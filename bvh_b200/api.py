@@ -421,6 +421,38 @@ class Bvh:
         self._nodes = self._node_index = None
         return int(rebuilt.value)
 
+    def add_shapes(self, shapes, max_growth: float = 1.5) -> int:
+        """Bvh::add_shape for every new shape (src/bvh/optimization.rs:67-207), batched: `shapes` (objects with .aabb(), or an AABB array)
+        get the indices num_shapes .. num_shapes+k-1.  max_growth >= 1: degraded subtrees on the changed paths are rebuilt; <= 0: the
+        grafts only (k = 1: the reference's own tree).  Returns the number of shapes in rebuilt subtrees.  The node index of every shape may
+        change: re-read node_index (set_bh_node_index) after every call.  Triangles set with set_triangles are discarded."""
+        aabbs = _gather_aabbs(shapes, self.prec)
+        rebuilt = C.c_size_t(0)
+        self._nodes = self._node_index = None
+        capi.check(getattr(capi.lib(), f"bvhgpu_add_shapes_{self._d['suffix']}")(self._h, _ptr(aabbs), len(aabbs), C.c_double(max_growth), C.byref(rebuilt)))
+        return int(rebuilt.value)
+
+    def remove_shapes(self, indices) -> np.ndarray:
+        """Bvh::remove_shape(i, swap_shape=true) for every index (src/bvh/optimization.rs:208-301), batched; indices are distinct, in the
+        numbering before the call.  Returns the renumbering as (m, 2) rows (new index, old index): apply it to your shape list, then
+        drop its last k entries.  The node index of every shape may change: re-read node_index after every call."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint32).reshape(-1)
+        n = self.num_shapes
+        self._nodes = self._node_index = None
+        capi.check(getattr(capi.lib(), f"bvhgpu_remove_shapes_{self._d['suffix']}")(self._h, _ptr(idx), len(idx)))
+        return swap_moves(n, idx)
+
+
+def swap_moves(n: int, indices) -> np.ndarray:
+    """The renumbering of Bvh.remove_shapes: (m, 2) rows (new index, old index) of the survivors that move.  Survivors with index
+    >= n-k take the vacated indices < n-k, smallest hole first (for k = 1: remove_shape(i, true) followed by pop())."""
+    rm = np.zeros(n, dtype=bool)
+    rm[np.asarray(indices, dtype=np.int64).reshape(-1)] = True
+    m = n - int(rm.sum())
+    holes = np.flatnonzero(rm[:m])
+    tail = m + np.flatnonzero(~rm[m:])
+    return np.stack([holes, tail], axis=1).astype(np.uint32).reshape(-1, 2)
+
 
 class Bvh2:
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays

@@ -118,6 +118,10 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_nearest_triangles_{s}").argtypes = [vp, C.c_int, vp, sz, vp, vp]
         getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, C.POINTER(C.c_size_t)]
         getattr(L, f"bvhgpu_optimize_{s}").argtypes = [vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
+        for f in ("add_shapes", "add_shapes_dev"):
+            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
+        for f in ("remove_shapes", "remove_shapes_dev"):
+            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz]
     for s in ("f32x2", "f64x2"):
         getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
         getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]

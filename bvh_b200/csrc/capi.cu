@@ -605,6 +605,115 @@ static int update_impl(Tree<T>* tree, const uint32_t* changed, const typename Tr
     return BVHGPU_OK;
 }
 
+// A relocation that failed half-way leaves arrays that no longer agree with each other: the failure is sticky, as a failed build's.
+template <class T> static int mark_failed(Tree<T>* tree, int rc, const char* who) {
+    char msg[1200];
+    snprintf(msg, sizeof msg, "%s failed after the tree was modified (%s); the tree is unusable", who, g_last_error.c_str());
+    tree->failed_status = rc; tree->failed_message = msg;
+    set_error("%s", msg);
+    return rc;
+}
+
+// Bvh::add_shape, batched: the k new shapes get indices n .. n+k-1.  The AABBs are staged next to the tree's own and checked for NaN
+// before the tree is touched.  n == 0: the call is bvhgpu_build_* over the k AABBs.
+template <class T>
+static int add_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size_t k, double max_growth, size_t* rebuilt, bool dev_input) {
+    if (!tree || (k && !aabbs)) { set_error("add_shapes: null argument"); return BVHGPU_ERR_INVALID; }
+    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("add_shapes: max_growth = %g, must be >= 1 (or <= 0 for no rebuild)", max_growth); return BVHGPU_ERR_INVALID; }
+    if (rebuilt) *rebuilt = 0;
+    if ((uint64_t)tree->n + k > (1ull << 30)) { set_error("add_shapes: %u + %zu shapes exceed 2^30 (u32 node indices); the tree was left unchanged", tree->n, k); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (k == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const typename Traits<T>::Aabb* d_in = aabbs;
+    if (!dev_input) {
+        typename Traits<T>::Aabb* staged = nullptr;
+        BVH_TRY(scratch.get(&staged, k));
+        BVH_CUDA_TRY(cudaMemcpyAsync(staged, aabbs, k * sizeof(*aabbs), cudaMemcpyHostToDevice, ctx->stream));
+        d_in = staged;
+    }
+    const uint32_t n = tree->n;
+    if (n == 0) {                                                       // an empty tree: exactly bvhgpu_build_*
+        Tree<T> fresh;
+        int rc = build_exact_sah<T>(ctx, d_in, (uint32_t)k, &fresh);
+        if (rc == BVHGPU_OK) rc = resolve_status(&fresh);
+        if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
+        dfree(ctx, tree->d_status); dfree(ctx, tree->d_sa_base); dfree(ctx, tree->d_tris);
+        tree->d_sa_base = nullptr; tree->d_tris = nullptr;
+        tree->n = fresh.n; tree->n_nodes = fresh.n_nodes; tree->d_status = fresh.d_status;
+        tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
+        BVH_TRY(build_traversal_records(tree));
+        if (tree->have_flat) BVH_TRY(build_flat(tree));
+        tree->status_pending = true;
+        return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+    }
+    typename Traits<T>::DAabb* all = nullptr;
+    uint32_t* flag = nullptr;
+    BVH_TRY(scratch.get(&flag, 1));
+    BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
+    int rc = cudaMemsetAsync(flag, 0, sizeof(uint32_t), ctx->stream) == cudaSuccess ? BVHGPU_OK : BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK && cudaMemcpyAsync(all, tree->d_aabb, sizeof(*all) * n, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) rc = BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK) rc = convert_aabbs<T>(ctx, d_in, (uint32_t)k, all + n, flag);
+    uint32_t* h = ctx->h_pinned + 212;
+    if (rc == BVHGPU_OK && (cudaMemcpyAsync(h, flag, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+                            cudaStreamSynchronize(ctx->stream) != cudaSuccess)) { set_error("add_shapes: CUDA error while staging the AABBs"); rc = BVHGPU_ERR_CUDA; }
+    if (rc == BVHGPU_OK && *h) { set_error("add_shapes: NaN coordinate in a new AABB; the tree was left unchanged"); rc = BVHGPU_ERR_NAN; }
+    if (rc != BVHGPU_OK) { dfree(ctx, all); return rc; }
+    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
+    rc = add_shapes<T>(tree, all, (uint32_t)k, max_growth);
+    if (rc != BVHGPU_OK) {
+        if (tree->d_aabb != all) { dfree(ctx, all); return rc; }            // failed before the tree was touched
+        return mark_failed(tree, rc, "add_shapes");
+    }
+    tree->status_pending = true;
+    if (dev_input && !rebuilt) return BVHGPU_OK;                        // asynchronous from here on
+    BuildStatus hs;
+    BVH_CUDA_TRY(cudaMemcpyAsync(&hs, tree->d_status, sizeof(hs), cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_TRY(resolve_status(tree));
+    if (rebuilt && max_growth > 0.0) *rebuilt = hs.rebuilt;
+    return BVHGPU_OK;
+}
+
+// Bvh::remove_shape(i, swap_shape = true), batched: `indices` are distinct shape indices before the call; survivors >= n-k take the
+// vacated indices < n-k, smallest hole first.  Checked (range, duplicates) before the tree is touched.
+template <class T>
+static int remove_impl(Tree<T>* tree, const uint32_t* indices, size_t k, bool dev_input) {
+    if (!tree || (k && !indices)) { set_error("remove_shapes: null argument"); return BVHGPU_ERR_INVALID; }
+    if (k > tree->n) { set_error("remove_shapes: %zu indices for a tree over %u shapes; the tree was left unchanged", k, tree->n); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (k == 0) return BVHGPU_OK;
+    const uint32_t n = tree->n;
+    Scratch scratch(ctx);
+    const uint32_t* d_idx = indices;
+    if (!dev_input) {
+        uint32_t* c = nullptr;
+        BVH_TRY(scratch.get(&c, k));
+        BVH_CUDA_TRY(cudaMemcpyAsync(c, indices, sizeof(uint32_t) * k, cudaMemcpyHostToDevice, ctx->stream));
+        d_idx = c;
+    }
+    uint32_t *rm = nullptr, *flags = nullptr;
+    BVH_TRY(scratch.get(&rm, (size_t)n + 1));
+    BVH_TRY(scratch.get(&flags, 2));
+    BVH_CUDA_TRY(cudaMemsetAsync(rm, 0, sizeof(uint32_t) * ((size_t)n + 1), ctx->stream));
+    BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), ctx->stream));
+    BVH_TRY(remove_check(ctx, d_idx, (uint32_t)k, n, rm, flags));
+    uint32_t* h = ctx->h_pinned + 216;
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (h[0]) { set_error("remove_shapes: a shape index is >= %u; the tree was left unchanged", n); return BVHGPU_ERR_INVALID; }
+    if (h[1]) { set_error("remove_shapes: a shape index is listed twice; the tree was left unchanged"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
+    const void* nodes_before = tree->d_nodes;
+    const int rrc = remove_shapes<T>(tree, rm, (uint32_t)k);
+    if (rrc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rrc : mark_failed(tree, rrc, "remove_shapes");
+    tree->status_pending = true;
+    return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+}
+
 }  // namespace bvhb200
 
 using namespace bvhb200;
@@ -963,6 +1072,18 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_update_dev_##SUF(TREE* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt) { \
         return update_impl<T>(tree, (const uint32_t*)dev_changed, (const AABB*)dev_changed_aabbs, m, max_growth, rebuilt, true); \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) { \
+        return add_impl<T>(tree, aabbs, k, max_growth, rebuilt, false);                                                   \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_add_shapes_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt) { \
+        return add_impl<T>(tree, (const AABB*)dev_aabbs, k, max_growth, rebuilt, true);                                   \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                            \
+        return remove_impl<T>(tree, indices, k, false);                                                                   \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_remove_shapes_dev_##SUF(TREE* tree, const void* dev_indices, size_t k) {                        \
+        return remove_impl<T>(tree, (const uint32_t*)dev_indices, k, true);                                               \
     }
 
 #define DEFINE_API2(T, SUF, TREE, AABB, RAY, NODE, FLAT)                                                                   \

@@ -569,7 +569,7 @@ int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, dou
     const uint32_t n = tree->n, nn = tree->n_nodes;
     const bool rebuild = max_growth > 0.0;
     if (n < 3) return rebuild ? optimize(tree, max_growth) : refit(tree);
-    const unsigned gn = (nn + 255) / 256, gm = (m + 255) / 256;
+    const unsigned gm = (m + 255) / 256;
     if (!tree->d_arrive) {
         BVH_TRY(dalloc_t(ctx, &tree->d_arrive, nn));
         BVH_CUDA_TRY(cudaMemsetAsync(tree->d_arrive, 0, sizeof(uint32_t) * nn, st));
@@ -578,14 +578,9 @@ int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, dou
         BVH_TRY(dalloc_t(ctx, &tree->d_bad, nn));
         BVH_CUDA_TRY(cudaMemsetAsync(tree->d_bad, 0, nn, st));
     }
-    if (rebuild && !tree->d_sa_base) {                                  // first update on this tree: the baseline is the tree before the motion
-        BVH_TRY(dalloc(ctx, &tree->d_sa_base, sizeof(T) * nn));
-        node_sa_kernel<T><<<gn, 256, 0, st>>>(tree->d_nodes, nn, reinterpret_cast<T*>(tree->d_sa_base));
-        ctx->launches++;
-    }
+    if (rebuild) BVH_TRY(ensure_sa_base(tree));                         // first update on this tree: the baseline is the tree before the motion
     Scratch scratch(ctx);
-    uint32_t *dirty = nullptr, *cnts = nullptr, *roots = nullptr, *idx0 = nullptr;
-    T* cb_roots = nullptr;
+    uint32_t *dirty = nullptr, *cnts = nullptr;
     BVH_TRY(scratch.get(&dirty, nn));
     BVH_TRY(scratch.get(&cnts, 2));                                     // [0] dirty nodes, [1] rebuild roots
     BVH_CUDA_TRY(cudaMemsetAsync(cnts, 0, 2 * sizeof(uint32_t), st));
@@ -593,22 +588,45 @@ int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, dou
     climb_paths_kernel<T><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
                                               reinterpret_cast<const T*>(tree->d_sa_base), (T)max_growth, rebuild ? tree->d_bad : nullptr, dirty, cnts);
     ctx->launches += 2;
-    if (rebuild) {
-        BVH_TRY(scratch.get(&roots, n));
-        BVH_TRY(scratch.get(&idx0, n));
-        BVH_TRY(scratch.get(&cb_roots, 6 * (size_t)n / 2 + 6));         // rebuild roots are inner nodes of disjoint subtrees: at most n / 2 of them
-        select_roots_dirty_kernel<T><<<gn, 256, 0, st>>>(tree->d_nodes, tree->d_bad, dirty, cnts, roots, cnts + 1);
-        root_prep_kernel<T><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, tree->d_aabb, roots, cnts + 1, idx0, cb_roots);
-        ctx->launches += 2;
-        BVH_CUDA_TRY(cudaGetLastError());
-        BVH_TRY(rebuild_subtrees(ctx, tree, roots, cnts + 1, cb_roots, idx0, true));
-        rebase_kernel<T><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, reinterpret_cast<T*>(tree->d_sa_base));
-        clear_bad_kernel<<<gn, 256, 0, st>>>(dirty, cnts, tree->d_bad);
-        ctx->launches += 2;
-    }
+    if (rebuild) BVH_TRY(rebuild_degraded(tree, dirty, cnts));
     BVH_CUDA_TRY(cudaGetLastError());
     BVH_TRY(build_traversal_records(tree));
     if (tree->have_flat) BVH_TRY(build_flat(tree));
+    return BVHGPU_OK;
+}
+
+// The surface-area baseline of the growth test: the tree as it is now, unless one exists already.
+template <class T> int ensure_sa_base(Tree<T>* tree) {
+    if (tree->d_sa_base || tree->n_nodes == 0) return BVHGPU_OK;
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_TRY(dalloc(ctx, &tree->d_sa_base, sizeof(T) * tree->n_nodes));
+    node_sa_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, reinterpret_cast<T*>(tree->d_sa_base));
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+// dirty[0 .. cnts[0]) = the nodes whose box changed, tree->d_bad = their growth flags.  Rebuilds in place the outermost degraded
+// subtrees (cnts[1], zero on entry, counts them), gives them fresh baselines and clears the flags.
+template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* dirty, uint32_t* cnts) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = tree->n, gn = (tree->n_nodes + 255) / 256;
+    Scratch scratch(ctx);
+    uint32_t *roots = nullptr, *idx0 = nullptr;
+    T* cb_roots = nullptr;
+    BVH_TRY(scratch.get(&roots, n));
+    BVH_TRY(scratch.get(&idx0, n));
+    BVH_TRY(scratch.get(&cb_roots, 6 * (size_t)n / 2 + 6));             // rebuild roots are inner nodes of disjoint subtrees: at most n / 2 of them
+    select_roots_dirty_kernel<T><<<gn, 256, 0, st>>>(tree->d_nodes, tree->d_bad, dirty, cnts, roots, cnts + 1);
+    root_prep_kernel<T><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, tree->d_aabb, roots, cnts + 1, idx0, cb_roots);
+    ctx->launches += 2;
+    BVH_CUDA_TRY(cudaGetLastError());
+    BVH_TRY(rebuild_subtrees(ctx, tree, roots, cnts + 1, cb_roots, idx0, true));
+    rebase_kernel<T><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, reinterpret_cast<T*>(tree->d_sa_base));
+    clear_bad_kernel<<<gn, 256, 0, st>>>(dirty, cnts, tree->d_bad);
+    ctx->launches += 2;
+    BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
 }
 
@@ -632,6 +650,8 @@ int update_scatter(Tree<T>* tree, const uint32_t* d_changed, const typename Trai
 
 #define INST(T)                                           \
     template int update_incremental<T>(Tree<T>*, const uint32_t*, uint32_t, double); \
+    template int ensure_sa_base<T>(Tree<T>*);             \
+    template int rebuild_degraded<T>(Tree<T>*, const uint32_t*, uint32_t*); \
     template int update_changed<T>(Tree<T>*, const uint32_t*, const typename Traits<T>::Aabb*, uint32_t, uint32_t*); \
     template int update_scatter<T>(Tree<T>*, const uint32_t*, const typename Traits<T>::Aabb*, uint32_t); \
     template int optimize<T>(Tree<T>*, double);           \

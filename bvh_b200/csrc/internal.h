@@ -174,6 +174,17 @@ template <class T> int optimize(Tree<T>* tree, double max_growth);   // refit + 
 template <class T> int update_changed(Tree<T>* tree, const uint32_t* d_changed, const typename Traits<T>::Aabb* d_fresh, uint32_t m, uint32_t* d_flags);
 template <class T> int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth);
 template <class T> int update_scatter(Tree<T>* tree, const uint32_t* d_changed, const typename Traits<T>::Aabb* d_fresh, uint32_t m);
+// growth test helpers shared by update_incremental and add_shapes
+template <class T> int ensure_sa_base(Tree<T>* tree);
+template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* d_dirty, uint32_t* d_cnts /* [0] dirty nodes, [1] roots (zeroed) */);
+
+// ---- dynamic.cu: Bvh::add_shape / remove_shape, batched ----
+// aabb_all: [n + k] device AABBs (the tree's n followed by the k new ones, checked for NaN); becomes tree->d_aabb.
+template <class T> int add_shapes(Tree<T>* tree, typename Traits<T>::DAabb* aabb_all, uint32_t k, double max_growth);
+// d_rm: [n + 1] removed flag of every shape (0 / 1, the last word 0), k = number of removed shapes, 1 <= k <= n.
+template <class T> int remove_shapes(Tree<T>* tree, const uint32_t* d_rm, uint32_t k);
+// validation of a removal list: d_rm[n + 1] zeroed by the caller; d_flags[0] = index >= n, d_flags[1] = duplicate index
+int remove_check(bvhgpu_ctx* ctx, const uint32_t* d_idx, uint32_t k, uint32_t n, uint32_t* d_rm, uint32_t* d_flags);
 
 // ---- traverse.cu ----
 // d_rays: rays on the device; fmt: BVHGPU_RAYS_FULL (9 scalars: the C-ABI Ray) or BVHGPU_RAYS_OD (6 scalars: origin, direction).

@@ -383,6 +383,38 @@ int bvhgpu_update_f64x3(bvhgpu_tree3d* tree, const uint32_t* changed, const bvh_
 int bvhgpu_update_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
 int bvhgpu_update_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
 
+/* ---- add / remove shapes: Bvh::add_shape / Bvh::remove_shape (src/bvh/optimization.rs:67-301), batched ----
+ * add: the k new shapes get indices n .. n+k-1 in the order given (the reference's shapes.push(s); add_shape(len-1)).  Every new
+ * shape picks its insertion point by the reference's descent, evaluated against the tree as it was before the call (all k descents
+ * are independent).  At each insertion point p a new inner node takes p's place: its left child is the exact-SAH subtree over the
+ * shapes that chose p (ascending index order; a leaf for one shape), its right child p's old subtree; the ancestors' boxes are
+ * refitted.  For k = 1 this is the reference's own topology, and its own tree whenever the boxes are tight (every built tree except
+ * f32 trees whose surface areas overflow, where the builder stores empty child boxes: there the device refits the affected paths up to
+ * the root, the reference stops at the first box that does not change, so boxes on those paths can differ).  max_growth >= 1: then the growth test of bvhgpu_update_* runs on the
+ * changed ancestors and the degraded subtrees are rebuilt in place; *rebuilt (may be NULL) = shapes in those subtrees.
+ * max_growth <= 0: no rebuild, *rebuilt = 0.  n == 0: the call is bvhgpu_build_* over the k AABBs.  Triangles set with
+ * bvhgpu_tree_set_triangles_* are discarded (the triangle forms of closest_hit / nearest return BVHGPU_ERR_INVALID until set again).
+ * remove: `indices` are distinct shape indices (numbering before the call).  Removed leaves go; an inner node left with one child
+ * is replaced by that child (the reference's connect_nodes); boxes on the affected paths are refitted (same caveat for non-tight trees
+ * as for add: the topology and node indices are the reference's, the boxes are on tight trees); nothing is rebuilt.
+ * Renumbering (remove_shape with swap_shape = true): the survivors with index >= n-k move into the vacated indices < n-k, in
+ * ascending order on both sides (smallest hole <- smallest surviving tail index).  For k = 1 that is remove_shape(i, true) + pop();
+ * for k > 1 it is NOT k sequential swap-removes (removing {0,1,2} of 5 shapes sequentially gives [4,3], here [3,4]).  Triangles
+ * follow their shapes.  swap_shape == false is not representable: device trees number their shapes densely.
+ * Both: NaN AABBs (BVHGPU_ERR_NAN), indices >= n, duplicates, k > n on remove and n + k > 2^30 (BVHGPU_ERR_INVALID) are rejected
+ * before the tree is touched.  The node index of EVERY shape may change (preorder positions shift): re-read them with
+ * bvhgpu_tree_nodes_* after every call.  The tree stays in Bvh::build's preorder layout: it is the same tree that
+ * bvhgpu_tree_from_nodes_* makes from its node array and AABBs.  _dev_: inputs on the device; validated synchronously, the rest
+ * is asynchronous (as bvhgpu_update_dev_*). */
+int bvhgpu_add_shapes_f32x3(bvhgpu_tree3f* tree, const bvh_aabb3f* aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_f64x3(bvhgpu_tree3d* tree, const bvh_aabb3d* aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_remove_shapes_f32x3(bvhgpu_tree3f* tree, const uint32_t* indices, size_t k);
+int bvhgpu_remove_shapes_f64x3(bvhgpu_tree3d* tree, const uint32_t* indices, size_t k);
+int bvhgpu_remove_shapes_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_indices, size_t k);
+int bvhgpu_remove_shapes_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_indices, size_t k);
+
 #ifdef __cplusplus
 }
 #endif

@@ -99,6 +99,8 @@ template <> struct Abi<float> {
     static int update(tree* t, const uint32_t* c, const aabb* a, size_t m, double g, size_t* r) { return bvhgpu_update_f32x3(t, c, a, m, g, r); }
     static int set_triangles(tree* t, const float* abc, size_t n) { return bvhgpu_tree_set_triangles_f32x3(t, abc, n); }
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_closest_hit_f32x3(t, r, n, tri, s, d, uv); }
+    static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f32x3(t, a, k, g, r); }
+    static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
 };
 template <> struct Abi<double> {
     using aabb = bvh_aabb3d; using ray = bvh_ray3d; using node = bvh_node3d; using flat = bvh_flat3d; using tree = bvhgpu_tree3d;
@@ -114,6 +116,8 @@ template <> struct Abi<double> {
     static int update(tree* t, const uint32_t* c, const aabb* a, size_t m, double g, size_t* r) { return bvhgpu_update_f64x3(t, c, a, m, g, r); }
     static int set_triangles(tree* t, const double* abc, size_t n) { return bvhgpu_tree_set_triangles_f64x3(t, abc, n); }
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_closest_hit_f64x3(t, r, n, tri, s, d, uv); }
+    static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f64x3(t, a, k, g, r); }
+    static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
 };
 struct Ctx {
     bvhgpu_ctx* h = nullptr;
@@ -330,7 +334,63 @@ template <class T> class Bvh {
     }
     size_t num_shapes() const { return n_; }
 
+    // Bvh::add_shape(shapes, new_shape_index) (src/bvh/optimization.rs:67-207): the caller has pushed the new shape, which must be the
+    // last one.  No rebuild (max_growth 0): the reference's own topology.  The node index of EVERY shape may change (preorder positions
+    // shift), so all of them are written back with set_bh_node_index.
+    template <class Shape> void add_shape(std::vector<Shape>& shapes, size_t new_shape_index) {
+        if (new_shape_index + 1 != shapes.size() || new_shape_index != n_)
+            throw Error(BVHGPU_ERR_INVALID, "add_shape: the new shape must be the last one, at index num_shapes()");
+        add_shapes(shapes, new_shape_index, 0.0);
+    }
+    // Batched add: shapes[first_new ..] are new (first_new == num_shapes()); max_growth >= 1 also rebuilds degraded subtrees.
+    // Returns the number of shapes in rebuilt subtrees.
+    template <class Shape> size_t add_shapes(std::vector<Shape>& shapes, size_t first_new, double max_growth = 1.5) {
+        if (first_new != n_ || first_new > shapes.size()) throw Error(BVHGPU_ERR_INVALID, "add_shapes: first_new must be num_shapes()");
+        std::vector<typename A::aabb> boxes(shapes.size() - first_new);
+        for (size_t i = 0; i < boxes.size(); ++i) {
+            const Aabb<T> a = shapes[first_new + i].aabb();
+            for (int k = 0; k < 3; ++k) { boxes[i].min[k] = a.min[k]; boxes[i].max[k] = a.max[k]; }
+        }
+        size_t rebuilt = 0;
+        check(A::add(tree_, boxes.data(), boxes.size(), max_growth, &rebuilt));
+        n_ = shapes.size();
+        write_node_indices(shapes);
+        return rebuilt;
+    }
+    // Bvh::remove_shape(shapes, i, swap_shape) (src/bvh/optimization.rs:208-301).  swap_shape == true: the last shape takes index i,
+    // in the tree and in `shapes` (swap_remove), as the reference does.  swap_shape == false is not representable -- device trees
+    // number their shapes densely -- and throws Error(BVHGPU_ERR_UNSUPPORTED).
+    template <class Shape> void remove_shape(std::vector<Shape>& shapes, size_t i, bool swap_shape) {
+        if (!swap_shape) throw Error(BVHGPU_ERR_UNSUPPORTED, "remove_shape: swap_shape == false is not supported (device trees number their shapes densely)");
+        remove_shapes(shapes, std::vector<size_t>{i});
+    }
+    // Batched remove of distinct indices: survivors with index >= n-k move into the vacated indices < n-k, smallest hole first, in the
+    // tree and in `shapes`, which then loses its last k entries.  For one index this is remove_shape(i, true).
+    template <class Shape> void remove_shapes(std::vector<Shape>& shapes, const std::vector<size_t>& indices) {
+        if (shapes.size() != n_) throw Error(BVHGPU_ERR_INVALID, "remove_shapes: shapes.size() != num_shapes()");
+        std::vector<uint32_t> idx(indices.size());
+        for (size_t j = 0; j < idx.size(); ++j) idx[j] = (uint32_t)indices[j];
+        check(A::remove(tree_, idx.data(), idx.size()));
+        const size_t k = indices.size(), m = n_ - k;
+        std::vector<char> gone(n_, 0);
+        for (size_t s : indices) gone[s] = 1;
+        size_t t = m;
+        for (size_t h = 0; h < m; ++h) {
+            if (!gone[h]) continue;
+            while (gone[t]) ++t;
+            std::swap(shapes[h], shapes[t++]);
+        }
+        shapes.erase(shapes.begin() + (std::ptrdiff_t)m, shapes.end());
+        n_ = m;
+        write_node_indices(shapes);
+    }
+
   private:
+    template <class Shape> void write_node_indices(std::vector<Shape>& shapes) {
+        std::vector<uint32_t> idx(shapes.size());
+        if (!idx.empty()) check(A::nodes(tree_, nullptr, idx.data()));
+        for (size_t i = 0; i < shapes.size(); ++i) shapes[i].set_bh_node_index(idx[i]);
+    }
     void release() { if (tree_) { A::free_tree(tree_); tree_ = nullptr; } }
     std::shared_ptr<detail::Ctx> ctx_;
     typename A::tree* tree_ = nullptr;
