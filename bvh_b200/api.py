@@ -23,7 +23,7 @@ from typing import Iterable, Sequence
 import numpy as np
 
 from . import capi
-from .dtypes import BY_PREC, BY_PREC_2D, U32_MAX
+from .dtypes import BY_PREC, BY_PREC_2D, BY_PREC_4D, U32_MAX
 
 
 def _ptr(a):
@@ -458,13 +458,15 @@ class Bvh2:
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays
     (bvhgpu_*_f32x2 / _f64x2).  Rays: structured array with 2-component origin, direction (normalised), inv_direction."""
 
+    _TABLE = BY_PREC_2D
+
     def __init__(self, handle, prec: str, ctx: Context, n: int):
-        self._h, self.prec, self.ctx, self._d, self.n = handle, prec, ctx, BY_PREC_2D[prec], n
+        self._h, self.prec, self.ctx, self._d, self.n = handle, prec, ctx, self._TABLE[prec], n
 
     @classmethod
     def build(cls, aabbs, prec: str = "f32", ctx: Context | None = None, mode: int = capi.BUILD_EXACT_SAH) -> "Bvh2":
         ctx = ctx or Context.default()
-        d = BY_PREC_2D[prec]
+        d = cls._TABLE[prec]
         a = np.ascontiguousarray(aabbs, dtype=d["aabb"])
         h = C.c_void_p()
         capi.check(getattr(capi.lib(), f"bvhgpu_build_{d['suffix']}")(ctx._h, _ptr(a), len(a), mode, C.byref(h)))
@@ -509,3 +511,20 @@ class Bvh2:
                 continue
             capi.check(st)
             return offsets, hits[: total.value]
+
+
+class Bvh4(Bvh2):
+    """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten and batched
+    ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction)."""
+
+    _TABLE = BY_PREC_4D
+
+    def traverse_dev(self, rays_ptr: int, nrays: int, offsets_ptr: int, hits_ptr: int, cap: int, mode: int = capi.TRAVERSE_BVH,
+                     want_total: bool = False):
+        """Device pointers (e.g. torch tensors' data_ptr()), enqueued on the context's stream.  want_total = False: no host
+        synchronisation, hits beyond `cap` are dropped."""
+        total = C.c_size_t(0)
+        fn = getattr(capi.lib(), f"bvhgpu_traverse_dev_{self._d['suffix']}")
+        capi.check(fn(self._h, mode, C.c_void_p(rays_ptr), nrays, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
+                      C.byref(total) if want_total else None))
+        return total.value if want_total else None

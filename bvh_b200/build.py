@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 SO = os.path.join(HERE, "libbvh_b200.so")
-SOURCES = ["capi.cu", "build_sah.cu", "flatten.cu", "traverse.cu", "lbvh.cu", "closest.cu", "dim2.cu", "dynamic.cu"]
+SOURCES = ["capi.cu", "build_sah.cu", "flatten.cu", "traverse.cu", "lbvh.cu", "closest.cu", "dim2.cu", "dynamic.cu", "dim4.cu"]
 HEADERS = ["common.cuh", "internal.h", "build_types.cuh", os.path.join("..", "..", "include", "bvh_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [

@@ -131,7 +131,17 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_tree_nodes_{s}").argtypes = [vp, vp, vp]
         getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
         getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-    missing = [n for n in declared_symbols() if not hasattr(L, n)]
+    for s in ("f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
+        getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]
+        getattr(L, f"bvhgpu_tree_free_{s}").restype = None
+        getattr(L, f"bvhgpu_tree_num_shapes_{s}").argtypes = [vp]
+        getattr(L, f"bvhgpu_tree_num_shapes_{s}").restype = sz
+        getattr(L, f"bvhgpu_tree_nodes_{s}").argtypes = [vp, vp, vp]
+        getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_traverse_dev_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
+    missing =[n for n in declared_symbols() if not hasattr(L, n)]
     if missing:
         raise ImportError(f"{SO_PATH} does not export {missing}")
     _lib = L

@@ -1,0 +1,932 @@
+// bvh_b200/csrc/dim4.cu -- D = 4: Bvh<T,4>::build (exact 6-bucket SAH), flatten and batched ray traversal, f32 and f64.
+//
+// The reference is generic in D (src/bvh/bvh_node.rs:81-279, src/flat_bvh.rs:60-143, src/ray/intersect_default.rs:16-37) and ships
+// 4-wide slab tests for Ray<f32,4> / Ray<f64,4> (src/ray/intersect_simd.rs).  A fourth axis cannot hide in the 3-D kernels the way
+// D = 2 hides in z = 0 (dim2.cu): surface areas, largest_axis and the slab test all see it.  So D = 4 has its own pipeline here, with
+// its own node / record types and its own Tree4<T>; it shares the exact-arithmetic helpers and keys of common.cuh, Scratch, and the
+// CSR scan kernels of traverse.cu.  DESIGN.md section 4.11 describes the design.
+//
+// Builder (bit-identical to Bvh::build in the sense of DESIGN.md section 2):
+//   ranges of more than SMALL4 shapes: level-synchronous.  Per level: prep (tile numbering, bucket identities), bin (one warp per
+//     TILE4 shapes: bucket counts + min/max keys of boxes and centres, folded with warp REDUX, flushed with global atomics), split
+//     (one warp per range: the 5 candidate costs in exact arithmetic, the node, the child ranges, the stable per-tile destinations),
+//     scatter (one warp per tile, stable by ballots).  The host reads back one word per level: the number of ranges left.
+//   ranges of at most SMALL4 shapes: one warp each, depth-first with an explicit stack in shared memory.  The smaller child is
+//     split first and the larger one is pushed, so the stack never holds more than log2(SMALL4) + 1 entries, however skewed the range.
+// Node positions depend only on counts (cl = me + 1, cr = me + 2 nl) and every reduction is a min / max / sum of integers, so the
+// order in which warps run never shows in the result: two builds of the same input are byte-identical.
+#include "internal.h"
+#include <algorithm>
+#include <new>
+
+namespace bvhb200 {
+
+// ---- device layouts -----------------------------------------------------------------------------------------------------------
+// Traversal record: the AABB the node has in its parent, `skip` (first record behind the subtree) and the shape index of a leaf.
+// Sized in whole 16-byte granules so that a record is fetched with 128-bit non-coherent loads only: 3 for f32, 5 for f64.
+struct __align__(16) TRec4F { float min[4]; float max[4]; uint32_t skip, shape, pad[2]; };    // 48 B
+struct __align__(16) TRec4D { double min[4]; double max[4]; uint32_t skip, shape, pad[2]; };  // 80 B
+static_assert(sizeof(TRec4F) == 48 && sizeof(TRec4D) == 80, "4-D record size");
+static_assert(sizeof(bvh_aabb4f) == 32 && sizeof(bvh_aabb4d) == 64 && sizeof(bvh_ray4f) == 48 && sizeof(bvh_ray4d) == 96, "4-D POD size");
+static_assert(sizeof(bvh_node4f) == 80 && sizeof(bvh_node4d) == 144 && sizeof(bvh_flat4f) == 44 && sizeof(bvh_flat4d) == 80, "4-D POD size");
+
+template <class T> struct D4;
+template <> struct D4<float> { using Aabb = bvh_aabb4f; using Ray = bvh_ray4f; using Node = bvh_node4f; using Flat = bvh_flat4f; using Rec = TRec4F; };
+template <> struct D4<double> { using Aabb = bvh_aabb4d; using Ray = bvh_ray4d; using Node = bvh_node4d; using Flat = bvh_flat4d; using Rec = TRec4D; };
+
+template <class T> struct Tree4 {
+    using Aabb = typename D4<T>::Aabb; using Node = typename D4<T>::Node; using Flat = typename D4<T>::Flat; using Rec = typename D4<T>::Rec;
+    bvhgpu_ctx* ctx = nullptr;
+    uint32_t n = 0, n_nodes = 0;
+    Aabb* d_aabb = nullptr;            // [n]      shape AABBs (ABI layout: already whole sectors)
+    Node* d_nodes = nullptr;           // [2n-1]   Bvh.nodes, reference preorder layout
+    uint32_t* d_node_index = nullptr;  // [n]      leaf node of every shape
+    uint32_t* d_node_start = nullptr;  // [2n-1]   first position of the node's shape range (== leaves before it)
+    Rec* d_trec = nullptr;             // [n_trec] traversal records (built on first use)
+    uint32_t n_trec = 0;
+    Flat* d_flat = nullptr;            // [n_flat] FlatBvh (built on demand)
+    size_t n_flat = 0;
+    int failed_status = 0;             // sticky (DESIGN.md section 1)
+    std::string failed_message;
+    uint32_t* d_offsets = nullptr; size_t offsets_cap = 0;   // result buffers of the host-pointer traversal
+    uint32_t* d_hits = nullptr;    size_t hits_cap = 0;
+};
+
+constexpr uint32_t SMALL4 = 256;     // ranges this small are finished by one warp (depth-first, shared-memory stack)
+constexpr uint32_t TILE4 = 512;      // shapes per warp tile of a large range
+constexpr int STACK4 = 12;           // > log2(SMALL4) + 1: the smaller-child-first order bounds the stack
+constexpr uint32_t CTL_NEXT = 0, CTL_SMALL = 1, CTL_ERROR = 2, CTL_NAN = 3;
+
+template <class T> struct __align__(16) Task4 {
+    uint32_t start, count, node, parent;
+    uint32_t buf, pad[3];              // index buffer that holds the range
+    T ab[8];                           // aabb_bounds      (min xyzw, max xyzw)
+    T cb[8];                           // centroid_bounds
+};
+
+// key slot k of a bucket: 0..3 box min, 4..7 box max, 8..11 centre min, 12..15 centre max
+__device__ __forceinline__ bool kmin4(int k) { return ((k >> 2) & 1) == 0; }
+template <class Key> __device__ __forceinline__ Key fold_key(int k, Key acc, Key v) { return kmin4(k) ? (v < acc ? v : acc) : (v > acc ? v : acc); }
+
+__device__ __forceinline__ void load4(const bvh_aabb4f* p, float mn[4], float mx[4]) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+    mn[0] = a.x; mn[1] = a.y; mn[2] = a.z; mn[3] = a.w; mx[0] = b.x; mx[1] = b.y; mx[2] = b.z; mx[3] = b.w;
+}
+__device__ __forceinline__ void load4(const bvh_aabb4d* p, double mn[4], double mx[4]) {
+    const double2* q = reinterpret_cast<const double2*>(p);
+    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);
+    mn[0] = a.x; mn[1] = a.y; mn[2] = b.x; mn[3] = b.y; mx[0] = c.x; mx[1] = c.y; mx[2] = d.x; mx[3] = d.y;
+}
+
+// Aabb::surface_area for D = 4: 2 * (((sx*sx + sy*sy) + sz*sz) + sw*sw), left to right, no FMA.
+template <class T> __device__ __forceinline__ T surface_area4(const T mn[4], const T mx[4]) {
+    T acc = add_rn(mul_rn(sub_rn(mx[0], mn[0]), sub_rn(mx[0], mn[0])), mul_rn(sub_rn(mx[1], mn[1]), sub_rn(mx[1], mn[1])));
+    acc = add_rn(acc, mul_rn(sub_rn(mx[2], mn[2]), sub_rn(mx[2], mn[2])));
+    acc = add_rn(acc, mul_rn(sub_rn(mx[3], mn[3]), sub_rn(mx[3], mn[3])));
+    return mul_rn(T(2), acc);
+}
+
+// How a range is split: largest_axis (first strict maximum) of the centroid extent, halving below T::EPSILON (bvh_node.rs:114-124).
+template <class T> struct Plan4 { int axis; T cmin, ext; bool halve; uint32_t half; };
+template <class T> __device__ __forceinline__ Plan4<T> plan4(const T cb[8], uint32_t count) {
+    Plan4<T> p;
+    T size[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) size[k] = sub_rn(cb[4 + k], cb[k]);
+    p.axis = 0; p.ext = size[0]; p.cmin = cb[0];
+#pragma unroll
+    for (int k = 1; k < 4; ++k) if (size[k] > p.ext) { p.axis = k; p.ext = size[k]; p.cmin = cb[k]; }
+    p.halve = p.ext < Traits<T>::eps();
+    p.half = count / 2;
+    return p;
+}
+// bucket of a shape (bvh_node.rs:204-222) or its half of a halved range
+template <class T> __device__ __forceinline__ int bucket4(const Plan4<T>& p, const T c[4], uint32_t rel_pos) {
+    if (p.halve) return rel_pos < p.half ? 0 : 1;
+    const T ca = p.axis == 0 ? c[0] : (p.axis == 1 ? c[1] : (p.axis == 2 ? c[2] : c[3]));
+    const T K = sub_rn(T(6), T(0.01));                       // T::from(NUM_BUCKETS) - T::from(0.01), bvh_node.rs:214-215
+    int b = (int)mul_rn(div_rn(sub_rn(ca, p.cmin), p.ext), K);   // to_usize(): truncation toward zero
+    return b < 0 ? 0 : (b > 5 ? 5 : b);                       // inert for tight bounds; keeps memory safe
+}
+
+// Bins positions [p0, p1) of src (range starting at r0).  Lane k < 16 folds key k of every bucket into acc[]; cnt[] is warp-uniform.
+// The bucket of every position is kept in bkt[] for the scatter.
+template <class T>
+__device__ __forceinline__ void bin4(const typename D4<T>::Aabb* __restrict__ aabb, const uint32_t* src, uint8_t* bkt, uint32_t r0,
+                                     uint32_t p0, uint32_t p1, const Plan4<T>& pl, typename Traits<T>::Key acc[6], uint32_t cnt[6]) {
+    using Tr = Traits<T>;
+    using Key = typename Tr::Key;
+    const int lane = (int)lane_id();
+#pragma unroll
+    for (int bb = 0; bb < 6; ++bb) { acc[bb] = kmin4(lane & 15) ? Tr::KEY_POS_INF : Tr::KEY_NEG_INF; cnt[bb] = 0; }
+    for (uint32_t base = p0; base < p1; base += 32) {
+        const uint32_t pos = base + lane;
+        T mn[4], mx[4], c[4];
+        int b = -1;
+        if (pos < p1) {
+            load4(aabb + __ldcg(src + pos), mn, mx);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) c[k] = center1(mn[k], mx[k]);
+            b = bucket4(pl, c, pos - r0);
+            bkt[pos] = (uint8_t)b;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) mn[k] = mx[k] = c[k] = T(0);
+        }
+#pragma unroll
+        for (int bb = 0; bb < 6; ++bb) {
+            const uint32_t m = __ballot_sync(0xffffffffu, b == bb);
+            if (!m) continue;                                      // warp-uniform
+            cnt[bb] += __popc(m);
+            const bool in = b == bb;
+#pragma unroll
+            for (int k = 0; k < 16; ++k) {
+                const T val = k < 4 ? mn[k & 3] : (k < 8 ? mx[k & 3] : c[k & 3]);
+                const bool is_min = kmin4(k);
+                const Key v = in ? f2key(val) : (is_min ? Tr::KEY_POS_INF : Tr::KEY_NEG_INF);
+                const Key r = is_min ? warp_min_key(v) : warp_max_key(v);
+                if (lane == k) acc[bb] = is_min ? (r < acc[bb] ? r : acc[bb]) : (r > acc[bb] ? r : acc[bb]);
+            }
+        }
+    }
+}
+
+// Stable 6-way partition of positions [p0, p1) of src into dst; dest[b] = next free position of bucket b (warp-uniform, advanced).
+__device__ __forceinline__ void scatter4(const uint32_t* src, uint32_t* dst, const uint8_t* bkt, uint32_t p0, uint32_t p1, uint32_t dest[6]) {
+    const uint32_t lane = lane_id(), lt = lanemask_lt();
+    for (uint32_t base = p0; base < p1; base += 32) {
+        const uint32_t pos = base + lane;
+        const bool valid = pos < p1;
+        const uint32_t id = valid ? __ldcg(src + pos) : 0u;
+        const int b = valid ? (int)bkt[pos] : -1;
+        uint32_t d = 0;
+#pragma unroll
+        for (int bb = 0; bb < 6; ++bb) {
+            const uint32_t m = __ballot_sync(0xffffffffu, b == bb);
+            if (b == bb) d = dest[bb] + __popc(m & lt);
+            dest[bb] += __popc(m);
+        }
+        if (valid) __stcg(dst + d, id);
+    }
+}
+
+// The split (bvh_node.rs:225-279) from the six buckets: keys[b * 16 + k], cnt[b].  One thread.  child = lab, lcb, rab, rcb (8 T each);
+// Aabb::empty() for all four when no candidate cost is < +inf.  Returns the left count.
+template <class T>
+__device__ uint32_t split4(const typename Traits<T>::Key* keys, const uint32_t cnt[6], const T ab[8], const Plan4<T>& pl, T child[32]) {
+    using Tr = Traits<T>;
+    using Key = typename Tr::Key;
+    if (pl.halve) {                                          // children = the two halves, bounds recomputed (joint_aabb / centroid)
+        for (int k = 0; k < 8; ++k) {
+            child[k] = key2f(keys[k]); child[8 + k] = key2f(keys[8 + k]);
+            child[16 + k] = key2f(keys[16 + k]); child[24 + k] = key2f(keys[16 + 8 + k]);
+        }
+        return pl.half;
+    }
+    int best = 0;
+    bool found = false;
+    T min_cost = Tr::inf();
+    const T sa_parent = surface_area4(ab, ab + 4);
+    for (int s = 0; s < 5; ++s) {
+        Key L[16], R[16];
+        uint32_t nL = 0, nR = 0;
+        for (int k = 0; k < 16; ++k) L[k] = R[k] = kmin4(k) ? Tr::KEY_POS_INF : Tr::KEY_NEG_INF;
+        for (int b = 0; b <= s; ++b) {
+            nL += cnt[b];
+            for (int k = 0; k < 16; ++k) L[k] = fold_key(k, L[k], keys[b * 16 + k]);
+        }
+        for (int b = s + 1; b < 6; ++b) {
+            nR += cnt[b];
+            for (int k = 0; k < 16; ++k) R[k] = fold_key(k, R[k], keys[b * 16 + k]);
+        }
+        T lmn[4], lmx[4], rmn[4], rmx[4];
+        for (int k = 0; k < 4; ++k) { lmn[k] = key2f(L[k]); lmx[k] = key2f(L[4 + k]); rmn[k] = key2f(R[k]); rmx[k] = key2f(R[4 + k]); }
+        // cost = (T(nL) * SA(L) + T(nR) * SA(R)) / SA(aabb_bounds), bvh_node.rs:236-238
+        const T cost = div_rn(add_rn(mul_rn((T)nL, surface_area4(lmn, lmx)), mul_rn((T)nR, surface_area4(rmn, rmx))), sa_parent);
+        if (cost < min_cost) {
+            best = s; min_cost = cost; found = true;
+            for (int k = 0; k < 8; ++k) { child[k] = key2f(L[k]); child[8 + k] = key2f(L[8 + k]); child[16 + k] = key2f(R[k]); child[24 + k] = key2f(R[8 + k]); }
+        }
+    }
+    if (!found)                                              // overflowing surface areas: bucket 0 left, empty child bounds
+        for (int q = 0; q < 4; ++q) for (int k = 0; k < 8; ++k) child[q * 8 + k] = k < 4 ? Tr::inf() : -Tr::inf();
+    uint32_t nl = 0;
+    for (int b = 0; b <= best; ++b) nl += cnt[b];
+    return nl;
+}
+
+template <class T> __device__ __forceinline__ void write_leaf4(typename D4<T>::Node* nodes, uint32_t* node_index, uint32_t* node_start,
+                                                               uint32_t node, uint32_t parent, uint32_t shape, uint32_t start) {
+    typename D4<T>::Node nd;
+    nd.parent = parent; nd.child_l = BVH_INVALID; nd.child_r = BVH_INVALID; nd.shape = shape;
+    for (int k = 0; k < 4; ++k) { nd.l_aabb.min[k] = nd.r_aabb.min[k] = Traits<T>::inf(); nd.l_aabb.max[k] = nd.r_aabb.max[k] = -Traits<T>::inf(); }
+    nodes[node] = nd;
+    node_index[shape] = node;                                // Shapes::set_node_index, bvh_node.rs:103
+    node_start[node] = start;
+}
+template <class T> __device__ __forceinline__ void write_inner4(typename D4<T>::Node* nodes, uint32_t* node_start, const Task4<T>& t,
+                                                                uint32_t nl, const T child[32]) {
+    typename D4<T>::Node nd;
+    nd.parent = t.parent; nd.child_l = t.node + 1; nd.child_r = t.node + 2 * nl; nd.shape = t.count;
+    for (int k = 0; k < 4; ++k) {
+        nd.l_aabb.min[k] = child[k]; nd.l_aabb.max[k] = child[4 + k];
+        nd.r_aabb.min[k] = child[16 + k]; nd.r_aabb.max[k] = child[20 + k];
+    }
+    nodes[t.node] = nd;
+    node_start[t.node] = t.start;
+}
+template <class T> __device__ __forceinline__ Task4<T> child_task(const Task4<T>& t, int side, uint32_t nl, const T child[32]) {
+    Task4<T> c;
+    c.start = side ? t.start + nl : t.start;
+    c.count = side ? t.count - nl : nl;
+    c.node = side ? t.node + 2 * nl : t.node + 1;
+    c.parent = t.node;
+    c.buf = t.buf ^ 1u;                                      // the split moved the range into the other index buffer
+    c.pad[0] = c.pad[1] = c.pad[2] = 0;
+    for (int k = 0; k < 8; ++k) { c.ab[k] = child[side * 16 + k]; c.cb[k] = child[side * 16 + 8 + k]; }
+    return c;
+}
+
+struct BuildArgs4 {
+    uint32_t* idx[2];          // index buffers
+    uint8_t* bkt;              // bucket of every position (bin -> scatter)
+    uint32_t* ctl;             // CTL_* words
+    void* small;               // Task4[]: ranges of <= SMALL4 shapes
+};
+
+// ---- upload pass: NaN check, root bounds (keys), identity permutation ----
+template <class T>
+__global__ void __launch_bounds__(256) upload4_kernel(const typename D4<T>::Aabb* __restrict__ aabb, uint32_t n, uint32_t* __restrict__ idx,
+                                                      typename Traits<T>::Key* __restrict__ root_keys, uint32_t* __restrict__ ctl) {
+    using Tr = Traits<T>;
+    using Key = typename Tr::Key;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    T mn[4], mx[4];
+    bool nan = false;
+    if (i < n) {
+        load4(aabb + i, mn, mx);
+        idx[i] = i;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) nan |= (mn[k] != mn[k]) | (mx[k] != mx[k]);
+    }
+    if (__any_sync(0xffffffffu, nan) && lane_id() == 0) atomicOr(ctl + CTL_NAN, 1u);
+    const int lane = (int)lane_id();
+    Key mine = 0;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+        const bool is_min = kmin4(k);
+        Key v = is_min ? Tr::KEY_POS_INF : Tr::KEY_NEG_INF;
+        if (i < n && !nan) v = f2key(k < 4 ? mn[k & 3] : (k < 8 ? mx[k & 3] : center1(mn[k & 3], mx[k & 3])));
+        const Key r = is_min ? warp_min_key(v) : warp_max_key(v);
+        if (lane == k) mine = r;
+    }
+    if (lane < 16) { if (kmin4(lane)) atomicMin(root_keys + lane, mine); else atomicMax(root_keys + lane, mine); }
+}
+template <class T> __global__ void keys_init_kernel(typename Traits<T>::Key* keys, uint32_t groups) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < 16 * groups; j += gridDim.x * blockDim.x)
+        keys[j] = kmin4((int)(j & 15)) ? Traits<T>::KEY_POS_INF : Traits<T>::KEY_NEG_INF;
+}
+template <class T> __global__ void root_task4_kernel(const typename Traits<T>::Key* __restrict__ root_keys, uint32_t n, Task4<T>* __restrict__ dst) {
+    Task4<T> t;
+    t.start = 0; t.count = n; t.node = 0; t.parent = 0; t.buf = 0; t.pad[0] = t.pad[1] = t.pad[2] = 0;
+    for (int k = 0; k < 8; ++k) { t.ab[k] = key2f(root_keys[k]); t.cb[k] = key2f(root_keys[8 + k]); }
+    *dst = t;
+}
+
+// ---- large ranges, one level ----
+// prep: first tile of every range (exclusive scan of ceil(count / TILE4)), total in tile0[m]; bucket identities; next-level counter.
+template <class T>
+__global__ void __launch_bounds__(1024) level_prep4_kernel(const Task4<T>* __restrict__ tasks, uint32_t m, uint32_t* __restrict__ tile0,
+                                                           typename Traits<T>::Key* __restrict__ acc, uint32_t* __restrict__ acnt, uint32_t* __restrict__ ctl) {
+    __shared__ uint32_t wsum[32];
+    __shared__ uint32_t carry;
+    if (threadIdx.x == 0) { carry = 0; ctl[CTL_NEXT] = 0; }
+    __syncthreads();
+    for (uint32_t j0 = 0; j0 < m; j0 += 1024) {
+        const uint32_t j = j0 + threadIdx.x;
+        const uint32_t v = j < m ? (tasks[j].count + TILE4 - 1) / TILE4 : 0u;
+        uint32_t incl = v;
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
+        if (lane_id() == 31) wsum[threadIdx.x >> 5] = incl;
+        __syncthreads();
+        uint32_t woff = 0;
+        for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) woff += wsum[w];
+        const uint32_t c = carry;
+        if (j < m) tile0[j] = c + woff + incl - v;
+        __syncthreads();
+        if (threadIdx.x == 1023) carry = c + woff + incl;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) tile0[m] = carry;
+    for (uint32_t j = threadIdx.x; j < 96 * m; j += 1024) acc[j] = kmin4((int)(j & 15)) ? Traits<T>::KEY_POS_INF : Traits<T>::KEY_NEG_INF;
+    for (uint32_t j = threadIdx.x; j < 6 * m; j += 1024) acnt[j] = 0;
+}
+
+__device__ __forceinline__ uint32_t tile_owner(const uint32_t* tile0, uint32_t m, uint32_t t) {   // last j with tile0[j] <= t
+    uint32_t lo = 0, hi = m - 1;
+    while (lo < hi) { const uint32_t mid = (lo + hi + 1) >> 1; if (tile0[mid] <= t) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+
+template <class T>
+__global__ void __launch_bounds__(256) level_bin4_kernel(const typename D4<T>::Aabb* __restrict__ aabb, const Task4<T>* __restrict__ tasks, uint32_t m,
+                                                         const uint32_t* __restrict__ tile0, BuildArgs4 A, typename Traits<T>::Key* __restrict__ acc,
+                                                         uint32_t* __restrict__ acnt, uint32_t* __restrict__ tilecnt) {
+    using Key = typename Traits<T>::Key;
+    const uint32_t ntiles = tile0[m];
+    const int lane = (int)lane_id();
+    for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < ntiles; t += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t j = tile_owner(tile0, m, t);
+        const Task4<T>& tk = tasks[j];
+        const uint32_t p0 = tk.start + (t - tile0[j]) * TILE4, p1 = min(p0 + TILE4, tk.start + tk.count);
+        const Plan4<T> pl = plan4<T>(tk.cb, tk.count);
+        Key a[6];
+        uint32_t cnt[6];
+        bin4<T>(aabb, A.idx[tk.buf], A.bkt, tk.start, p0, p1, pl, a, cnt);
+#pragma unroll
+        for (int bb = 0; bb < 6; ++bb) {
+            if (!cnt[bb]) continue;
+            if (lane < 16) { if (kmin4(lane)) atomicMin(acc + 96 * (size_t)j + 16 * bb + lane, a[bb]); else atomicMax(acc + 96 * (size_t)j + 16 * bb + lane, a[bb]); }
+            if (lane == 0) atomicAdd(acnt + 6 * (size_t)j + bb, cnt[bb]);
+        }
+        if (lane < 6) {
+            uint32_t c = cnt[0];
+#pragma unroll
+            for (int bb = 1; bb < 6; ++bb) c = lane == bb ? cnt[bb] : c;
+            tilecnt[6 * (size_t)t + lane] = c;
+        }
+    }
+}
+
+// one warp per range: the split, the node, the children, and the stable destination of every (tile, bucket)
+template <class T>
+__global__ void __launch_bounds__(256) level_split4_kernel(const Task4<T>* __restrict__ tasks, uint32_t m, const uint32_t* __restrict__ tile0,
+                                                           const typename Traits<T>::Key* __restrict__ acc, const uint32_t* __restrict__ acnt,
+                                                           uint32_t* __restrict__ tiledest, Task4<T>* __restrict__ next, BuildArgs4 A,
+                                                           typename D4<T>::Node* __restrict__ nodes, uint32_t* __restrict__ node_index, uint32_t* __restrict__ node_start) {
+    const uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (j >= m) return;
+    const uint32_t lane = lane_id();
+    const Task4<T> t = tasks[j];
+    uint32_t cnt[6], dest[6], run = t.start;
+    for (int b = 0; b < 6; ++b) { cnt[b] = acnt[6 * (size_t)j + b]; dest[b] = run; run += cnt[b]; }
+    for (uint32_t q0 = tile0[j]; q0 < tile0[j + 1]; q0 += 32) {
+        const uint32_t q = q0 + lane;
+        const bool in = q < tile0[j + 1];
+        for (int b = 0; b < 6; ++b) {
+            const uint32_t v = in ? tiledest[6 * (size_t)q + b] : 0u;
+            uint32_t incl = v;
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane >= o) incl += x; }
+            if (in) tiledest[6 * (size_t)q + b] = dest[b] + incl - v;
+            dest[b] += __shfl_sync(0xffffffffu, incl, 31);
+        }
+    }
+    if (lane != 0) return;
+    const Plan4<T> pl = plan4<T>(t.cb, t.count);
+    T child[32];
+    const uint32_t nl = split4<T>(acc + 96 * (size_t)j, cnt, t.ab, pl, child);
+    if (nl == 0 || nl >= t.count) { atomicCAS(A.ctl + CTL_ERROR, 0u, (uint32_t)BVHGPU_ERR_INTERNAL); return; }
+    write_inner4<T>(nodes, node_start, t, nl, child);
+    Task4<T>* small = reinterpret_cast<Task4<T>*>(A.small);
+    for (int side = 0; side < 2; ++side) {
+        const Task4<T> c = child_task<T>(t, side, nl, child);
+        if (c.count > SMALL4) next[atomicAdd(A.ctl + CTL_NEXT, 1u)] = c;
+        else small[atomicAdd(A.ctl + CTL_SMALL, 1u)] = c;
+    }
+}
+
+template <class T>
+__global__ void __launch_bounds__(256) level_scatter4_kernel(const Task4<T>* __restrict__ tasks, uint32_t m, const uint32_t* __restrict__ tile0,
+                                                             const uint32_t* __restrict__ tiledest, BuildArgs4 A) {
+    const uint32_t ntiles = tile0[m];
+    for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < ntiles; t += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t j = tile_owner(tile0, m, t);
+        const Task4<T>& tk = tasks[j];
+        const uint32_t p0 = tk.start + (t - tile0[j]) * TILE4, p1 = min(p0 + TILE4, tk.start + tk.count);
+        uint32_t dest[6];
+        for (int b = 0; b < 6; ++b) dest[b] = tiledest[6 * (size_t)t + b];
+        scatter4(A.idx[tk.buf], A.idx[tk.buf ^ 1u], A.bkt, p0, p1, dest);
+    }
+}
+
+// ---- small ranges: one warp each, depth-first ----
+template <class T> struct __align__(16) WarpState4 {
+    typename Traits<T>::Key keys[96];
+    T child[32];
+    uint32_t nl;
+    uint32_t pad[3];
+    Task4<T> stack[STACK4];
+};
+
+template <class T>
+__global__ void __launch_bounds__(256) small4_kernel(const typename D4<T>::Aabb* __restrict__ aabb, uint32_t count, BuildArgs4 A,
+                                                     typename D4<T>::Node* __restrict__ nodes, uint32_t* __restrict__ node_index, uint32_t* __restrict__ node_start) {
+    using Key = typename Traits<T>::Key;
+    __shared__ WarpState4<T> st[8];
+    const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= count) return;
+    WarpState4<T>& ws = st[threadIdx.x >> 5];
+    const int lane = (int)lane_id();
+    Task4<T> t = reinterpret_cast<const Task4<T>*>(A.small)[w];
+    int top = 0;
+    for (;;) {
+        if (t.count == 1) {
+            if (lane == 0) write_leaf4<T>(nodes, node_index, node_start, t.node, t.parent, __ldcg(A.idx[t.buf] + t.start), t.start);
+        } else {
+            const Plan4<T> pl = plan4<T>(t.cb, t.count);
+            Key a[6];
+            uint32_t cnt[6];
+            bin4<T>(aabb, A.idx[t.buf], A.bkt, t.start, t.start, t.start + t.count, pl, a, cnt);
+            if (lane < 16) {
+#pragma unroll
+                for (int bb = 0; bb < 6; ++bb) ws.keys[16 * bb + lane] = a[bb];
+            }
+            __syncwarp();
+            if (lane == 0) {
+                ws.nl = split4<T>(ws.keys, cnt, t.ab, pl, ws.child);
+                if (ws.nl == 0 || ws.nl >= t.count) atomicCAS(A.ctl + CTL_ERROR, 0u, (uint32_t)BVHGPU_ERR_INTERNAL);
+                else write_inner4<T>(nodes, node_start, t, ws.nl, ws.child);
+            }
+            __syncwarp();
+            const uint32_t nl = ws.nl;
+            if (nl == 0 || nl >= t.count) return;
+            uint32_t dest[6], run = t.start;
+#pragma unroll
+            for (int b = 0; b < 6; ++b) { dest[b] = run; run += cnt[b]; }
+            scatter4(A.idx[t.buf], A.idx[t.buf ^ 1u], A.bkt, t.start, t.start + t.count, dest);
+            __syncwarp();
+            const Task4<T> l = child_task<T>(t, 0, nl, ws.child), r = child_task<T>(t, 1, nl, ws.child);
+            const bool left_first = l.count <= r.count;           // continue with the smaller child, push the larger
+            if (top == STACK4) { if (lane == 0) atomicCAS(A.ctl + CTL_ERROR, 0u, (uint32_t)BVHGPU_ERR_INTERNAL); return; }
+            if (lane == 0) ws.stack[top] = left_first ? r : l;
+            ++top;
+            t = left_first ? l : r;
+            __syncwarp();
+            continue;
+        }
+        if (top == 0) break;
+        __syncwarp();
+        t = ws.stack[--top];
+        __syncwarp();
+    }
+}
+
+// ---- flatten and traversal records: closed forms over the preorder node array (as flatten.cu) ----
+template <class T>
+__global__ void __launch_bounds__(256) flat4_kernel(const typename D4<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ node_start,
+                                                    uint32_t n_nodes, typename D4<T>::Flat* __restrict__ flat) {
+    using Flat = typename D4<T>::Flat;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_nodes) return;
+    const typename D4<T>::Node& nd = nodes[i];
+    const bool leaf = nd.child_l == BVH_INVALID;
+    Flat g;
+    for (int k = 0; k < 4; ++k) { g.aabb.min[k] = Traits<T>::inf(); g.aabb.max[k] = -Traits<T>::inf(); }
+    if constexpr (sizeof(T) == 8) g._pad = 0;
+    if (i == 0) {
+        if (leaf) { g.entry_index = BVH_INVALID; g.exit_index = 1; g.shape_index = nd.shape; flat[0] = g; }   // flat_bvh.rs:129-141 only
+        return;
+    }
+    const uint32_t nav = (i - 1) + node_start[i];
+    const uint32_t count = leaf ? 1u : nd.shape;
+    const typename D4<T>::Node& par = nodes[nd.parent];
+    const bool is_left = par.child_l == i;
+    Flat f = g;
+    for (int k = 0; k < 4; ++k) {
+        f.aabb.min[k] = is_left ? par.l_aabb.min[k] : par.r_aabb.min[k];
+        f.aabb.max[k] = is_left ? par.l_aabb.max[k] : par.r_aabb.max[k];
+    }
+    f.entry_index = nav + 1; f.exit_index = nav + 3 * count - 1; f.shape_index = BVH_INVALID;   // flat_bvh.rs:80-88
+    flat[nav] = f;
+    if (leaf) { g.entry_index = BVH_INVALID; g.exit_index = nav + 2; g.shape_index = nd.shape; flat[nav + 1] = g; }
+}
+
+// record r = node r+1 (the root has no box of its own); a root leaf gets the shape's own box (bvh_node.rs:314)
+template <class T>
+__global__ void __launch_bounds__(256) trec4_kernel(const typename D4<T>::Node* __restrict__ nodes, uint32_t n_nodes,
+                                                    const typename D4<T>::Aabb* __restrict__ aabb, typename D4<T>::Rec* __restrict__ trec) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_nodes) return;
+    typename D4<T>::Rec r;
+    r.pad[0] = r.pad[1] = 0;
+    if (n_nodes == 1) {
+        const uint32_t s = nodes[0].shape;
+        for (int k = 0; k < 4; ++k) { r.min[k] = aabb[s].min[k]; r.max[k] = aabb[s].max[k]; }
+        r.skip = 1; r.shape = s;
+        trec[0] = r;
+        return;
+    }
+    if (i == 0) return;
+    const typename D4<T>::Node& nd = nodes[i];
+    const bool leaf = nd.child_l == BVH_INVALID;
+    const typename D4<T>::Node& par = nodes[nd.parent];
+    const bool is_left = par.child_l == i;
+    for (int k = 0; k < 4; ++k) {
+        r.min[k] = is_left ? par.l_aabb.min[k] : par.r_aabb.min[k];
+        r.max[k] = is_left ? par.l_aabb.max[k] : par.r_aabb.max[k];
+    }
+    r.skip = (i - 1) + (2 * (leaf ? 1u : nd.shape) - 1);
+    r.shape = leaf ? nd.shape : BVH_INVALID;
+    trec[i - 1] = r;
+}
+
+// ---- walk: one ray per thread over the records, the 4-wide slab test (intersect_default.rs:16-37, intersect_simd.rs) ----
+template <class T>
+__device__ __forceinline__ bool slab4(const T o[4], const T inv[4], const T mn[4], const T mx[4]) {
+    T lo[4], hi[4];
+    bool nan = false;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const T l = mul_rn(sub_rn(mn[k], o[k]), inv[k]), r = mul_rn(sub_rn(mx[k], o[k]), inv[k]);
+        nan |= (l != l) | (r != r);                            // any NaN rejects the box
+        lo[k] = min_t(l, r); hi[k] = max_t(l, r);
+    }
+    const T tmin = max_t(max_t(lo[0], lo[1]), max_t(lo[2], lo[3]));
+    const T tmax = min_t(min_t(hi[0], hi[1]), min_t(hi[2], hi[3]));
+    return !nan && tmax >= (tmin > T(0) ? tmin : T(0));
+}
+__device__ __forceinline__ void fetch4(const TRec4F* p, float mn[4], float mx[4], uint32_t& skip, uint32_t& shape) {
+    uint32_t a, b, c, d;
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mn[0]), "=f"(mn[1]), "=f"(mn[2]), "=f"(mn[3]) : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mx[0]), "=f"(mx[1]), "=f"(mx[2]), "=f"(mx[3]) : "l"(reinterpret_cast<const char*>(p) + 16));
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "l"(reinterpret_cast<const char*>(p) + 32));
+    skip = a; shape = b;
+}
+__device__ __forceinline__ void fetch4(const TRec4D* p, double mn[4], double mx[4], uint32_t& skip, uint32_t& shape) {
+    const char* c = reinterpret_cast<const char*>(p);
+    uint32_t a, b, x, y;
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[0]), "=d"(mn[1]) : "l"(c));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[2]), "=d"(mn[3]) : "l"(c + 16));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[0]), "=d"(mx[1]) : "l"(c + 32));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[2]), "=d"(mx[3]) : "l"(c + 48));
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(x), "=r"(y) : "l"(c + 64));
+    skip = a; shape = b;
+}
+__device__ __forceinline__ void load_ray4(const bvh_ray4f* p, float o[4], float inv[4]) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 2);
+    o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; inv[0] = b.x; inv[1] = b.y; inv[2] = b.z; inv[3] = b.w;
+}
+__device__ __forceinline__ void load_ray4(const bvh_ray4d* p, double o[4], double inv[4]) {
+    const double2* q = reinterpret_cast<const double2*>(p);
+    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 4), d = __ldg(q + 5);
+    o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y; inv[0] = c.x; inv[1] = c.y; inv[2] = d.x; inv[3] = d.y;
+}
+
+template <class T, bool FLAT, class Emit>
+__device__ __forceinline__ void walk4(const typename D4<T>::Rec* __restrict__ trec, uint32_t n_rec, const typename D4<T>::Aabb* __restrict__ aabb,
+                                      const T o[4], const T inv[4], Emit emit) {
+    uint32_t i = 0;
+    while (i < n_rec) {
+        T mn[4], mx[4];
+        uint32_t skip, shape;
+        fetch4(trec + i, mn, mx, skip, shape);
+        if (slab4(o, inv, mn, mx)) {
+            if (shape != BVH_INVALID) {
+                bool report = true;
+                if (FLAT) {                                    // flat_bvh.rs:412-416: a reached leaf re-tests the shape's AABB
+                    T smn[4], smx[4];
+                    load4(aabb + shape, smn, smx);
+                    report = slab4(o, inv, smn, smx);
+                }
+                if (report) emit(shape);
+            }
+            ++i;
+        } else {
+            i = skip;
+        }
+    }
+}
+
+// count pass (FILL = false) and fill pass (FILL = true); hits beyond cap are dropped
+template <class T, bool FLAT, bool FILL>
+__global__ void __launch_bounds__(256) walk4_kernel(const typename D4<T>::Rec* __restrict__ trec, uint32_t n_rec, const typename D4<T>::Aabb* __restrict__ aabb,
+                                                    const typename D4<T>::Ray* __restrict__ rays, uint32_t nrays, uint32_t* __restrict__ counts,
+                                                    const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
+                                                    const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits,
+                                                    unsigned long long cap) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (FILL && r == 0) { const unsigned long long t = *total; offsets[nrays] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
+    if (r >= nrays) return;
+    T o[4], inv[4];
+    load_ray4(rays + r, o, inv);
+    if (!FILL) {
+        uint32_t cnt = 0;
+        walk4<T, FLAT>(trec, n_rec, aabb, o, inv, [&](uint32_t) { ++cnt; });
+        counts[r] = cnt;
+    } else {
+        unsigned long long w = blocksum[r / CSR_SCAN_TILE] + local[r];
+        offsets[r] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
+        if (hits) walk4<T, FLAT>(trec, n_rec, aabb, o, inv, [&](uint32_t shape) { if (w < cap) hits[w] = shape; ++w; });
+    }
+}
+
+// ================================================================================================================================
+// host side
+// ================================================================================================================================
+#define LAUNCHED(ctx, k) do { (ctx)->launches += (k); BVH_CUDA_TRY(cudaGetLastError()); } while (0)
+
+template <class T> static void release4(Tree4<T>* t) {
+    if (!t || !t->ctx) return;
+    bvhgpu_ctx* ctx = t->ctx;
+    dfree(ctx, t->d_aabb); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
+    dfree(ctx, t->d_trec); dfree(ctx, t->d_flat); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
+}
+template <class T> static int sticky4(const Tree4<T>* t) {
+    if (t->failed_status != BVHGPU_OK) set_error("%s", t->failed_message.c_str());
+    return t->failed_status;
+}
+template <class T> static int fail4(Tree4<T>* t, int rc, const char* msg) {
+    t->failed_status = rc; t->failed_message = msg;
+    set_error("%s", msg);
+    return rc;
+}
+
+// The exact SAH build.  h_aabbs: host pointer.  Synchronous (the host learns the range count of every level anyway).
+template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb* h_aabbs) {
+    using Key = typename Traits<T>::Key;
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = tree->n;
+    BVH_TRY(dalloc_t(ctx, &tree->d_aabb, n));
+    BVH_TRY(dalloc_t(ctx, &tree->d_nodes, tree->n_nodes));
+    BVH_TRY(dalloc_t(ctx, &tree->d_node_index, n));
+    BVH_TRY(dalloc_t(ctx, &tree->d_node_start, tree->n_nodes));
+    BVH_CUDA_TRY(cudaMemcpyAsync(tree->d_aabb, h_aabbs, sizeof(*h_aabbs) * n, cudaMemcpyHostToDevice, st));
+
+    const uint32_t max_tasks = n / (SMALL4 + 1) + 1;           // disjoint ranges of > SMALL4 shapes on one level
+    const uint32_t max_tiles = n / TILE4 + max_tasks;
+    Scratch scratch(ctx);
+    BuildArgs4 A{};
+    uint32_t *idx = nullptr, *tile0 = nullptr, *tilecnt = nullptr, *acnt = nullptr;
+    Key *root_keys = nullptr, *acc = nullptr;
+    Task4<T>* tasks = nullptr;
+    Task4<T>* small = nullptr;
+    BVH_TRY(scratch.get(&idx, 2 * (size_t)n));
+    BVH_TRY(scratch.get(&A.bkt, n));
+    BVH_TRY(scratch.get(&A.ctl, 8));
+    BVH_TRY(scratch.get(&root_keys, 16));
+    BVH_TRY(scratch.get(&small, n));
+    A.idx[0] = idx; A.idx[1] = idx + n; A.small = small;
+    BVH_CUDA_TRY(cudaMemsetAsync(A.ctl, 0, 8 * sizeof(uint32_t), st));
+    keys_init_kernel<T><<<1, 32, 0, st>>>(root_keys, 1);
+    upload4_kernel<T><<<(n + 255) / 256, 256, 0, st>>>(tree->d_aabb, n, idx, root_keys, A.ctl);
+    LAUNCHED(ctx, 2);
+    uint32_t* h = ctx->h_pinned + 232;
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    if (h[CTL_NAN]) return fail4(tree, BVHGPU_ERR_NAN, "build: NaN coordinate in an input AABB (the reference panics here, src/bvh/bvh_node.rs:214-217)");
+
+    uint32_t m = 0, n_small = 1;
+    if (n > SMALL4) {
+        BVH_TRY(scratch.get(&tasks, 2 * (size_t)max_tasks));
+        BVH_TRY(scratch.get(&acc, 96 * (size_t)max_tasks));
+        BVH_TRY(scratch.get(&acnt, 6 * (size_t)max_tasks));
+        BVH_TRY(scratch.get(&tile0, (size_t)max_tasks + 1));
+        BVH_TRY(scratch.get(&tilecnt, 6 * (size_t)max_tiles));
+        root_task4_kernel<T><<<1, 1, 0, st>>>(root_keys, n, tasks);
+        LAUNCHED(ctx, 1);
+        m = 1;
+    } else {
+        root_task4_kernel<T><<<1, 1, 0, st>>>(root_keys, n, small);
+        LAUNCHED(ctx, 1);
+    }
+    const int wave = std::max(ctx->sm_count, 1) * 8;           // blocks of the grid-stride tile kernels
+    int cur = 0;
+    while (m) {
+        Task4<T>* tc = tasks + (size_t)cur * max_tasks;
+        Task4<T>* tn = tasks + (size_t)(cur ^ 1) * max_tasks;
+        const uint32_t tiles_bound = n / TILE4 + m;
+        const int grid = (int)std::min<uint32_t>((tiles_bound + 7) / 8, (uint32_t)wave);
+        level_prep4_kernel<T><<<1, 1024, 0, st>>>(tc, m, tile0, acc, acnt, A.ctl);
+        level_bin4_kernel<T><<<grid, 256, 0, st>>>(tree->d_aabb, tc, m, tile0, A, acc, acnt, tilecnt);
+        level_split4_kernel<T><<<(m + 7) / 8, 256, 0, st>>>(tc, m, tile0, acc, acnt, tilecnt, tn, A, tree->d_nodes, tree->d_node_index, tree->d_node_start);
+        level_scatter4_kernel<T><<<grid, 256, 0, st>>>(tc, m, tile0, tilecnt, A);
+        LAUNCHED(ctx, 4);
+        BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        BVH_CUDA_TRY(cudaStreamSynchronize(st));
+        if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], "build: the device reported an empty split (non-finite input?); the tree is unusable");
+        m = h[CTL_NEXT];
+        n_small = h[CTL_SMALL];
+        cur ^= 1;
+    }
+    if (n_small) {
+        small4_kernel<T><<<(n_small + 7) / 8, 256, 0, st>>>(tree->d_aabb, n_small, A, tree->d_nodes, tree->d_node_index, tree->d_node_start);
+        LAUNCHED(ctx, 1);
+    }
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], "build: the device reported an empty split (non-finite input?); the tree is unusable");
+    return BVHGPU_OK;
+}
+
+template <class T, class TreeT> static int build4_impl(bvhgpu_ctx* ctx, const typename D4<T>::Aabb* aabbs, size_t n, int mode, TreeT** out) {
+    if (!ctx || !out || (n && !aabbs)) { set_error("build: null argument"); return BVHGPU_ERR_INVALID; }
+    *out = nullptr;
+    if (n > (1ull << 30)) { set_error("build: n = %zu exceeds 2^30 shapes", n); return BVHGPU_ERR_INVALID; }
+    if (mode == BVHGPU_BUILD_LBVH || mode == BVHGPU_BUILD_LBVH_TREELET) {
+        set_error("build: D = 4 has the exact SAH build only (BVHGPU_BUILD_EXACT_SAH); the LBVH modes are not implemented for D = 4");
+        return BVHGPU_ERR_UNSUPPORTED;
+    }
+    if (mode != BVHGPU_BUILD_EXACT_SAH) { set_error("build: unknown mode %d", mode); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    TreeT* tree = new (std::nothrow) TreeT();
+    if (!tree) { set_error("build: out of host memory"); return BVHGPU_ERR_INTERNAL; }
+    tree->ctx = ctx;
+    tree->n = (uint32_t)n;
+    tree->n_nodes = n ? 2 * (uint32_t)n - 1 : 0;
+    const int rc = n ? build4<T>(tree, aabbs) : (int)BVHGPU_OK;
+    if (rc != BVHGPU_OK) { release4<T>(tree); delete tree; return rc; }
+    *out = tree;
+    return BVHGPU_OK;
+}
+
+template <class T> static int nodes4_impl(Tree4<T>* tree, typename D4<T>::Node* out_nodes, uint32_t* out_node_index) {
+    if (!tree) { set_error("tree_nodes: null tree"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (tree->n == 0) return BVHGPU_OK;
+    if (out_nodes) BVH_CUDA_TRY(cudaMemcpyAsync(out_nodes, tree->d_nodes, sizeof(*out_nodes) * tree->n_nodes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_node_index) BVH_CUDA_TRY(cudaMemcpyAsync(out_node_index, tree->d_node_index, sizeof(uint32_t) * tree->n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+
+template <class T> static int flatten4_impl(Tree4<T>* tree, typename D4<T>::Flat* out, size_t cap, size_t* len) {
+    if (!tree) { set_error("flatten: null tree"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    tree->n_flat = tree->n == 0 ? 0 : (tree->n == 1 ? 1 : 3 * (size_t)tree->n - 2);
+    if (len) *len = tree->n_flat;
+    if (tree->n && !tree->d_flat) {
+        BVH_TRY(dalloc_t(ctx, &tree->d_flat, tree->n_flat));
+        flat4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_start, tree->n_nodes, tree->d_flat);
+        LAUNCHED(ctx, 1);
+    }
+    if (out) {
+        if (cap < tree->n_flat) { set_error("flatten: capacity %zu < %zu flat nodes", cap, tree->n_flat); return BVHGPU_ERR_CAPACITY; }
+        if (tree->n_flat) BVH_CUDA_TRY(cudaMemcpyAsync(out, tree->d_flat, sizeof(*out) * tree->n_flat, cudaMemcpyDeviceToHost, ctx->stream));
+        BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
+    return BVHGPU_OK;
+}
+
+// Count pass + scan on the stream; leaves the 64-bit total at sums[nblk].  Needs n > 0 and nrays > 0.
+template <class T> static int count_and_scan4(Tree4<T>* tree, bool flat, const typename D4<T>::Ray* d_rays, uint32_t R, Scratch& scratch,
+                                              uint32_t** counts, uint32_t** local, unsigned long long** sums) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    if (!tree->d_trec) {
+        tree->n_trec = tree->n == 1 ? 1u : tree->n_nodes - 1;
+        BVH_TRY(dalloc_t(ctx, &tree->d_trec, tree->n_trec));
+        trec4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, st>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec);
+        LAUNCHED(ctx, 1);
+    }
+    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
+    BVH_TRY(scratch.get(counts, R));
+    BVH_TRY(scratch.get(local, R));
+    BVH_TRY(scratch.get(sums, (size_t)nblk + 1));
+    BVH_CUDA_TRY(cudaMemsetAsync(*sums + nblk, 0, sizeof(unsigned long long), st));
+    const int grid = (R + 255) / 256;
+    if (flat) walk4_kernel<T, true, false><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    else      walk4_kernel<T, false, false><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    scan_local_kernel<<<nblk, CSR_SCAN_THREADS, 0, st>>>(*counts, R, *local, *sums, nullptr);
+    scan_blocks_kernel<<<1, 1024, 0, st>>>(*sums, nblk, *sums + nblk);
+    LAUNCHED(ctx, 3);
+    return BVHGPU_OK;
+}
+template <class T> static int fill4(Tree4<T>* tree, bool flat, const typename D4<T>::Ray* d_rays, uint32_t R, const uint32_t* local,
+                                    const unsigned long long* sums, uint32_t* d_offsets, uint32_t* d_hits, size_t cap) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
+    const int grid = (R + 255) / 256;
+    if (flat) walk4_kernel<T, true, true><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
+    else      walk4_kernel<T, false, true><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
+    LAUNCHED(ctx, 1);
+    return BVHGPU_OK;
+}
+
+template <class T> static int check_traverse_args(Tree4<T>* tree, int mode, size_t nrays) {
+    if (nrays > 0x7FFFFFFFull) { set_error("traverse: nrays %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+    return sticky4(tree);
+}
+
+// device pointers, enqueued on the context's stream; synchronises only to return *total
+template <class T> static int traverse4_dev_impl(Tree4<T>* tree, int mode, const void* d_rays, size_t nrays, uint32_t* d_offsets, uint32_t* d_hits,
+                                                 size_t cap, size_t* total) {
+    if (!tree || !d_offsets || (nrays && !d_rays)) { set_error("traverse_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_traverse_args(tree, mode, nrays));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nrays == 0 || tree->n == 0) {                              // no rays / empty Bvh: no hits (bvh_impl.rs:109-112)
+        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (nrays + 1), st));
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    const uint32_t R = (uint32_t)nrays;
+    const auto* rays = reinterpret_cast<const typename D4<T>::Ray*>(d_rays);
+    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    Scratch scratch(ctx);
+    uint32_t *counts = nullptr, *local = nullptr;
+    unsigned long long* sums = nullptr;
+    BVH_TRY(count_and_scan4(tree, flat, rays, R, scratch, &counts, &local, &sums));
+    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
+    unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned + 236);
+    if (total) {                                                   // the total is known before the hit lists are written
+        BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        BVH_CUDA_TRY(cudaEventRecord(ctx->ev_total, st));
+    }
+    BVH_TRY(fill4(tree, flat, rays, R, local, sums, d_offsets, d_hits, cap));
+    if (!total) return BVHGPU_OK;
+    BVH_CUDA_TRY(cudaEventSynchronize(ctx->ev_total));
+    *total = (size_t)*h;
+    if (*h > 0xFFFFFFFFull) { set_error("traverse: %llu hits overflow the u32 CSR offsets", *h); return BVHGPU_ERR_CAPACITY; }
+    if (d_hits && *h > cap) { set_error("traverse: %llu hits do not fit capacity %zu", *h, cap); return BVHGPU_ERR_CAPACITY; }
+    return BVHGPU_OK;
+}
+
+// host pointers: count, read the total, size the retained hit buffer, fill, copy back
+template <class T> static int traverse4_host_impl(Tree4<T>* tree, int mode, const typename D4<T>::Ray* rays, size_t nrays, uint32_t* offsets,
+                                                  uint32_t* hits, size_t cap, size_t* total) {
+    if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_traverse_args(tree, mode, nrays));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nrays == 0 || tree->n == 0) {
+        std::fill(offsets, offsets + nrays + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    const uint32_t R = (uint32_t)nrays;
+    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    Scratch scratch(ctx);
+    typename D4<T>::Ray* d_rays = nullptr;
+    BVH_TRY(scratch.get(&d_rays, nrays));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, st));
+    uint32_t *counts = nullptr, *local = nullptr;
+    unsigned long long* sums = nullptr;
+    BVH_TRY(count_and_scan4(tree, flat, d_rays, R, scratch, &counts, &local, &sums));
+    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
+    unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned + 236);
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    const unsigned long long tot = *h;
+    if (total) *total = (size_t)tot;
+    if (tot > 0xFFFFFFFFull) { set_error("traverse: %llu hits overflow the u32 CSR offsets", tot); return BVHGPU_ERR_CAPACITY; }
+    if (tree->offsets_cap < nrays + 1) {
+        dfree(ctx, tree->d_offsets); tree->d_offsets = nullptr; tree->offsets_cap = 0;
+        BVH_TRY(dalloc_t(ctx, &tree->d_offsets, nrays + 1));
+        tree->offsets_cap = nrays + 1;
+    }
+    const bool fits = hits && tot <= cap;
+    if (fits && tree->hits_cap < tot) {
+        dfree(ctx, tree->d_hits); tree->d_hits = nullptr; tree->hits_cap = 0;
+        BVH_TRY(dalloc_t(ctx, &tree->d_hits, tot));
+        tree->hits_cap = tot;
+    }
+    BVH_TRY(fill4(tree, flat, d_rays, R, local, sums, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
+    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, st));
+    if (fits && tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    if (tot > cap) { set_error("traverse: %llu hits do not fit the caller's capacity %zu (call again with cap = *total)", tot, cap); return BVHGPU_ERR_CAPACITY; }
+    return BVHGPU_OK;
+}
+
+}  // namespace bvhb200
+
+using namespace bvhb200;
+
+struct bvhgpu_tree4f : Tree4<float> {};
+struct bvhgpu_tree4d : Tree4<double> {};
+
+#define BVH_EXPORT4 extern "C" __attribute__((visibility("default")))
+#define DEFINE_API4(T, SUF, TREE, AABB, RAY, NODE, FLAT)                                                                   \
+    BVH_EXPORT4 int bvhgpu_build_##SUF(bvhgpu_ctx* ctx, const AABB* aabbs, size_t n, int mode, TREE** out) {              \
+        return build4_impl<T, TREE>(ctx, aabbs, n, mode, out);                                                            \
+    }                                                                                                                     \
+    BVH_EXPORT4 void bvhgpu_tree_free_##SUF(TREE* tree) {                                                                 \
+        if (!tree) return;                                                                                                \
+        if (tree->ctx) cudaSetDevice(tree->ctx->device);                                                                  \
+        release4<T>(tree);                                                                                                \
+        delete tree;                                                                                                      \
+    }                                                                                                                     \
+    BVH_EXPORT4 size_t bvhgpu_tree_num_shapes_##SUF(const TREE* tree) { return tree ? tree->n : 0; }                      \
+    BVH_EXPORT4 int bvhgpu_tree_nodes_##SUF(TREE* tree, NODE* out_nodes, uint32_t* out_node_index) {                      \
+        return nodes4_impl<T>(tree, out_nodes, out_node_index);                                                           \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_flatten_##SUF(TREE* tree, FLAT* out, size_t cap, size_t* len) { return flatten4_impl<T>(tree, out, cap, len); } \
+    BVH_EXPORT4 int bvhgpu_traverse_##SUF(TREE* tree, int mode, const RAY* rays, size_t nrays, uint32_t* offsets, uint32_t* hits, \
+                                          size_t cap, size_t* total) {                                                    \
+        return traverse4_host_impl<T>(tree, mode, rays, nrays, offsets, hits, cap, total);                                \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_traverse_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, void* dev_offsets, \
+                                              void* dev_hits, size_t cap, size_t* total) {                                \
+        return traverse4_dev_impl<T>(tree, mode, dev_rays, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+    }
+
+DEFINE_API4(float, f32x4, bvhgpu_tree4f, bvh_aabb4f, bvh_ray4f, bvh_node4f, bvh_flat4f)
+DEFINE_API4(double, f64x4, bvhgpu_tree4d, bvh_aabb4d, bvh_ray4d, bvh_node4d, bvh_flat4d)

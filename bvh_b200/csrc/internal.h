@@ -203,6 +203,14 @@ template <class T> int query_device(Tree<T>* tree, int mode, int kind, const T* 
 // nearest_to for a batch of points (device pointers): exact reference walk for AABB-distance shapes; candidate lists for any shape
 template <class T> int nearest_device(Tree<T>* tree, int mode, const T* d_points, size_t nq, uint32_t* d_shape, T* d_dist, int use_triangles = 0);
 template <class T> int nearest_candidates_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t* d_offsets, uint32_t* d_cand, size_t cap, size_t* total);
+// CSR scan of per-ray counts (traverse.cu), shared with dim4.cu: scan_local_kernel runs CSR_SCAN_THREADS threads per block over
+// CSR_SCAN_TILE counts and leaves local exclusive offsets and block totals; scan_blocks_kernel (one block of 1024 threads) turns the
+// block totals into exclusive 64-bit block offsets and adds the grand total to *total (zeroed by the caller).
+constexpr int CSR_SCAN_THREADS = 256;
+constexpr int CSR_SCAN_TILE = 2048;
+__global__ void __launch_bounds__(256) scan_local_kernel(const uint32_t* __restrict__ counts, uint32_t n, uint32_t* __restrict__ local,
+                                                         unsigned long long* __restrict__ blocksum, uint32_t* __restrict__ maxcount);
+__global__ void __launch_bounds__(1024) scan_blocks_kernel(unsigned long long* __restrict__ blocksum, uint32_t nblocks, unsigned long long* __restrict__ total);
 // ---- dim2.cu ----
 template <class T> int dim2_expand_aabbs(bvhgpu_ctx* ctx, const T* d_in4, uint32_t n, T* d_out6);
 template <class T> int dim2_expand_rays(bvhgpu_ctx* ctx, const T* d_in6, uint32_t n, T* d_out9);

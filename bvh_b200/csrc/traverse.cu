@@ -45,6 +45,7 @@ template <class T> static inline const typename Traits<T>::DAabb* walk_aabbs(con
 constexpr int SCAN_ITEMS = 8;
 constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_TILE = SCAN_ITEMS * SCAN_THREADS;     // 2048 counts per block
+static_assert(SCAN_THREADS == CSR_SCAN_THREADS && SCAN_TILE == CSR_SCAN_TILE, "scan geometry declared in internal.h");
 
 // ---- slab test: intersect_default.rs:16-37 --------------------------------------------------------
 template <class T> __device__ __forceinline__ T tmin2(T a, T b);

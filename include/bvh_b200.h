@@ -68,6 +68,16 @@ typedef struct { uint32_t parent, child_l, child_r, shape; bvh_aabb2d l_aabb, r_
 typedef struct { bvh_aabb2f aabb; uint32_t entry_index, exit_index, shape_index; } bvh_flat2f;               /* 28 B */
 typedef struct { bvh_aabb2d aabb; uint32_t entry_index, exit_index, shape_index, _pad; } bvh_flat2d;         /* 48 B */
 
+/* D = 4 twins (4-wide slab tests: src/ray/intersect_simd.rs:38-45, 123-133 (f32), 202-209, 226-246, 260-270 (f64)) */
+typedef struct { float min[4]; float max[4]; } bvh_aabb4f;                                                   /* 32 B */
+typedef struct { double min[4]; double max[4]; } bvh_aabb4d;                                                 /* 64 B */
+typedef struct { float origin[4]; float direction[4]; float inv_direction[4]; } bvh_ray4f;                   /* 48 B */
+typedef struct { double origin[4]; double direction[4]; double inv_direction[4]; } bvh_ray4d;                /* 96 B */
+typedef struct { uint32_t parent, child_l, child_r, shape; bvh_aabb4f l_aabb, r_aabb; } bvh_node4f;          /* 80 B */
+typedef struct { uint32_t parent, child_l, child_r, shape; bvh_aabb4d l_aabb, r_aabb; } bvh_node4d;          /* 144 B */
+typedef struct { bvh_aabb4f aabb; uint32_t entry_index, exit_index, shape_index; } bvh_flat4f;               /* 44 B */
+typedef struct { bvh_aabb4d aabb; uint32_t entry_index, exit_index, shape_index, _pad; } bvh_flat4d;         /* 80 B */
+
 typedef enum {
     BVHGPU_OK = 0,
     BVHGPU_ERR_INVALID = 1,     /* bad argument */
@@ -101,6 +111,8 @@ typedef struct bvhgpu_tree3f bvhgpu_tree3f; /* device-resident Bvh<f32,3> (+ Fla
 typedef struct bvhgpu_tree3d bvhgpu_tree3d; /* device-resident Bvh<f64,3>                      */
 typedef struct bvhgpu_tree2f bvhgpu_tree2f; /* device-resident Bvh<f32,2>                      */
 typedef struct bvhgpu_tree2d bvhgpu_tree2d; /* device-resident Bvh<f64,2>                      */
+typedef struct bvhgpu_tree4f bvhgpu_tree4f; /* device-resident Bvh<f32,4>                      */
+typedef struct bvhgpu_tree4d bvhgpu_tree4d; /* device-resident Bvh<f64,4>                      */
 
 /* ---- context ------------------------------------------------------------------ */
 int bvhgpu_create(int device, bvhgpu_ctx** out);
@@ -184,6 +196,37 @@ int bvhgpu_traverse_f32x2(bvhgpu_tree2f* tree, int mode, const bvh_ray2f* rays, 
                           uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
 int bvhgpu_traverse_f64x2(bvhgpu_tree2d* tree, int mode, const bvh_ray2d* rays, size_t nrays,
                           uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+
+/* ---- D = 4: Bvh<T,4>::build / nodes / flatten / traverse (the reference is generic in D, src/bvh/bvh_node.rs:81-279,
+ * src/flat_bvh.rs:60-143, 396-431; 4-wide slab tests src/ray/intersect_simd.rs; generic slab test src/ray/intersect_default.rs:16-37).
+ * Its own device pipeline (dim4.cu): a fourth axis cannot be embedded in the 3-D kernels.  Semantics, error codes and the CSR output as
+ * the 3-D entry points, except:
+ *   - build: only BVHGPU_BUILD_EXACT_SAH exists (bit-identical to Bvh<T,4>::build); the LBVH modes return BVHGPU_ERR_UNSUPPORTED.
+ *     NaN in any coordinate: BVHGPU_ERR_NAN; n > 2^30 or a null argument: BVHGPU_ERR_INVALID.  The build is synchronous and a build
+ *     that fails hands out no tree.  Node layout, leaves and inner-node `shape` (= shapes below the node) as bvh_node3f.
+ *   - traverse: there is no fetch call.  When the hits do not fit `cap`, offsets and *total are valid and the call returns
+ *     BVHGPU_ERR_CAPACITY; call again with cap = *total.  BVHGPU_TRAVERSE_BVH re-tests the shape AABB only at a root leaf
+ *     (src/bvh/bvh_node.rs:314), BVHGPU_TRAVERSE_FLAT at every reached leaf.
+ *   - traverse_dev: device pointers, enqueued on the context's stream; `total` may be NULL (no host synchronisation); hits beyond
+ *     `cap` are dropped, as bvhgpu_traverse_dev_f32x3. */
+int bvhgpu_build_f32x4(bvhgpu_ctx* ctx, const bvh_aabb4f* aabbs, size_t n, int mode, bvhgpu_tree4f** out);
+int bvhgpu_build_f64x4(bvhgpu_ctx* ctx, const bvh_aabb4d* aabbs, size_t n, int mode, bvhgpu_tree4d** out);
+void bvhgpu_tree_free_f32x4(bvhgpu_tree4f* tree);
+void bvhgpu_tree_free_f64x4(bvhgpu_tree4d* tree);
+size_t bvhgpu_tree_num_shapes_f32x4(const bvhgpu_tree4f* tree);
+size_t bvhgpu_tree_num_shapes_f64x4(const bvhgpu_tree4d* tree);
+int bvhgpu_tree_nodes_f32x4(bvhgpu_tree4f* tree, bvh_node4f* out_nodes, uint32_t* out_node_index);
+int bvhgpu_tree_nodes_f64x4(bvhgpu_tree4d* tree, bvh_node4d* out_nodes, uint32_t* out_node_index);
+int bvhgpu_flatten_f32x4(bvhgpu_tree4f* tree, bvh_flat4f* out, size_t cap, size_t* len);
+int bvhgpu_flatten_f64x4(bvhgpu_tree4d* tree, bvh_flat4d* out, size_t cap, size_t* len);
+int bvhgpu_traverse_f32x4(bvhgpu_tree4f* tree, int mode, const bvh_ray4f* rays, size_t nrays,
+                          uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_traverse_f64x4(bvhgpu_tree4d* tree, int mode, const bvh_ray4d* rays, size_t nrays,
+                          uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_traverse_dev_f32x4(bvhgpu_tree4f* tree, int mode, const void* dev_rays, size_t nrays,
+                              void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_traverse_dev_f64x4(bvhgpu_tree4d* tree, int mode, const void* dev_rays, size_t nrays,
+                              void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 
 /* ---- flatten: replaces Bvh::flatten (src/flat_bvh.rs:60-143, 240-251, 312-319) -----
  * Writes the FlatBvh (3n-2 FlatNodes for n >= 2, 1 for n == 1, 0 for n == 0) into `out`
