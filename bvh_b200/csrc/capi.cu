@@ -1006,6 +1006,8 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_query_dev_##SUF(TREE* tree, int mode, int kind, const void* dev_queries, size_t n, void* dev_offsets, \
                                           void* dev_hits, size_t cap, size_t* total) {                                    \
         if (!tree || !dev_offsets || (n && !dev_queries)) { set_error("query_dev: null argument"); return BVHGPU_ERR_INVALID; } \
+        /* query_device also serves the library's internal kinds (nearest_candidates): only the public ones get through here */ \
+        if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; } \
         BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
         return query_device<T>(tree, mode, kind, (const T*)dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
     }                                                                                                                     \

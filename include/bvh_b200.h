@@ -312,7 +312,12 @@ int bvhgpu_traverse_stats_f64x3(bvhgpu_tree3d* tree, uint64_t* out2);
 /* ---- the other IntersectsAabb implementors as batched queries (SURVEY.md 8f N2) ------------------------------
  * Bvh::traverse / FlatBvh::traverse with an Aabb (src/aabb/aabb_impl.rs:240-248, src/aabb/intersection.rs:35-39),
  * a Point (Aabb::contains, src/aabb/aabb_impl.rs:175-177, intersection.rs:41-45) or a Ball (src/ball.rs:85-106) as the
- * query.  `queries` holds n records of 6 T {min,max}, 3 T {point} or 4 T {center, radius}.  Output: CSR as for rays. */
+ * query.  `queries` holds n records of 6 T {min,max}, 3 T {point} or 4 T {center, radius}.  Output: CSR as for rays.
+ * `kind` other than the three below: BVHGPU_ERR_INVALID, nothing is read or written.
+ * query_dev: device pointers, enqueued on the context's stream.  `total` may be NULL (no host synchronisation, no capacity
+ * check).  The offsets are always complete; hits[0 .. cap) receives the first `cap` entries of the full CSR hit list (a prefix:
+ * the hits at positions >= cap are dropped).  With `total` given and more than `cap` hits, *total holds the full count and the
+ * call returns BVHGPU_ERR_CAPACITY. */
 typedef enum { BVHGPU_QUERY_AABB = 1, BVHGPU_QUERY_POINT = 2, BVHGPU_QUERY_BALL = 3 } bvhgpu_query_kind;
 int bvhgpu_query_f32x3(bvhgpu_tree3f* tree, int mode, int kind, const float* queries, size_t n,
                        uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);

@@ -23,6 +23,41 @@ def test_library_exports_every_declared_symbol():
     assert all(e.startswith("bvhgpu_") for e in exported), sorted(e for e in exported if not e.startswith("bvhgpu_"))[:5]
 
 
+# Declared entry points that no test, tool or wrapper calls, with the reason each one is allowed to stay that way.
+UNCALLED_ENTRY_POINTS: dict[str, str] = {}
+
+
+def test_every_declared_entry_point_is_called_somewhere():
+    """Every function of include/bvh_b200.h is called from the suite, tools/check_sharded.py, the Python wrappers or the C++
+    mirror.  A symbol counts as called when its literal name appears there, or when an f-string stem `bvhgpu_<stem>_{` does
+    (a stem stands for every precision / dimension suffix).  bvh_b200/capi.py is not scanned: its argtypes table names
+    every symbol.  This file is not scanned either, so that an entry in the exemption list above does not cover itself."""
+    import glob
+    import re
+
+    from bvh_b200 import capi
+
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    files = sorted(set(glob.glob(os.path.join(root, "tests", "**", "*.py"), recursive=True)) - {os.path.abspath(__file__)})
+    files += sorted(f for f in glob.glob(os.path.join(root, "tests", "cpp", "*")) if os.path.isfile(f))      # not the build directory
+    files += [os.path.join(root, *p.split("/")) for p in ("tools/check_sharded.py", "bvh_b200/api.py", "bvh_b200/dist.py", "include/bvh_b200.hpp")]
+    names, stems = set(), set()
+    for f in files:
+        text = open(f, encoding="utf-8").read()
+        names |= set(re.findall(r"\bbvhgpu_[a-z0-9_]+", text))
+        stems |= set(re.findall(r"\bbvhgpu_([a-z0-9_]+)_\{", text))
+    suffix = re.compile(r"(f32|f64)x[234]")
+
+    def covered(sym):
+        if sym in names:
+            return True
+        rest = sym[len("bvhgpu_"):]
+        return any(rest.startswith(s + "_") and suffix.fullmatch(rest[len(s) + 1:]) for s in stems)
+
+    uncovered = {s for s in capi.declared_symbols() if not covered(s)}
+    assert uncovered == set(UNCALLED_ENTRY_POINTS), sorted(uncovered ^ set(UNCALLED_ENTRY_POINTS))
+
+
 def test_pod_sizes_match_the_header():
     from bvh_b200 import dtypes as D
 

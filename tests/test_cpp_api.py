@@ -1,30 +1,29 @@
 """Builds tests/cpp/test_api.cpp (the reference's fixed-scene tests written against the C++ host mirror
-include/bvh_b200.hpp) with g++, links libbvh_b200.so, and runs it on the GPU."""
+include/bvh_b200.hpp) with g++, links libbvh_b200.so, and runs it on the GPU.  The executable goes to a temporary directory:
+the source tree may be read-only."""
 import os
 import subprocess
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cpp", "build", "test_api")
 
 
-def _build():
-    os.makedirs(os.path.dirname(EXE), exist_ok=True)
+def _build(out_dir):
+    exe = os.path.join(out_dir, "test_api")
     lib_dir = os.path.join(ROOT, "bvh_b200")
     cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "test_api.cpp"),
-           "-L", lib_dir, "-lbvh_b200", f"-Wl,-rpath,{lib_dir}", "-o", EXE]
+           "-L", lib_dir, "-lbvh_b200", f"-Wl,-rpath,{lib_dir}", "-o", exe]
     subprocess.run(cmd, check=True)
+    return exe
 
 
-def test_cpp_host_mirror_compiles_and_links():
-    _build()
-    assert os.path.exists(EXE)
+def test_cpp_host_mirror_compiles_and_links(tmp_path):
+    assert os.path.exists(_build(str(tmp_path)))
 
 
 @pytest.mark.gpu
-def test_cpp_reference_fixed_scene_tests():
-    _build()
-    r = subprocess.run([EXE], capture_output=True, text=True, timeout=120)
+def test_cpp_reference_fixed_scene_tests(tmp_path):
+    r = subprocess.run([_build(str(tmp_path))], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "all reference fixed-scene tests passed" in r.stdout
