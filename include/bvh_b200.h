@@ -329,9 +329,12 @@ int bvhgpu_query_dev_f64x3(bvhgpu_tree3d* tree, int mode, int kind, const void* 
                            void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 
 /* ---- distance-ordered traversal (SURVEY.md 8f N3): batched counterpart of Bvh::nearest_traverse_iterator /
- * farthest_traverse_iterator (src/bvh/distance_traverse.rs, src/bvh/bvh_impl.rs).  Per ray: the shapes whose AABB the ray
- * hits (same set as bvhgpu_traverse_*, BVH semantics), sorted by AABB entry distance ascending (`ascending` != 0) or by
- * exit distance descending, with that distance in `dists` (Ray::intersection_slice_for_aabb, src/ray/ray_impl.rs:118-145).
+ * farthest_traverse_iterator (src/bvh/distance_traverse.rs, src/bvh/bvh_impl.rs).  Per ray: the same set as
+ * bvhgpu_traverse_* in BVH semantics, sorted by the entry distance ascending
+ * (`ascending` != 0) or the exit distance descending of the child box the tree stores for each leaf, with that distance in
+ * `dists` (Ray::intersection_slice_for_aabb, src/ray/ray_impl.rs:118-145; distance_traverse.rs:100-116 slices the same box).
+ * On tight trees that box is the shape's AABB.  Where surface areas overflow, "no split wins" nodes store Aabb::empty()
+ * children, which every ray passes at entry 0 / exit inf: those leaves are listed whether or not the ray hits the shape itself.
  * The reference iterator is best-effort ("not necessarily perfectly sorted"); this result is perfectly sorted, ties in the
  * reference's DFS order.  Host pointers; `cap` entries in hits and dists. */
 int bvhgpu_traverse_ordered_f32x3(bvhgpu_tree3f* tree, const bvh_ray3f* rays, size_t nrays, int ascending,
@@ -437,8 +440,9 @@ int bvhgpu_update_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_changed, const 
  * are independent).  At each insertion point p a new inner node takes p's place: its left child is the exact-SAH subtree over the
  * shapes that chose p (ascending index order; a leaf for one shape), its right child p's old subtree; the ancestors' boxes are
  * refitted.  For k = 1 this is the reference's own topology, and its own tree whenever the boxes are tight (every built tree except
- * f32 trees whose surface areas overflow, where the builder stores empty child boxes: there the device refits the affected paths up to
- * the root, the reference stops at the first box that does not change, so boxes on those paths can differ).  max_growth >= 1: then the growth test of bvhgpu_update_* runs on the
+ * trees whose surface areas overflow -- coordinates from about 1e19 in f32, 1e154 in f64 -- where the builder stores empty child
+ * boxes: there the device refits the affected paths up to the root, the reference stops at the first box that does not change, so
+ * boxes on those paths can differ; traversal then follows the device's boxes).  max_growth >= 1: then the growth test of bvhgpu_update_* runs on the
  * changed ancestors and the degraded subtrees are rebuilt in place; *rebuilt (may be NULL) = shapes in those subtrees.
  * max_growth <= 0: no rebuild, *rebuilt = 0.  n == 0: the call is bvhgpu_build_* over the k AABBs.  Triangles set with
  * bvhgpu_tree_set_triangles_* are discarded (the triangle forms of closest_hit / nearest return BVHGPU_ERR_INVALID until set again).

@@ -171,3 +171,20 @@ def traverse_recursive(nodes, aabbs, ray, F=np.float32):
 
     rec(0)
     return out
+
+
+def traverse_flat(flat, aabbs, ray, F=np.float32):
+    """FlatBvh::traverse (src/flat_bvh.rs:396-431) over flatten()'s output: a leaf re-tests its shape's own AABB."""
+    out = []
+    i = 0
+    while i < len(flat):
+        box, entry, exit_, shape = flat[i]
+        if entry == U32_MAX:
+            if hit(F, ray, aabbs[shape]["min"], aabbs[shape]["max"]):
+                out.append(shape)
+            i = exit_
+        elif hit(F, ray, *box):
+            i = entry
+        else:
+            i = exit_
+    return out
