@@ -456,9 +456,11 @@ def swap_moves(n: int, indices) -> np.ndarray:
 
 class Bvh2:
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays
-    (bvhgpu_*_f32x2 / _f64x2).  Rays: structured array with 2-component origin, direction (normalised), inv_direction."""
+    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries and nearest_to.  Rays: structured array with 2-component origin, direction
+    (normalised), inv_direction."""
 
     _TABLE = BY_PREC_2D
+    _DIM = 2
 
     def __init__(self, handle, prec: str, ctx: Context, n: int):
         self._h, self.prec, self.ctx, self._d, self.n = handle, prec, ctx, self._TABLE[prec], n
@@ -512,12 +514,65 @@ class Bvh2:
             capi.check(st)
             return offsets, hits[: total.value]
 
+    def _query_stride(self, kind: int) -> int:
+        D = self._DIM
+        return {capi.QUERY_AABB: 2 * D, capi.QUERY_POINT: D, capi.QUERY_BALL: D + 1}[kind]
+
+    def _csr_call(self, fn, n: int, cap: int, *args):
+        """Calls fn(*args, offsets, out, cap, &total) again with cap = total when the first capacity is short (there is no fetch call)."""
+        offsets = np.zeros(n + 1, dtype=np.uint32)
+        while True:
+            out = np.zeros(cap, dtype=np.uint32)
+            total = C.c_size_t(0)
+            st = fn(*args, _ptr(offsets), _ptr(out), cap, C.byref(total))
+            if st == capi.ERR_CAPACITY and total.value > cap and total.value <= U32_MAX:
+                cap = total.value
+                continue
+            capi.check(st)
+            return offsets, out[: total.value]
+
+    def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
+        """Bvh::traverse with Aabb / Point / Ball queries: (n, 2D) {min, max} for capi.QUERY_AABB, (n, D) points for QUERY_POINT,
+        (n, D+1) {center, radius} for QUERY_BALL.  CSR (offsets, hits), hits of a query in the reference's DFS order."""
+        q = np.ascontiguousarray(queries, dtype=self._d["scalar"]).reshape(-1, self._query_stride(kind))
+        fn = getattr(capi.lib(), f"bvhgpu_query_{self._d['suffix']}")
+        return self._csr_call(fn, len(q), max(16 * len(q), 1024), self._h, mode, kind, _ptr(q), len(q))
+
+    def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
+        """Bvh::nearest_to / FlatBvh::nearest_to for shapes whose distance is their AABB's: (shape index per point, U32_MAX for an
+        empty tree; distance per point).  points: (n, D)."""
+        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, self._DIM)
+        shape = np.zeros(len(p), dtype=np.uint32)
+        dist = np.zeros(len(p), dtype=self._d["scalar"])
+        capi.check(getattr(capi.lib(), f"bvhgpu_nearest_{self._d['suffix']}")(self._h, mode, _ptr(p), len(p), _ptr(shape), _ptr(dist)))
+        return shape, dist
+
+    def nearest_candidates(self, points):
+        """CSR (offsets, shape indices) of candidate lists that contain the nearest shape of every point, for shapes with their own
+        distance (see `nearest_to`).  points: (n, D)."""
+        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, self._DIM)
+        fn = getattr(capi.lib(), f"bvhgpu_nearest_candidates_{self._d['suffix']}")
+        return self._csr_call(fn, len(p), max(64 * len(p), 1024), self._h, _ptr(p), len(p))
+
+    def nearest_to(self, point, shapes, distance_squared):
+        """BoundingHierarchy::nearest_to for one point and an arbitrary shape distance: `distance_squared(shape, point)` is the shape's
+        PointDistance::distance_squared.  Returns (shape, distance) or None for an empty tree."""
+        off, cand = self.nearest_candidates([point])
+        best = None
+        for s in cand[off[0]:off[1]]:
+            d = distance_squared(shapes[int(s)], point)
+            if best is None or d < best[1]:
+                best = (shapes[int(s)], d)
+        return None if best is None else (best[0], float(np.sqrt(best[1])))
+
 
 class Bvh4(Bvh2):
-    """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten and batched
-    ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction)."""
+    """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten, batched
+    ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction), and the queries and nearest_to
+    of Bvh2 with 4 components, plus query_dev."""
 
     _TABLE = BY_PREC_4D
+    _DIM = 4
 
     def traverse_dev(self, rays_ptr: int, nrays: int, offsets_ptr: int, hits_ptr: int, cap: int, mode: int = capi.TRAVERSE_BVH,
                      want_total: bool = False):
@@ -526,5 +581,15 @@ class Bvh4(Bvh2):
         total = C.c_size_t(0)
         fn = getattr(capi.lib(), f"bvhgpu_traverse_dev_{self._d['suffix']}")
         capi.check(fn(self._h, mode, C.c_void_p(rays_ptr), nrays, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
+                      C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
+    def query_dev(self, kind: int, queries_ptr: int, n: int, offsets_ptr: int, hits_ptr: int, cap: int, mode: int = capi.TRAVERSE_BVH,
+                  want_total: bool = False):
+        """Aabb / Point / Ball queries from device pointers (records of 8 / 4 / 5 scalars), enqueued on the context's stream.  The
+        offsets are always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        total = C.c_size_t(0)
+        fn = getattr(capi.lib(), f"bvhgpu_query_dev_{self._d['suffix']}")
+        capi.check(fn(self._h, mode, kind, C.c_void_p(queries_ptr), n, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
                       C.byref(total) if want_total else None))
         return total.value if want_total else None

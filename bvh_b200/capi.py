@@ -131,6 +131,9 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_tree_nodes_{s}").argtypes = [vp, vp, vp]
         getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
         getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_query_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_nearest_{s}").argtypes = [vp, i32, vp, sz, vp, vp]
+        getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
     for s in ("f32x4", "f64x4"):
         getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
         getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]
@@ -141,6 +144,10 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
         getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_traverse_dev_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_query_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_query_dev_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_nearest_{s}").argtypes = [vp, i32, vp, sz, vp, vp]
+        getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
     missing =[n for n in declared_symbols() if not hasattr(L, n)]
     if missing:
         raise ImportError(f"{SO_PATH} does not export {missing}")

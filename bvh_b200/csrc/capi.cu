@@ -245,20 +245,37 @@ static int traverse_host_impl(Tree<T>* tree, int mode, const void* rays, uint32_
     return BVHGPU_OK;
 }
 
-template <class T>
+// D = 3: the C-ABI records as they are.  D = 2: records of 2-vectors (a Bvh<T,2> embedded in z = 0), lifted on the device
+// (dim2_lift) before they reach the 3-D kernels; there is no fetch call for D = 2, so a short `cap` is answered with
+// "call again with cap = *total" and the retained buffers are re-used by that call.
+template <int D, class T> static int upload_records(Tree<T>* tree, Scratch& scratch, const T* h, size_t n, int nvec, int nscal, T** d_out) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    const size_t in_w = (size_t)D * nvec + nscal;
+    T* d_in = nullptr;
+    BVH_TRY(scratch.get(&d_in, n * in_w));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_in, h, sizeof(T) * n * in_w, cudaMemcpyHostToDevice, ctx->stream));
+    if (D == 3) { *d_out = d_in; return BVHGPU_OK; }
+    T* d_lift = nullptr;
+    BVH_TRY(scratch.get(&d_lift, n * (3 * (size_t)nvec + nscal)));
+    BVH_TRY(dim2_lift<T>(ctx, d_in, (uint32_t)n, nvec, nscal, d_lift));
+    *d_out = d_lift;
+    return BVHGPU_OK;
+}
+static const char* capacity_hint(int D) { return D == 3 ? "use bvhgpu_traverse_fetch_*" : "call again with cap = *total"; }
+
+template <class T, int D = 3>
 static int query_host_impl(Tree<T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || (n && !queries) || !offsets) { set_error("query: null argument"); return BVHGPU_ERR_INVALID; }
     if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
+    if (D != 3 && n > 0x7FFFFFFFull) { set_error("query: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
+    if (D != 3 && mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("query: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
-    const size_t stride = kind == BVHGPU_QUERY_AABB ? 6 : (kind == BVHGPU_QUERY_POINT ? 3 : 4);
+    const int nvec = kind == BVHGPU_QUERY_AABB ? 2 : 1, nscal = kind == BVHGPU_QUERY_BALL ? 1 : 0;
     T* d_q = nullptr;
     Scratch scratch(ctx);                                           // released on every return path
-    if (n) {
-        BVH_TRY(scratch.get(&d_q, n * stride));
-        BVH_CUDA_TRY(cudaMemcpyAsync(d_q, queries, sizeof(T) * n * stride, cudaMemcpyHostToDevice, ctx->stream));
-    }
+    if (n) BVH_TRY(upload_records<D>(tree, scratch, queries, n, nvec, nscal, &d_q));
     size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 16 * n), 1024), tot = 0;
     int rc = BVHGPU_OK;
     for (int attempt = 0; attempt < 2; ++attempt) {
@@ -273,14 +290,16 @@ static int query_host_impl(Tree<T>* tree, int mode, int kind, const T* queries, 
     BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
     int ret = BVHGPU_OK;
     if (hits && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
-    else if (tot > cap) { set_error("query: %zu hits do not fit the caller's capacity %zu (use bvhgpu_traverse_fetch_*)", tot, cap); ret = BVHGPU_ERR_CAPACITY; }
+    else if (tot > cap) { set_error("query: %zu hits do not fit the caller's capacity %zu (%s)", tot, cap, capacity_hint(D)); ret = BVHGPU_ERR_CAPACITY; }
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return ret;
 }
 
-template <class T>
+template <class T, int D = 3>
 static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist, int use_triangles = 0) {
     if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("nearest: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D != 3 && n > 0x7FFFFFFFull) { set_error("nearest: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
+    if (D != 3 && mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("nearest: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
@@ -288,10 +307,9 @@ static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n,
     T *d_p = nullptr, *d_d = nullptr;
     uint32_t* d_s = nullptr;
     Scratch scratch(ctx);
-    BVH_TRY(scratch.get(&d_p, n * 3));
+    BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
     BVH_TRY(scratch.get(&d_d, n));
     BVH_TRY(scratch.get(&d_s, n));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_p, points, sizeof(T) * n * 3, cudaMemcpyHostToDevice, ctx->stream));
     int rc = nearest_device<T>(tree, mode, d_p, n, d_s, d_d, use_triangles);
     if (rc == BVHGPU_OK) {
         BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -301,18 +319,16 @@ static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n,
     return rc;
 }
 
-template <class T>
+template <class T, int D = 3>
 static int nearest_candidates_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
     if (!tree || (n && !points) || !offsets) { set_error("nearest_candidates: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D != 3 && n > 0x7FFFFFFFull) { set_error("nearest_candidates: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
     T* d_p = nullptr;
     Scratch scratch(ctx);
-    if (n) {
-        BVH_TRY(scratch.get(&d_p, n * 3));
-        BVH_CUDA_TRY(cudaMemcpyAsync(d_p, points, sizeof(T) * n * 3, cudaMemcpyHostToDevice, ctx->stream));
-    }
+    if (n) BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
     size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 16 * n), 1024), tot = 0;
     int rc = BVHGPU_OK;
     for (int attempt = 0; attempt < 2; ++attempt) {
@@ -327,7 +343,7 @@ static int nearest_candidates_host_impl(Tree<T>* tree, const T* points, size_t n
     BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
     int ret = BVHGPU_OK;
     if (cand && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(cand, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
-    else if (tot > cap) { set_error("nearest_candidates: %zu candidates do not fit the caller's capacity %zu (use bvhgpu_traverse_fetch_*)", tot, cap); ret = BVHGPU_ERR_CAPACITY; }
+    else if (tot > cap) { set_error("nearest_candidates: %zu candidates do not fit the caller's capacity %zu (%s)", tot, cap, capacity_hint(D)); ret = BVHGPU_ERR_CAPACITY; }
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return ret;
 }
@@ -1106,6 +1122,17 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_traverse_##SUF(TREE* tree, int mode, const RAY* rays, size_t nrays, uint32_t* offsets, uint32_t* hits, \
                                          size_t cap, size_t* total) {                                                      \
         return traverse2_impl<T, RAY>(tree, mode, rays, nrays, offsets, hits, cap, total);                                 \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, \
+                                      size_t cap, size_t* total) {                                                        \
+        return query_host_impl<T, 2>(tree, mode, kind, queries, n, offsets, hits, cap, total);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
+        return nearest_host_impl<T, 2>(tree, mode, points, n, out_shape, out_dist);                                        \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
+                                                   size_t cap, size_t* total) {                                            \
+        return nearest_candidates_host_impl<T, 2>(tree, points, n, offsets, cand, cap, total);                             \
     }
 
 DEFINE_API2(float, f32x2, bvhgpu_tree2f, bvh_aabb2f, bvh_ray2f, bvh_node2f, bvh_flat2f)

@@ -8,6 +8,14 @@
 //   traverse  the traversal records (and the shape AABBs the FLAT leaf re-test reads) get z = [-1, +1]; rays get origin.z = 0 and
 //             inv_direction.z = +inf: the z slab is (-1 - 0) * inf = -inf, (1 - 0) * inf = +inf -- never NaN, and max(tmin, -inf),
 //             min(tmax, +inf) are identities, so the 3-D slab test returns exactly what the 2-D one does.
+//   queries   Aabb / Point / Ball records and nearest_to points are lifted to z = 0 (lift2_kernel) and run through the 3-D query and
+//             nearest kernels.  Every z term is exactly neutral, so the results are the 2-D ones bit for bit:
+//               - Aabb and Point tests pass on z: the records and the FLAT re-test boxes span z = [-1, +1] and contain 0.
+//               - Ball: the centre's z = 0 clamps to itself, so the z difference is +0 and adds +0 to the sum of squares.
+//               - Aabb::min_distance_squared on d_nodes / d_flat / d_aabb (z = [0, 0]): half size 0, centre 0, o_z = max(|0 - 0| - 0, 0)
+//                 = 0; on an empty child box (z = [+inf, -inf]) the centre is NaN and o_z = 0 as well (NaN.max(0) = 0, as in Rust).
+//               - the QUERY_WITHIN lower bound on a record: max(-1 - 0, 0 - 1) = -1 -> 0; the farthest-corner bound on a shape: |0 - 0| = 0.
+//               - adding +0 to a non-negative sum is exact, and the squares are summed left to right, so z comes last.
 // The 2-D PODs are converted on the device (expand on the way in, drop z on the way out).
 #include "internal.h"
 
@@ -56,6 +64,17 @@ template <class T, class F2> __global__ void __launch_bounds__(256) shrink_flat_
     out[i] = o;
 }
 
+// Query records and points lifted into the plane z = 0: every 2-vector of a record gets z = 0, trailing scalars are copied.
+//   Aabb {min, max}: nvec = 2 (z = [0, 0]);  Point and nearest_to points: nvec = 1 (z = 0);  Ball {center, radius}: nvec = 1, nscal = 1.
+template <class T> __global__ void __launch_bounds__(256) lift2_kernel(const T* __restrict__ in, uint32_t n, int nvec, int nscal, T* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const T* p = in + (size_t)(2 * nvec + nscal) * i;
+    T* q = out + (size_t)(3 * nvec + nscal) * i;
+    for (int v = 0; v < nvec; ++v) { q[3 * v] = p[2 * v]; q[3 * v + 1] = p[2 * v + 1]; q[3 * v + 2] = T(0); }
+    for (int s = 0; s < nscal; ++s) q[3 * nvec + s] = p[2 * nvec + s];
+}
+
 template <class T> int dim2_expand_aabbs(bvhgpu_ctx* ctx, const T* d_in4, uint32_t n, T* d_out6) {
     expand_aabb2_kernel<T><<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_in4, n, d_out6);
     ctx->launches++;
@@ -64,6 +83,12 @@ template <class T> int dim2_expand_aabbs(bvhgpu_ctx* ctx, const T* d_in4, uint32
 }
 template <class T> int dim2_expand_rays(bvhgpu_ctx* ctx, const T* d_in6, uint32_t n, T* d_out9) {
     expand_ray2_kernel<T><<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_in6, n, d_out9);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+template <class T> int dim2_lift(bvhgpu_ctx* ctx, const T* d_in, uint32_t n, int nvec, int nscal, T* d_out) {
+    lift2_kernel<T><<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_in, n, nvec, nscal, d_out);
     ctx->launches++;
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
@@ -97,6 +122,8 @@ template int dim2_expand_aabbs<float>(bvhgpu_ctx*, const float*, uint32_t, float
 template int dim2_expand_aabbs<double>(bvhgpu_ctx*, const double*, uint32_t, double*);
 template int dim2_expand_rays<float>(bvhgpu_ctx*, const float*, uint32_t, float*);
 template int dim2_expand_rays<double>(bvhgpu_ctx*, const double*, uint32_t, double*);
+template int dim2_lift<float>(bvhgpu_ctx*, const float*, uint32_t, int, int, float*);
+template int dim2_lift<double>(bvhgpu_ctx*, const double*, uint32_t, int, int, double*);
 template int dim2_finish_build<float>(Tree<float>*);
 template int dim2_finish_build<double>(Tree<double>*);
 template int dim2_nodes_out<float, bvh_node2f>(Tree<float>*, bvh_node2f*);

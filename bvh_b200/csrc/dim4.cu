@@ -16,6 +16,7 @@
 // Node positions depend only on counts (cl = me + 1, cr = me + 2 nl) and every reduction is a min / max / sum of integers, so the
 // order in which warps run never shows in the result: two builds of the same input are byte-identical.
 #include "internal.h"
+#include "queries.cuh"
 #include <algorithm>
 #include <new>
 
@@ -572,21 +573,36 @@ __device__ __forceinline__ void load_ray4(const bvh_ray4d* p, double o[4], doubl
     o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y; inv[0] = c.x; inv[1] = c.y; inv[2] = d.x; inv[3] = d.y;
 }
 
-template <class T, bool FLAT, class Emit>
+// What one thread walks the records with: hit(mn, mx) is the predicate, load(src, r) reads item r of the batch.
+//   RayProbe4         the 4-wide slab test of a Ray<T,4>
+//   QueryProbe4<KIND> an Aabb / Point / Ball query (aabb_impl.rs:240-248, :175-177, ball.rs:85-99) or the internal QUERY_WITHIN
+//                     bound of nearest_candidates, with D = 4 (queries.cuh)
+template <class T> struct RayProbe4 {
+    T o[4], inv[4];
+    __device__ __forceinline__ void load(const void* src, uint32_t r) { load_ray4(reinterpret_cast<const typename D4<T>::Ray*>(src) + r, o, inv); }
+    __device__ __forceinline__ bool hit(const T mn[4], const T mx[4]) const { return slab4(o, inv, mn, mx); }
+};
+template <class T, int KIND> struct QueryProbe4 : Query<T, KIND, 4> {
+    __device__ __forceinline__ void load(const void* src, uint32_t r) {
+        Query<T, KIND, 4>::load(reinterpret_cast<const T*>(src) + (size_t)r * Query<T, KIND, 4>::STRIDE);
+    }
+};
+
+template <class T, bool FLAT, class P, class Emit>
 __device__ __forceinline__ void walk4(const typename D4<T>::Rec* __restrict__ trec, uint32_t n_rec, const typename D4<T>::Aabb* __restrict__ aabb,
-                                      const T o[4], const T inv[4], Emit emit) {
+                                      const P& probe, Emit emit) {
     uint32_t i = 0;
     while (i < n_rec) {
         T mn[4], mx[4];
         uint32_t skip, shape;
         fetch4(trec + i, mn, mx, skip, shape);
-        if (slab4(o, inv, mn, mx)) {
+        if (probe.hit(mn, mx)) {
             if (shape != BVH_INVALID) {
                 bool report = true;
                 if (FLAT) {                                    // flat_bvh.rs:412-416: a reached leaf re-tests the shape's AABB
                     T smn[4], smx[4];
                     load4(aabb + shape, smn, smx);
-                    report = slab4(o, inv, smn, smx);
+                    report = probe.hit(smn, smx);
                 }
                 if (report) emit(shape);
             }
@@ -597,27 +613,60 @@ __device__ __forceinline__ void walk4(const typename D4<T>::Rec* __restrict__ tr
     }
 }
 
-// count pass (FILL = false) and fill pass (FILL = true); hits beyond cap are dropped
-template <class T, bool FLAT, bool FILL>
+// count pass (FILL = false) and fill pass (FILL = true) for a batch of n items of probe P; hits beyond cap are dropped
+template <class T, bool FLAT, bool FILL, class P>
 __global__ void __launch_bounds__(256) walk4_kernel(const typename D4<T>::Rec* __restrict__ trec, uint32_t n_rec, const typename D4<T>::Aabb* __restrict__ aabb,
-                                                    const typename D4<T>::Ray* __restrict__ rays, uint32_t nrays, uint32_t* __restrict__ counts,
+                                                    const void* __restrict__ src, uint32_t n, uint32_t* __restrict__ counts,
                                                     const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
                                                     const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits,
                                                     unsigned long long cap) {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (FILL && r == 0) { const unsigned long long t = *total; offsets[nrays] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
-    if (r >= nrays) return;
-    T o[4], inv[4];
-    load_ray4(rays + r, o, inv);
+    if (FILL && r == 0) { const unsigned long long t = *total; offsets[n] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
+    if (r >= n) return;
+    P probe;
+    probe.load(src, r);
     if (!FILL) {
         uint32_t cnt = 0;
-        walk4<T, FLAT>(trec, n_rec, aabb, o, inv, [&](uint32_t) { ++cnt; });
+        walk4<T, FLAT>(trec, n_rec, aabb, probe, [&](uint32_t) { ++cnt; });
         counts[r] = cnt;
     } else {
         unsigned long long w = blocksum[r / CSR_SCAN_TILE] + local[r];
         offsets[r] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
-        if (hits) walk4<T, FLAT>(trec, n_rec, aabb, o, inv, [&](uint32_t shape) { if (w < cap) hits[w] = shape; ++w; });
+        if (hits) walk4<T, FLAT>(trec, n_rec, aabb, probe, [&](uint32_t shape) { if (w < cap) hits[w] = shape; ++w; });
     }
+}
+
+// ---- nearest_to: the walks of queries.cuh over the 4-D nodes / flat array; the leaf value is the shape AABB's distance ----
+template <class T, bool FLAT>
+__global__ void __launch_bounds__(128) nearest4_kernel(const typename D4<T>::Node* __restrict__ nodes, const typename D4<T>::Flat* __restrict__ flat,
+                                                       uint32_t n_flat, const typename D4<T>::Aabb* __restrict__ aabb, const T* __restrict__ points,
+                                                       uint32_t nq, uint32_t* __restrict__ out_shape, T* __restrict__ out_dist) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    T p[4];
+    for (int k = 0; k < 4; ++k) p[k] = points[4 * (size_t)i + k];
+    uint32_t best = BVH_INVALID;
+    T best_d = T(0);
+    auto leaf = [&](uint32_t shape) { T mn[4], mx[4]; load4(aabb + shape, mn, mx); return aabb_min_d2<4>(p, mn, mx); };
+    if (!FLAT) nearest_walk<4, T, true>(nodes, p, best, best_d, leaf);
+    else       nearest_flat<4, T>(flat, n_flat, p, best, best_d, leaf);
+    out_shape[i] = best;
+    out_dist[i] = sqrt_rn(best_d);                          // bvh_impl.rs:237
+}
+// nearest_candidates, first pass: the farthest-corner bound U of every point (as nearest_bound_kernel), records {p, U} for QUERY_WITHIN
+template <class T>
+__global__ void __launch_bounds__(128) nearest_bound4_kernel(const typename D4<T>::Node* __restrict__ nodes, const typename D4<T>::Aabb* __restrict__ aabb,
+                                                             const T* __restrict__ points, uint32_t nq, T* __restrict__ records) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    T p[4];
+    for (int k = 0; k < 4; ++k) p[k] = points[4 * (size_t)i + k];
+    uint32_t best;
+    T u;
+    nearest_walk<4, T, false>(nodes, p, best, u, [&](uint32_t shape) { T mn[4], mx[4]; load4(aabb + shape, mn, mx); return box_upper_d2<4>(p, mn, mx); });
+    u = mul_rn(u, add_rn(T(1), mul_rn(T(16), Traits<T>::eps())));      // the bound itself is a rounded sum: keep it an upper bound
+    for (int k = 0; k < 4; ++k) records[5 * (size_t)i + k] = p[k];
+    records[5 * (size_t)i + 4] = u;
 }
 
 // ================================================================================================================================
@@ -772,9 +821,9 @@ template <class T> static int flatten4_impl(Tree4<T>* tree, typename D4<T>::Flat
     return BVHGPU_OK;
 }
 
-// Count pass + scan on the stream; leaves the 64-bit total at sums[nblk].  Needs n > 0 and nrays > 0.
-template <class T> static int count_and_scan4(Tree4<T>* tree, bool flat, const typename D4<T>::Ray* d_rays, uint32_t R, Scratch& scratch,
-                                              uint32_t** counts, uint32_t** local, unsigned long long** sums) {
+// Count pass + scan on the stream; leaves the 64-bit total at sums[nblk].  Needs tree->n > 0 and R > 0.  src: R items of probe P.
+template <class P, class T> static int count_and_scan4(Tree4<T>* tree, bool flat, const void* d_src, uint32_t R, Scratch& scratch,
+                                                       uint32_t** counts, uint32_t** local, unsigned long long** sums) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
     if (!tree->d_trec) {
@@ -789,98 +838,89 @@ template <class T> static int count_and_scan4(Tree4<T>* tree, bool flat, const t
     BVH_TRY(scratch.get(sums, (size_t)nblk + 1));
     BVH_CUDA_TRY(cudaMemsetAsync(*sums + nblk, 0, sizeof(unsigned long long), st));
     const int grid = (R + 255) / 256;
-    if (flat) walk4_kernel<T, true, false><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    else      walk4_kernel<T, false, false><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    if (flat) walk4_kernel<T, true, false, P><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    else      walk4_kernel<T, false, false, P><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
     scan_local_kernel<<<nblk, CSR_SCAN_THREADS, 0, st>>>(*counts, R, *local, *sums, nullptr);
     scan_blocks_kernel<<<1, 1024, 0, st>>>(*sums, nblk, *sums + nblk);
     LAUNCHED(ctx, 3);
     return BVHGPU_OK;
 }
-template <class T> static int fill4(Tree4<T>* tree, bool flat, const typename D4<T>::Ray* d_rays, uint32_t R, const uint32_t* local,
-                                    const unsigned long long* sums, uint32_t* d_offsets, uint32_t* d_hits, size_t cap) {
+template <class P, class T> static int fill4(Tree4<T>* tree, bool flat, const void* d_src, uint32_t R, const uint32_t* local,
+                                             const unsigned long long* sums, uint32_t* d_offsets, uint32_t* d_hits, size_t cap) {
     bvhgpu_ctx* ctx = tree->ctx;
     const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
     const int grid = (R + 255) / 256;
-    if (flat) walk4_kernel<T, true, true><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
-    else      walk4_kernel<T, false, true><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_rays, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
+    if (flat) walk4_kernel<T, true, true, P><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
+    else      walk4_kernel<T, false, true, P><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
 }
 
-template <class T> static int check_traverse_args(Tree4<T>* tree, int mode, size_t nrays) {
-    if (nrays > 0x7FFFFFFFull) { set_error("traverse: nrays %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+// `what` names the entry point in error messages
+template <class T> static int check_batch_args(Tree4<T>* tree, int mode, size_t n, const char* what) {
+    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
+    if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("%s: bad mode %d", what, mode); return BVHGPU_ERR_INVALID; }
     return sticky4(tree);
 }
+static bool public_query_kind(int kind) { return kind >= BVHGPU_QUERY_AABB && kind <= BVHGPU_QUERY_BALL; }
+template <class T> static size_t query_stride4(int kind) {
+    return kind == BVHGPU_QUERY_AABB ? Query<T, BVHGPU_QUERY_AABB, 4>::STRIDE : kind == BVHGPU_QUERY_POINT ? Query<T, BVHGPU_QUERY_POINT, 4>::STRIDE
+                                                                            : Query<T, BVHGPU_QUERY_BALL, 4>::STRIDE;
+}
 
-// device pointers, enqueued on the context's stream; synchronises only to return *total
-template <class T> static int traverse4_dev_impl(Tree4<T>* tree, int mode, const void* d_rays, size_t nrays, uint32_t* d_offsets, uint32_t* d_hits,
-                                                 size_t cap, size_t* total) {
-    if (!tree || !d_offsets || (nrays && !d_rays)) { set_error("traverse_dev: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_traverse_args(tree, mode, nrays));
+// Device pointers, enqueued on the context's stream; synchronises only to return *total.  Arguments checked by the caller.
+template <class P, class T> static int csr4_dev(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* d_offsets, uint32_t* d_hits,
+                                                size_t cap, size_t* total, const char* what) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (nrays == 0 || tree->n == 0) {                              // no rays / empty Bvh: no hits (bvh_impl.rs:109-112)
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (nrays + 1), st));
+    if (n == 0 || tree->n == 0) {                                  // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
+        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (n + 1), st));
         if (total) *total = 0;
         return BVHGPU_OK;
     }
-    const uint32_t R = (uint32_t)nrays;
-    const auto* rays = reinterpret_cast<const typename D4<T>::Ray*>(d_rays);
-    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    const uint32_t R = (uint32_t)n;
     Scratch scratch(ctx);
     uint32_t *counts = nullptr, *local = nullptr;
     unsigned long long* sums = nullptr;
-    BVH_TRY(count_and_scan4(tree, flat, rays, R, scratch, &counts, &local, &sums));
+    BVH_TRY(count_and_scan4<P>(tree, flat, d_src, R, scratch, &counts, &local, &sums));
     const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
     unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned + 236);
     if (total) {                                                   // the total is known before the hit lists are written
         BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
         BVH_CUDA_TRY(cudaEventRecord(ctx->ev_total, st));
     }
-    BVH_TRY(fill4(tree, flat, rays, R, local, sums, d_offsets, d_hits, cap));
+    BVH_TRY(fill4<P>(tree, flat, d_src, R, local, sums, d_offsets, d_hits, cap));
     if (!total) return BVHGPU_OK;
     BVH_CUDA_TRY(cudaEventSynchronize(ctx->ev_total));
     *total = (size_t)*h;
-    if (*h > 0xFFFFFFFFull) { set_error("traverse: %llu hits overflow the u32 CSR offsets", *h); return BVHGPU_ERR_CAPACITY; }
-    if (d_hits && *h > cap) { set_error("traverse: %llu hits do not fit capacity %zu", *h, cap); return BVHGPU_ERR_CAPACITY; }
+    if (*h > 0xFFFFFFFFull) { set_error("%s: %llu hits overflow the u32 CSR offsets", what, *h); return BVHGPU_ERR_CAPACITY; }
+    if (d_hits && *h > cap) { set_error("%s: %llu hits do not fit capacity %zu", what, *h, cap); return BVHGPU_ERR_CAPACITY; }
     return BVHGPU_OK;
 }
 
-// host pointers: count, read the total, size the retained hit buffer, fill, copy back
-template <class T> static int traverse4_host_impl(Tree4<T>* tree, int mode, const typename D4<T>::Ray* rays, size_t nrays, uint32_t* offsets,
-                                                  uint32_t* hits, size_t cap, size_t* total) {
-    if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_traverse_args(tree, mode, nrays));
+// Host CSR out of a batch already on the device (d_src, n > 0, tree->n > 0): count, read the total, size the retained hit buffer
+// exactly, fill, copy back.  Hits that do not fit `cap` are not copied; offsets and *total are, and the call returns
+// BVHGPU_ERR_CAPACITY -- the caller's second call with cap = *total is the only extra walk.
+template <class P, class T> static int csr4_host(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
+                                                 size_t cap, size_t* total, const char* what) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (nrays == 0 || tree->n == 0) {
-        std::fill(offsets, offsets + nrays + 1, 0u);
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    const uint32_t R = (uint32_t)nrays;
-    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    const uint32_t R = (uint32_t)n;
     Scratch scratch(ctx);
-    typename D4<T>::Ray* d_rays = nullptr;
-    BVH_TRY(scratch.get(&d_rays, nrays));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, st));
     uint32_t *counts = nullptr, *local = nullptr;
     unsigned long long* sums = nullptr;
-    BVH_TRY(count_and_scan4(tree, flat, d_rays, R, scratch, &counts, &local, &sums));
+    BVH_TRY(count_and_scan4<P>(tree, flat, d_src, R, scratch, &counts, &local, &sums));
     const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
     unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned + 236);
     BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
     const unsigned long long tot = *h;
     if (total) *total = (size_t)tot;
-    if (tot > 0xFFFFFFFFull) { set_error("traverse: %llu hits overflow the u32 CSR offsets", tot); return BVHGPU_ERR_CAPACITY; }
-    if (tree->offsets_cap < nrays + 1) {
+    if (tot > 0xFFFFFFFFull) { set_error("%s: %llu hits overflow the u32 CSR offsets", what, tot); return BVHGPU_ERR_CAPACITY; }
+    if (tree->offsets_cap < n + 1) {
         dfree(ctx, tree->d_offsets); tree->d_offsets = nullptr; tree->offsets_cap = 0;
-        BVH_TRY(dalloc_t(ctx, &tree->d_offsets, nrays + 1));
-        tree->offsets_cap = nrays + 1;
+        BVH_TRY(dalloc_t(ctx, &tree->d_offsets, n + 1));
+        tree->offsets_cap = n + 1;
     }
     const bool fits = hits && tot <= cap;
     if (fits && tree->hits_cap < tot) {
@@ -888,12 +928,136 @@ template <class T> static int traverse4_host_impl(Tree4<T>* tree, int mode, cons
         BVH_TRY(dalloc_t(ctx, &tree->d_hits, tot));
         tree->hits_cap = tot;
     }
-    BVH_TRY(fill4(tree, flat, d_rays, R, local, sums, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, st));
+    BVH_TRY(fill4<P>(tree, flat, d_src, R, local, sums, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
+    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
     if (fits && tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (tot > cap) { set_error("traverse: %llu hits do not fit the caller's capacity %zu (call again with cap = *total)", tot, cap); return BVHGPU_ERR_CAPACITY; }
+    if (tot > cap) { set_error("%s: %llu hits do not fit the caller's capacity %zu (call again with cap = *total)", what, tot, cap); return BVHGPU_ERR_CAPACITY; }
     return BVHGPU_OK;
+}
+
+// host batch -> device scratch (n items of `bytes` each)
+static int upload4(bvhgpu_ctx* ctx, Scratch& scratch, const void* h_src, size_t bytes, void** d_out) {
+    char* d = nullptr;
+    BVH_TRY(scratch.get(&d, bytes));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d, h_src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    *d_out = d;
+    return BVHGPU_OK;
+}
+
+// ---- rays ----
+template <class T> static int traverse4_dev_impl(Tree4<T>* tree, int mode, const void* d_rays, size_t nrays, uint32_t* d_offsets, uint32_t* d_hits,
+                                                 size_t cap, size_t* total) {
+    if (!tree || !d_offsets || (nrays && !d_rays)) { set_error("traverse_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_batch_args(tree, mode, nrays, "traverse"));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return csr4_dev<RayProbe4<T>>(tree, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, d_offsets, d_hits, cap, total, "traverse");
+}
+template <class T> static int traverse4_host_impl(Tree4<T>* tree, int mode, const typename D4<T>::Ray* rays, size_t nrays, uint32_t* offsets,
+                                                  uint32_t* hits, size_t cap, size_t* total) {
+    if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_batch_args(tree, mode, nrays, "traverse"));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nrays == 0 || tree->n == 0) {
+        std::fill(offsets, offsets + nrays + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    Scratch scratch(ctx);
+    void* d_rays = nullptr;
+    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
+    return csr4_host<RayProbe4<T>>(tree, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, offsets, hits, cap, total, "traverse");
+}
+
+// ---- Aabb / Point / Ball queries: records of 8 / 4 / 5 T ----
+template <class T> static int query4_dev_impl(Tree4<T>* tree, int mode, int kind, const void* d_queries, size_t n, uint32_t* d_offsets,
+                                              uint32_t* d_hits, size_t cap, size_t* total) {
+    if (!tree || !d_offsets || (n && !d_queries)) { set_error("query_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    if (!public_query_kind(kind)) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_batch_args(tree, mode, n, "query_dev"));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    const int rc = kind == BVHGPU_QUERY_AABB  ? csr4_dev<QueryProbe4<T, BVHGPU_QUERY_AABB>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
+                 : kind == BVHGPU_QUERY_POINT ? csr4_dev<QueryProbe4<T, BVHGPU_QUERY_POINT>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
+                                              : csr4_dev<QueryProbe4<T, BVHGPU_QUERY_BALL>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev");
+    // as bvhgpu_query_dev_f32x3: with `total` given the call synchronises, and the CSR is complete when it returns
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
+    return rc;
+}
+template <class T> static int query4_host_impl(Tree4<T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits,
+                                               size_t cap, size_t* total) {
+    if (!tree || (n && !queries) || !offsets) { set_error("query: null argument"); return BVHGPU_ERR_INVALID; }
+    if (!public_query_kind(kind)) { set_error("query: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_batch_args(tree, mode, n, "query"));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0 || tree->n == 0) {
+        std::fill(offsets, offsets + n + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    Scratch scratch(ctx);
+    void* d_q = nullptr;
+    BVH_TRY(upload4(ctx, scratch, queries, sizeof(T) * query_stride4<T>(kind) * n, &d_q));
+    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    return kind == BVHGPU_QUERY_AABB  ? csr4_host<QueryProbe4<T, BVHGPU_QUERY_AABB>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
+         : kind == BVHGPU_QUERY_POINT ? csr4_host<QueryProbe4<T, BVHGPU_QUERY_POINT>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
+                                      : csr4_host<QueryProbe4<T, BVHGPU_QUERY_BALL>>(tree, flat, d_q, n, offsets, hits, cap, total, "query");
+}
+
+// ---- nearest_to: 4 T per point ----
+template <class T> static int nearest4_host_impl(Tree4<T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("nearest: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_batch_args(tree, mode, n, "nearest"));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return BVHGPU_OK;
+    if (tree->n == 0) {                                            // empty tree: None (bvh_impl.rs:229-231)
+        std::fill(out_shape, out_shape + n, BVH_INVALID);
+        std::fill(out_dist, out_dist + n, T(0));
+        return BVHGPU_OK;
+    }
+    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    if (flat) BVH_TRY(flatten4_impl(tree, nullptr, 0, nullptr));    // builds d_flat once
+    Scratch scratch(ctx);
+    void* d_p = nullptr;
+    uint32_t* d_s = nullptr;
+    T* d_d = nullptr;
+    BVH_TRY(upload4(ctx, scratch, points, sizeof(T) * 4 * n, &d_p));
+    BVH_TRY(scratch.get(&d_s, n));
+    BVH_TRY(scratch.get(&d_d, n));
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    if (flat) nearest4_kernel<T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->d_flat, (uint32_t)tree->n_flat, tree->d_aabb, (const T*)d_p, (uint32_t)n, d_s, d_d);
+    else      nearest4_kernel<T, false><<<grid, 128, 0, st>>>(tree->d_nodes, nullptr, 0u, tree->d_aabb, (const T*)d_p, (uint32_t)n, d_s, d_d);
+    LAUNCHED(ctx, 1);
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    return BVHGPU_OK;
+}
+// Candidate lists that contain the nearest shape of every point, for shapes with their own distance (bvh_b200.h): the bound walk,
+// then a QUERY_WITHIN pass over the records in FLAT semantics (leaves re-test the shape's own AABB).
+template <class T> static int nearest_candidates4_host_impl(Tree4<T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand,
+                                                            size_t cap, size_t* total) {
+    if (!tree || (n && !points) || !offsets) { set_error("nearest_candidates: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_batch_args(tree, BVHGPU_TRAVERSE_FLAT, n, "nearest_candidates"));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0 || tree->n == 0) {
+        std::fill(offsets, offsets + n + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    Scratch scratch(ctx);
+    void* d_p = nullptr;
+    T* rec = nullptr;
+    BVH_TRY(upload4(ctx, scratch, points, sizeof(T) * 4 * n, &d_p));
+    BVH_TRY(scratch.get(&rec, 5 * n));
+    nearest_bound4_kernel<T><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, (const T*)d_p, (uint32_t)n, rec);
+    LAUNCHED(ctx, 1);
+    return csr4_host<QueryProbe4<T, QUERY_WITHIN>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
 }
 
 }  // namespace bvhb200
@@ -926,6 +1090,21 @@ struct bvhgpu_tree4d : Tree4<double> {};
     BVH_EXPORT4 int bvhgpu_traverse_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, void* dev_offsets, \
                                               void* dev_hits, size_t cap, size_t* total) {                                \
         return traverse4_dev_impl<T>(tree, mode, dev_rays, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets,     \
+                                       uint32_t* hits, size_t cap, size_t* total) {                                       \
+        return query4_host_impl<T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                              \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_query_dev_##SUF(TREE* tree, int mode, int kind, const void* dev_queries, size_t n,             \
+                                           void* dev_offsets, void* dev_hits, size_t cap, size_t* total) {                \
+        return query4_dev_impl<T>(tree, mode, kind, dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
+        return nearest4_host_impl<T>(tree, mode, points, n, out_shape, out_dist);                                         \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
+                                                    size_t cap, size_t* total) {                                          \
+        return nearest_candidates4_host_impl<T>(tree, points, n, offsets, cand, cap, total);                              \
     }
 
 DEFINE_API4(float, f32x4, bvhgpu_tree4f, bvh_aabb4f, bvh_ray4f, bvh_node4f, bvh_flat4f)

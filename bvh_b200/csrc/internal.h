@@ -214,6 +214,8 @@ __global__ void __launch_bounds__(1024) scan_blocks_kernel(unsigned long long* _
 // ---- dim2.cu ----
 template <class T> int dim2_expand_aabbs(bvhgpu_ctx* ctx, const T* d_in4, uint32_t n, T* d_out6);
 template <class T> int dim2_expand_rays(bvhgpu_ctx* ctx, const T* d_in6, uint32_t n, T* d_out9);
+// n records of nvec 2-vectors and nscal scalars -> the same with every vector lifted to z = 0 (query records, nearest_to points)
+template <class T> int dim2_lift(bvhgpu_ctx* ctx, const T* d_in, uint32_t n, int nvec, int nscal, T* d_out);
 template <class T> int dim2_finish_build(Tree<T>* tree);
 template <class T, class N2> int dim2_nodes_out(Tree<T>* tree, N2* d_out);
 template <class T, class F2> int dim2_flat_out(Tree<T>* tree, F2* d_out);

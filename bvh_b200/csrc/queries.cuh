@@ -1,0 +1,177 @@
+// bvh_b200/csrc/queries.cuh -- the IntersectsAabb predicates other than Ray and the nearest_to walks, generic in the dimension D.
+// Shared by traverse.cu (D = 3, and D = 2 through the z = 0 embedding of dim2.cu) and dim4.cu (D = 4).  Every sum runs over the axes
+// left to right in T without FMA, so the instantiation for D = 3 performs exactly the operations the 3-D kernels always did.
+#pragma once
+#include "common.cuh"
+
+namespace bvhb200 {
+
+#ifdef __CUDACC__
+// ---- query records: Aabb {min, max} (2D T), Point (D T), Ball {center, radius} (D + 1 T) (src/aabb/intersection.rs:35-45,
+// src/ball.rs:85-106) ----
+template <class T, int KIND, int D> struct Query;
+template <class T, int D> struct Query<T, BVHGPU_QUERY_AABB, D> {
+    T mn[D], mx[D];
+    __device__ __forceinline__ void load(const T* p) { for (int k = 0; k < D; ++k) { mn[k] = __ldg(p + k); mx[k] = __ldg(p + D + k); } }
+    static constexpr int STRIDE = 2 * D;
+    __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {            // aabb_impl.rs:240-248
+        bool h = true;
+#pragma unroll
+        for (int i = 0; i < D; ++i) if (mx[i] < bmn[i] || bmx[i] < mn[i]) h = false;
+        return h;
+    }
+};
+template <class T, int D> struct Query<T, BVHGPU_QUERY_POINT, D> {
+    T p[D];
+    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < D; ++k) p[k] = __ldg(q + k); }
+    static constexpr int STRIDE = D;
+    __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {            // Aabb::contains, aabb_impl.rs:175-177
+        bool h = true;
+#pragma unroll
+        for (int i = 0; i < D; ++i) if (!(p[i] >= bmn[i]) || !(p[i] <= bmx[i])) h = false;
+        return h;
+    }
+};
+template <class T, int D> struct Query<T, BVHGPU_QUERY_BALL, D> {
+    T c[D], r2;
+    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < D; ++k) c[k] = __ldg(q + k); const T r = __ldg(q + D); r2 = mul_rn(r, r); }
+    static constexpr int STRIDE = D + 1;
+    __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {            // Ball::intersects_aabb, ball.rs:85-99
+        T d2 = T(0);
+#pragma unroll
+        for (int i = 0; i < D; ++i) {
+            T x = c[i];
+            if (x < bmn[i]) x = bmn[i];
+            if (x > bmx[i]) x = bmx[i];
+            const T d = sub_rn(x, c[i]);
+            d2 = add_rn(d2, mul_rn(d, d));
+        }
+        return d2 <= r2;
+    }
+};
+
+// Internal kind: every shape whose AABB lies within squared distance U of a point, record {p, U} (D + 1 T).  The lower bound
+// sum_k max(min_k - p_k, p_k - max_k, 0)^2 is monotone under box containment in floating point (subtraction, squaring
+// and addition of non-negative terms are monotone), so pruning an inner box can never lose a shape it contains.  An empty
+// child box (min > max on some axis: the Aabb::empty() a "no split wins" node stores where surface areas overflow) contains
+// nothing it bounds, so it is always entered.
+constexpr int QUERY_WITHIN = 4;
+template <int D, class T> __device__ __forceinline__ T box_lower_d2(const T p[D], const T bmn[D], const T bmx[D]) {
+    T d2 = T(0);
+#pragma unroll
+    for (int i = 0; i < D; ++i) {
+        const T a = sub_rn(bmn[i], p[i]), b = sub_rn(p[i], bmx[i]);
+        T d = a > b ? a : b;
+        d = d > T(0) ? d : T(0);
+        d2 = add_rn(d2, mul_rn(d, d));
+    }
+    return d2;
+}
+template <int D, class T> __device__ __forceinline__ T box_upper_d2(const T p[D], const T bmn[D], const T bmx[D]) {   // farthest corner
+    T d2 = T(0);
+#pragma unroll
+    for (int i = 0; i < D; ++i) {
+        const T a = fabs(sub_rn(p[i], bmn[i])), b = fabs(sub_rn(p[i], bmx[i]));
+        const T d = a > b ? a : b;
+        d2 = add_rn(d2, mul_rn(d, d));
+    }
+    return d2;
+}
+template <class T, int D> struct Query<T, QUERY_WITHIN, D> {
+    T p[D], u;
+    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < D; ++k) p[k] = __ldg(q + k); u = __ldg(q + D); }
+    static constexpr int STRIDE = D + 1;
+    __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {
+        bool empty = false;
+#pragma unroll
+        for (int i = 0; i < D; ++i) empty |= bmn[i] > bmx[i];
+        return empty || box_lower_d2<D>(p, bmn, bmx) <= u;
+    }
+};
+
+// Aabb::min_distance_squared (aabb_impl.rs:618-629): per axis max(|p - centre| - half_size, 0), then the dot product
+// ((o0*o0 + o1*o1) + o2*o2) [+ o3*o3].  An empty box (min = +inf, max = -inf) gives a NaN centre and o = 0 on that axis, as
+// NaN.max(0) = 0 in Rust.
+template <int D, class T> __device__ __forceinline__ T aabb_min_d2(const T p[D], const T mn[D], const T mx[D]) {
+    T o[D];
+#pragma unroll
+    for (int k = 0; k < D; ++k) {
+        const T hs = mul_rn(sub_rn(mx[k], mn[k]), T(0.5));             // half_size(), :479-481
+        const T c = add_rn(mn[k], hs);
+        const T q = sub_rn(fabs(sub_rn(p[k], c)), hs);
+        o[k] = q > T(0) ? q : T(0);
+    }
+    T acc = add_rn(mul_rn(o[0], o[0]), mul_rn(o[1], o[1]));
+#pragma unroll
+    for (int k = 2; k < D; ++k) acc = add_rn(acc, mul_rn(o[k], o[k]));
+    return acc;
+}
+__device__ __forceinline__ float sqrt_rn(float x) { return __fsqrt_rn(x); }
+__device__ __forceinline__ double sqrt_rn(double x) { return __dsqrt_rn(x); }
+
+// ---- nearest_to: Bvh::nearest_to (bvh_impl.rs:221-238, bvh_node.rs:327-372) over the reference node array ----
+// EXACT: reference semantics (children ordered by min_distance_squared, prune with `<`, first minimum kept).
+// !EXACT: children ordered and pruned by the monotone lower bound box_lower_d2, ties kept (`<=`).
+// leaf(shape) returns the leaf's value.  The recursion is a stackless walk over parent links: on the way back up the two child
+// distances are recomputed (same bits), so any tree depth works without a stack.  Node: a bvh_node{D}{f,d} POD.
+template <int D, class T, bool EXACT, class Node, class Leaf>
+__device__ __forceinline__ void nearest_walk(const Node* __restrict__ nodes, const T p[D], uint32_t& best, T& best_d, Leaf leaf) {
+    best = BVH_INVALID;
+    best_d = Traits<T>::inf();
+    uint32_t node = 0, from = BVH_INVALID;                 // from: the child we are returning from (BVH_INVALID = arriving from the parent)
+    for (;;) {
+        const uint4 meta = __ldg(reinterpret_cast<const uint4*>(nodes + node));      // parent, child_l, child_r, shape
+        if (meta.y == BVH_INVALID) {                       // leaf
+            const T d = leaf(meta.w);
+            if (best == BVH_INVALID || d < best_d) { best = meta.w; best_d = d; }
+            if (node == 0) return;
+            from = node; node = meta.x;
+            continue;
+        }
+        const Node& nd = nodes[node];
+        T lmn[D], lmx[D], rmn[D], rmx[D];
+#pragma unroll
+        for (int k = 0; k < D; ++k) { lmn[k] = __ldg(&nd.l_aabb.min[k]); lmx[k] = __ldg(&nd.l_aabb.max[k]); rmn[k] = __ldg(&nd.r_aabb.min[k]); rmx[k] = __ldg(&nd.r_aabb.max[k]); }
+        const T dl = EXACT ? aabb_min_d2<D>(p, lmn, lmx) : box_lower_d2<D>(p, lmn, lmx);
+        const T dr = EXACT ? aabb_min_d2<D>(p, rmn, rmx) : box_lower_d2<D>(p, rmn, rmx);
+        const bool swap = dl > dr;                          // bvh_node.rs:349-351
+        const uint32_t near_i = swap ? meta.z : meta.y, far_i = swap ? meta.y : meta.z;
+        const T near_d = swap ? dr : dl, far_d = swap ? dl : dr;
+        uint32_t next = BVH_INVALID;
+        if (from == BVH_INVALID) {                          // first visit: the nearer child, if it can still win
+            if (best == BVH_INVALID || (EXACT ? near_d < best_d : near_d <= best_d)) next = near_i;
+            else from = near_i;                             // skipped: as if we had just returned from it
+        }
+        if (next == BVH_INVALID && from == near_i) {        // back from (or past) the nearer child: now the farther one
+            if (best == BVH_INVALID || (EXACT ? far_d < best_d : far_d <= best_d)) next = far_i;
+            else from = far_i;
+        }
+        if (next != BVH_INVALID) { node = next; from = BVH_INVALID; continue; }
+        if (node == 0) return;                              // back from the farther child of the root
+        from = node; node = meta.x;
+    }
+}
+
+// FlatBvh::nearest_to (flat_bvh.rs:513-562) over the reference FlatNode array.  Flat: a bvh_flat{D}{f,d} POD.
+template <int D, class T, class Flat, class Leaf>
+__device__ __forceinline__ void nearest_flat(const Flat* __restrict__ flat, uint32_t n_flat, const T p[D], uint32_t& best, T& best_d, Leaf leaf) {
+    uint32_t index = 0;
+    while (index < n_flat) {                                // flat_bvh.rs:524-558
+        const Flat& f = flat[index];
+        const uint32_t entry = f.entry_index, exit_i = f.exit_index;
+        if (entry == BVH_INVALID) {
+            const uint32_t shape = f.shape_index;
+            const T d = leaf(shape);
+            if (best == BVH_INVALID || d < best_d) { best = shape; best_d = d; }
+            index = exit_i;
+        } else {
+            T mn[D], mx[D];
+            for (int k = 0; k < D; ++k) { mn[k] = f.aabb.min[k]; mx[k] = f.aabb.max[k]; }
+            const T md = aabb_min_d2<D>(p, mn, mx);
+            index = (best == BVH_INVALID || md < best_d) ? entry : exit_i;
+        }
+    }
+}
+#endif  // __CUDACC__
+
+}  // namespace bvhb200

@@ -12,6 +12,7 @@
 // them; an exclusive scan turns counts into offsets; the emit kernel copies the slots into place and
 // re-walks only rays with more than K hits.  K = 0 degenerates to the classic count / scan / fill.
 #include "internal.h"
+#include "queries.cuh"
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
@@ -1313,83 +1314,11 @@ template int traverse_host_pipelined<float>(Tree<float>*, int, const void*, uint
 template int traverse_host_pipelined<double>(Tree<double>*, int, const void*, uint32_t, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 
 // ---- the other IntersectsAabb implementors: Aabb, Point, Ball (src/aabb/intersection.rs:35-45, src/ball.rs:85-106) ----
-// Same stackless walk, another predicate.  Query records: Aabb {min,max} (6 T), Point (3 T), Ball {center, radius} (4 T).
-template <class T, int KIND> struct Query;
-template <class T> struct Query<T, BVHGPU_QUERY_AABB> {
-    T mn[3], mx[3];
-    __device__ __forceinline__ void load(const T* p) { for (int k = 0; k < 3; ++k) { mn[k] = __ldg(p + k); mx[k] = __ldg(p + 3 + k); } }
-    static constexpr int STRIDE = 6;
-    __device__ __forceinline__ bool hit(const T bmn[3], const T bmx[3]) const {            // aabb_impl.rs:240-248
-        bool h = true;
-#pragma unroll
-        for (int i = 0; i < 3; ++i) if (mx[i] < bmn[i] || bmx[i] < mn[i]) h = false;
-        return h;
-    }
-};
-template <class T> struct Query<T, BVHGPU_QUERY_POINT> {
-    T p[3];
-    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < 3; ++k) p[k] = __ldg(q + k); }
-    static constexpr int STRIDE = 3;
-    __device__ __forceinline__ bool hit(const T bmn[3], const T bmx[3]) const {            // Aabb::contains, aabb_impl.rs:175-177
-        bool h = true;
-#pragma unroll
-        for (int i = 0; i < 3; ++i) if (!(p[i] >= bmn[i]) || !(p[i] <= bmx[i])) h = false;
-        return h;
-    }
-};
-template <class T> struct Query<T, BVHGPU_QUERY_BALL> {
-    T c[3], r2;
-    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < 3; ++k) c[k] = __ldg(q + k); const T r = __ldg(q + 3); r2 = mul_rn(r, r); }
-    static constexpr int STRIDE = 4;
-    __device__ __forceinline__ bool hit(const T bmn[3], const T bmx[3]) const {            // Ball::intersects_aabb, ball.rs:85-99
-        T d2 = T(0);
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            T x = c[i];
-            if (x < bmn[i]) x = bmn[i];
-            if (x > bmx[i]) x = bmx[i];
-            const T d = sub_rn(x, c[i]);
-            d2 = add_rn(d2, mul_rn(d, d));
-        }
-        return d2 <= r2;
-    }
-};
-
-// Internal kind: every shape whose AABB lies within squared distance U of a point, record {p, U}.  The lower bound
-// sum_k max(min_k - p_k, p_k - max_k, 0)^2 is monotone under box containment in floating point (subtraction, squaring
-// and addition of non-negative terms are monotone), so pruning an inner box can never lose a shape it contains.
-constexpr int QUERY_WITHIN = 4;
-template <class T> __device__ __forceinline__ T box_lower_d2(const T p[3], const T bmn[3], const T bmx[3]) {
-    T d2 = T(0);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-        const T a = sub_rn(bmn[i], p[i]), b = sub_rn(p[i], bmx[i]);
-        T d = a > b ? a : b;
-        d = d > T(0) ? d : T(0);
-        d2 = add_rn(d2, mul_rn(d, d));
-    }
-    return d2;
-}
-template <class T> __device__ __forceinline__ T box_upper_d2(const T p[3], const T bmn[3], const T bmx[3]) {   // farthest corner
-    T d2 = T(0);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-        const T a = fabs(sub_rn(p[i], bmn[i])), b = fabs(sub_rn(p[i], bmx[i]));
-        const T d = a > b ? a : b;
-        d2 = add_rn(d2, mul_rn(d, d));
-    }
-    return d2;
-}
-template <class T> struct Query<T, QUERY_WITHIN> {
-    T p[3], u;
-    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < 3; ++k) p[k] = __ldg(q + k); u = __ldg(q + 3); }
-    static constexpr int STRIDE = 4;
-    __device__ __forceinline__ bool hit(const T bmn[3], const T bmx[3]) const { return box_lower_d2(p, bmn, bmx) <= u; }
-};
+// Same stackless walk, another predicate (queries.cuh).
 
 template <class T, int KIND, bool FLAT, class Emit>
 __device__ __forceinline__ void walk_query(const typename Traits<T>::TNode* __restrict__ trec, uint32_t n_rec,
-                                           const typename Traits<T>::DAabb* __restrict__ aabb, const Query<T, KIND>& q, Emit emit) {
+                                           const typename Traits<T>::DAabb* __restrict__ aabb, const Query<T, KIND, 3>& q, Emit emit) {
     uint32_t i = 0;
     while (i < n_rec) {
         T mn[3], mx[3];
@@ -1416,8 +1345,8 @@ __global__ void __launch_bounds__(256) query_kernel(const typename Traits<T>::TN
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (FILL && r == 0) { const unsigned long long t = *total; offsets[nq] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
     if (r >= nq) return;
-    Query<T, KIND> q;
-    q.load(queries + (size_t)r * Query<T, KIND>::STRIDE);
+    Query<T, KIND, 3> q;
+    q.load(queries + (size_t)r * Query<T, KIND, 3>::STRIDE);
     if (!FILL) {
         uint32_t cnt = 0;
         walk_query<T, KIND, FLAT>(trec, n_rec, aabb, q, [&](uint32_t) { ++cnt; });
@@ -1499,20 +1428,7 @@ template int query_device<double>(Tree<double>*, int, int, const double*, size_t
 //                           corner of the shape's AABB bounds the true nearest distance from above; the candidates
 //                           {s : lower(AABB_s) <= U} (QUERY_WITHIN) contain the nearest shape, and the caller evaluates its
 //                           own distance on that short list.
-template <class T> __device__ __forceinline__ T aabb_min_d2(const T p[3], const T mn[3], const T mx[3]) {     // aabb_impl.rs:618-629
-    T o[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const T hs = mul_rn(sub_rn(mx[k], mn[k]), T(0.5));             // half_size(), :479-481
-        const T c = add_rn(mn[k], hs);
-        const T q = sub_rn(fabs(sub_rn(p[k], c)), hs);
-        o[k] = q > T(0) ? q : T(0);
-    }
-    return add_rn(add_rn(mul_rn(o[0], o[0]), mul_rn(o[1], o[1])), mul_rn(o[2], o[2]));
-}
-__device__ __forceinline__ float sqrt_rn(float x) { return __fsqrt_rn(x); }
-__device__ __forceinline__ double sqrt_rn(double x) { return __dsqrt_rn(x); }
-
+// Both walks (nearest_walk, nearest_flat) are generic in the dimension and live in queries.cuh, shared with dim4.cu.
 // Triangle::distance_squared of the reference's test shape (src/testbase.rs:353-443: closest_point_segment, closest_point_triangle),
 // operation for operation -- the PointDistance every benchmark scene of the reference uses.  tri: {a.xyz,-, b.xyz,-, c.xyz,-}.
 template <class T> __device__ __forceinline__ T dot3_rn(const T a[3], const T b[3]) { return add_rn(add_rn(mul_rn(a[0], b[0]), mul_rn(a[1], b[1])), mul_rn(a[2], b[2])); }
@@ -1561,53 +1477,6 @@ template <class T> __device__ __forceinline__ T triangle_distance_squared(const 
     return dot3_rn(d, d);
 }
 
-// One walk for both kernels.  EXACT: reference semantics (order by min distance, prune with `<`, leaf value = AABB distance).
-// !EXACT: leaf value = farthest-corner bound, children ordered and pruned by the monotone lower bound, ties kept (`<=`).
-// tris != nullptr (EXACT only): the leaf value is the triangle's own distance (Triangle::distance_squared).
-template <class T, bool EXACT>
-__device__ __forceinline__ void nearest_walk(const typename Traits<T>::Node* __restrict__ nodes, const typename Traits<T>::DAabb* __restrict__ aabb,
-                                             const T p[3], uint32_t& best, T& best_d, const T* __restrict__ tris = nullptr) {
-    best = BVH_INVALID;
-    best_d = Traits<T>::inf();
-    uint32_t node = 0, from = BVH_INVALID;                 // from: the child we are returning from (BVH_INVALID = arriving from the parent)
-    for (;;) {
-        const uint4 meta = __ldg(reinterpret_cast<const uint4*>(nodes + node));      // parent, child_l, child_r, shape
-        if (meta.y == BVH_INVALID) {                       // leaf
-            T d;
-            if (EXACT && tris) d = triangle_distance_squared(p, tris + 12 * (size_t)meta.w);
-            else {
-                T mn[3], mx[3];
-                load_aabb(aabb + meta.w, mn, mx);
-                d = EXACT ? aabb_min_d2(p, mn, mx) : box_upper_d2(p, mn, mx);
-            }
-            if (best == BVH_INVALID || d < best_d) { best = meta.w; best_d = d; }
-            if (node == 0) return;
-            from = node; node = meta.x;
-            continue;
-        }
-        const typename Traits<T>::Node& nd = nodes[node];
-        T lmn[3], lmx[3], rmn[3], rmx[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { lmn[k] = __ldg(&nd.l_aabb.min[k]); lmx[k] = __ldg(&nd.l_aabb.max[k]); rmn[k] = __ldg(&nd.r_aabb.min[k]); rmx[k] = __ldg(&nd.r_aabb.max[k]); }
-        const T dl = EXACT ? aabb_min_d2(p, lmn, lmx) : box_lower_d2(p, lmn, lmx);
-        const T dr = EXACT ? aabb_min_d2(p, rmn, rmx) : box_lower_d2(p, rmn, rmx);
-        const bool swap = dl > dr;                          // bvh_node.rs:349-351
-        const uint32_t near_i = swap ? meta.z : meta.y, far_i = swap ? meta.y : meta.z;
-        const T near_d = swap ? dr : dl, far_d = swap ? dl : dr;
-        uint32_t next = BVH_INVALID;
-        if (from == BVH_INVALID) {                          // first visit: the nearer child, if it can still win
-            if (best == BVH_INVALID || (EXACT ? near_d < best_d : near_d <= best_d)) next = near_i;
-            else from = near_i;                             // skipped: as if we had just returned from it
-        }
-        if (next == BVH_INVALID && from == near_i) {        // back from (or past) the nearer child: now the farther one
-            if (best == BVH_INVALID || (EXACT ? far_d < best_d : far_d <= best_d)) next = far_i;
-            else from = far_i;
-        }
-        if (next != BVH_INVALID) { node = next; from = BVH_INVALID; continue; }
-        if (node == 0) return;                              // back from the farther child of the root
-        from = node; node = meta.x;
-    }
-}
 template <class T, bool FLAT>
 __global__ void __launch_bounds__(128) nearest_kernel(const typename Traits<T>::Node* __restrict__ nodes, const typename Traits<T>::Flat* __restrict__ flat,
                                                       uint32_t n_flat, const typename Traits<T>::DAabb* __restrict__ aabb,
@@ -1619,29 +1488,14 @@ __global__ void __launch_bounds__(128) nearest_kernel(const typename Traits<T>::
     for (int k = 0; k < 3; ++k) p[k] = points[3 * (size_t)i + k];
     uint32_t best = BVH_INVALID;
     T best_d = T(0);
-    if (!FLAT) {
-        nearest_walk<T, true>(nodes, aabb, p, best, best_d, tris);
-    } else {                                                // flat_bvh.rs:524-558
-        uint32_t index = 0;
-        while (index < n_flat) {
-            const typename Traits<T>::Flat& f = flat[index];
-            const uint32_t entry = f.entry_index, exit_i = f.exit_index;
-            if (entry == BVH_INVALID) {
-                T mn[3], mx[3];
-                const uint32_t shape = f.shape_index;
-                T d;
-                if (tris) d = triangle_distance_squared(p, tris + 12 * (size_t)shape);
-                else { load_aabb(aabb + shape, mn, mx); d = aabb_min_d2(p, mn, mx); }
-                if (best == BVH_INVALID || d < best_d) { best = shape; best_d = d; }
-                index = exit_i;
-            } else {
-                T mn[3], mx[3];
-                for (int k = 0; k < 3; ++k) { mn[k] = f.aabb.min[k]; mx[k] = f.aabb.max[k]; }
-                const T md = aabb_min_d2(p, mn, mx);
-                index = (best == BVH_INVALID || md < best_d) ? entry : exit_i;
-            }
-        }
-    }
+    auto leaf = [&](uint32_t shape) -> T {                  // tris != nullptr: the triangle's own distance (Triangle::distance_squared)
+        if (tris) return triangle_distance_squared(p, tris + 12 * (size_t)shape);
+        T mn[3], mx[3];
+        load_aabb(aabb + shape, mn, mx);
+        return aabb_min_d2<3>(p, mn, mx);
+    };
+    if (!FLAT) nearest_walk<3, T, true>(nodes, p, best, best_d, leaf);
+    else       nearest_flat<3, T>(flat, n_flat, p, best, best_d, leaf);
     out_shape[i] = best;
     out_dist[i] = sqrt_rn(best_d);                          // bvh_impl.rs:237
 }
@@ -1654,7 +1508,7 @@ __global__ void __launch_bounds__(128) nearest_bound_kernel(const typename Trait
     for (int k = 0; k < 3; ++k) p[k] = points[3 * (size_t)i + k];
     uint32_t best;
     T u;
-    nearest_walk<T, false>(nodes, aabb, p, best, u);
+    nearest_walk<3, T, false>(nodes, p, best, u, [&](uint32_t shape) { T mn[3], mx[3]; load_aabb(aabb + shape, mn, mx); return box_upper_d2<3>(p, mn, mx); });
     u = mul_rn(u, add_rn(T(1), mul_rn(T(16), Traits<T>::eps())));      // the bound itself is a rounded sum: keep it an upper bound
     for (int k = 0; k < 3; ++k) records[4 * (size_t)i + k] = p[k];
     records[4 * (size_t)i + 3] = u;

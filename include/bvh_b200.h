@@ -196,6 +196,23 @@ int bvhgpu_traverse_f32x2(bvhgpu_tree2f* tree, int mode, const bvh_ray2f* rays, 
                           uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
 int bvhgpu_traverse_f64x2(bvhgpu_tree2d* tree, int mode, const bvh_ray2d* rays, size_t nrays,
                           uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+/* D = 2 queries and nearest_to: the semantics of bvhgpu_query_f32x3 / bvhgpu_nearest_f32x3 / bvhgpu_nearest_candidates_f32x3 below
+ * (section "the other IntersectsAabb implementors" and section "nearest_to") with 2 components, host pointers.  Query records:
+ * Aabb {min, max} = 4 T, Point = 2 T, Ball {center, radius} = 3 T; nearest points: 2 T.  The records are lifted to z = 0 and run
+ * through the 3-D kernels on the embedded tree; every z term is exactly neutral, so the results are the 2-D ones bit for bit (dim2.cu).
+ * `kind` outside 1..3, a bad mode, a null argument or n > 2^31-1: BVHGPU_ERR_INVALID, nothing is read or written.  There is no fetch
+ * call: when the hits (candidates) do not fit `cap`, offsets and *total are valid and the call returns BVHGPU_ERR_CAPACITY; call
+ * again with cap = *total. */
+int bvhgpu_query_f32x2(bvhgpu_tree2f* tree, int mode, int kind, const float* queries, size_t n,
+                       uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_query_f64x2(bvhgpu_tree2d* tree, int mode, int kind, const double* queries, size_t n,
+                       uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_nearest_f32x2(bvhgpu_tree2f* tree, int mode, const float* points, size_t n, uint32_t* out_shape, float* out_dist);
+int bvhgpu_nearest_f64x2(bvhgpu_tree2d* tree, int mode, const double* points, size_t n, uint32_t* out_shape, double* out_dist);
+int bvhgpu_nearest_candidates_f32x2(bvhgpu_tree2f* tree, const float* points, size_t n, uint32_t* offsets, uint32_t* cand,
+                                    size_t cap, size_t* total);
+int bvhgpu_nearest_candidates_f64x2(bvhgpu_tree2d* tree, const double* points, size_t n, uint32_t* offsets, uint32_t* cand,
+                                    size_t cap, size_t* total);
 
 /* ---- D = 4: Bvh<T,4>::build / nodes / flatten / traverse (the reference is generic in D, src/bvh/bvh_node.rs:81-279,
  * src/flat_bvh.rs:60-143, 396-431; 4-wide slab tests src/ray/intersect_simd.rs; generic slab test src/ray/intersect_default.rs:16-37).
@@ -227,6 +244,28 @@ int bvhgpu_traverse_dev_f32x4(bvhgpu_tree4f* tree, int mode, const void* dev_ray
                               void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 int bvhgpu_traverse_dev_f64x4(bvhgpu_tree4d* tree, int mode, const void* dev_rays, size_t nrays,
                               void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+/* D = 4 queries and nearest_to: the semantics of the 3-D functions (section "the other IntersectsAabb implementors" and section
+ * "nearest_to") with 4 components, run by dim4.cu's own kernels.  Query records: Aabb {min, max} = 8 T, Point = 4 T,
+ * Ball {center, radius} = 5 T; nearest points: 4 T.  `kind` outside 1..3, a bad mode, a null argument or n > 2^31-1:
+ * BVHGPU_ERR_INVALID, nothing is read or written.  An empty tree gives all-zero offsets; nearest gives BVHGPU_INVALID_INDEX and
+ * distance 0.  Host forms: no fetch call; when the hits (candidates) do not fit `cap`, offsets and *total are valid and the call
+ * returns BVHGPU_ERR_CAPACITY; call again with cap = *total.  query_dev: device pointers, enqueued on the context's stream, the
+ * contract of bvhgpu_query_dev_f32x3 (offsets always complete, hits[0 .. cap) a prefix of the full list, `total` may be NULL: then
+ * there is no host synchronisation). */
+int bvhgpu_query_f32x4(bvhgpu_tree4f* tree, int mode, int kind, const float* queries, size_t n,
+                       uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_query_f64x4(bvhgpu_tree4d* tree, int mode, int kind, const double* queries, size_t n,
+                       uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_query_dev_f32x4(bvhgpu_tree4f* tree, int mode, int kind, const void* dev_queries, size_t n,
+                           void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_query_dev_f64x4(bvhgpu_tree4d* tree, int mode, int kind, const void* dev_queries, size_t n,
+                           void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_nearest_f32x4(bvhgpu_tree4f* tree, int mode, const float* points, size_t n, uint32_t* out_shape, float* out_dist);
+int bvhgpu_nearest_f64x4(bvhgpu_tree4d* tree, int mode, const double* points, size_t n, uint32_t* out_shape, double* out_dist);
+int bvhgpu_nearest_candidates_f32x4(bvhgpu_tree4f* tree, const float* points, size_t n, uint32_t* offsets, uint32_t* cand,
+                                    size_t cap, size_t* total);
+int bvhgpu_nearest_candidates_f64x4(bvhgpu_tree4d* tree, const double* points, size_t n, uint32_t* offsets, uint32_t* cand,
+                                    size_t cap, size_t* total);
 
 /* ---- flatten: replaces Bvh::flatten (src/flat_bvh.rs:60-143, 240-251, 312-319) -----
  * Writes the FlatBvh (3n-2 FlatNodes for n >= 2, 1 for n == 1, 0 for n == 0) into `out`
@@ -378,7 +417,8 @@ int bvhgpu_closest_hit_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_rays, int 
  *   bvhgpu_nearest_candidates_* for ANY shape contained in its AABB: CSR lists that are guaranteed to contain the nearest shape
  *                               of every point (all shapes whose AABB is at most as far as the smallest farthest-corner
  *                               distance of any shape's AABB); the shim evaluates distance_squared on that short list and
- *                               keeps the minimum. */
+ *                               keeps the minimum.  Below an empty child box ("no split wins" nodes, where surface areas
+ *                               overflow) the box bounds nothing, so every shape under it is listed. */
 int bvhgpu_nearest_f32x3(bvhgpu_tree3f* tree, int mode, const float* points, size_t n, uint32_t* out_shape, float* out_dist);
 int bvhgpu_nearest_f64x3(bvhgpu_tree3d* tree, int mode, const double* points, size_t n, uint32_t* out_shape, double* out_dist);
 /* The same walk with the TRIANGLE's own distance at the leaves -- Triangle::distance_squared of the reference's test shape
