@@ -565,11 +565,27 @@ class Bvh2:
                 best = (shapes[int(s)], d)
         return None if best is None else (best[0], float(np.sqrt(best[1])))
 
+    def refit(self, aabbs):
+        """Bvh::update_shapes' refit (fix_aabbs_ascending) for all shapes: `aabbs` = the new boxes of every shape.  Topology is kept."""
+        a = np.ascontiguousarray(aabbs, dtype=self._d["aabb"])
+        capi.check(getattr(capi.lib(), f"bvhgpu_refit_{self._d['suffix']}")(self._h, _ptr(a), len(a)))
+
+    def update_shapes(self, changed, aabbs, max_growth: float = 1.5) -> int:
+        """Bvh::update_shapes(changed_shape_indices, shapes): only the changed shapes' boxes are sent.  `aabbs` = the boxes of all
+        shapes (an AABB array); max_growth >= 1: degraded subtrees are rebuilt, <= 0: boxes only.  Returns the number of shapes in
+        rebuilt subtrees; node indices must be re-read (nodes_and_index) when it is non-zero."""
+        idx = np.ascontiguousarray(changed, dtype=np.uint32).reshape(-1)
+        fresh = np.ascontiguousarray(np.asarray(aabbs)[idx], dtype=self._d["aabb"])
+        rebuilt = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_update_{self._d['suffix']}")(self._h, _ptr(idx), _ptr(fresh), len(idx), C.c_double(max_growth),
+                                                                            C.byref(rebuilt)))
+        return int(rebuilt.value)
+
 
 class Bvh4(Bvh2):
     """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten, batched
     ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction), and the queries and nearest_to
-    of Bvh2 with 4 components, plus query_dev."""
+    of Bvh2 with 4 components (refit and update_shapes included), plus query_dev, refit_dev and update_dev."""
 
     _TABLE = BY_PREC_4D
     _DIM = 4
@@ -593,3 +609,15 @@ class Bvh4(Bvh2):
         capi.check(fn(self._h, mode, kind, C.c_void_p(queries_ptr), n, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
                       C.byref(total) if want_total else None))
         return total.value if want_total else None
+
+    def refit_dev(self, aabbs_ptr: int, n: int):
+        """refit from the new boxes of all n shapes on the device (C-ABI layout), enqueued on the context's stream."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_refit_dev_{self._d['suffix']}")(self._h, C.c_void_p(aabbs_ptr), n))
+
+    def update_dev(self, changed_ptr: int, aabbs_ptr: int, m: int, max_growth: float = 1.5, want_rebuilt: bool = True):
+        """update_shapes from device pointers: m u32 shape indices and their m new boxes (C-ABI layout), on the context's stream.
+        Returns the number of shapes in rebuilt subtrees (None with want_rebuilt = False)."""
+        rebuilt = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_update_dev_{self._d['suffix']}")(self._h, C.c_void_p(changed_ptr), C.c_void_p(aabbs_ptr), m,
+                                                                                C.c_double(max_growth), C.byref(rebuilt) if want_rebuilt else None))
+        return int(rebuilt.value) if want_rebuilt else None

@@ -134,7 +134,13 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_query_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_nearest_{s}").argtypes = [vp, i32, vp, sz, vp, vp]
         getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
+        getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
     for s in ("f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
+        getattr(L, f"bvhgpu_refit_dev_{s}").argtypes = [vp, vp, sz]
+        getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
+        getattr(L, f"bvhgpu_update_dev_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
         getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
         getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]
         getattr(L, f"bvhgpu_tree_free_{s}").restype = None

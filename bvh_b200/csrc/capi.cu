@@ -452,6 +452,7 @@ static int refit_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size
     BVH_TRY(resolve_status(tree));
     if (n == 0) return BVHGPU_OK;
     BVH_TRY(stage_new_aabbs<T>(tree, aabbs, n, dev_input, "refit"));
+    if (tree->dims == 2) BVH_TRY(dim2_finish_build<T>(tree));          // the FLAT leaf boxes follow d_aabb before the records are rebuilt
     BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
     BVH_TRY(refit(tree));
     tree->status_pending = true;
@@ -610,6 +611,7 @@ static int update_impl(Tree<T>* tree, const uint32_t* changed, const typename Tr
     if (h[1]) { set_error("update: a changed shape index is >= %u; the tree was left unchanged", tree->n); return BVHGPU_ERR_INVALID; }
     if (h[0]) { set_error("update: NaN coordinate in a new AABB; the tree was left unchanged"); return BVHGPU_ERR_NAN; }
     BVH_TRY(update_scatter<T>(tree, d_changed, d_fresh, (uint32_t)m));
+    if (tree->dims == 2) BVH_TRY(dim2_finish_build<T>(tree));          // the FLAT leaf boxes follow d_aabb before the records are rebuilt
     BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
     BVH_TRY(update_incremental<T>(tree, d_changed, (uint32_t)m, max_growth));      // touches the root paths of the changed leaves only
     tree->status_pending = true;
@@ -618,6 +620,56 @@ static int update_impl(Tree<T>* tree, const uint32_t* changed, const typename Tr
     BVH_CUDA_TRY(cudaMemcpyAsync(&hs, tree->d_status, sizeof(hs), cudaMemcpyDeviceToHost, ctx->stream));
     BVH_TRY(resolve_status(tree));
     if (rebuilt) *rebuilt = hs.rebuilt;
+    return BVHGPU_OK;
+}
+
+// D = 2 refit / update_shapes: the 2-D boxes are lifted to z = [0, 0] on the device and run through refit_impl / update_impl above.
+// Surface areas with z = [0, 0] are exact and largest_axis never picks z (dim2.cu), so the 3-D refit, growth test and rebuild are the
+// 2-D ones.  Host pointers; synchronous.
+template <class T, class AABB2>
+static int lift2_aabbs(Tree<T>* tree, Scratch& scratch, const AABB2* aabbs, size_t n, const typename Traits<T>::Aabb** d_out) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    T *in4 = nullptr, *in6 = nullptr;
+    BVH_TRY(scratch.get(&in4, 4 * n));
+    BVH_TRY(scratch.get(&in6, 6 * n));
+    BVH_CUDA_TRY(cudaMemcpyAsync(in4, aabbs, sizeof(AABB2) * n, cudaMemcpyHostToDevice, ctx->stream));
+    BVH_TRY(dim2_expand_aabbs<T>(ctx, in4, (uint32_t)n, in6));
+    *d_out = reinterpret_cast<const typename Traits<T>::Aabb*>(in6);
+    return BVHGPU_OK;
+}
+template <class T, class AABB2>
+static int refit2_impl(Tree<T>* tree, const AABB2* aabbs, size_t n) {
+    if (!tree || (n && !aabbs)) { set_error("refit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (n != tree->n) { set_error("refit: %zu AABBs for a tree over %u shapes", n, tree->n); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const typename Traits<T>::Aabb* d6 = nullptr;
+    BVH_TRY((lift2_aabbs<T, AABB2>(tree, scratch, aabbs, n, &d6)));
+    BVH_TRY(refit_impl<T>(tree, d6, n, true));
+    return resolve_status(tree);
+}
+template <class T, class AABB2>
+static int update2_impl(Tree<T>* tree, const uint32_t* changed, const AABB2* fresh, size_t m, double max_growth, size_t* rebuilt) {
+    if (!tree || (m && (!changed || !fresh))) { set_error("update: null argument"); return BVHGPU_ERR_INVALID; }
+    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("update: max_growth = %g, must be >= 1 (or <= 0 for a pure refit)", max_growth); return BVHGPU_ERR_INVALID; }
+    if (m > 0xFFFFFFFFull) { set_error("update: too many changed shapes"); return BVHGPU_ERR_INVALID; }
+    if (rebuilt) *rebuilt = 0;
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (m == 0 || tree->n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    uint32_t* d_changed = nullptr;
+    BVH_TRY(scratch.get(&d_changed, m));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_changed, changed, sizeof(uint32_t) * m, cudaMemcpyHostToDevice, ctx->stream));
+    const typename Traits<T>::Aabb* d6 = nullptr;
+    BVH_TRY((lift2_aabbs<T, AABB2>(tree, scratch, fresh, m, &d6)));
+    size_t r = 0;
+    BVH_TRY(update_impl<T>(tree, d_changed, d6, m, max_growth, &r, true));   // with `rebuilt` given, the call synchronises
+    if (rebuilt) *rebuilt = r;
     return BVHGPU_OK;
 }
 
@@ -1133,6 +1185,11 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                    size_t cap, size_t* total) {                                            \
         return nearest_candidates_host_impl<T, 2>(tree, points, n, offsets, cand, cap, total);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit2_impl<T, AABB>(tree, aabbs, n); } \
+    BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, \
+                                       size_t* rebuilt) {                                                                  \
+        return update2_impl<T, AABB>(tree, changed, changed_aabbs, m, max_growth, rebuilt);                                \
     }
 
 DEFINE_API2(float, f32x2, bvhgpu_tree2f, bvh_aabb2f, bvh_ray2f, bvh_node2f, bvh_flat2f)

@@ -17,6 +17,7 @@
 // order in which warps run never shows in the result: two builds of the same input are byte-identical.
 #include "internal.h"
 #include "queries.cuh"
+#include "update.cuh"
 #include <algorithm>
 #include <new>
 
@@ -51,12 +52,15 @@ template <class T> struct Tree4 {
     std::string failed_message;
     uint32_t* d_offsets = nullptr; size_t offsets_cap = 0;   // result buffers of the host-pointer traversal
     uint32_t* d_hits = nullptr;    size_t hits_cap = 0;
+    T* d_sa_base = nullptr;            // [2n-1] surface area of every inner node when it was last (re)built: baseline of update (first update)
+    uint32_t* d_arrive = nullptr;      // [2n-1] arrival counters of the incremental update (all zero between calls)
+    uint8_t* d_bad = nullptr;          // [2n-1] growth flags of the incremental update (all zero between calls)
 };
 
 constexpr uint32_t SMALL4 = 256;     // ranges this small are finished by one warp (depth-first, shared-memory stack)
 constexpr uint32_t TILE4 = 512;      // shapes per warp tile of a large range
 constexpr int STACK4 = 12;           // > log2(SMALL4) + 1: the smaller-child-first order bounds the stack
-constexpr uint32_t CTL_NEXT = 0, CTL_SMALL = 1, CTL_ERROR = 2, CTL_NAN = 3;
+constexpr uint32_t CTL_NEXT = 0, CTL_SMALL = 1, CTL_ERROR = 2, CTL_NAN = 3, CTL_REBUILT = 4;
 
 template <class T> struct __align__(16) Task4 {
     uint32_t start, count, node, parent;
@@ -68,24 +72,6 @@ template <class T> struct __align__(16) Task4 {
 // key slot k of a bucket: 0..3 box min, 4..7 box max, 8..11 centre min, 12..15 centre max
 __device__ __forceinline__ bool kmin4(int k) { return ((k >> 2) & 1) == 0; }
 template <class Key> __device__ __forceinline__ Key fold_key(int k, Key acc, Key v) { return kmin4(k) ? (v < acc ? v : acc) : (v > acc ? v : acc); }
-
-__device__ __forceinline__ void load4(const bvh_aabb4f* p, float mn[4], float mx[4]) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
-    mn[0] = a.x; mn[1] = a.y; mn[2] = a.z; mn[3] = a.w; mx[0] = b.x; mx[1] = b.y; mx[2] = b.z; mx[3] = b.w;
-}
-__device__ __forceinline__ void load4(const bvh_aabb4d* p, double mn[4], double mx[4]) {
-    const double2* q = reinterpret_cast<const double2*>(p);
-    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);
-    mn[0] = a.x; mn[1] = a.y; mn[2] = b.x; mn[3] = b.y; mx[0] = c.x; mx[1] = c.y; mx[2] = d.x; mx[3] = d.y;
-}
-
-// Aabb::surface_area for D = 4: 2 * (((sx*sx + sy*sy) + sz*sz) + sw*sw), left to right, no FMA.
-template <class T> __device__ __forceinline__ T surface_area4(const T mn[4], const T mx[4]) {
-    T acc = add_rn(mul_rn(sub_rn(mx[0], mn[0]), sub_rn(mx[0], mn[0])), mul_rn(sub_rn(mx[1], mn[1]), sub_rn(mx[1], mn[1])));
-    acc = add_rn(acc, mul_rn(sub_rn(mx[2], mn[2]), sub_rn(mx[2], mn[2])));
-    acc = add_rn(acc, mul_rn(sub_rn(mx[3], mn[3]), sub_rn(mx[3], mn[3])));
-    return mul_rn(T(2), acc);
-}
 
 // How a range is split: largest_axis (first strict maximum) of the centroid extent, halving below T::EPSILON (bvh_node.rs:114-124).
 template <class T> struct Plan4 { int axis; T cmin, ext; bool halve; uint32_t half; };
@@ -294,18 +280,15 @@ template <class T> __global__ void root_task4_kernel(const typename Traits<T>::K
     *dst = t;
 }
 
-// ---- large ranges, one level ----
-// prep: first tile of every range (exclusive scan of ceil(count / TILE4)), total in tile0[m]; bucket identities; next-level counter.
-template <class T>
-__global__ void __launch_bounds__(1024) level_prep4_kernel(const Task4<T>* __restrict__ tasks, uint32_t m, uint32_t* __restrict__ tile0,
-                                                           typename Traits<T>::Key* __restrict__ acc, uint32_t* __restrict__ acnt, uint32_t* __restrict__ ctl) {
+// One block of 1024 threads: tile0[j] = first tile of item j (exclusive scan of tiles(j) over j < m), total in tile0[m].
+template <class F> __device__ __forceinline__ void tile_scan1024(uint32_t m, F tiles, uint32_t* __restrict__ tile0) {
     __shared__ uint32_t wsum[32];
     __shared__ uint32_t carry;
-    if (threadIdx.x == 0) { carry = 0; ctl[CTL_NEXT] = 0; }
+    if (threadIdx.x == 0) carry = 0;
     __syncthreads();
     for (uint32_t j0 = 0; j0 < m; j0 += 1024) {
         const uint32_t j = j0 + threadIdx.x;
-        const uint32_t v = j < m ? (tasks[j].count + TILE4 - 1) / TILE4 : 0u;
+        const uint32_t v = j < m ? tiles(j) : 0u;
         uint32_t incl = v;
         for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
         if (lane_id() == 31) wsum[threadIdx.x >> 5] = incl;
@@ -319,6 +302,15 @@ __global__ void __launch_bounds__(1024) level_prep4_kernel(const Task4<T>* __res
         __syncthreads();
     }
     if (threadIdx.x == 0) tile0[m] = carry;
+}
+
+// ---- large ranges, one level ----
+// prep: first tile of every range (exclusive scan of ceil(count / TILE4)), total in tile0[m]; bucket identities; next-level counter.
+template <class T>
+__global__ void __launch_bounds__(1024) level_prep4_kernel(const Task4<T>* __restrict__ tasks, uint32_t m, uint32_t* __restrict__ tile0,
+                                                           typename Traits<T>::Key* __restrict__ acc, uint32_t* __restrict__ acnt, uint32_t* __restrict__ ctl) {
+    if (threadIdx.x == 0) ctl[CTL_NEXT] = 0;
+    tile_scan1024(m, [&](uint32_t j) { return (tasks[j].count + TILE4 - 1) / TILE4; }, tile0);
     for (uint32_t j = threadIdx.x; j < 96 * m; j += 1024) acc[j] = kmin4((int)(j & 15)) ? Traits<T>::KEY_POS_INF : Traits<T>::KEY_NEG_INF;
     for (uint32_t j = threadIdx.x; j < 6 * m; j += 1024) acnt[j] = 0;
 }
@@ -669,6 +661,139 @@ __global__ void __launch_bounds__(128) nearest_bound4_kernel(const typename D4<T
     records[5 * (size_t)i + 4] = u;
 }
 
+// ---- refit and update_shapes (Bvh::update_shapes, src/bvh/optimization.rs:304-351; DESIGN.md section 4.12) ----
+// refit: one thread per shape climbs from its leaf and writes its box into the parent's child slot; the second thread to reach a node
+// joins the two slots and carries on (flatten.cu: refit_kernel).  Topology, node_index and node_start are kept; leaves keep their
+// Aabb::empty() child boxes.
+template <class T>
+__global__ void __launch_bounds__(256) refit4_kernel(typename D4<T>::Node* nodes, const uint32_t* __restrict__ node_index,
+                                                     const typename D4<T>::Aabb* __restrict__ aabb, uint32_t n, uint32_t* arrivals) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    T mn[4], mx[4];
+    load4(aabb + s, mn, mx);
+    uint32_t node = node_index[s];
+    while (node != 0) {
+        const uint32_t p = __ldcg(&nodes[node].parent);
+        typename D4<T>::Node* pn = nodes + p;
+        const bool is_left = __ldcg(&pn->child_l) == node;
+        auto* dst = is_left ? &pn->l_aabb : &pn->r_aabb;
+        for (int k = 0; k < 4; ++k) { __stcg(&dst->min[k], mn[k]); __stcg(&dst->max[k], mx[k]); }
+        __threadfence();
+        if (atomicAdd(arrivals + p, 1u) == 0u) return;      // sibling subtree not finished yet
+        __threadfence();
+        const auto* sib = is_left ? &pn->r_aabb : &pn->l_aabb;
+        for (int k = 0; k < 4; ++k) { mn[k] = min_t(__ldcg(&sib->min[k]), mn[k]); mx[k] = max_t(__ldcg(&sib->max[k]), mx[k]); }
+        node = p;
+    }
+}
+// New boxes, checked before anything is written: flags[0] NaN, flags[1] an index >= n (changed == nullptr: box i belongs to shape i).
+template <class T>
+__global__ void __launch_bounds__(256) check4_kernel(const uint32_t* __restrict__ changed, const typename D4<T>::Aabb* __restrict__ fresh,
+                                                     uint32_t m, uint32_t n, uint32_t* __restrict__ flags) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    if (changed && changed[i] >= n) atomicExch(flags + 1, 1u);
+    const T* p = reinterpret_cast<const T*>(fresh + i);
+    bool nan = false;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) nan |= p[c] != p[c];
+    if (nan) atomicExch(flags, 1u);
+}
+template <class T>
+__global__ void __launch_bounds__(256) put4_kernel(const uint32_t* __restrict__ changed, const typename D4<T>::Aabb* __restrict__ fresh, uint32_t m,
+                                                   typename D4<T>::Aabb* __restrict__ aabb) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < m) aabb[changed[i]] = fresh[i];                  // an index listed twice: one of its boxes wins
+}
+
+// Seeding the builder from the rebuild roots roots[0 .. *n_roots) (disjoint inner nodes).  The subtree of root r with c shapes is the
+// node range [r, r + 2c - 1) over the leaf positions [node_start[r], node_start[r] + c).  Its nodes are cut into tiles of TILE4, so
+// that a root that holds every shape (global motion) is reduced by many warps, as level_bin4 does.
+// prep (one block): first tile of every root, total in tile0[nr]; centre-bound keys (min xyzw, max xyzw per root) at their identities.
+template <class T>
+__global__ void __launch_bounds__(1024) root_tiles4_kernel(const typename D4<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ roots,
+                                                           const uint32_t* __restrict__ n_roots, uint32_t* __restrict__ tile0,
+                                                           typename Traits<T>::Key* __restrict__ keys) {
+    const uint32_t nr = *n_roots;
+    tile_scan1024(nr, [&](uint32_t j) { return (2 * nodes[roots[j]].shape - 1 + TILE4 - 1) / TILE4; }, tile0);
+    for (uint32_t j = threadIdx.x; j < 8 * nr; j += 1024) keys[j] = (j & 7) < 4 ? Traits<T>::KEY_POS_INF : Traits<T>::KEY_NEG_INF;
+}
+// bin (one warp per tile): every leaf of the tile puts its shape at its leaf position of index buffer 0 and folds its centre into the
+// root's keys
+template <class T>
+__global__ void __launch_bounds__(256) root_bin4_kernel(const typename D4<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ node_start,
+                                                        const typename D4<T>::Aabb* __restrict__ aabb, const uint32_t* __restrict__ roots,
+                                                        const uint32_t* __restrict__ n_roots, const uint32_t* __restrict__ tile0, uint32_t* __restrict__ idx0,
+                                                        typename Traits<T>::Key* __restrict__ keys) {
+    const uint32_t nr = *n_roots;
+    if (nr == 0) return;
+    const uint32_t ntiles = tile0[nr];
+    for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < ntiles; t += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t j = tile_owner(tile0, nr, t), r = roots[j];
+        const uint32_t end = r + 2 * nodes[r].shape - 1, i0 = r + (t - tile0[j]) * TILE4, i1 = min(i0 + TILE4, end);
+        T cmn[4], cmx[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { cmn[k] = Traits<T>::inf(); cmx[k] = -Traits<T>::inf(); }
+        for (uint32_t i = i0 + lane_id(); i < i1; i += 32) {
+            const uint4 meta = *reinterpret_cast<const uint4*>(nodes + i);    // parent, child_l, child_r, shape
+            if (meta.y != BVH_INVALID) continue;
+            idx0[node_start[i]] = meta.w;
+            T mn[4], mx[4];
+            load4(aabb + meta.w, mn, mx);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { const T c = center1(mn[k], mx[k]); cmn[k] = min_t(cmn[k], c); cmx[k] = max_t(cmx[k], c); }
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const typename Traits<T>::Key a = warp_min_key(f2key(cmn[k])), b = warp_max_key(f2key(cmx[k]));
+            if (lane_id() == 0) { atomicMin(keys + 8 * (size_t)j + k, a); atomicMax(keys + 8 * (size_t)j + 4 + k, b); }
+        }
+    }
+}
+// rebase (one warp per tile of root_tiles4): the nodes of the rebuilt subtrees get their new surface area as the growth baseline.  The
+// tiles matter when a root holds every shape: rebase_kernel (update.cuh) gives each root a single warp.
+template <class T>
+__global__ void __launch_bounds__(256) rebase4_kernel(const typename D4<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ roots,
+                                                      const uint32_t* __restrict__ n_roots, const uint32_t* __restrict__ tile0, T* __restrict__ sa_base) {
+    const uint32_t nr = *n_roots;
+    if (nr == 0) return;
+    const uint32_t ntiles = tile0[nr];
+    for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < ntiles; t += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t j = tile_owner(tile0, nr, t), r = roots[j];
+        const uint32_t end = r + 2 * __ldcg(&nodes[r].shape) - 1, i0 = r + (t - tile0[j]) * TILE4, i1 = min(i0 + TILE4, end);
+        for (uint32_t i = i0 + lane_id(); i < i1; i += 32) {
+            const typename D4<T>::Node& nd = nodes[i];
+            if (__ldcg(&nd.child_l) == BVH_INVALID) { sa_base[i] = T(0); continue; }
+            T mn[4], mx[4];
+            for (int c = 0; c < 4; ++c) { mn[c] = min_t(__ldcg(&nd.l_aabb.min[c]), __ldcg(&nd.r_aabb.min[c])); mx[c] = max_t(__ldcg(&nd.l_aabb.max[c]), __ldcg(&nd.r_aabb.max[c])); }
+            sa_base[i] = surface_area4(mn, mx);
+        }
+    }
+}
+// seed (one thread per root): the root's task -- its leaf range, node, parent, box (the join of its two child boxes, as the 3-D
+// rebuild takes it: tight after the climb) and centre bounds -- into the level list (> SMALL4 shapes) or the small list
+template <class T>
+__global__ void __launch_bounds__(256) root_seed4_kernel(const typename D4<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ node_start,
+                                                         const uint32_t* __restrict__ roots, const uint32_t* __restrict__ n_roots,
+                                                         const typename Traits<T>::Key* __restrict__ keys, Task4<T>* __restrict__ tasks, BuildArgs4 A) {
+    const uint32_t nr = *n_roots;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < nr; j += gridDim.x * blockDim.x) {
+        const uint32_t r = roots[j];
+        const typename D4<T>::Node& nd = nodes[r];
+        Task4<T> t;
+        t.start = node_start[r]; t.count = nd.shape; t.node = r; t.parent = nd.parent;
+        t.buf = 0; t.pad[0] = t.pad[1] = t.pad[2] = 0;
+        for (int k = 0; k < 4; ++k) {
+            t.ab[k] = min_t(nd.l_aabb.min[k], nd.r_aabb.min[k]); t.ab[4 + k] = max_t(nd.l_aabb.max[k], nd.r_aabb.max[k]);
+            t.cb[k] = key2f(keys[8 * (size_t)j + k]); t.cb[4 + k] = key2f(keys[8 * (size_t)j + 4 + k]);
+        }
+        atomicAdd(A.ctl + CTL_REBUILT, t.count);
+        if (t.count > SMALL4) tasks[atomicAdd(A.ctl + CTL_NEXT, 1u)] = t;
+        else reinterpret_cast<Task4<T>*>(A.small)[atomicAdd(A.ctl + CTL_SMALL, 1u)] = t;
+    }
+}
+
 // ================================================================================================================================
 // host side
 // ================================================================================================================================
@@ -679,6 +804,7 @@ template <class T> static void release4(Tree4<T>* t) {
     bvhgpu_ctx* ctx = t->ctx;
     dfree(ctx, t->d_aabb); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
     dfree(ctx, t->d_trec); dfree(ctx, t->d_flat); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
+    dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad);
 }
 template <class T> static int sticky4(const Tree4<T>* t) {
     if (t->failed_status != BVHGPU_OK) set_error("%s", t->failed_message.c_str());
@@ -688,6 +814,62 @@ template <class T> static int fail4(Tree4<T>* t, int rc, const char* msg) {
     t->failed_status = rc; t->failed_message = msg;
     set_error("%s", msg);
     return rc;
+}
+
+// Buffers of the level loop, sized for n shapes: at most max_tasks disjoint ranges of > SMALL4 shapes on one level.
+template <class T> struct Levels4 {
+    Task4<T>* tasks = nullptr;                   // [2 max_tasks]: this level's ranges, the next level's
+    typename Traits<T>::Key* acc = nullptr;      // [96 max_tasks] bucket keys
+    uint32_t *acnt = nullptr, *tile0 = nullptr, *tilecnt = nullptr;
+    uint32_t max_tasks = 0;
+};
+template <class T> static int levels4_alloc(Scratch& scratch, uint32_t n, Levels4<T>* L) {
+    L->max_tasks = n / (SMALL4 + 1) + 1;
+    const uint32_t max_tiles = n / TILE4 + L->max_tasks;
+    BVH_TRY(scratch.get(&L->tasks, 2 * (size_t)L->max_tasks));
+    BVH_TRY(scratch.get(&L->acc, 96 * (size_t)L->max_tasks));
+    BVH_TRY(scratch.get(&L->acnt, 6 * (size_t)L->max_tasks));
+    BVH_TRY(scratch.get(&L->tile0, (size_t)L->max_tasks + 1));
+    BVH_TRY(scratch.get(&L->tilecnt, 6 * (size_t)max_tiles));
+    return BVHGPU_OK;
+}
+
+// The builder from seeded tasks: the ranges of more than SMALL4 shapes in L.tasks[0 .. m) go through the level loop, then the n_small
+// ranges in A.small (the seeds' and the loop's) are finished by small4_kernel.  Build and rebuild run this same code.  Synchronous: the
+// host reads the range count of every level.  `who` names the caller in error messages.
+template <class T> static int run_levels4(Tree4<T>* tree, const BuildArgs4& A, const Levels4<T>& L, uint32_t m, uint32_t n_small, const char* who) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = tree->n;
+    uint32_t* h = ctx->h_pinned + 232;
+    const std::string err = std::string(who) + ": the device reported an empty split (non-finite input?); the tree is unusable";
+    const int wave = std::max(ctx->sm_count, 1) * 8;           // blocks of the grid-stride tile kernels
+    int cur = 0;
+    while (m) {
+        Task4<T>* tc = L.tasks + (size_t)cur * L.max_tasks;
+        Task4<T>* tn = L.tasks + (size_t)(cur ^ 1) * L.max_tasks;
+        const uint32_t tiles_bound = n / TILE4 + m;
+        const int grid = (int)std::min<uint32_t>((tiles_bound + 7) / 8, (uint32_t)wave);
+        level_prep4_kernel<T><<<1, 1024, 0, st>>>(tc, m, L.tile0, L.acc, L.acnt, A.ctl);
+        level_bin4_kernel<T><<<grid, 256, 0, st>>>(tree->d_aabb, tc, m, L.tile0, A, L.acc, L.acnt, L.tilecnt);
+        level_split4_kernel<T><<<(m + 7) / 8, 256, 0, st>>>(tc, m, L.tile0, L.acc, L.acnt, L.tilecnt, tn, A, tree->d_nodes, tree->d_node_index, tree->d_node_start);
+        level_scatter4_kernel<T><<<grid, 256, 0, st>>>(tc, m, L.tile0, L.tilecnt, A);
+        LAUNCHED(ctx, 4);
+        BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        BVH_CUDA_TRY(cudaStreamSynchronize(st));
+        if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], err.c_str());
+        m = h[CTL_NEXT];
+        n_small = h[CTL_SMALL];
+        cur ^= 1;
+    }
+    if (n_small) {
+        small4_kernel<T><<<(n_small + 7) / 8, 256, 0, st>>>(tree->d_aabb, n_small, A, tree->d_nodes, tree->d_node_index, tree->d_node_start);
+        LAUNCHED(ctx, 1);
+    }
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], err.c_str());
+    return BVHGPU_OK;
 }
 
 // The exact SAH build.  h_aabbs: host pointer.  Synchronous (the host learns the range count of every level anyway).
@@ -702,13 +884,10 @@ template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb*
     BVH_TRY(dalloc_t(ctx, &tree->d_node_start, tree->n_nodes));
     BVH_CUDA_TRY(cudaMemcpyAsync(tree->d_aabb, h_aabbs, sizeof(*h_aabbs) * n, cudaMemcpyHostToDevice, st));
 
-    const uint32_t max_tasks = n / (SMALL4 + 1) + 1;           // disjoint ranges of > SMALL4 shapes on one level
-    const uint32_t max_tiles = n / TILE4 + max_tasks;
     Scratch scratch(ctx);
     BuildArgs4 A{};
-    uint32_t *idx = nullptr, *tile0 = nullptr, *tilecnt = nullptr, *acnt = nullptr;
-    Key *root_keys = nullptr, *acc = nullptr;
-    Task4<T>* tasks = nullptr;
+    uint32_t* idx = nullptr;
+    Key* root_keys = nullptr;
     Task4<T>* small = nullptr;
     BVH_TRY(scratch.get(&idx, 2 * (size_t)n));
     BVH_TRY(scratch.get(&A.bkt, n));
@@ -725,47 +904,15 @@ template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb*
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
     if (h[CTL_NAN]) return fail4(tree, BVHGPU_ERR_NAN, "build: NaN coordinate in an input AABB (the reference panics here, src/bvh/bvh_node.rs:214-217)");
 
-    uint32_t m = 0, n_small = 1;
-    if (n > SMALL4) {
-        BVH_TRY(scratch.get(&tasks, 2 * (size_t)max_tasks));
-        BVH_TRY(scratch.get(&acc, 96 * (size_t)max_tasks));
-        BVH_TRY(scratch.get(&acnt, 6 * (size_t)max_tasks));
-        BVH_TRY(scratch.get(&tile0, (size_t)max_tasks + 1));
-        BVH_TRY(scratch.get(&tilecnt, 6 * (size_t)max_tiles));
-        root_task4_kernel<T><<<1, 1, 0, st>>>(root_keys, n, tasks);
-        LAUNCHED(ctx, 1);
-        m = 1;
+    Levels4<T> L;
+    if (n > SMALL4) {                                          // one root task: the level list, or the small list
+        BVH_TRY(levels4_alloc(scratch, n, &L));
+        root_task4_kernel<T><<<1, 1, 0, st>>>(root_keys, n, L.tasks);
     } else {
         root_task4_kernel<T><<<1, 1, 0, st>>>(root_keys, n, small);
-        LAUNCHED(ctx, 1);
     }
-    const int wave = std::max(ctx->sm_count, 1) * 8;           // blocks of the grid-stride tile kernels
-    int cur = 0;
-    while (m) {
-        Task4<T>* tc = tasks + (size_t)cur * max_tasks;
-        Task4<T>* tn = tasks + (size_t)(cur ^ 1) * max_tasks;
-        const uint32_t tiles_bound = n / TILE4 + m;
-        const int grid = (int)std::min<uint32_t>((tiles_bound + 7) / 8, (uint32_t)wave);
-        level_prep4_kernel<T><<<1, 1024, 0, st>>>(tc, m, tile0, acc, acnt, A.ctl);
-        level_bin4_kernel<T><<<grid, 256, 0, st>>>(tree->d_aabb, tc, m, tile0, A, acc, acnt, tilecnt);
-        level_split4_kernel<T><<<(m + 7) / 8, 256, 0, st>>>(tc, m, tile0, acc, acnt, tilecnt, tn, A, tree->d_nodes, tree->d_node_index, tree->d_node_start);
-        level_scatter4_kernel<T><<<grid, 256, 0, st>>>(tc, m, tile0, tilecnt, A);
-        LAUNCHED(ctx, 4);
-        BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaStreamSynchronize(st));
-        if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], "build: the device reported an empty split (non-finite input?); the tree is unusable");
-        m = h[CTL_NEXT];
-        n_small = h[CTL_SMALL];
-        cur ^= 1;
-    }
-    if (n_small) {
-        small4_kernel<T><<<(n_small + 7) / 8, 256, 0, st>>>(tree->d_aabb, n_small, A, tree->d_nodes, tree->d_node_index, tree->d_node_start);
-        LAUNCHED(ctx, 1);
-    }
-    BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], "build: the device reported an empty split (non-finite input?); the tree is unusable");
-    return BVHGPU_OK;
+    LAUNCHED(ctx, 1);
+    return run_levels4(tree, A, L, n > SMALL4 ? 1u : 0u, n > SMALL4 ? 0u : 1u, "build");
 }
 
 template <class T, class TreeT> static int build4_impl(bvhgpu_ctx* ctx, const typename D4<T>::Aabb* aabbs, size_t n, int mode, TreeT** out) {
@@ -1060,6 +1207,191 @@ template <class T> static int nearest_candidates4_host_impl(Tree4<T>* tree, cons
     return csr4_host<QueryProbe4<T, QUERY_WITHIN>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
 }
 
+// ---- refit / update_shapes ----
+// A failure after the tree was modified leaves arrays that no longer agree with each other: sticky, as a failed build.
+template <class T> static int failed4(Tree4<T>* t, int rc, const char* who) {
+    if (t->failed_status != BVHGPU_OK) return t->failed_status;               // already sticky (run_levels4)
+    char msg[1200];
+    snprintf(msg, sizeof msg, "%s failed after the tree was modified (%s); the tree is unusable", who, bvhgpu_last_error());
+    return fail4(t, rc, msg);
+}
+
+// The traversal records and the flat array, if they were built, are rewritten in place from the new boxes (their sizes do not change);
+// otherwise traverse, query, flatten and FLAT nearest_to would keep using the old boxes.
+template <class T> static int refresh_caches4(Tree4<T>* tree) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    const unsigned g = (tree->n_nodes + 255) / 256;
+    if (tree->d_trec) { trec4_kernel<T><<<g, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec); LAUNCHED(ctx, 1); }
+    if (tree->d_flat) { flat4_kernel<T><<<g, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_start, tree->n_nodes, tree->d_flat); LAUNCHED(ctx, 1); }
+    return BVHGPU_OK;
+}
+
+// m new boxes (and their shape indices, when `d_changed` is given) are checked on the device and the verdict is read back before the
+// tree is touched.
+template <class T> static int check4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m, Scratch& scratch,
+                                     const char* who) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    uint32_t* flags = nullptr;
+    BVH_TRY(scratch.get(&flags, 2));
+    BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), ctx->stream));
+    check4_kernel<T><<<(m + 255) / 256, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->n, flags);
+    LAUNCHED(ctx, 1);
+    uint32_t* h = ctx->h_pinned + 240;
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    if (h[1]) { set_error("%s: a changed shape index is >= %u; the tree was left unchanged", who, tree->n); return BVHGPU_ERR_INVALID; }
+    if (h[0]) { set_error("%s: NaN coordinate in a new AABB; the tree was left unchanged", who); return BVHGPU_ERR_NAN; }
+    return BVHGPU_OK;
+}
+
+// Bottom-up refit of every node from tree->d_aabb.
+template <class T> static int refit4(Tree4<T>* tree) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    if (tree->n >= 2) {
+        Scratch scratch(ctx);
+        uint32_t* arrivals = nullptr;
+        BVH_TRY(scratch.get(&arrivals, tree->n_nodes));
+        BVH_CUDA_TRY(cudaMemsetAsync(arrivals, 0, sizeof(uint32_t) * tree->n_nodes, ctx->stream));
+        refit4_kernel<T><<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, tree->n, arrivals);
+        LAUNCHED(ctx, 1);
+    }
+    return refresh_caches4(tree);                               // n = 1: the root record holds the shape's own box
+}
+
+// dirty[0 .. cnts[0]) = the nodes whose box changed, tree->d_bad = their growth flags.  Rebuilds in place, with the level loop and
+// small4_kernel of the build, the outermost degraded subtrees (cnts[1], zero on entry, counts them), gives their nodes fresh baselines
+// and clears the flags.  *rebuilt = shapes in the rebuilt subtrees.
+template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* dirty, uint32_t* cnts, size_t* rebuilt) {
+    using Key = typename Traits<T>::Key;
+    using Node = typename D4<T>::Node;
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = tree->n, gn = (tree->n_nodes + 255) / 256;
+    const uint32_t max_roots = n / 2 + 1;                       // rebuild roots are inner nodes of disjoint subtrees
+    const int wave = std::max(ctx->sm_count, 1) * 8;
+    Scratch scratch(ctx);
+    BuildArgs4 A{};
+    uint32_t *roots = nullptr, *idx = nullptr, *tile0 = nullptr;
+    Key* keys = nullptr;
+    Task4<T>* small = nullptr;
+    Levels4<T> L;
+    BVH_TRY(scratch.get(&roots, max_roots));
+    BVH_TRY(scratch.get(&tile0, (size_t)max_roots + 1));
+    BVH_TRY(scratch.get(&keys, 8 * (size_t)max_roots));
+    BVH_TRY(scratch.get(&idx, 2 * (size_t)n));
+    BVH_TRY(scratch.get(&A.bkt, n));
+    BVH_TRY(scratch.get(&A.ctl, 8));
+    BVH_TRY(scratch.get(&small, n));
+    BVH_TRY(levels4_alloc(scratch, n, &L));
+    A.idx[0] = idx; A.idx[1] = idx + n; A.small = small;
+    BVH_CUDA_TRY(cudaMemsetAsync(A.ctl, 0, 8 * sizeof(uint32_t), st));
+    select_roots_dirty_kernel<Node><<<gn, 256, 0, st>>>(tree->d_nodes, tree->d_bad, dirty, cnts, roots, cnts + 1);
+    root_tiles4_kernel<T><<<1, 1024, 0, st>>>(tree->d_nodes, roots, cnts + 1, tile0, keys);
+    root_bin4_kernel<T><<<wave, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, tree->d_aabb, roots, cnts + 1, tile0, idx, keys);
+    root_seed4_kernel<T><<<std::min<uint32_t>((max_roots + 255) / 256, (uint32_t)wave), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, roots, cnts + 1,
+                                                                                                       keys, L.tasks, A);
+    LAUNCHED(ctx, 4);
+    uint32_t* h = ctx->h_pinned + 244;
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 5 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    const uint32_t m = h[CTL_NEXT], n_small = h[CTL_SMALL], shapes = h[CTL_REBUILT];
+    if (m || n_small) BVH_TRY(run_levels4(tree, A, L, m, n_small, "update"));
+    rebase4_kernel<T><<<wave, 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, tile0, tree->d_sa_base);
+    clear_bad_kernel<<<gn, 256, 0, st>>>(dirty, cnts, tree->d_bad);
+    LAUNCHED(ctx, 2);
+    if (rebuilt) *rebuilt = shapes;
+    return BVHGPU_OK;
+}
+
+// The shapes d_changed[0 .. m) already carry their new boxes in tree->d_aabb.  max_growth <= 0: boxes only.  The same steps as the 3-D
+// update_incremental (flatten.cu) with the shared kernels of update.cuh.
+template <class T> static int update4(Tree4<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt) {
+    using Node = typename D4<T>::Node;
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t nn = tree->n_nodes;
+    const bool rebuild = max_growth > 0.0;
+    if (tree->n < 3) return refit4(tree);                       // one or two shapes: nothing a rebuild could change
+    if (!tree->d_arrive) {
+        BVH_TRY(dalloc_t(ctx, &tree->d_arrive, nn));
+        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_arrive, 0, sizeof(uint32_t) * nn, st));
+    }
+    if (rebuild && !tree->d_bad) {
+        BVH_TRY(dalloc_t(ctx, &tree->d_bad, nn));
+        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_bad, 0, nn, st));
+    }
+    if (rebuild && !tree->d_sa_base) {                          // first update on this tree: the baseline is the tree before the motion
+        BVH_TRY(dalloc_t(ctx, &tree->d_sa_base, nn));
+        node_sa_kernel<4, T, Node><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn, tree->d_sa_base);
+        LAUNCHED(ctx, 1);
+    }
+    Scratch scratch(ctx);
+    uint32_t *dirty = nullptr, *cnts = nullptr;
+    BVH_TRY(scratch.get(&dirty, nn));
+    BVH_TRY(scratch.get(&cnts, 2));                             // [0] dirty nodes, [1] rebuild roots
+    BVH_CUDA_TRY(cudaMemsetAsync(cnts, 0, 2 * sizeof(uint32_t), st));
+    const unsigned gm = (m + 255) / 256;
+    mark_paths_kernel<Node><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, d_changed, m, tree->d_arrive);
+    climb_paths_kernel<4, T, Node, typename D4<T>::Aabb><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
+                                                                              tree->d_sa_base, (T)max_growth, rebuild ? tree->d_bad : nullptr, dirty, cnts);
+    LAUNCHED(ctx, 2);
+    if (rebuild) BVH_TRY(rebuild_degraded4(tree, dirty, cnts, rebuilt));
+    return refresh_caches4(tree);
+}
+
+template <class T> static int refit4_impl(Tree4<T>* tree, const typename D4<T>::Aabb* aabbs, size_t n, bool dev_input) {
+    if (!tree || (n && !aabbs)) { set_error("refit: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    if (n != tree->n) { set_error("refit: %zu AABBs for a tree over %u shapes", n, tree->n); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const typename D4<T>::Aabb* d_in = aabbs;
+    if (!dev_input) {
+        void* d = nullptr;
+        BVH_TRY(upload4(ctx, scratch, aabbs, sizeof(*aabbs) * n, &d));
+        d_in = static_cast<const typename D4<T>::Aabb*>(d);
+    }
+    BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)n, scratch, "refit"));
+    int rc = cudaMemcpyAsync(tree->d_aabb, d_in, sizeof(*d_in) * n, cudaMemcpyDeviceToDevice, ctx->stream) == cudaSuccess ? (int)BVHGPU_OK : (int)BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK) rc = refit4(tree);
+    if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("refit: CUDA error"); rc = BVHGPU_ERR_CUDA; }
+    return rc == BVHGPU_OK ? rc : failed4(tree, rc, "refit");
+}
+
+// Bvh::update_shapes(changed_shape_indices, shapes): only the m changed shapes cross the boundary.
+template <class T> static int update4_impl(Tree4<T>* tree, const uint32_t* changed, const typename D4<T>::Aabb* fresh, size_t m, double max_growth,
+                                           size_t* rebuilt, bool dev_input) {
+    if (!tree || (m && (!changed || !fresh))) { set_error("update: null argument"); return BVHGPU_ERR_INVALID; }
+    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("update: max_growth = %g, must be >= 1 (or <= 0 for a pure refit)", max_growth); return BVHGPU_ERR_INVALID; }
+    if (m > 0xFFFFFFFFull) { set_error("update: too many changed shapes"); return BVHGPU_ERR_INVALID; }
+    if (rebuilt) *rebuilt = 0;
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (m == 0 || tree->n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const uint32_t* d_changed = changed;
+    const typename D4<T>::Aabb* d_fresh = fresh;
+    if (!dev_input) {
+        void *c = nullptr, *f = nullptr;
+        BVH_TRY(upload4(ctx, scratch, changed, sizeof(uint32_t) * m, &c));
+        BVH_TRY(upload4(ctx, scratch, fresh, sizeof(*fresh) * m, &f));
+        d_changed = static_cast<const uint32_t*>(c); d_fresh = static_cast<const typename D4<T>::Aabb*>(f);
+    }
+    BVH_TRY(check4(tree, d_changed, d_fresh, (uint32_t)m, scratch, "update"));
+    put4_kernel<T><<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(d_changed, d_fresh, (uint32_t)m, tree->d_aabb);
+    ctx->launches++;
+    size_t shapes = 0;
+    int rc = cudaGetLastError() == cudaSuccess ? (int)BVHGPU_OK : (int)BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK) rc = update4(tree, d_changed, (uint32_t)m, max_growth, &shapes);     // touches the root paths of the changed leaves only
+    if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("update: CUDA error"); rc = BVHGPU_ERR_CUDA; }
+    if (rc != BVHGPU_OK) return failed4(tree, rc, "update");
+    if (rebuilt) *rebuilt = shapes;
+    return BVHGPU_OK;
+}
+
 }  // namespace bvhb200
 
 using namespace bvhb200;
@@ -1105,6 +1437,18 @@ struct bvhgpu_tree4d : Tree4<double> {};
     BVH_EXPORT4 int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                     size_t cap, size_t* total) {                                          \
         return nearest_candidates4_host_impl<T>(tree, points, n, offsets, cand, cap, total);                              \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit4_impl<T>(tree, aabbs, n, false); } \
+    BVH_EXPORT4 int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) {                                 \
+        return refit4_impl<T>(tree, (const AABB*)dev_aabbs, n, true);                                                     \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m,         \
+                                        double max_growth, size_t* rebuilt) {                                             \
+        return update4_impl<T>(tree, changed, changed_aabbs, m, max_growth, rebuilt, false);                              \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_update_dev_##SUF(TREE* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, \
+                                            double max_growth, size_t* rebuilt) {                                         \
+        return update4_impl<T>(tree, (const uint32_t*)dev_changed, (const AABB*)dev_changed_aabbs, m, max_growth, rebuilt, true); \
     }
 
 DEFINE_API4(float, f32x4, bvhgpu_tree4f, bvh_aabb4f, bvh_ray4f, bvh_node4f, bvh_flat4f)

@@ -7,6 +7,7 @@
 //     nav(i) = (i - 1) + start(i)          start(i) = number of leaves before i = first shape position
 // with entry = nav+1 and exit = nav + 3*count(i) - 1.  One thread per node, no recursion, no scan.
 #include "internal.h"
+#include "update.cuh"
 
 namespace bvhb200 {
 
@@ -340,16 +341,6 @@ template <class T> int refit(Tree<T>* tree) {
 //      the subtree of a node with k shapes the contiguous node range [i, i + 2k - 1) over the contiguous leaf range
 //      [start(i), start(i) + k), so a rebuild only rewrites its own ranges.
 template <class T>
-__global__ void __launch_bounds__(256) node_sa_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_nodes, T* __restrict__ sa) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_nodes) return;
-    const typename Traits<T>::Node& nd = nodes[i];
-    if (nd.child_l == BVH_INVALID) { sa[i] = T(0); return; }
-    T mn[3], mx[3];
-    for (int k = 0; k < 3; ++k) { mn[k] = min_t(nd.l_aabb.min[k], nd.r_aabb.min[k]); mx[k] = max_t(nd.l_aabb.max[k], nd.r_aabb.max[k]); }
-    sa[i] = surface_area(mn, mx);
-}
-template <class T>
 __global__ void __launch_bounds__(256) mark_bad_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_nodes,
                                                        const T* __restrict__ sa_old, T max_growth, uint8_t* __restrict__ bad) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -359,11 +350,6 @@ __global__ void __launch_bounds__(256) mark_bad_kernel(const typename Traits<T>:
     T mn[3], mx[3];
     for (int k = 0; k < 3; ++k) { mn[k] = min_t(nd.l_aabb.min[k], nd.r_aabb.min[k]); mx[k] = max_t(nd.l_aabb.max[k], nd.r_aabb.max[k]); }
     bad[i] = surface_area(mn, mx) > mul_rn(max_growth, sa_old[i]) ? 1 : 0;
-}
-__device__ __forceinline__ bool rebuild_candidate(uint32_t i, uint32_t child_l, uint32_t child_r, const uint8_t* bad) {
-    if (child_l == BVH_INVALID) return false;
-    if (bad[i]) return i == 0;
-    return bad[child_l] || bad[child_r];
 }
 template <class T>
 __global__ void __launch_bounds__(256) select_roots_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_nodes,
@@ -387,25 +373,6 @@ __global__ void __launch_bounds__(256) leaf_order_kernel(const uint32_t* __restr
     if (s < n) idx[node_start[node_index[s]]] = s;
 }
 
-// After a rebuild the nodes of the rebuilt subtrees get a new surface-area baseline; every other node keeps the one it had when
-// it was last built (so slow drift accumulates against it instead of being forgiven at every call).
-template <class T>
-__global__ void __launch_bounds__(256) rebase_kernel(const typename Traits<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ roots,
-                                                     const uint32_t* __restrict__ n_roots, T* __restrict__ sa_base) {
-    const uint32_t warps = gridDim.x * (blockDim.x >> 5), nr = *n_roots;
-    for (uint32_t k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); k < nr; k += warps) {
-        const uint32_t r = roots[k];
-        const uint32_t cnt = __ldcg(&nodes[r].shape);                        // shapes below the root: its subtree is the node range [r, r + 2 cnt - 1)
-        for (uint32_t i = r + lane_id(); i < r + 2 * cnt - 1; i += 32) {
-            const typename Traits<T>::Node& nd = nodes[i];
-            if (__ldcg(&nd.child_l) == BVH_INVALID) { sa_base[i] = T(0); continue; }
-            T mn[3], mx[3];
-            for (int c = 0; c < 3; ++c) { mn[c] = min_t(__ldcg(&nd.l_aabb.min[c]), __ldcg(&nd.r_aabb.min[c])); mx[c] = max_t(__ldcg(&nd.l_aabb.max[c]), __ldcg(&nd.r_aabb.max[c])); }
-            sa_base[i] = surface_area(mn, mx);
-        }
-    }
-}
-
 template <class T> int optimize(Tree<T>* tree, double max_growth) {
     bvhgpu_ctx* ctx = tree->ctx;
     if (tree->n < 3) return refit(tree);                                // one or two shapes: nothing a rebuild could change
@@ -417,7 +384,7 @@ template <class T> int optimize(Tree<T>* tree, double max_growth) {
     const unsigned gn0 = (nn + 255) / 256;
     if (!tree->d_sa_base) {                                             // first optimize on this tree: the baseline is the tree as built
         BVH_TRY(dalloc(ctx, &tree->d_sa_base, sizeof(T) * nn));
-        node_sa_kernel<T><<<gn0, 256, 0, st>>>(tree->d_nodes, nn, reinterpret_cast<T*>(tree->d_sa_base));
+        node_sa_kernel<3, T, typename Traits<T>::Node><<<gn0, 256, 0, st>>>(tree->d_nodes, nn, reinterpret_cast<T*>(tree->d_sa_base));
         ctx->launches++;
     }
     T* sa_old = reinterpret_cast<T*>(tree->d_sa_base);
@@ -438,7 +405,7 @@ template <class T> int optimize(Tree<T>* tree, double max_growth) {
     ctx->launches += 4;
     BVH_CUDA_TRY(cudaGetLastError());
     BVH_TRY(rebuild_subtrees(ctx, tree, roots, n_roots, cb, idx0, false));
-    rebase_kernel<T><<<std::max(1, std::min(ctx->sm_count * 4, (int)n)), 256, 0, st>>>(tree->d_nodes, roots, n_roots, sa_old);
+    rebase_kernel<3, T, typename Traits<T>::Node><<<std::max(1, std::min(ctx->sm_count * 4, (int)n)), 256, 0, st>>>(tree->d_nodes, roots, n_roots, sa_old);
     ctx->launches++;
     BVH_TRY(build_traversal_records(tree));
     if (tree->have_flat) BVH_TRY(build_flat(tree));
@@ -471,67 +438,6 @@ __global__ void __launch_bounds__(256) update_scatter_kernel(const uint32_t* __r
     if constexpr (sizeof(T) == 4) { d.pad0 = 0; d.pad1 = 0; }
     aabb[changed[i]] = d;                                               // an index listed twice: one of its AABBs wins (the reference would use shapes[i] for both)
 }
-// ---- incremental form: only the root paths of the changed leaves are touched ----------------------------------------------------
-// mark: every changed leaf walks up and counts, in arrive[p], how many of p's children lie on a changed path (the first walker through
-// a node carries on, later ones stop).  climb: every changed leaf writes its box into its parent and decrements; the LAST arrival at a
-// node joins the two stored child boxes (both final by then), tests the growth against the node's baseline, logs the node as dirty and
-// carries on.  Work = number of nodes on the changed paths, not n.
-template <class T>
-__global__ void __launch_bounds__(256) mark_paths_kernel(const typename Traits<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ node_index,
-                                                         const uint32_t* __restrict__ changed, uint32_t m, uint32_t* __restrict__ arrive) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    uint32_t node = node_index[changed[i]];
-    while (node != 0) {
-        const uint32_t p = nodes[node].parent;
-        if (atomicAdd(arrive + p, 1u) != 0u) break;
-        node = p;
-    }
-}
-template <class T>
-__global__ void __launch_bounds__(256) climb_paths_kernel(typename Traits<T>::Node* nodes, const uint32_t* __restrict__ node_index,
-                                                          const typename Traits<T>::DAabb* __restrict__ aabb, const uint32_t* __restrict__ changed, uint32_t m,
-                                                          uint32_t* __restrict__ arrive, const T* __restrict__ sa_base, T max_growth, uint8_t* __restrict__ bad,
-                                                          uint32_t* __restrict__ dirty, uint32_t* __restrict__ n_dirty) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const uint32_t s = changed[i];
-    T mn[3], mx[3];
-    load_aabb(aabb + s, mn, mx);
-    uint32_t node = node_index[s];
-    while (node != 0) {
-        const uint32_t p = __ldcg(&nodes[node].parent);
-        typename Traits<T>::Node* pn = nodes + p;
-        const bool is_left = __ldcg(&pn->child_l) == node;
-        auto* dst = is_left ? &pn->l_aabb : &pn->r_aabb;
-        for (int k = 0; k < 3; ++k) { __stcg(&dst->min[k], mn[k]); __stcg(&dst->max[k], mx[k]); }
-        __threadfence();
-        if (atomicSub(arrive + p, 1u) != 1u) return;        // another changed path still has to come through p
-        __threadfence();
-        const auto* sib = is_left ? &pn->r_aabb : &pn->l_aabb;
-        for (int k = 0; k < 3; ++k) { mn[k] = min_t(__ldcg(&sib->min[k]), mn[k]); mx[k] = max_t(__ldcg(&sib->max[k]), mx[k]); }
-        if (bad && surface_area(mn, mx) > mul_rn(max_growth, sa_base[p])) bad[p] = 1;
-        dirty[atomicAdd(n_dirty, 1u)] = p;
-        node = p;
-    }
-}
-template <class T>
-__global__ void __launch_bounds__(256) select_roots_dirty_kernel(const typename Traits<T>::Node* __restrict__ nodes, const uint8_t* __restrict__ bad,
-                                                                 const uint32_t* __restrict__ dirty, const uint32_t* __restrict__ n_dirty,
-                                                                 uint32_t* __restrict__ roots, uint32_t* n_roots) {
-    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= *n_dirty) return;
-    const uint32_t i = dirty[k];
-    const uint4 meta = *reinterpret_cast<const uint4*>(nodes + i);
-    if (!rebuild_candidate(i, meta.y, meta.z, bad)) return;
-    uint32_t a = i;
-    while (a != 0) {                                                   // an outer candidate takes this subtree with it
-        a = nodes[a].parent;
-        const uint4 mm = *reinterpret_cast<const uint4*>(nodes + a);
-        if (rebuild_candidate(a, mm.y, mm.z, bad)) return;
-    }
-    roots[atomicAdd(n_roots, 1u)] = i;
-}
 // one warp per rebuild root: the shapes of its subtree in leaf order (index buffer of the rebuild) and the bounds of their centres
 template <class T>
 __global__ void __launch_bounds__(256) root_prep_kernel(const typename Traits<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ node_start,
@@ -556,11 +462,6 @@ __global__ void __launch_bounds__(256) root_prep_kernel(const typename Traits<T>
         }
     }
 }
-__global__ void __launch_bounds__(256) clear_bad_kernel(const uint32_t* __restrict__ dirty, const uint32_t* __restrict__ n_dirty, uint8_t* __restrict__ bad) {
-    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k < *n_dirty) bad[dirty[k]] = 0;
-}
-
 // The shapes `d_changed[0..m)` already carry their new AABBs in tree->d_aabb.  max_growth <= 0: boxes only.
 template <class T>
 int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth) {
@@ -584,8 +485,8 @@ int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, dou
     BVH_TRY(scratch.get(&dirty, nn));
     BVH_TRY(scratch.get(&cnts, 2));                                     // [0] dirty nodes, [1] rebuild roots
     BVH_CUDA_TRY(cudaMemsetAsync(cnts, 0, 2 * sizeof(uint32_t), st));
-    mark_paths_kernel<T><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, d_changed, m, tree->d_arrive);
-    climb_paths_kernel<T><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
+    mark_paths_kernel<typename Traits<T>::Node><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, d_changed, m, tree->d_arrive);
+    climb_paths_kernel<3, T, typename Traits<T>::Node, typename Traits<T>::DAabb><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
                                               reinterpret_cast<const T*>(tree->d_sa_base), (T)max_growth, rebuild ? tree->d_bad : nullptr, dirty, cnts);
     ctx->launches += 2;
     if (rebuild) BVH_TRY(rebuild_degraded(tree, dirty, cnts));
@@ -600,7 +501,7 @@ template <class T> int ensure_sa_base(Tree<T>* tree) {
     if (tree->d_sa_base || tree->n_nodes == 0) return BVHGPU_OK;
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_TRY(dalloc(ctx, &tree->d_sa_base, sizeof(T) * tree->n_nodes));
-    node_sa_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, reinterpret_cast<T*>(tree->d_sa_base));
+    node_sa_kernel<3, T, typename Traits<T>::Node><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, reinterpret_cast<T*>(tree->d_sa_base));
     ctx->launches++;
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
@@ -618,12 +519,12 @@ template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* dirty, ui
     BVH_TRY(scratch.get(&roots, n));
     BVH_TRY(scratch.get(&idx0, n));
     BVH_TRY(scratch.get(&cb_roots, 6 * (size_t)n / 2 + 6));             // rebuild roots are inner nodes of disjoint subtrees: at most n / 2 of them
-    select_roots_dirty_kernel<T><<<gn, 256, 0, st>>>(tree->d_nodes, tree->d_bad, dirty, cnts, roots, cnts + 1);
+    select_roots_dirty_kernel<typename Traits<T>::Node><<<gn, 256, 0, st>>>(tree->d_nodes, tree->d_bad, dirty, cnts, roots, cnts + 1);
     root_prep_kernel<T><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, tree->d_aabb, roots, cnts + 1, idx0, cb_roots);
     ctx->launches += 2;
     BVH_CUDA_TRY(cudaGetLastError());
     BVH_TRY(rebuild_subtrees(ctx, tree, roots, cnts + 1, cb_roots, idx0, true));
-    rebase_kernel<T><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, reinterpret_cast<T*>(tree->d_sa_base));
+    rebase_kernel<3, T, typename Traits<T>::Node><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, reinterpret_cast<T*>(tree->d_sa_base));
     clear_bad_kernel<<<gn, 256, 0, st>>>(dirty, cnts, tree->d_bad);
     ctx->launches += 2;
     BVH_CUDA_TRY(cudaGetLastError());

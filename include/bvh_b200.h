@@ -267,6 +267,37 @@ int bvhgpu_nearest_candidates_f32x4(bvhgpu_tree4f* tree, const float* points, si
 int bvhgpu_nearest_candidates_f64x4(bvhgpu_tree4d* tree, const double* points, size_t n, uint32_t* offsets, uint32_t* cand,
                                     size_t cap, size_t* total);
 
+/* ---- D = 2 and D = 4 refit and update_shapes (Bvh::update_shapes and its refit fix_aabbs_ascending, src/bvh/optimization.rs:17,
+ * 304-351, generic in D).  The contract of bvhgpu_refit_f32x3 / bvhgpu_update_f32x3 below, with D components:
+ *   - refit: `aabbs` are the new boxes of all n shapes; every node's child boxes are recomputed bottom-up.  Topology, node indices and
+ *     node_start are kept; leaves keep their Aabb::empty() child boxes.  n != the tree's shape count: BVHGPU_ERR_INVALID.
+ *   - update: `changed[i]` is a shape index, `changed_aabbs[i]` its new box; only the root paths of the changed leaves are refitted.
+ *     max_growth >= 1: then the outermost subtrees that hold a node whose surface area grew by more than max_growth are rebuilt in
+ *     place with the exact builder (the node array stays in Bvh::build's preorder layout; node indices of the shapes in them change).
+ *     Growth is judged against the surface area every node had when it was last (re)built; the baseline is taken at the first update,
+ *     so slow drift over many calls adds up.  max_growth <= 0: boxes only.  0 < max_growth < 1: BVHGPU_ERR_INVALID.  *rebuilt (may
+ *     be NULL) = number of shapes in the rebuilt subtrees.  m = 0 is a no-op.
+ *   - every changed index (< n) and every new box (no NaN) is checked on the device, and the verdict read back, before anything is
+ *     written: a refused call (BVHGPU_ERR_INVALID / BVHGPU_ERR_NAN) leaves the tree byte for byte as it was.
+ *   - traversal records and the flat array built by earlier traverse / query / flatten / nearest_to calls are rewritten in place, so
+ *     every later call sees the new boxes.
+ *   - a failure after the tree was modified is sticky, as a failed build's.
+ * D = 2 runs the 3-D refit and update on the tree embedded in z = [0, 0] (exact, dim2.cu); host pointers only.  D = 4 has its own
+ * kernels (dim4.cu) and rebuilds with the 4-D exact builder; the calls are synchronous (the builder reads one word per level).
+ * update_dev / refit_dev: device pointers (C-ABI layout), enqueued on the context's stream. */
+int bvhgpu_refit_f32x2(bvhgpu_tree2f* tree, const bvh_aabb2f* aabbs, size_t n);
+int bvhgpu_refit_f64x2(bvhgpu_tree2d* tree, const bvh_aabb2d* aabbs, size_t n);
+int bvhgpu_update_f32x2(bvhgpu_tree2f* tree, const uint32_t* changed, const bvh_aabb2f* changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
+int bvhgpu_update_f64x2(bvhgpu_tree2d* tree, const uint32_t* changed, const bvh_aabb2d* changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
+int bvhgpu_refit_f32x4(bvhgpu_tree4f* tree, const bvh_aabb4f* aabbs, size_t n);
+int bvhgpu_refit_f64x4(bvhgpu_tree4d* tree, const bvh_aabb4d* aabbs, size_t n);
+int bvhgpu_refit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_aabbs, size_t n);
+int bvhgpu_refit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_aabbs, size_t n);
+int bvhgpu_update_f32x4(bvhgpu_tree4f* tree, const uint32_t* changed, const bvh_aabb4f* changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
+int bvhgpu_update_f64x4(bvhgpu_tree4d* tree, const uint32_t* changed, const bvh_aabb4d* changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
+int bvhgpu_update_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
+int bvhgpu_update_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
+
 /* ---- flatten: replaces Bvh::flatten (src/flat_bvh.rs:60-143, 240-251, 312-319) -----
  * Writes the FlatBvh (3n-2 FlatNodes for n >= 2, 1 for n == 1, 0 for n == 0) into `out`
  * (may be NULL to only build the device copy) and its length into *len. */
