@@ -12,9 +12,11 @@
 //   triangle mode  result = the triangle with the smallest Ray::intersects_triangle distance (Moeller-Trumbore with backface culling,
 //                  same operation order, no FMA), ties to the lower shape index.  A subtree is skipped when its entry distance exceeds
 //                  best * (1 + 2^-16): the slab distance and the Moeller-Trumbore distance are different roundings of the same
-//                  quantity, so pruning at exactly `entry > best` could drop a hit that wins by an ulp; with the margin the result can
-//                  differ from the unpruned minimum only between two hits whose distances agree to ~1e-5 relative (stated in the
-//                  tests as the tolerance).
+//                  quantity, so pruning at exactly `entry > best` could drop a hit that wins by an ulp.  The margin does not bound
+//                  how far a grazing hit's rounded distance can fall in front of its own box (17 % was seen in f32), so the result
+//                  G differs from the unpruned minimum W only where W's Moeller-Trumbore distance lies more than 2^-16 in front of
+//                  the slab entry of W's own AABB; then d_W <= d_G, that entry exceeds fl(d_G * (1 + 2^-16)), and W's exact
+//                  intersection lies behind d_G.  G's distance, u and v are always the reference's Moeller-Trumbore result for G.
 // The walk needs no stack: nodes carry parent links, a lane remembers which child it comes back from and re-derives the near / far
 // order from the node (same loads, same bits), so any tree depth works (the reference's iterators use a 32-slot stack / a heap).
 #include "internal.h"

@@ -654,8 +654,9 @@ __global__ void __launch_bounds__(128) nearest_bound4_kernel(const typename D4<T
     T p[4];
     for (int k = 0; k < 4; ++k) p[k] = points[4 * (size_t)i + k];
     uint32_t best;
-    T u;
-    nearest_walk<4, T, false>(nodes, p, best, u, [&](uint32_t shape) { T mn[4], mx[4]; load4(aabb + shape, mn, mx); return box_upper_d2<4>(p, mn, mx); });
+    T u, g[4];
+    root_magnitude<4>(nodes, p, g);
+    nearest_walk<4, T, false>(nodes, p, best, u, [&](uint32_t shape) { T mn[4], mx[4]; load4(aabb + shape, mn, mx); return box_upper_d2<4>(p, mn, mx, g); });
     u = mul_rn(u, add_rn(T(1), mul_rn(T(16), Traits<T>::eps())));      // the bound itself is a rounded sum: keep it an upper bound
     for (int k = 0; k < 4; ++k) records[5 * (size_t)i + k] = p[k];
     records[5 * (size_t)i + 4] = u;

@@ -50,32 +50,69 @@ template <class T, int D> struct Query<T, BVHGPU_QUERY_BALL, D> {
     }
 };
 
-// Internal kind: every shape whose AABB lies within squared distance U of a point, record {p, U} (D + 1 T).  The lower bound
-// sum_k max(min_k - p_k, p_k - max_k, 0)^2 is monotone under box containment in floating point (subtraction, squaring
-// and addition of non-negative terms are monotone), so pruning an inner box can never lose a shape it contains.  An empty
-// child box (min > max on some axis: the Aabb::empty() a "no split wins" node stores where surface areas overflow) contains
-// nothing it bounds, so it is always entered.
+// Internal kind: every shape whose AABB lies within squared distance U of a point, record {p, U} (D + 1 T).
+//
+// The per-axis gap of a box is judged against two distances: the exact one, and the reference's rounded
+// Aabb::min_distance_squared (aabb_impl.rs:618-629: |p - centre| - half_size), which cancels badly far from the origin.  The
+// reference's gap differs from the exact gap by less than 9 u m (u = eps / 2, m = max(|p|, -min, max, max - min) on that axis,
+// plus a few subnormal steps), and min - p, p - max are off by at most 2 u m.  axis_slack is 16 eps m + 16 subnormal steps, so
+// the lower bound sum_k max(max(min_k - p_k, p_k - max_k) - slack_k, 0)^2 stays below both distances.  It is monotone under box
+// containment in floating point (a larger box has smaller differences and a larger m; subtraction, squaring and addition of
+// non-negative terms are monotone), so pruning an inner box can never lose a shape it contains.  An empty child box (min > max
+// on some axis: the Aabb::empty() a "no split wins" node stores where surface areas overflow) contains nothing it bounds, so it
+// is always entered.
 constexpr int QUERY_WITHIN = 4;
+template <class T> __device__ __forceinline__ T slack_floor();
+template <> __device__ __forceinline__ float slack_floor<float>() { return 0x1p-145f; }        // 16 f32 subnormal steps
+template <> __device__ __forceinline__ double slack_floor<double>() { return 0x1p-1070; }      // 16 f64 subnormal steps
+// m of one axis of one box; an empty axis (min = +inf, max = -inf) gives |p|, a NaN term is ignored
+template <class T> __device__ __forceinline__ T axis_magnitude(T p, T mn, T mx) {
+    T m = fabs(p);
+    const T nmn = -mn, ext = sub_rn(mx, mn);
+    m = nmn > m ? nmn : m;
+    m = mx > m ? mx : m;
+    return ext > m ? ext : m;
+}
+template <class T> __device__ __forceinline__ T axis_slack(T m) { return add_rn(mul_rn(m, mul_rn(T(16), Traits<T>::eps())), slack_floor<T>()); }
 template <int D, class T> __device__ __forceinline__ T box_lower_d2(const T p[D], const T bmn[D], const T bmx[D]) {
     T d2 = T(0);
 #pragma unroll
     for (int i = 0; i < D; ++i) {
         const T a = sub_rn(bmn[i], p[i]), b = sub_rn(p[i], bmx[i]);
         T d = a > b ? a : b;
+        d = sub_rn(d, axis_slack(axis_magnitude(p[i], bmn[i], bmx[i])));
         d = d > T(0) ? d : T(0);
         d2 = add_rn(d2, mul_rn(d, d));
     }
     return d2;
 }
-template <int D, class T> __device__ __forceinline__ T box_upper_d2(const T p[D], const T bmn[D], const T bmx[D]) {   // farthest corner
+// The U of nearest_candidates at a shape: the squared distance to the farthest corner, each non-zero axis term widened by the
+// slack of m = max(that axis's m of the shape, g[axis]).  g is the magnitude of the root's child boxes: every node below them
+// has a smaller m, so U also bounds the reference's rounded distance of any node Bvh::nearest_to prunes (see nearest_bound_kernel).
+// A zero farthest distance means min = max = p on that axis, where the reference's term is exactly 0 as well.
+template <int D, class T> __device__ __forceinline__ T box_upper_d2(const T p[D], const T bmn[D], const T bmx[D], const T g[D]) {
     T d2 = T(0);
 #pragma unroll
     for (int i = 0; i < D; ++i) {
         const T a = fabs(sub_rn(p[i], bmn[i])), b = fabs(sub_rn(p[i], bmx[i]));
-        const T d = a > b ? a : b;
+        T d = a > b ? a : b;
+        if (d > T(0)) {
+            const T m = axis_magnitude(p[i], bmn[i], bmx[i]);
+            d = add_rn(d, axis_slack(g[i] > m ? g[i] : m));
+        }
         d2 = add_rn(d2, mul_rn(d, d));
     }
     return d2;
+}
+// g of box_upper_d2 for one point: the axis magnitudes of the root's two child boxes.  Empty boxes (those of a root leaf, or of
+// a "no split wins" root) give |p|.
+template <int D, class T, class Node> __device__ __forceinline__ void root_magnitude(const Node* __restrict__ nodes, const T p[D], T g[D]) {
+#pragma unroll
+    for (int k = 0; k < D; ++k) {
+        const T l = axis_magnitude(p[k], __ldg(&nodes[0].l_aabb.min[k]), __ldg(&nodes[0].l_aabb.max[k]));
+        const T r = axis_magnitude(p[k], __ldg(&nodes[0].r_aabb.min[k]), __ldg(&nodes[0].r_aabb.max[k]));
+        g[k] = l > r ? l : r;
+    }
 }
 template <class T, int D> struct Query<T, QUERY_WITHIN, D> {
     T p[D], u;

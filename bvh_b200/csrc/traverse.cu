@@ -1507,8 +1507,9 @@ __global__ void __launch_bounds__(128) nearest_bound_kernel(const typename Trait
     T p[3];
     for (int k = 0; k < 3; ++k) p[k] = points[3 * (size_t)i + k];
     uint32_t best;
-    T u;
-    nearest_walk<3, T, false>(nodes, p, best, u, [&](uint32_t shape) { T mn[3], mx[3]; load_aabb(aabb + shape, mn, mx); return box_upper_d2<3>(p, mn, mx); });
+    T u, g[3];
+    root_magnitude<3>(nodes, p, g);
+    nearest_walk<3, T, false>(nodes, p, best, u, [&](uint32_t shape) { T mn[3], mx[3]; load_aabb(aabb + shape, mn, mx); return box_upper_d2<3>(p, mn, mx, g); });
     u = mul_rn(u, add_rn(T(1), mul_rn(T(16), Traits<T>::eps())));      // the bound itself is a rounded sum: keep it an upper bound
     for (int k = 0; k < 3; ++k) records[4 * (size_t)i + k] = p[k];
     records[4 * (size_t)i + 3] = u;

@@ -421,8 +421,9 @@ int bvhgpu_traverse_ordered_f64x3(bvhgpu_tree3d* tree, const bvh_ray3d* rays, si
  *   use_triangles != 0: the triangles given with bvhgpu_tree_set_triangles_* (9 scalars per shape: a, b, c; shape i's AABB must
  *       contain triangle i); out_shape = the triangle with the smallest Moeller-Trumbore distance (backface culled, the reference's
  *       operation order, no FMA), ties to the lower index; out_dist = that distance, out_uv (may be NULL) = its u, v.  A subtree is
- *       skipped when its entry distance exceeds best * (1 + 2^-16): results can differ from the unpruned minimum only between hits
- *       whose distances agree to ~1e-5 relative.
+ *       skipped when its entry distance exceeds best * (1 + 2^-16).  The result G differs from the unpruned minimum W (the loop over
+ *       Bvh::traverse) only where W's Moeller-Trumbore distance lies more than 2^-16 in front of the slab entry of W's own AABB
+ *       (grazing hits); then d_W <= d_G, that entry exceeds fl(d_G * (1 + 2^-16)), and W's exact intersection lies behind d_G.
  * No hit: out_shape = BVHGPU_INVALID_INDEX, out_dist = +inf. */
 int bvhgpu_tree_set_triangles_f32x3(bvhgpu_tree3f* tree, const float* triangles, size_t n);
 int bvhgpu_tree_set_triangles_f64x3(bvhgpu_tree3d* tree, const double* triangles, size_t n);
@@ -445,10 +446,13 @@ int bvhgpu_closest_hit_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_rays, int 
  *                               src/aabb/aabb_impl.rs:618-629; strict `<`; first minimum kept).  out_shape[i] = shape index
  *                               (BVHGPU_INVALID_INDEX for an empty tree), out_dist[i] = distance (sqrt, as the reference returns).
  *                               `mode` selects Bvh (BVHGPU_TRAVERSE_BVH) or FlatBvh (BVHGPU_TRAVERSE_FLAT) visiting order.
- *   bvhgpu_nearest_candidates_* for ANY shape contained in its AABB: CSR lists that are guaranteed to contain the nearest shape
- *                               of every point (all shapes whose AABB is at most as far as the smallest farthest-corner
- *                               distance of any shape's AABB); the shim evaluates distance_squared on that short list and
- *                               keeps the minimum.  Below an empty child box ("no split wins" nodes, where surface areas
+ *   bvhgpu_nearest_candidates_* for ANY shape contained in its AABB: CSR lists of the shapes whose AABB is at most as far as
+ *                               the smallest farthest-corner distance of any shape's AABB, both sides widened per axis by a
+ *                               rounding slack of 16 eps max(|p|, -min, max, max - min).  Every list contains every shape at the
+ *                               minimal exact distance, the shape bvhgpu_nearest_* (Bvh::nearest_to) returns, and the shape of
+ *                               smallest Aabb::min_distance_squared over all shapes.  A shape's own distance is guaranteed only
+ *                               in exact arithmetic; its rounded form is user code.  The shim evaluates distance_squared on the
+ *                               short list and keeps the minimum.  Below an empty child box ("no split wins" nodes, where surface areas
  *                               overflow) the box bounds nothing, so every shape under it is listed. */
 int bvhgpu_nearest_f32x3(bvhgpu_tree3f* tree, int mode, const float* points, size_t n, uint32_t* out_shape, float* out_dist);
 int bvhgpu_nearest_f64x3(bvhgpu_tree3d* tree, int mode, const double* points, size_t n, uint32_t* out_shape, double* out_dist);
