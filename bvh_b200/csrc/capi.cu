@@ -210,6 +210,39 @@ template <class T> static int ensure_result_buffers(Tree<T>* tree, size_t nrays,
     return BVHGPU_OK;
 }
 
+// The host-pointer CSR calls of a 3-D (or lifted 2-D) tree run into the tree's retained buffers, which bvhgpu_traverse_fetch_*
+// reads later.  The hit buffer starts at max(hits_cap, per_item * n, 1024).  When run(d_offsets, d_hits, cap, &tot) reports
+// BVHGPU_ERR_CAPACITY with a total the u32 offsets can hold, the buffer grows to that total and the call runs once more.
+template <class T, class Run> static int run_retained(Tree<T>* tree, size_t n, size_t per_item, size_t* tot, Run run) {
+    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, per_item * n), 1024);
+    int rc = BVHGPU_OK;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        rc = ensure_result_buffers(tree, n, want);
+        if (rc != BVHGPU_OK) break;
+        rc = run(tree->d_offsets, tree->d_hits, tree->hits_cap, tot);
+        if (rc == BVHGPU_ERR_CAPACITY && *tot <= 0xFFFFFFFFull && *tot > tree->hits_cap && attempt == 0) { want = *tot; continue; }   // grow once and redo
+        break;
+    }
+    return rc;
+}
+static const char* capacity_hint(int D) { return D == 3 ? "use bvhgpu_traverse_fetch_*" : "call again with cap = *total"; }
+// run_retained, then the CSR copied from the retained buffers: the offsets always, the hits when they fit `cap`.
+template <int D, class T, class Run>
+static int retained_to_host(Tree<T>* tree, const char* what, size_t n, size_t per_item, uint32_t* offsets, uint32_t* hits, size_t cap,
+                            size_t* total, Run run) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    size_t tot = 0;
+    const int rc = run_retained(tree, n, per_item, &tot, run);
+    if (total) *total = tot;
+    if (rc != BVHGPU_OK) return rc;
+    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
+    int ret = BVHGPU_OK;
+    if (hits && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
+    else if (tot > cap) { set_error("%s: %zu hits do not fit the caller's capacity %zu (%s)", what, tot, cap, capacity_hint(D)); ret = BVHGPU_ERR_CAPACITY; }
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return ret;
+}
+
 template <class T>
 static int traverse_host_impl(Tree<T>* tree, int mode, const void* rays, uint32_t fmt, size_t nrays,
                               uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
@@ -226,16 +259,10 @@ static int traverse_host_impl(Tree<T>* tree, int mode, const void* rays, uint32_
         if (total) *total = 0;
         return BVHGPU_OK;
     }
-    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 4 * nrays), 1024);
     size_t tot = 0;
-    int rc = BVHGPU_OK;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        rc = ensure_result_buffers(tree, nrays, want);
-        if (rc != BVHGPU_OK) break;
-        rc = traverse_host_pipelined<T>(tree, mode, rays, fmt, nrays, offsets, hits, cap, &tot);
-        if (rc == BVHGPU_ERR_CAPACITY && tot <= 0xFFFFFFFFull && tot > tree->hits_cap && attempt == 0) { want = tot; continue; }   // grow once and redo
-        break;
-    }
+    const int rc = run_retained(tree, nrays, 4, &tot, [&](uint32_t*, uint32_t*, size_t, size_t* t) {   // copies back for itself
+        return traverse_host_pipelined<T>(tree, mode, rays, fmt, nrays, offsets, hits, cap, t);
+    });
     if (total) *total = tot;
     if (rc != BVHGPU_OK) return rc;
     if (tot > cap) {
@@ -261,8 +288,6 @@ template <int D, class T> static int upload_records(Tree<T>* tree, Scratch& scra
     *d_out = d_lift;
     return BVHGPU_OK;
 }
-static const char* capacity_hint(int D) { return D == 3 ? "use bvhgpu_traverse_fetch_*" : "call again with cap = *total"; }
-
 template <class T, int D = 3>
 static int query_host_impl(Tree<T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || (n && !queries) || !offsets) { set_error("query: null argument"); return BVHGPU_ERR_INVALID; }
@@ -276,23 +301,9 @@ static int query_host_impl(Tree<T>* tree, int mode, int kind, const T* queries, 
     T* d_q = nullptr;
     Scratch scratch(ctx);                                           // released on every return path
     if (n) BVH_TRY(upload_records<D>(tree, scratch, queries, n, nvec, nscal, &d_q));
-    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 16 * n), 1024), tot = 0;
-    int rc = BVHGPU_OK;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        rc = ensure_result_buffers(tree, n, want);
-        if (rc != BVHGPU_OK) break;
-        rc = query_device<T>(tree, mode, kind, d_q, n, tree->d_offsets, tree->d_hits, tree->hits_cap, &tot);
-        if (rc == BVHGPU_ERR_CAPACITY && tot <= 0xFFFFFFFFull && attempt == 0) { want = tot; continue; }
-        break;
-    }
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
-    int ret = BVHGPU_OK;
-    if (hits && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
-    else if (tot > cap) { set_error("query: %zu hits do not fit the caller's capacity %zu (%s)", tot, cap, capacity_hint(D)); ret = BVHGPU_ERR_CAPACITY; }
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return ret;
+    return retained_to_host<D>(tree, "query", n, 16, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+        return query_device<T>(tree, mode, kind, d_q, n, d_off, d_hits, hcap, t);
+    });
 }
 
 template <class T, int D = 3>
@@ -329,23 +340,9 @@ static int nearest_candidates_host_impl(Tree<T>* tree, const T* points, size_t n
     T* d_p = nullptr;
     Scratch scratch(ctx);
     if (n) BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
-    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 16 * n), 1024), tot = 0;
-    int rc = BVHGPU_OK;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        rc = ensure_result_buffers(tree, n, want);
-        if (rc != BVHGPU_OK) break;
-        rc = nearest_candidates_device<T>(tree, d_p, n, tree->d_offsets, tree->d_hits, tree->hits_cap, &tot);
-        if (rc == BVHGPU_ERR_CAPACITY && tot <= 0xFFFFFFFFull && attempt == 0) { want = tot; continue; }
-        break;
-    }
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
-    int ret = BVHGPU_OK;
-    if (cand && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(cand, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
-    else if (tot > cap) { set_error("nearest_candidates: %zu candidates do not fit the caller's capacity %zu (%s)", tot, cap, capacity_hint(D)); ret = BVHGPU_ERR_CAPACITY; }
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return ret;
+    return retained_to_host<D>(tree, "nearest_candidates", n, 16, offsets, cand, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+        return nearest_candidates_device<T>(tree, d_p, n, d_off, d_hits, hcap, t);
+    });
 }
 
 template <class T>
@@ -558,23 +555,9 @@ static int traverse2_impl(Tree<T>* tree, int mode, const RAY2* rays, size_t nray
         BVH_CUDA_TRY(cudaMemcpyAsync(r6, rays, sizeof(RAY2) * nrays, cudaMemcpyHostToDevice, ctx->stream));
         BVH_TRY(dim2_expand_rays<T>(ctx, r6, (uint32_t)nrays, r9));
     }
-    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 4 * nrays), 1024), tot = 0;
-    int rc = BVHGPU_OK;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        rc = ensure_result_buffers(tree, nrays, want);
-        if (rc != BVHGPU_OK) break;
-        rc = traverse_device<T>(tree, mode, r9, BVHGPU_RAYS_FULL, nrays, tree->d_offsets, tree->d_hits, tree->hits_cap, &tot);
-        if (rc == BVHGPU_ERR_CAPACITY && tot <= 0xFFFFFFFFull && tot > tree->hits_cap && attempt == 0) { want = tot; continue; }
-        break;
-    }
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, ctx->stream));
-    int ret = BVHGPU_OK;
-    if (hits && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
-    else if (tot > cap) { set_error("traverse: %zu hits do not fit the caller's capacity %zu", tot, cap); ret = BVHGPU_ERR_CAPACITY; }
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return ret;
+    return retained_to_host<2>(tree, "traverse", nrays, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+        return traverse_device<T>(tree, mode, r9, BVHGPU_RAYS_FULL, nrays, d_off, d_hits, hcap, t);
+    });
 }
 
 // Bvh::update_shapes(changed_shape_indices, shapes): only the m changed shapes cross the boundary.  The tree is touched only after
@@ -1077,7 +1060,10 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
         /* query_device also serves the library's internal kinds (nearest_candidates): only the public ones get through here */ \
         if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; } \
         BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        return query_device<T>(tree, mode, kind, (const T*)dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+        const int rc = query_device<T>(tree, mode, kind, (const T*)dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+        /* with `total` given the call synchronises, and the CSR is complete when it returns */                         \
+        if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream)); \
+        return rc;                                                                                                        \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<T>(tree, mode, points, n, out_shape, out_dist);                                         \

@@ -1,0 +1,213 @@
+// bvh_b200/csrc/csr.cuh -- the two-pass CSR walk that every batched walk except the 3-D ray traversal produces its hit lists with:
+// the traversal records of D = 3 and D = 4 and their fetch, the record walk generic in D, the count / fill kernel, and the host
+// driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries and nearest_candidates, D = 2 through the z = 0 lift, the
+// ordered traversal) and dim4.cu (D = 4 rays, queries and nearest_candidates).  The 3-D ray kernels of traverse.cu use the same fetch.
+//
+// CSR: offsets[n + 1] (u32, saturated to 0xFFFFFFFF) and the hit list hits[total]; the fill pass stores hits[0 .. cap) only, so a
+// short `cap` leaves a prefix of the full list.
+#pragma once
+#include "internal.h"
+
+namespace bvhb200 {
+
+// ---- 4-D traversal record: the AABB the node has in its parent, `skip` (first record behind the subtree) and the shape index of a
+// leaf.  Sized in whole 16-byte granules so that a record is fetched with 128-bit non-coherent loads only: 3 for f32, 5 for f64.
+struct __align__(16) TRec4F { float min[4]; float max[4]; uint32_t skip, shape, pad[2]; };    // 48 B
+struct __align__(16) TRec4D { double min[4]; double max[4]; uint32_t skip, shape, pad[2]; };  // 80 B
+static_assert(sizeof(TRec4F) == 48 && sizeof(TRec4D) == 80, "4-D record size");
+
+// record and shape-box types of the walk in D (3: TNodeF / TNodeD and the padded device boxes; 4: TRec4F / TRec4D and the ABI boxes)
+template <int D, class T> struct CsrRecords;
+template <class T> struct CsrRecords<3, T> { using Rec = typename Traits<T>::TNode; using Box = typename Traits<T>::DAabb; };
+template <> struct CsrRecords<4, float> { using Rec = TRec4F; using Box = bvh_aabb4f; };
+template <> struct CsrRecords<4, double> { using Rec = TRec4D; using Box = bvh_aabb4d; };
+
+#ifdef __CUDACC__
+// ---- record fetch: 128-bit non-coherent loads (LDG.E.128, the widest global load sm_90a has) ------------
+// A divergent warp pays one L1 tag lookup ("wavefront") per distinct line per load instruction, and the ray
+// kernels are L1-wavefront bound, so a record is fetched with as few load instructions as the ISA allows:
+// two for a 32-byte f32 record, four for a 64-byte f64 record.
+__device__ __forceinline__ void fetch(const TNodeF* __restrict__ p, float mn[3], float mx[3], uint32_t& skip, uint32_t& shape) {
+    float sk, sh;
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mn[0]), "=f"(mn[1]), "=f"(mn[2]), "=f"(sk) : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mx[0]), "=f"(mx[1]), "=f"(mx[2]), "=f"(sh) : "l"(reinterpret_cast<const char*>(p) + 16));
+    skip = __float_as_uint(sk);
+    shape = __float_as_uint(sh);
+}
+__device__ __forceinline__ void fetch(const TNodeD* __restrict__ p, double mn[3], double mx[3], uint32_t& skip, uint32_t& shape) {
+    double links, pad;                         // {skip, shape} travel as the bits of the 7th double of the 64-byte record
+    const char* c = reinterpret_cast<const char*>(p);
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[0]), "=d"(mn[1]) : "l"(c));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[2]), "=d"(mx[0]) : "l"(c + 16));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[1]), "=d"(mx[2]) : "l"(c + 32));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(links), "=d"(pad) : "l"(c + 48));
+    const unsigned long long b = (unsigned long long)__double_as_longlong(links);
+    skip = (uint32_t)b; shape = (uint32_t)(b >> 32);
+}
+__device__ __forceinline__ void fetch(const TRec4F* p, float mn[4], float mx[4], uint32_t& skip, uint32_t& shape) {
+    uint32_t a, b, c, d;
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mn[0]), "=f"(mn[1]), "=f"(mn[2]), "=f"(mn[3]) : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mx[0]), "=f"(mx[1]), "=f"(mx[2]), "=f"(mx[3]) : "l"(reinterpret_cast<const char*>(p) + 16));
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "l"(reinterpret_cast<const char*>(p) + 32));
+    skip = a; shape = b;
+}
+__device__ __forceinline__ void fetch(const TRec4D* p, double mn[4], double mx[4], uint32_t& skip, uint32_t& shape) {
+    const char* c = reinterpret_cast<const char*>(p);
+    uint32_t a, b, x, y;
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[0]), "=d"(mn[1]) : "l"(c));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[2]), "=d"(mn[3]) : "l"(c + 16));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[0]), "=d"(mx[1]) : "l"(c + 32));
+    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[2]), "=d"(mx[3]) : "l"(c + 48));
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(x), "=r"(y) : "l"(c + 64));
+    skip = a; shape = b;
+}
+
+// ---- shape boxes: the padded 3-D device layout and the 4-D ABI layout (already whole sectors) ----
+__device__ __forceinline__ void load4(const bvh_aabb4f* p, float mn[4], float mx[4]) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+    mn[0] = a.x; mn[1] = a.y; mn[2] = a.z; mn[3] = a.w; mx[0] = b.x; mx[1] = b.y; mx[2] = b.z; mx[3] = b.w;
+}
+__device__ __forceinline__ void load4(const bvh_aabb4d* p, double mn[4], double mx[4]) {
+    const double2* q = reinterpret_cast<const double2*>(p);
+    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);
+    mn[0] = a.x; mn[1] = a.y; mn[2] = b.x; mn[3] = b.y; mx[0] = c.x; mx[1] = c.y; mx[2] = d.x; mx[3] = d.y;
+}
+__device__ __forceinline__ void load_box(const DAabbF* p, float mn[3], float mx[3]) { load_aabb(p, mn, mx); }
+__device__ __forceinline__ void load_box(const DAabbD* p, double mn[3], double mx[3]) { load_aabb(p, mn, mx); }
+__device__ __forceinline__ void load_box(const bvh_aabb4f* p, float mn[4], float mx[4]) { load4(p, mn, mx); }
+__device__ __forceinline__ void load_box(const bvh_aabb4d* p, double mn[4], double mx[4]) { load4(p, mn, mx); }
+
+// ---- the walk: stackless over the preorder records, hit -> next record, miss -> skip, so hits come out in the reference's
+// left-first DFS order.  `probe.hit(mn, mx)` is the predicate; `emit(shape)` is called for every reported shape. ----
+template <int D, class T, bool FLAT, class Rec, class Box, class Probe, class Emit>
+__device__ __forceinline__ void walk_records(const Rec* __restrict__ trec, uint32_t n_rec, const Box* __restrict__ aabb, const Probe& probe, Emit emit) {
+    uint32_t i = 0;
+    while (i < n_rec) {
+        T mn[D], mx[D];
+        uint32_t skip, shape;
+        fetch(trec + i, mn, mx, skip, shape);
+        if (probe.hit(mn, mx)) {
+            if (shape != BVH_INVALID) {
+                bool report = true;
+                if (FLAT) {                                    // flat_bvh.rs:412-416: a reached leaf re-tests the shape's AABB
+                    T smn[D], smx[D];
+                    load_box(aabb + shape, smn, smx);
+                    report = probe.hit(smn, smx);
+                }
+                if (report) emit(shape);
+            }
+            ++i;
+        } else {
+            i = skip;
+        }
+    }
+}
+
+// Count pass (FILL = false) and fill pass (FILL = true) over n items, one per thread.  A probe has load(src, r), which reads item r
+// of the batch, and hit(mn, mx).  The fill pass writes offsets[0 .. n] from the scan (saturated to 0xFFFFFFFF) and drops the hits
+// at positions >= cap.
+template <int D, class T, bool FLAT, bool FILL, class Probe>
+__global__ void __launch_bounds__(256) csr_walk_kernel(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                                       const typename CsrRecords<D, T>::Box* __restrict__ aabb,
+                                                       const void* __restrict__ src, uint32_t n, uint32_t* __restrict__ counts,
+                                                       const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
+                                                       const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits,
+                                                       unsigned long long cap) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (FILL && r == 0) { const unsigned long long t = *total; offsets[n] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
+    if (r >= n) return;
+    Probe probe;
+    probe.load(src, r);
+    if (!FILL) {
+        uint32_t cnt = 0;
+        walk_records<D, T, FLAT>(trec, n_rec, aabb, probe, [&](uint32_t) { ++cnt; });
+        counts[r] = cnt;
+    } else {
+        unsigned long long w = blocksum[r / CSR_SCAN_TILE] + local[r];
+        offsets[r] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
+        if (hits) walk_records<D, T, FLAT>(trec, n_rec, aabb, probe, [&](uint32_t shape) { if (w < cap) hits[w] = shape; ++w; });
+    }
+}
+
+// ---- host: count -> scan -> fill ----
+// A walk is what the driver launches: walk.count(stream, n, counts) enqueues the count pass, walk.fill(stream, n, local, sums, total,
+// offsets, hits, cap) the fill pass.  CsrWalk is the one of csr_walk_kernel; the ordered traversal has its own (traverse.cu).
+template <int D, class T, class Probe> struct CsrWalk {
+    bool flat;
+    const typename CsrRecords<D, T>::Rec* trec;
+    uint32_t n_rec;
+    const typename CsrRecords<D, T>::Box* aabb;       // the FLAT leaf re-test's shape boxes
+    const void* src;                                  // the batch, read by Probe::load
+    template <bool FILL> void launch(cudaStream_t st, uint32_t n, uint32_t* counts, const uint32_t* local, const unsigned long long* sums,
+                                     const unsigned long long* total, uint32_t* offsets, uint32_t* hits, size_t cap) const {
+        const unsigned grid = (n + 255) / 256;
+        if (flat) csr_walk_kernel<D, T, true, FILL, Probe><<<grid, 256, 0, st>>>(trec, n_rec, aabb, src, n, counts, local, sums, total, offsets, hits, (unsigned long long)cap);
+        else      csr_walk_kernel<D, T, false, FILL, Probe><<<grid, 256, 0, st>>>(trec, n_rec, aabb, src, n, counts, local, sums, total, offsets, hits, (unsigned long long)cap);
+    }
+    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const { launch<false>(st, n, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0); }
+    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
+              uint32_t* offsets, uint32_t* hits, size_t cap) const { launch<true>(st, n, nullptr, local, sums, total, offsets, hits, cap); }
+};
+
+// One CSR over n items (0 < n <= 2^31 - 1) on the context's stream, in two steps so that a caller can read the total between them.
+// count_and_scan: the count pass, then the shared scan (scan_local_kernel / scan_blocks_kernel) into local offsets, 64-bit block
+// offsets sums[0 .. nblk) and the total sums[nblk].  With read_total it also copies the total into the pinned word CSR_TOTAL_WORD
+// and records ctx->ev_total, so that total() waits for that copy only, not for a fill enqueued after it.  The scratch lives as long
+// as the object (released stream-ordered, after the fill).
+struct CsrPasses {
+    bvhgpu_ctx* ctx;
+    uint32_t n, nblk;
+    Scratch scratch;
+    uint32_t *counts = nullptr, *local = nullptr;
+    unsigned long long* sums = nullptr;
+
+    CsrPasses(bvhgpu_ctx* c, uint32_t items) : ctx(c), n(items), nblk((items + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE), scratch(c) {}
+    unsigned long long* pinned_total() const { return reinterpret_cast<unsigned long long*>(ctx->h_pinned + CSR_TOTAL_WORD); }
+
+    template <class Walk> int count_and_scan(const Walk& walk, bool read_total) {
+        cudaStream_t st = ctx->stream;
+        BVH_TRY(scratch.get(&counts, n));
+        BVH_TRY(scratch.get(&local, n));
+        BVH_TRY(scratch.get(&sums, (size_t)nblk + 1));
+        BVH_CUDA_TRY(cudaMemsetAsync(sums + nblk, 0, sizeof(unsigned long long), st));
+        walk.count(st, n, counts);
+        scan_local_kernel<<<nblk, CSR_SCAN_THREADS, 0, st>>>(counts, n, local, sums, nullptr);
+        scan_blocks_kernel<<<1, 1024, 0, st>>>(sums, nblk, sums + nblk);
+        ctx->launches += 3;
+        BVH_CUDA_TRY(cudaGetLastError());
+        if (read_total) {
+            BVH_CUDA_TRY(cudaMemcpyAsync(pinned_total(), sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            BVH_CUDA_TRY(cudaEventRecord(ctx->ev_total, st));
+        }
+        return BVHGPU_OK;
+    }
+    template <class Walk> int fill(const Walk& walk, uint32_t* offsets, uint32_t* hits, size_t cap) {
+        walk.fill(ctx->stream, n, local, sums, sums + nblk, offsets, hits, cap);
+        ctx->launches++;
+        BVH_CUDA_TRY(cudaGetLastError());
+        return BVHGPU_OK;
+    }
+    // Waits for the total (count_and_scan with read_total) and stores it in *out.  BVHGPU_ERR_CAPACITY when it overflows the u32
+    // offsets, or when hits != nullptr and it exceeds cap.  `what` names the entry point in the message.
+    int total(const char* what, const uint32_t* hits, size_t cap, size_t* out) const {
+        BVH_CUDA_TRY(cudaEventSynchronize(ctx->ev_total));
+        const unsigned long long t = *pinned_total();
+        *out = (size_t)t;
+        if (t > 0xFFFFFFFFull) { set_error("%s: %llu hits overflow the u32 CSR offsets", what, t); return BVHGPU_ERR_CAPACITY; }
+        if (hits && t > cap) { set_error("%s: %llu hits do not fit capacity %zu", what, t, cap); return BVHGPU_ERR_CAPACITY; }
+        return BVHGPU_OK;
+    }
+};
+
+// The whole CSR of a device-pointer call.  Without `total` nothing synchronises.  With it, the call waits for the total only (the
+// fill pass may still run when it returns) and returns CsrPasses::total's verdict.
+template <class Walk> int csr_two_pass(bvhgpu_ctx* ctx, const Walk& walk, uint32_t n, const char* what, uint32_t* offsets, uint32_t* hits,
+                                       size_t cap, size_t* total) {
+    CsrPasses passes(ctx, n);
+    BVH_TRY(passes.count_and_scan(walk, total != nullptr));
+    BVH_TRY(passes.fill(walk, offsets, hits, cap));
+    return total ? passes.total(what, hits, cap, total) : BVHGPU_OK;
+}
+#endif  // __CUDACC__
+
+}  // namespace bvhb200

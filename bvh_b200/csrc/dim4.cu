@@ -3,8 +3,8 @@
 // The reference is generic in D (src/bvh/bvh_node.rs:81-279, src/flat_bvh.rs:60-143, src/ray/intersect_default.rs:16-37) and ships
 // 4-wide slab tests for Ray<f32,4> / Ray<f64,4> (src/ray/intersect_simd.rs).  A fourth axis cannot hide in the 3-D kernels the way
 // D = 2 hides in z = 0 (dim2.cu): surface areas, largest_axis and the slab test all see it.  So D = 4 has its own pipeline here, with
-// its own node / record types and its own Tree4<T>; it shares the exact-arithmetic helpers and keys of common.cuh, Scratch, and the
-// CSR scan kernels of traverse.cu.  DESIGN.md section 4.11 describes the design.
+// its own node types and its own Tree4<T>; it shares the exact-arithmetic helpers and keys of common.cuh, Scratch, the records,
+// walk and count -> scan -> fill driver of csr.cuh, and the predicates of queries.cuh.  DESIGN.md section 4.11 describes the design.
 //
 // Builder (bit-identical to Bvh::build in the sense of DESIGN.md section 2):
 //   ranges of more than SMALL4 shapes: level-synchronous.  Per level: prep (tile numbering, bucket identities), bin (one warp per
@@ -16,6 +16,7 @@
 // Node positions depend only on counts (cl = me + 1, cr = me + 2 nl) and every reduction is a min / max / sum of integers, so the
 // order in which warps run never shows in the result: two builds of the same input are byte-identical.
 #include "internal.h"
+#include "csr.cuh"
 #include "queries.cuh"
 #include "update.cuh"
 #include <algorithm>
@@ -23,12 +24,7 @@
 
 namespace bvhb200 {
 
-// ---- device layouts -----------------------------------------------------------------------------------------------------------
-// Traversal record: the AABB the node has in its parent, `skip` (first record behind the subtree) and the shape index of a leaf.
-// Sized in whole 16-byte granules so that a record is fetched with 128-bit non-coherent loads only: 3 for f32, 5 for f64.
-struct __align__(16) TRec4F { float min[4]; float max[4]; uint32_t skip, shape, pad[2]; };    // 48 B
-struct __align__(16) TRec4D { double min[4]; double max[4]; uint32_t skip, shape, pad[2]; };  // 80 B
-static_assert(sizeof(TRec4F) == 48 && sizeof(TRec4D) == 80, "4-D record size");
+// ---- device layouts (the traversal records TRec4F / TRec4D are in csr.cuh) ------------------------------------------------------
 static_assert(sizeof(bvh_aabb4f) == 32 && sizeof(bvh_aabb4d) == 64 && sizeof(bvh_ray4f) == 48 && sizeof(bvh_ray4d) == 96, "4-D POD size");
 static_assert(sizeof(bvh_node4f) == 80 && sizeof(bvh_node4d) == 144 && sizeof(bvh_flat4f) == 44 && sizeof(bvh_flat4d) == 80, "4-D POD size");
 
@@ -538,23 +534,6 @@ __device__ __forceinline__ bool slab4(const T o[4], const T inv[4], const T mn[4
     const T tmax = min_t(min_t(hi[0], hi[1]), min_t(hi[2], hi[3]));
     return !nan && tmax >= (tmin > T(0) ? tmin : T(0));
 }
-__device__ __forceinline__ void fetch4(const TRec4F* p, float mn[4], float mx[4], uint32_t& skip, uint32_t& shape) {
-    uint32_t a, b, c, d;
-    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mn[0]), "=f"(mn[1]), "=f"(mn[2]), "=f"(mn[3]) : "l"(p));
-    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mx[0]), "=f"(mx[1]), "=f"(mx[2]), "=f"(mx[3]) : "l"(reinterpret_cast<const char*>(p) + 16));
-    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "l"(reinterpret_cast<const char*>(p) + 32));
-    skip = a; shape = b;
-}
-__device__ __forceinline__ void fetch4(const TRec4D* p, double mn[4], double mx[4], uint32_t& skip, uint32_t& shape) {
-    const char* c = reinterpret_cast<const char*>(p);
-    uint32_t a, b, x, y;
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[0]), "=d"(mn[1]) : "l"(c));
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[2]), "=d"(mn[3]) : "l"(c + 16));
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[0]), "=d"(mx[1]) : "l"(c + 32));
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[2]), "=d"(mx[3]) : "l"(c + 48));
-    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(x), "=r"(y) : "l"(c + 64));
-    skip = a; shape = b;
-}
 __device__ __forceinline__ void load_ray4(const bvh_ray4f* p, float o[4], float inv[4]) {
     const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 2);
     o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; inv[0] = b.x; inv[1] = b.y; inv[2] = b.z; inv[3] = b.w;
@@ -565,68 +544,13 @@ __device__ __forceinline__ void load_ray4(const bvh_ray4d* p, double o[4], doubl
     o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y; inv[0] = c.x; inv[1] = c.y; inv[2] = d.x; inv[3] = d.y;
 }
 
-// What one thread walks the records with: hit(mn, mx) is the predicate, load(src, r) reads item r of the batch.
-//   RayProbe4         the 4-wide slab test of a Ray<T,4>
-//   QueryProbe4<KIND> an Aabb / Point / Ball query (aabb_impl.rs:240-248, :175-177, ball.rs:85-99) or the internal QUERY_WITHIN
-//                     bound of nearest_candidates, with D = 4 (queries.cuh)
+// The probe of a ray batch for csr_walk_kernel (csr.cuh): load(src, r) reads ray r, hit(mn, mx) is the 4-wide slab test.  Queries
+// use Query<T, KIND, 4> of queries.cuh directly.
 template <class T> struct RayProbe4 {
     T o[4], inv[4];
     __device__ __forceinline__ void load(const void* src, uint32_t r) { load_ray4(reinterpret_cast<const typename D4<T>::Ray*>(src) + r, o, inv); }
     __device__ __forceinline__ bool hit(const T mn[4], const T mx[4]) const { return slab4(o, inv, mn, mx); }
 };
-template <class T, int KIND> struct QueryProbe4 : Query<T, KIND, 4> {
-    __device__ __forceinline__ void load(const void* src, uint32_t r) {
-        Query<T, KIND, 4>::load(reinterpret_cast<const T*>(src) + (size_t)r * Query<T, KIND, 4>::STRIDE);
-    }
-};
-
-template <class T, bool FLAT, class P, class Emit>
-__device__ __forceinline__ void walk4(const typename D4<T>::Rec* __restrict__ trec, uint32_t n_rec, const typename D4<T>::Aabb* __restrict__ aabb,
-                                      const P& probe, Emit emit) {
-    uint32_t i = 0;
-    while (i < n_rec) {
-        T mn[4], mx[4];
-        uint32_t skip, shape;
-        fetch4(trec + i, mn, mx, skip, shape);
-        if (probe.hit(mn, mx)) {
-            if (shape != BVH_INVALID) {
-                bool report = true;
-                if (FLAT) {                                    // flat_bvh.rs:412-416: a reached leaf re-tests the shape's AABB
-                    T smn[4], smx[4];
-                    load4(aabb + shape, smn, smx);
-                    report = probe.hit(smn, smx);
-                }
-                if (report) emit(shape);
-            }
-            ++i;
-        } else {
-            i = skip;
-        }
-    }
-}
-
-// count pass (FILL = false) and fill pass (FILL = true) for a batch of n items of probe P; hits beyond cap are dropped
-template <class T, bool FLAT, bool FILL, class P>
-__global__ void __launch_bounds__(256) walk4_kernel(const typename D4<T>::Rec* __restrict__ trec, uint32_t n_rec, const typename D4<T>::Aabb* __restrict__ aabb,
-                                                    const void* __restrict__ src, uint32_t n, uint32_t* __restrict__ counts,
-                                                    const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
-                                                    const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits,
-                                                    unsigned long long cap) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (FILL && r == 0) { const unsigned long long t = *total; offsets[n] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
-    if (r >= n) return;
-    P probe;
-    probe.load(src, r);
-    if (!FILL) {
-        uint32_t cnt = 0;
-        walk4<T, FLAT>(trec, n_rec, aabb, probe, [&](uint32_t) { ++cnt; });
-        counts[r] = cnt;
-    } else {
-        unsigned long long w = blocksum[r / CSR_SCAN_TILE] + local[r];
-        offsets[r] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
-        if (hits) walk4<T, FLAT>(trec, n_rec, aabb, probe, [&](uint32_t shape) { if (w < cap) hits[w] = shape; ++w; });
-    }
-}
 
 // ---- nearest_to: the walks of queries.cuh over the 4-D nodes / flat array; the leaf value is the shape AABB's distance ----
 template <class T, bool FLAT>
@@ -969,37 +893,13 @@ template <class T> static int flatten4_impl(Tree4<T>* tree, typename D4<T>::Flat
     return BVHGPU_OK;
 }
 
-// Count pass + scan on the stream; leaves the 64-bit total at sums[nblk].  Needs tree->n > 0 and R > 0.  src: R items of probe P.
-template <class P, class T> static int count_and_scan4(Tree4<T>* tree, bool flat, const void* d_src, uint32_t R, Scratch& scratch,
-                                                       uint32_t** counts, uint32_t** local, unsigned long long** sums) {
+// The traversal records of the two-pass walks, built on first use.
+template <class T> static int ensure_trec4(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    if (!tree->d_trec) {
-        tree->n_trec = tree->n == 1 ? 1u : tree->n_nodes - 1;
-        BVH_TRY(dalloc_t(ctx, &tree->d_trec, tree->n_trec));
-        trec4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, st>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec);
-        LAUNCHED(ctx, 1);
-    }
-    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
-    BVH_TRY(scratch.get(counts, R));
-    BVH_TRY(scratch.get(local, R));
-    BVH_TRY(scratch.get(sums, (size_t)nblk + 1));
-    BVH_CUDA_TRY(cudaMemsetAsync(*sums + nblk, 0, sizeof(unsigned long long), st));
-    const int grid = (R + 255) / 256;
-    if (flat) walk4_kernel<T, true, false, P><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    else      walk4_kernel<T, false, false, P><<<grid, 256, 0, st>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, *counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    scan_local_kernel<<<nblk, CSR_SCAN_THREADS, 0, st>>>(*counts, R, *local, *sums, nullptr);
-    scan_blocks_kernel<<<1, 1024, 0, st>>>(*sums, nblk, *sums + nblk);
-    LAUNCHED(ctx, 3);
-    return BVHGPU_OK;
-}
-template <class P, class T> static int fill4(Tree4<T>* tree, bool flat, const void* d_src, uint32_t R, const uint32_t* local,
-                                             const unsigned long long* sums, uint32_t* d_offsets, uint32_t* d_hits, size_t cap) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
-    const int grid = (R + 255) / 256;
-    if (flat) walk4_kernel<T, true, true, P><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
-    else      walk4_kernel<T, false, true, P><<<grid, 256, 0, ctx->stream>>>(tree->d_trec, tree->n_trec, tree->d_aabb, d_src, R, nullptr, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
+    if (tree->d_trec) return BVHGPU_OK;
+    tree->n_trec = tree->n == 1 ? 1u : tree->n_nodes - 1;
+    BVH_TRY(dalloc_t(ctx, &tree->d_trec, tree->n_trec));
+    trec4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec);
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
 }
@@ -1026,24 +926,9 @@ template <class P, class T> static int csr4_dev(Tree4<T>* tree, bool flat, const
         if (total) *total = 0;
         return BVHGPU_OK;
     }
-    const uint32_t R = (uint32_t)n;
-    Scratch scratch(ctx);
-    uint32_t *counts = nullptr, *local = nullptr;
-    unsigned long long* sums = nullptr;
-    BVH_TRY(count_and_scan4<P>(tree, flat, d_src, R, scratch, &counts, &local, &sums));
-    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
-    unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned + 236);
-    if (total) {                                                   // the total is known before the hit lists are written
-        BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaEventRecord(ctx->ev_total, st));
-    }
-    BVH_TRY(fill4<P>(tree, flat, d_src, R, local, sums, d_offsets, d_hits, cap));
-    if (!total) return BVHGPU_OK;
-    BVH_CUDA_TRY(cudaEventSynchronize(ctx->ev_total));
-    *total = (size_t)*h;
-    if (*h > 0xFFFFFFFFull) { set_error("%s: %llu hits overflow the u32 CSR offsets", what, *h); return BVHGPU_ERR_CAPACITY; }
-    if (d_hits && *h > cap) { set_error("%s: %llu hits do not fit capacity %zu", what, *h, cap); return BVHGPU_ERR_CAPACITY; }
-    return BVHGPU_OK;
+    BVH_TRY(ensure_trec4(tree));
+    const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
+    return csr_two_pass(ctx, walk, (uint32_t)n, what, d_offsets, d_hits, cap, total);
 }
 
 // Host CSR out of a batch already on the device (d_src, n > 0, tree->n > 0): count, read the total, size the retained hit buffer
@@ -1053,18 +938,14 @@ template <class P, class T> static int csr4_host(Tree4<T>* tree, bool flat, cons
                                                  size_t cap, size_t* total, const char* what) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
-    const uint32_t R = (uint32_t)n;
-    Scratch scratch(ctx);
-    uint32_t *counts = nullptr, *local = nullptr;
-    unsigned long long* sums = nullptr;
-    BVH_TRY(count_and_scan4<P>(tree, flat, d_src, R, scratch, &counts, &local, &sums));
-    const uint32_t nblk = (R + CSR_SCAN_TILE - 1) / CSR_SCAN_TILE;
-    unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned + 236);
-    BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    const unsigned long long tot = *h;
-    if (total) *total = (size_t)tot;
-    if (tot > 0xFFFFFFFFull) { set_error("%s: %llu hits overflow the u32 CSR offsets", what, tot); return BVHGPU_ERR_CAPACITY; }
+    BVH_TRY(ensure_trec4(tree));
+    const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
+    CsrPasses passes(ctx, (uint32_t)n);
+    BVH_TRY(passes.count_and_scan(walk, true));
+    size_t tot = 0;
+    const int rc = passes.total(what, nullptr, 0, &tot);
+    if (total) *total = tot;
+    if (rc != BVHGPU_OK) return rc;
     if (tree->offsets_cap < n + 1) {
         dfree(ctx, tree->d_offsets); tree->d_offsets = nullptr; tree->offsets_cap = 0;
         BVH_TRY(dalloc_t(ctx, &tree->d_offsets, n + 1));
@@ -1076,11 +957,11 @@ template <class P, class T> static int csr4_host(Tree4<T>* tree, bool flat, cons
         BVH_TRY(dalloc_t(ctx, &tree->d_hits, tot));
         tree->hits_cap = tot;
     }
-    BVH_TRY(fill4<P>(tree, flat, d_src, R, local, sums, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
+    BVH_TRY(passes.fill(walk, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
     BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
     if (fits && tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (tot > cap) { set_error("%s: %llu hits do not fit the caller's capacity %zu (call again with cap = *total)", what, tot, cap); return BVHGPU_ERR_CAPACITY; }
+    if (tot > cap) { set_error("%s: %zu hits do not fit the caller's capacity %zu (call again with cap = *total)", what, tot, cap); return BVHGPU_ERR_CAPACITY; }
     return BVHGPU_OK;
 }
 
@@ -1126,9 +1007,9 @@ template <class T> static int query4_dev_impl(Tree4<T>* tree, int mode, int kind
     BVH_TRY(check_batch_args(tree, mode, n, "query_dev"));
     BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
     const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    const int rc = kind == BVHGPU_QUERY_AABB  ? csr4_dev<QueryProbe4<T, BVHGPU_QUERY_AABB>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
-                 : kind == BVHGPU_QUERY_POINT ? csr4_dev<QueryProbe4<T, BVHGPU_QUERY_POINT>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
-                                              : csr4_dev<QueryProbe4<T, BVHGPU_QUERY_BALL>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev");
+    const int rc = kind == BVHGPU_QUERY_AABB  ? csr4_dev<Query<T, BVHGPU_QUERY_AABB, 4>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
+                 : kind == BVHGPU_QUERY_POINT ? csr4_dev<Query<T, BVHGPU_QUERY_POINT, 4>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
+                                              : csr4_dev<Query<T, BVHGPU_QUERY_BALL, 4>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev");
     // as bvhgpu_query_dev_f32x3: with `total` given the call synchronises, and the CSR is complete when it returns
     if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
     return rc;
@@ -1149,9 +1030,9 @@ template <class T> static int query4_host_impl(Tree4<T>* tree, int mode, int kin
     void* d_q = nullptr;
     BVH_TRY(upload4(ctx, scratch, queries, sizeof(T) * query_stride4<T>(kind) * n, &d_q));
     const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    return kind == BVHGPU_QUERY_AABB  ? csr4_host<QueryProbe4<T, BVHGPU_QUERY_AABB>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
-         : kind == BVHGPU_QUERY_POINT ? csr4_host<QueryProbe4<T, BVHGPU_QUERY_POINT>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
-                                      : csr4_host<QueryProbe4<T, BVHGPU_QUERY_BALL>>(tree, flat, d_q, n, offsets, hits, cap, total, "query");
+    return kind == BVHGPU_QUERY_AABB  ? csr4_host<Query<T, BVHGPU_QUERY_AABB, 4>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
+         : kind == BVHGPU_QUERY_POINT ? csr4_host<Query<T, BVHGPU_QUERY_POINT, 4>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
+                                      : csr4_host<Query<T, BVHGPU_QUERY_BALL, 4>>(tree, flat, d_q, n, offsets, hits, cap, total, "query");
 }
 
 // ---- nearest_to: 4 T per point ----
@@ -1205,7 +1086,7 @@ template <class T> static int nearest_candidates4_host_impl(Tree4<T>* tree, cons
     BVH_TRY(scratch.get(&rec, 5 * n));
     nearest_bound4_kernel<T><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, (const T*)d_p, (uint32_t)n, rec);
     LAUNCHED(ctx, 1);
-    return csr4_host<QueryProbe4<T, QUERY_WITHIN>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
+    return csr4_host<Query<T, QUERY_WITHIN, 4>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
 }
 
 // ---- refit / update_shapes ----

@@ -50,7 +50,10 @@ struct bvhgpu_ctx {
     int64_t build_gang = -1;       // exact builder: co-resident warp gangs for the top levels (-1 / 1 on, 0 off = queue tiles only)
     int64_t build_subtree = -1;    // exact builder: in-register subtrees for ranges <= 32 shapes (-1 auto, 0 never, 1 always)
     int64_t build_small = -1;      // exact builder: defer ranges <= 16 shapes to the thread-per-range kernel (-1 auto by size, 0 never, 1 always)
-    uint32_t* h_pinned = nullptr;  // small pinned read-back area (256 words)
+    // small pinned read-back area (256 words): 0-25 the ray traversal's scan tail, 64-79 the streamed path's per-chunk values,
+    // 128-129 the stream probe, 200-221 the capi / dynamic checks, 232-235 the 4-D build, CSR_TOTAL_WORD (236-237) the total of
+    // the two-pass CSR walks (csr.cuh), 240-248 the 4-D update checks
+    uint32_t* h_pinned = nullptr;
     int64_t profile = 0;           // bracket dominant kernels with events
     cudaEvent_t ev_walk[2] = {nullptr, nullptr};
     cudaEvent_t ev_build[2] = {nullptr, nullptr};
@@ -203,11 +206,13 @@ template <class T> int query_device(Tree<T>* tree, int mode, int kind, const T* 
 // nearest_to for a batch of points (device pointers): exact reference walk for AABB-distance shapes; candidate lists for any shape
 template <class T> int nearest_device(Tree<T>* tree, int mode, const T* d_points, size_t nq, uint32_t* d_shape, T* d_dist, int use_triangles = 0);
 template <class T> int nearest_candidates_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t* d_offsets, uint32_t* d_cand, size_t cap, size_t* total);
-// CSR scan of per-ray counts (traverse.cu), shared with dim4.cu: scan_local_kernel runs CSR_SCAN_THREADS threads per block over
-// CSR_SCAN_TILE counts and leaves local exclusive offsets and block totals; scan_blocks_kernel (one block of 1024 threads) turns the
-// block totals into exclusive 64-bit block offsets and adds the grand total to *total (zeroed by the caller).
+// CSR scan of per-item counts (traverse.cu), launched by the count -> scan -> fill driver of csr.cuh (CsrPasses) for every two-pass
+// walk: scan_local_kernel runs CSR_SCAN_THREADS threads per block over CSR_SCAN_TILE counts and leaves local exclusive offsets and
+// block totals; scan_blocks_kernel (one block of 1024 threads) turns the block totals into exclusive 64-bit block offsets and adds the
+// grand total to *total (zeroed by the caller).
 constexpr int CSR_SCAN_THREADS = 256;
 constexpr int CSR_SCAN_TILE = 2048;
+constexpr int CSR_TOTAL_WORD = 236;        // h_pinned word (8-byte aligned) of the two-pass total
 __global__ void __launch_bounds__(256) scan_local_kernel(const uint32_t* __restrict__ counts, uint32_t n, uint32_t* __restrict__ local,
                                                          unsigned long long* __restrict__ blocksum, uint32_t* __restrict__ maxcount);
 __global__ void __launch_bounds__(1024) scan_blocks_kernel(unsigned long long* __restrict__ blocksum, uint32_t nblocks, unsigned long long* __restrict__ total);

@@ -8,12 +8,13 @@ namespace bvhb200 {
 
 #ifdef __CUDACC__
 // ---- query records: Aabb {min, max} (2D T), Point (D T), Ball {center, radius} (D + 1 T) (src/aabb/intersection.rs:35-45,
-// src/ball.rs:85-106) ----
+// src/ball.rs:85-106).  Each is a probe of csr_walk_kernel (csr.cuh): load(src, r) reads record r of the batch at src,
+// hit(mn, mx) is the predicate. ----
 template <class T, int KIND, int D> struct Query;
 template <class T, int D> struct Query<T, BVHGPU_QUERY_AABB, D> {
     T mn[D], mx[D];
-    __device__ __forceinline__ void load(const T* p) { for (int k = 0; k < D; ++k) { mn[k] = __ldg(p + k); mx[k] = __ldg(p + D + k); } }
     static constexpr int STRIDE = 2 * D;
+    __device__ __forceinline__ void load(const void* src, uint32_t r) { const T* p = static_cast<const T*>(src) + (size_t)r * STRIDE; for (int k = 0; k < D; ++k) { mn[k] = __ldg(p + k); mx[k] = __ldg(p + D + k); } }
     __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {            // aabb_impl.rs:240-248
         bool h = true;
 #pragma unroll
@@ -23,8 +24,8 @@ template <class T, int D> struct Query<T, BVHGPU_QUERY_AABB, D> {
 };
 template <class T, int D> struct Query<T, BVHGPU_QUERY_POINT, D> {
     T p[D];
-    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < D; ++k) p[k] = __ldg(q + k); }
     static constexpr int STRIDE = D;
+    __device__ __forceinline__ void load(const void* src, uint32_t r) { const T* q = static_cast<const T*>(src) + (size_t)r * STRIDE; for (int k = 0; k < D; ++k) p[k] = __ldg(q + k); }
     __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {            // Aabb::contains, aabb_impl.rs:175-177
         bool h = true;
 #pragma unroll
@@ -34,8 +35,8 @@ template <class T, int D> struct Query<T, BVHGPU_QUERY_POINT, D> {
 };
 template <class T, int D> struct Query<T, BVHGPU_QUERY_BALL, D> {
     T c[D], r2;
-    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < D; ++k) c[k] = __ldg(q + k); const T r = __ldg(q + D); r2 = mul_rn(r, r); }
     static constexpr int STRIDE = D + 1;
+    __device__ __forceinline__ void load(const void* src, uint32_t r) { const T* q = static_cast<const T*>(src) + (size_t)r * STRIDE; for (int k = 0; k < D; ++k) c[k] = __ldg(q + k); const T rad = __ldg(q + D); r2 = mul_rn(rad, rad); }
     __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {            // Ball::intersects_aabb, ball.rs:85-99
         T d2 = T(0);
 #pragma unroll
@@ -116,8 +117,8 @@ template <int D, class T, class Node> __device__ __forceinline__ void root_magni
 }
 template <class T, int D> struct Query<T, QUERY_WITHIN, D> {
     T p[D], u;
-    __device__ __forceinline__ void load(const T* q) { for (int k = 0; k < D; ++k) p[k] = __ldg(q + k); u = __ldg(q + D); }
     static constexpr int STRIDE = D + 1;
+    __device__ __forceinline__ void load(const void* src, uint32_t r) { const T* q = static_cast<const T*>(src) + (size_t)r * STRIDE; for (int k = 0; k < D; ++k) p[k] = __ldg(q + k); u = __ldg(q + D); }
     __device__ __forceinline__ bool hit(const T bmn[D], const T bmx[D]) const {
         bool empty = false;
 #pragma unroll

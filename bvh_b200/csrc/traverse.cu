@@ -12,6 +12,7 @@
 // them; an exclusive scan turns counts into offsets; the emit kernel copies the slots into place and
 // re-walks only rays with more than K hits.  K = 0 degenerates to the classic count / scan / fill.
 #include "internal.h"
+#include "csr.cuh"
 #include "queries.cuh"
 #include <cstdlib>
 #include <cstring>
@@ -70,28 +71,6 @@ __device__ __forceinline__ bool slab_hit(const T o[3], const T inv[3], const T m
     const T tmax = tmin2(tmin2(tmax2(l0, r0), tmax2(l1, r1)), tmax2(l2, r2));
     const T lo = tmin > T(0) ? tmin : T(0);                     // fast_max(tmin, 0), utils.rs:52-54
     return !nan && tmax >= lo;                                  // :35
-}
-
-// ---- record fetch: 128-bit non-coherent loads (LDG.E.128, the widest global load sm_90a has) ------------
-// A divergent warp pays one L1 tag lookup ("wavefront") per distinct line per load instruction, and this
-// kernel is L1-wavefront bound, so a record is fetched with as few load instructions as the ISA allows:
-// two for a 32-byte f32 record, four for a 64-byte f64 record.
-__device__ __forceinline__ void fetch(const TNodeF* __restrict__ p, float mn[3], float mx[3], uint32_t& skip, uint32_t& shape) {
-    float sk, sh;
-    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mn[0]), "=f"(mn[1]), "=f"(mn[2]), "=f"(sk) : "l"(p));
-    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(mx[0]), "=f"(mx[1]), "=f"(mx[2]), "=f"(sh) : "l"(reinterpret_cast<const char*>(p) + 16));
-    skip = __float_as_uint(sk);
-    shape = __float_as_uint(sh);
-}
-__device__ __forceinline__ void fetch(const TNodeD* __restrict__ p, double mn[3], double mx[3], uint32_t& skip, uint32_t& shape) {
-    double links, pad;                         // {skip, shape} travel as the bits of the 7th double of the 64-byte record
-    const char* c = reinterpret_cast<const char*>(p);
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[0]), "=d"(mn[1]) : "l"(c));
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mn[2]), "=d"(mx[0]) : "l"(c + 16));
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(mx[1]), "=d"(mx[2]) : "l"(c + 32));
-    asm volatile("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(links), "=d"(pad) : "l"(c + 48));
-    const unsigned long long b = (unsigned long long)__double_as_longlong(links);
-    skip = (uint32_t)b; shape = (uint32_t)(b >> 32);
 }
 
 // The walk.  `emit(shape)` is called for every reported shape in reference order.
@@ -1314,64 +1293,11 @@ template int traverse_host_pipelined<float>(Tree<float>*, int, const void*, uint
 template int traverse_host_pipelined<double>(Tree<double>*, int, const void*, uint32_t, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 
 // ---- the other IntersectsAabb implementors: Aabb, Point, Ball (src/aabb/intersection.rs:35-45, src/ball.rs:85-106) ----
-// Same stackless walk, another predicate (queries.cuh).
-
-template <class T, int KIND, bool FLAT, class Emit>
-__device__ __forceinline__ void walk_query(const typename Traits<T>::TNode* __restrict__ trec, uint32_t n_rec,
-                                           const typename Traits<T>::DAabb* __restrict__ aabb, const Query<T, KIND, 3>& q, Emit emit) {
-    uint32_t i = 0;
-    while (i < n_rec) {
-        T mn[3], mx[3];
-        uint32_t skip, shape;
-        fetch(trec + i, mn, mx, skip, shape);
-        if (q.hit(mn, mx)) {
-            if (shape != BVH_INVALID) {
-                bool report = true;
-                if (FLAT) { T smn[3], smx[3]; load_aabb(aabb + shape, smn, smx); report = q.hit(smn, smx); }
-                if (report) emit(shape);
-            }
-            i = i + 1;
-        } else i = skip;
-    }
-}
-
-// count pass (FILL = false) and fill pass (FILL = true) of the classic two-pass scheme: query batches are small
-template <class T, int KIND, bool FLAT, bool FILL>
-__global__ void __launch_bounds__(256) query_kernel(const typename Traits<T>::TNode* __restrict__ trec, uint32_t n_rec,
-                                                    const typename Traits<T>::DAabb* __restrict__ aabb, const T* __restrict__ queries, uint32_t nq,
-                                                    uint32_t* __restrict__ counts, const uint32_t* __restrict__ local,
-                                                    const unsigned long long* __restrict__ blocksum, const unsigned long long* __restrict__ total,
-                                                    uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits, unsigned long long cap) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (FILL && r == 0) { const unsigned long long t = *total; offsets[nq] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
-    if (r >= nq) return;
-    Query<T, KIND, 3> q;
-    q.load(queries + (size_t)r * Query<T, KIND, 3>::STRIDE);
-    if (!FILL) {
-        uint32_t cnt = 0;
-        walk_query<T, KIND, FLAT>(trec, n_rec, aabb, q, [&](uint32_t) { ++cnt; });
-        counts[r] = cnt;
-    } else {
-        unsigned long long w = blocksum[r / SCAN_TILE] + local[r];
-        offsets[r] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
-        if (hits) walk_query<T, KIND, FLAT>(trec, n_rec, aabb, q, [&](uint32_t shape) { if (w < cap) hits[w] = shape; ++w; });
-    }
-}
-
+// The two-pass walk of csr.cuh with the predicates of queries.cuh; query batches are small.
 template <class T, int KIND>
-static int query_launch(Tree<T>* tree, bool flat, const T* d_queries, uint32_t nq, uint32_t* counts, uint32_t* local,
-                        unsigned long long* sums, uint32_t nblk, uint32_t* d_offsets, uint32_t* d_hits, size_t cap) {
-    cudaStream_t st = tree->ctx->stream;
-    const int grid = (nq + 255) / 256;
-    if (flat) query_kernel<T, KIND, true, false><<<grid, 256, 0, st>>>(tree->d_tnodes, tree->n_trec, walk_aabbs(tree), d_queries, nq, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    else      query_kernel<T, KIND, false, false><<<grid, 256, 0, st>>>(tree->d_tnodes, tree->n_trec, walk_aabbs(tree), d_queries, nq, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    scan_local_kernel<<<nblk, SCAN_THREADS, 0, st>>>(counts, nq, local, sums, nullptr);
-    scan_blocks_kernel<<<1, 1024, 0, st>>>(sums, nblk, sums + nblk);
-    if (flat) query_kernel<T, KIND, true, true><<<grid, 256, 0, st>>>(tree->d_tnodes, tree->n_trec, walk_aabbs(tree), d_queries, nq, counts, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
-    else      query_kernel<T, KIND, false, true><<<grid, 256, 0, st>>>(tree->d_tnodes, tree->n_trec, walk_aabbs(tree), d_queries, nq, counts, local, sums, sums + nblk, d_offsets, d_hits, (unsigned long long)cap);
-    tree->ctx->launches += 4;
-    BVH_CUDA_TRY(cudaGetLastError());
-    return BVHGPU_OK;
+static int query_passes(Tree<T>* tree, bool flat, const T* d_queries, uint32_t nq, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
+    const CsrWalk<3, T, Query<T, KIND, 3>> walk{flat, tree->d_tnodes, tree->n_trec, walk_aabbs(tree), d_queries};
+    return csr_two_pass(tree->ctx, walk, nq, "query", d_offsets, d_hits, cap, total);
 }
 
 template <class T>
@@ -1389,27 +1315,13 @@ int query_device(Tree<T>* tree, int mode, int kind, const T* d_queries, size_t n
     }
     BVH_TRY(resolve_status(tree));
     if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
-    const uint32_t R = (uint32_t)nq, nblk = (R + SCAN_TILE - 1) / SCAN_TILE;
-    uint32_t *counts = nullptr, *local = nullptr;
-    unsigned long long* sums = nullptr;
-    Scratch scratch(ctx);                                      // released on every return path
-    BVH_TRY(scratch.get(&counts, R));
-    BVH_TRY(scratch.get(&local, R));
-    BVH_TRY(scratch.get(&sums, (size_t)nblk + 2));
-    BVH_CUDA_TRY(cudaMemsetAsync(sums + nblk, 0, 2 * sizeof(unsigned long long), st));
+    const uint32_t R = (uint32_t)nq;
     const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    int rc = kind == BVHGPU_QUERY_AABB  ? query_launch<T, BVHGPU_QUERY_AABB>(tree, flat, d_queries, R, counts, local, sums, nblk, d_offsets, d_hits, cap)
-           : kind == BVHGPU_QUERY_POINT ? query_launch<T, BVHGPU_QUERY_POINT>(tree, flat, d_queries, R, counts, local, sums, nblk, d_offsets, d_hits, cap)
-           : kind == BVHGPU_QUERY_BALL  ? query_launch<T, BVHGPU_QUERY_BALL>(tree, flat, d_queries, R, counts, local, sums, nblk, d_offsets, d_hits, cap)
-                                        : query_launch<T, QUERY_WITHIN>(tree, flat, d_queries, R, counts, local, sums, nblk, d_offsets, d_hits, cap);
-    if (rc == BVHGPU_OK && total) {
-        unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned);
-        BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaStreamSynchronize(st));
-        *total = (size_t)h[0];
-        tree->last_total = (size_t)h[0];
-        if (h[0] > 0xFFFFFFFFull || (d_hits && h[0] > cap)) { set_error("query: %llu hits do not fit capacity %zu", h[0], cap); rc = BVHGPU_ERR_CAPACITY; }
-    }
+    const int rc = kind == BVHGPU_QUERY_AABB  ? query_passes<T, BVHGPU_QUERY_AABB>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total)
+                 : kind == BVHGPU_QUERY_POINT ? query_passes<T, BVHGPU_QUERY_POINT>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total)
+                 : kind == BVHGPU_QUERY_BALL  ? query_passes<T, BVHGPU_QUERY_BALL>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total)
+                                              : query_passes<T, QUERY_WITHIN>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total);
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) tree->last_total = *total;
     return rc;
 }
 template int query_device<float>(Tree<float>*, int, int, const float*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
@@ -1615,6 +1527,22 @@ __global__ void __launch_bounds__(256) ordered_kernel(const typename Traits<T>::
     }
 }
 
+// the two passes of ordered_kernel, launched by the driver of csr.cuh
+template <class T> struct OrderedWalk {
+    const typename Traits<T>::TNode* trec;
+    uint32_t n_rec;
+    const typename Traits<T>::Ray* rays;
+    int ascending;
+    T* dists;
+    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const {
+        ordered_kernel<T, false><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    }
+    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
+              uint32_t* offsets, uint32_t* hits, size_t cap) const {
+        ordered_kernel<T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, nullptr, local, sums, total, offsets, hits, dists, (unsigned long long)cap);
+    }
+};
+
 template <class T>
 int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays, size_t nrays, int ascending,
                             uint32_t* d_offsets, uint32_t* d_hits, T* d_dists, size_t cap, size_t* total) {
@@ -1628,30 +1556,8 @@ int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays
     }
     BVH_TRY(resolve_status(tree));
     if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
-    const uint32_t R = (uint32_t)nrays, nblk = (R + SCAN_TILE - 1) / SCAN_TILE;
-    uint32_t *counts = nullptr, *local = nullptr;
-    unsigned long long* sums = nullptr;
-    Scratch scratch(ctx);
-    BVH_TRY(scratch.get(&counts, R));
-    BVH_TRY(scratch.get(&local, R));
-    BVH_TRY(scratch.get(&sums, (size_t)nblk + 2));
-    BVH_CUDA_TRY(cudaMemsetAsync(sums + nblk, 0, 2 * sizeof(unsigned long long), st));
-    const int grid = (R + 255) / 256;
-    ordered_kernel<T, false><<<grid, 256, 0, st>>>(tree->d_tnodes, tree->n_trec, d_rays, R, ascending, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    scan_local_kernel<<<nblk, SCAN_THREADS, 0, st>>>(counts, R, local, sums, nullptr);
-    scan_blocks_kernel<<<1, 1024, 0, st>>>(sums, nblk, sums + nblk);
-    ordered_kernel<T, true><<<grid, 256, 0, st>>>(tree->d_tnodes, tree->n_trec, d_rays, R, ascending, counts, local, sums, sums + nblk, d_offsets, d_hits, d_dists, (unsigned long long)cap);
-    ctx->launches += 4;
-    BVH_CUDA_TRY(cudaGetLastError());
-    int rc = BVHGPU_OK;
-    if (total) {
-        unsigned long long* h = reinterpret_cast<unsigned long long*>(ctx->h_pinned);
-        BVH_CUDA_TRY(cudaMemcpyAsync(h, sums + nblk, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaStreamSynchronize(st));
-        *total = (size_t)h[0];
-        if (h[0] > 0xFFFFFFFFull || h[0] > cap) { set_error("traverse_ordered: %llu hits do not fit capacity %zu", h[0], cap); rc = BVHGPU_ERR_CAPACITY; }
-    }
-    return rc;
+    const OrderedWalk<T> walk{tree->d_tnodes, tree->n_trec, d_rays, ascending, d_dists};
+    return csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_offsets, d_hits, cap, total);
 }
 template int traverse_ordered_device<float>(Tree<float>*, const bvh_ray3f*, size_t, int, uint32_t*, uint32_t*, float*, size_t, size_t*);
 template int traverse_ordered_device<double>(Tree<double>*, const bvh_ray3d*, size_t, int, uint32_t*, uint32_t*, double*, size_t, size_t*);

@@ -2,27 +2,17 @@
 // D = 3 (flatten.cu, and D = 2 through the z = 0 embedding of dim2.cu) and D = 4 (dim4.cu) share.
 //
 // Every node POD starts with the same 16 bytes {parent, child_l, child_r, shape}, so the kernels that only follow links are
-// templated on the node type.  The kernels that touch boxes are templated on D as well: they load a shape box with load_box (the
-// padded 3-D device layout or the 4-D ABI layout) and take surface areas with surface_area_d<D>, which is the 3-D surface_area for
-// D = 3 and surface_area4 for D = 4.  Both sum the squared extents left to right without FMA, so the D = 3 instantiations perform
-// exactly the operations the 3-D kernels always did.
+// templated on the node type.  The kernels that touch boxes are templated on D as well: they load a shape box with load_box of
+// csr.cuh (the padded 3-D device layout or the 4-D ABI layout) and take surface areas with surface_area_d<D>, which is the 3-D
+// surface_area for D = 3 and surface_area4 for D = 4.  Both sum the squared extents left to right without FMA, so the D = 3
+// instantiations perform exactly the operations the 3-D kernels always did.
 #pragma once
-#include "common.cuh"
+#include "csr.cuh"
 
 namespace bvhb200 {
 
 #ifdef __CUDACC__
-// ---- 4-D shape boxes (ABI layout: already whole sectors) and Aabb::surface_area for D = 4 ----
-__device__ __forceinline__ void load4(const bvh_aabb4f* p, float mn[4], float mx[4]) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
-    mn[0] = a.x; mn[1] = a.y; mn[2] = a.z; mn[3] = a.w; mx[0] = b.x; mx[1] = b.y; mx[2] = b.z; mx[3] = b.w;
-}
-__device__ __forceinline__ void load4(const bvh_aabb4d* p, double mn[4], double mx[4]) {
-    const double2* q = reinterpret_cast<const double2*>(p);
-    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);
-    mn[0] = a.x; mn[1] = a.y; mn[2] = b.x; mn[3] = b.y; mx[0] = c.x; mx[1] = c.y; mx[2] = d.x; mx[3] = d.y;
-}
-// 2 * (((sx*sx + sy*sy) + sz*sz) + sw*sw), left to right, no FMA.
+// ---- Aabb::surface_area for D = 4: 2 * (((sx*sx + sy*sy) + sz*sz) + sw*sw), left to right, no FMA ----
 template <class T> __device__ __forceinline__ T surface_area4(const T mn[4], const T mx[4]) {
     T acc = add_rn(mul_rn(sub_rn(mx[0], mn[0]), sub_rn(mx[0], mn[0])), mul_rn(sub_rn(mx[1], mn[1]), sub_rn(mx[1], mn[1])));
     acc = add_rn(acc, mul_rn(sub_rn(mx[2], mn[2]), sub_rn(mx[2], mn[2])));
@@ -30,10 +20,6 @@ template <class T> __device__ __forceinline__ T surface_area4(const T mn[4], con
     return mul_rn(T(2), acc);
 }
 
-__device__ __forceinline__ void load_box(const DAabbF* p, float mn[3], float mx[3]) { load_aabb(p, mn, mx); }
-__device__ __forceinline__ void load_box(const DAabbD* p, double mn[3], double mx[3]) { load_aabb(p, mn, mx); }
-__device__ __forceinline__ void load_box(const bvh_aabb4f* p, float mn[4], float mx[4]) { load4(p, mn, mx); }
-__device__ __forceinline__ void load_box(const bvh_aabb4d* p, double mn[4], double mx[4]) { load4(p, mn, mx); }
 template <int D, class T> __device__ __forceinline__ T surface_area_d(const T mn[D], const T mx[D]) {
     static_assert(D == 3 || D == 4, "surface_area_d: D = 3 or 4");
     if constexpr (D == 3) return surface_area(mn, mx);
