@@ -581,11 +581,39 @@ class Bvh2:
                                                                             C.byref(rebuilt)))
         return int(rebuilt.value)
 
+    def _sync_n(self):
+        self.n = int(getattr(capi.lib(), f"bvhgpu_tree_num_shapes_{self._d['suffix']}")(self._h))
+
+    def add_shapes(self, aabbs, max_growth: float = 1.5) -> int:
+        """Bvh::add_shape for every new box, batched (the contract of Bvh.add_shapes): the k boxes get the indices n .. n+k-1.
+        max_growth >= 1: degraded subtrees on the changed paths are rebuilt; <= 0: the grafts only.  Returns the number of shapes in
+        subtrees rebuilt by the growth test.  The node index of every shape may change: re-read nodes_and_index after every call."""
+        a = np.ascontiguousarray(aabbs, dtype=self._d["aabb"]).reshape(-1)
+        rebuilt = C.c_size_t(0)
+        try:
+            capi.check(getattr(capi.lib(), f"bvhgpu_add_shapes_{self._d['suffix']}")(self._h, _ptr(a), len(a), C.c_double(max_growth),
+                                                                                    C.byref(rebuilt)))
+        finally:
+            self._sync_n()
+        return int(rebuilt.value)
+
+    def remove_shapes(self, indices) -> np.ndarray:
+        """Bvh::remove_shape(i, swap_shape=true) for every index, batched (the contract of Bvh.remove_shapes): indices are distinct, in
+        the numbering before the call.  Returns the renumbering as (m, 2) rows (new index, old index)."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint32).reshape(-1)
+        n = self.n
+        try:
+            capi.check(getattr(capi.lib(), f"bvhgpu_remove_shapes_{self._d['suffix']}")(self._h, _ptr(idx), len(idx)))
+        finally:
+            self._sync_n()
+        return swap_moves(n, idx)
+
 
 class Bvh4(Bvh2):
     """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten, batched
     ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction), and the queries and nearest_to
-    of Bvh2 with 4 components (refit and update_shapes included), plus query_dev, refit_dev and update_dev."""
+    of Bvh2 with 4 components (refit, update_shapes, add_shapes and remove_shapes included), plus query_dev, refit_dev, update_dev,
+    add_shapes_dev and remove_shapes_dev."""
 
     _TABLE = BY_PREC_4D
     _DIM = 4
@@ -621,3 +649,24 @@ class Bvh4(Bvh2):
         capi.check(getattr(capi.lib(), f"bvhgpu_update_dev_{self._d['suffix']}")(self._h, C.c_void_p(changed_ptr), C.c_void_p(aabbs_ptr), m,
                                                                                 C.c_double(max_growth), C.byref(rebuilt) if want_rebuilt else None))
         return int(rebuilt.value) if want_rebuilt else None
+
+    def add_shapes_dev(self, aabbs_ptr: int, k: int, max_growth: float = 1.5) -> int:
+        """add_shapes from k new boxes on the device (C-ABI layout).  Returns the number of shapes in subtrees rebuilt by the growth
+        test."""
+        rebuilt = C.c_size_t(0)
+        try:
+            capi.check(getattr(capi.lib(), f"bvhgpu_add_shapes_dev_{self._d['suffix']}")(self._h, C.c_void_p(aabbs_ptr), k,
+                                                                                        C.c_double(max_growth), C.byref(rebuilt)))
+        finally:
+            self._sync_n()
+        return int(rebuilt.value)
+
+    def remove_shapes_dev(self, indices_ptr: int, k: int, indices=None) -> np.ndarray | None:
+        """remove_shapes from k u32 shape indices on the device.  Returns the renumbering when the same indices are also given on the
+        host (`indices`), else None."""
+        n = self.n
+        try:
+            capi.check(getattr(capi.lib(), f"bvhgpu_remove_shapes_dev_{self._d['suffix']}")(self._h, C.c_void_p(indices_ptr), k))
+        finally:
+            self._sync_n()
+        return None if indices is None else swap_moves(n, indices)

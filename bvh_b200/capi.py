@@ -136,7 +136,13 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
         getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
+        getattr(L, f"bvhgpu_add_shapes_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
+        getattr(L, f"bvhgpu_remove_shapes_{s}").argtypes = [vp, vp, sz]
     for s in ("f32x4", "f64x4"):
+        for f in ("add_shapes", "add_shapes_dev"):
+            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
+        for f in ("remove_shapes", "remove_shapes_dev"):
+            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz]
         getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
         getattr(L, f"bvhgpu_refit_dev_{s}").argtypes = [vp, vp, sz]
         getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]

@@ -695,6 +695,10 @@ static int add_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size_t
         tree->d_sa_base = nullptr; tree->d_tris = nullptr;
         tree->n = fresh.n; tree->n_nodes = fresh.n_nodes; tree->d_status = fresh.d_status;
         tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
+        if (tree->dims == 2) {                                          // the FLAT leaf boxes, read by the records, at the new n
+            dfree(ctx, tree->d_aabb_trav); tree->d_aabb_trav = nullptr;
+            BVH_TRY(dim2_finish_build<T>(tree));
+        }
         BVH_TRY(build_traversal_records(tree));
         if (tree->have_flat) BVH_TRY(build_flat(tree));
         tree->status_pending = true;
@@ -763,6 +767,30 @@ static int remove_impl(Tree<T>* tree, const uint32_t* indices, size_t k, bool de
     if (rrc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rrc : mark_failed(tree, rrc, "remove_shapes");
     tree->status_pending = true;
     return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+}
+
+// D = 2 add_shapes: the new 2-D boxes are lifted to z = [0, 0] and run through add_impl above; the descent's surface areas and the
+// exact builder of the group subtrees see z = [0, 0] only (exact, dim2.cu).  remove_shapes is remove_impl itself.  finish_relayout
+// (dynamic.cu) rebuilds the z = [-1, +1] boxes of the FLAT leaf re-test at the new n before the traversal records.  Host pointers;
+// synchronous.
+template <class T, class AABB2>
+static int add2_impl(Tree<T>* tree, const AABB2* aabbs, size_t k, double max_growth, size_t* rebuilt) {
+    if (!tree || (k && !aabbs)) { set_error("add_shapes: null argument"); return BVHGPU_ERR_INVALID; }
+    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("add_shapes: max_growth = %g, must be >= 1 (or <= 0 for no rebuild)", max_growth); return BVHGPU_ERR_INVALID; }
+    if (rebuilt) *rebuilt = 0;
+    if ((uint64_t)tree->n + k > (1ull << 30)) { set_error("add_shapes: %u + %zu shapes exceed 2^30 (u32 node indices); the tree was left unchanged", tree->n, k); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (k == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const typename Traits<T>::Aabb* d6 = nullptr;
+    BVH_TRY((lift2_aabbs<T, AABB2>(tree, scratch, aabbs, k, &d6)));
+    size_t r = 0;
+    BVH_TRY(add_impl<T>(tree, d6, k, max_growth, &r, true));
+    BVH_TRY(resolve_status(tree));
+    if (rebuilt) *rebuilt = r;
+    return BVHGPU_OK;
 }
 
 }  // namespace bvhb200
@@ -1176,6 +1204,12 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, \
                                        size_t* rebuilt) {                                                                  \
         return update2_impl<T, AABB>(tree, changed, changed_aabbs, m, max_growth, rebuilt);                                \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) {  \
+        return add2_impl<T, AABB>(tree, aabbs, k, max_growth, rebuilt);                                                    \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                             \
+        return remove_impl<T>(tree, indices, k, false);                                                                    \
     }
 
 DEFINE_API2(float, f32x2, bvhgpu_tree2f, bvh_aabb2f, bvh_ray2f, bvh_node2f, bvh_flat2f)

@@ -19,6 +19,7 @@
 #include "csr.cuh"
 #include "queries.cuh"
 #include "update.cuh"
+#include "dynamic.cuh"
 #include <algorithm>
 #include <new>
 
@@ -797,8 +798,8 @@ template <class T> static int run_levels4(Tree4<T>* tree, const BuildArgs4& A, c
     return BVHGPU_OK;
 }
 
-// The exact SAH build.  h_aabbs: host pointer.  Synchronous (the host learns the range count of every level anyway).
-template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb* h_aabbs) {
+// The exact SAH build.  h_aabbs: host pointer (device pointer with kind = cudaMemcpyDeviceToDevice).  Synchronous (the host learns the range count of every level anyway).
+template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb* h_aabbs, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
     using Key = typename Traits<T>::Key;
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
@@ -807,7 +808,7 @@ template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb*
     BVH_TRY(dalloc_t(ctx, &tree->d_nodes, tree->n_nodes));
     BVH_TRY(dalloc_t(ctx, &tree->d_node_index, n));
     BVH_TRY(dalloc_t(ctx, &tree->d_node_start, tree->n_nodes));
-    BVH_CUDA_TRY(cudaMemcpyAsync(tree->d_aabb, h_aabbs, sizeof(*h_aabbs) * n, cudaMemcpyHostToDevice, st));
+    BVH_CUDA_TRY(cudaMemcpyAsync(tree->d_aabb, h_aabbs, sizeof(*h_aabbs) * n, kind, st));
 
     Scratch scratch(ctx);
     BuildArgs4 A{};
@@ -1142,8 +1143,8 @@ template <class T> static int refit4(Tree4<T>* tree) {
 
 // dirty[0 .. cnts[0]) = the nodes whose box changed, tree->d_bad = their growth flags.  Rebuilds in place, with the level loop and
 // small4_kernel of the build, the outermost degraded subtrees (cnts[1], zero on entry, counts them), gives their nodes fresh baselines
-// and clears the flags.  *rebuilt = shapes in the rebuilt subtrees.
-template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* dirty, uint32_t* cnts, size_t* rebuilt) {
+// and clears the flags.  *rebuilt = shapes in the rebuilt subtrees.  `who` names the caller in error messages.
+template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* dirty, uint32_t* cnts, size_t* rebuilt, const char* who) {
     using Key = typename Traits<T>::Key;
     using Node = typename D4<T>::Node;
     bvhgpu_ctx* ctx = tree->ctx;
@@ -1177,7 +1178,7 @@ template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* 
     BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 5 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
     const uint32_t m = h[CTL_NEXT], n_small = h[CTL_SMALL], shapes = h[CTL_REBUILT];
-    if (m || n_small) BVH_TRY(run_levels4(tree, A, L, m, n_small, "update"));
+    if (m || n_small) BVH_TRY(run_levels4(tree, A, L, m, n_small, who));
     rebase4_kernel<T><<<wave, 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, tile0, tree->d_sa_base);
     clear_bad_kernel<<<gn, 256, 0, st>>>(dirty, cnts, tree->d_bad);
     LAUNCHED(ctx, 2);
@@ -1217,7 +1218,7 @@ template <class T> static int update4(Tree4<T>* tree, const uint32_t* d_changed,
     climb_paths_kernel<4, T, Node, typename D4<T>::Aabb><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
                                                                               tree->d_sa_base, (T)max_growth, rebuild ? tree->d_bad : nullptr, dirty, cnts);
     LAUNCHED(ctx, 2);
-    if (rebuild) BVH_TRY(rebuild_degraded4(tree, dirty, cnts, rebuilt));
+    if (rebuild) BVH_TRY(rebuild_degraded4(tree, dirty, cnts, rebuilt, "update"));
     return refresh_caches4(tree);
 }
 
@@ -1271,6 +1272,266 @@ template <class T> static int update4_impl(Tree4<T>* tree, const uint32_t* chang
     if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("update: CUDA error"); rc = BVHGPU_ERR_CUDA; }
     if (rc != BVHGPU_OK) return failed4(tree, rc, "update");
     if (rebuilt) *rebuilt = shapes;
+    return BVHGPU_OK;
+}
+
+// ---- add_shapes / remove_shapes (Bvh::add_shape / Bvh::remove_shape, src/bvh/optimization.rs:67-301; DESIGN.md section 4.13) ----
+// The relocation, grafting, contraction and climb of the 3-D drivers (dynamic.cu) with the kernels of dynamic.cuh at D = 4.  The group
+// subtrees and the growth rebuilds are built by the level loop and small4_kernel of the build, seeded with one task per root.
+
+// Arrays that depend on the node count or the shape numbering, after a relocation: the traversal records and the flat array are
+// rebuilt at the new size on first use (refresh_caches4 rewrites them in place and assumes the node count did not change); the
+// update's arrival counters and growth flags are reallocated by the next update.
+template <class T> static void drop_caches4(Tree4<T>* tree) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    dfree(ctx, tree->d_trec); tree->d_trec = nullptr;
+    dfree(ctx, tree->d_flat); tree->d_flat = nullptr;
+    dfree(ctx, tree->d_arrive); tree->d_arrive = nullptr;
+    dfree(ctx, tree->d_bad); tree->d_bad = nullptr;
+    tree->n_trec = tree->n == 0 ? 0u : (tree->n == 1 ? 1u : tree->n_nodes - 1);
+    tree->n_flat = tree->n == 0 ? 0 : (tree->n == 1 ? 1 : 3 * (size_t)tree->n - 2);
+}
+
+// aabb_all: [n + k] shape boxes (the tree's n followed by the k new ones, checked for NaN); becomes tree->d_aabb.  *rebuilt = shapes in
+// the subtrees rebuilt by the growth test (the group subtrees are not counted).  A failure with tree->d_aabb != aabb_all left the tree
+// untouched.
+template <class T> static int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* aabb_all, uint32_t k, double max_growth, size_t* rebuilt) {
+    using Node = typename D4<T>::Node;
+    using Key = typename Traits<T>::Key;
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = tree->n, nn = tree->n_nodes, nn2 = nn + 2 * k, N = n + k;
+    const bool rebuild = max_growth > 0.0;
+    const int wave = std::max(ctx->sm_count, 1) * 8;
+    if (rebuild && !tree->d_sa_base) {                          // the baseline is the tree before the call
+        BVH_TRY(dalloc_t(ctx, &tree->d_sa_base, nn));
+        node_sa_kernel<4, T, Node><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn, tree->d_sa_base);
+        LAUNCHED(ctx, 1);
+    }
+    T* sa_old = tree->d_sa_base;
+    Scratch scratch(ctx);
+    uint32_t *point = nullptr, *ng = nullptr;
+    BVH_TRY(scratch.get(&point, k));
+    // [0] groups, [1] group subtrees to build, [2] dirty nodes, [3] growth rebuild roots, [4] unused, [5] nodes that failed the growth test
+    BVH_TRY(scratch.get(&ng, 6));
+    BVH_CUDA_TRY(cudaMemsetAsync(ng, 0, 6 * sizeof(uint32_t), st));
+    descend_kernel<4, T><<<(k + 255) / 256, 256, 0, st>>>(tree->d_nodes, aabb_all, n, k, point);
+    LAUNCHED(ctx, 1);
+    Groups G;
+    BVH_TRY(group_insertions(ctx, scratch, point, k, nn, ng, &G));
+    Scratch scratch2(ctx);
+    uint32_t *idx = nullptr, *roots = nullptr, *gbase = nullptr, *arrive = nullptr, *dirty = nullptr;
+    uint8_t* aff = nullptr;
+    Key* keys = nullptr;
+    BVH_TRY(scratch2.get(&aff, nn2));
+    BVH_TRY(scratch2.get(&idx, 2 * (size_t)N));               // the builder's two index buffers; the groups' shapes go into the first
+    BVH_TRY(scratch2.get(&roots, k));
+    BVH_TRY(scratch2.get(&gbase, k));
+    BVH_TRY(scratch2.get(&keys, 8 * (size_t)k));
+    BVH_TRY(scratch2.get(&arrive, nn2));
+    BVH_TRY(scratch2.get(&dirty, nn2));
+    Node* nw = nullptr;
+    uint32_t *nstart = nullptr, *nidx = nullptr;
+    T* sa_new = nullptr;
+    int rc = dalloc_t(ctx, &nw, nn2);
+    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nstart, nn2);
+    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nidx, N);
+    if (rc == BVHGPU_OK && sa_old) rc = dalloc_t(ctx, &sa_new, nn2);
+    if (rc == BVHGPU_OK && cudaMemsetAsync(aff, 0, nn2, st) != cudaSuccess) rc = BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK) {
+        graft_relayout_kernel<4, T><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, sa_old, nn, G.a, G.S, nw, nstart, nidx, aff, sa_new);
+        graft_groups_kernel<4, T><<<wave, 256, 0, st>>>(G.uniq, G.cnt, G.goff, ng, G.sshape, tree->d_node_start, G.S, aabb_all, n,
+                                                        nw, nstart, nidx, idx, roots, ng + 1, keys, gbase);
+        ctx->launches += 2;
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) { set_error("add_shapes: %s", cudaGetErrorString(e)); rc = BVHGPU_ERR_CUDA; }
+    }
+    if (rc != BVHGPU_OK) { dfree(ctx, nw); dfree(ctx, nstart); dfree(ctx, nidx); dfree(ctx, sa_new); return rc; }
+    // the tree now is the new one (its boxes on the affected paths are still to be recomputed); from here on a failure leaves it
+    // half-done, and the caller marks it failed
+    dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
+    tree->d_nodes = nw; tree->d_node_start = nstart; tree->d_node_index = nidx; tree->d_aabb = aabb_all; tree->d_sa_base = sa_new;
+    tree->n = N; tree->n_nodes = nn2;
+    drop_caches4(tree);
+    uint32_t* h = ctx->h_pinned + 224;
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, ng + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    if (*h) {                                                   // exact-SAH subtrees of the groups with >= 2 shapes
+        Scratch scratch3(ctx);
+        BuildArgs4 A{};
+        Task4<T>* small = nullptr;
+        Levels4<T> L;
+        BVH_TRY(scratch3.get(&A.bkt, N));
+        BVH_TRY(scratch3.get(&A.ctl, 8));
+        BVH_TRY(scratch3.get(&small, N));
+        BVH_TRY(levels4_alloc(scratch3, N, &L));
+        A.idx[0] = idx; A.idx[1] = idx + N; A.small = small;
+        BVH_CUDA_TRY(cudaMemsetAsync(A.ctl, 0, 8 * sizeof(uint32_t), st));
+        root_seed4_kernel<T><<<std::min<uint32_t>((k + 255) / 256, (uint32_t)wave), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, roots, ng + 1,
+                                                                                                 keys, L.tasks, A);
+        LAUNCHED(ctx, 1);
+        BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        BVH_CUDA_TRY(cudaStreamSynchronize(st));
+        BVH_TRY(run_levels4(tree, A, L, h[CTL_NEXT], h[CTL_SMALL], "add_shapes"));
+    }
+    // boxes of the affected paths (+ the growth test)
+    BVH_CUDA_TRY(cudaMemsetAsync(arrive, 0, sizeof(uint32_t) * nn2, st));
+    if (rebuild) {
+        BVH_TRY(dalloc_t(ctx, &tree->d_bad, nn2));
+        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_bad, 0, nn2, st));
+    }
+    climb_affected_kernel<4, T><<<(nn2 + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn2, aff, tree->d_aabb, arrive, sa_new, (T)max_growth,
+                                                                 rebuild ? tree->d_bad : nullptr, ng + 5, dirty, ng + 2);
+    LAUNCHED(ctx, 1);
+    if (sa_new) { graft_rebase_kernel<4, T><<<wave, 256, 0, st>>>(tree->d_nodes, gbase, G.cnt, ng, sa_new); LAUNCHED(ctx, 1); }
+    if (rebuild) {
+        BVH_CUDA_TRY(cudaMemcpyAsync(h, ng + 5, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        BVH_CUDA_TRY(cudaStreamSynchronize(st));
+        if (*h) BVH_TRY(rebuild_degraded4(tree, dirty, ng + 2, rebuilt, "add_shapes"));   // a node failed the growth test
+    }
+    drop_caches4(tree);                                         // (the growth flags: all clear again, dropped with the counters)
+    return BVHGPU_OK;
+}
+
+// d_rm: [n + 1] removed flag of every shape (0 / 1, the last word 0), 1 <= k <= n.  A failure with tree->d_nodes unchanged left the
+// tree untouched.
+template <class T> static int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint32_t k) {
+    using Node = typename D4<T>::Node;
+    using Aabb = typename D4<T>::Aabb;
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t n = tree->n, nn = tree->n_nodes, m = n - k, nn2 = m ? 2 * m - 1 : 0;
+    if (m == 0) {                                               // everything goes: the tree of an n == 0 build
+        dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
+        tree->d_nodes = nullptr; tree->d_node_start = nullptr; tree->d_node_index = nullptr; tree->d_aabb = nullptr; tree->d_sa_base = nullptr;
+        tree->n = 0; tree->n_nodes = 0;
+        drop_caches4(tree);
+        return BVHGPU_OK;
+    }
+    Scratch scratch(ctx);
+    uint32_t *flag = nullptr, *newidx = nullptr, *arrive = nullptr;
+    uint8_t* aff = nullptr;
+    Ranks rk;
+    BVH_TRY(remove_ranks(ctx, scratch, d_rm, n, k, tree->d_node_index, tree->d_node_start, &rk));
+    BVH_TRY(scratch.get(&flag, (size_t)nn + 1));
+    BVH_TRY(scratch.get(&newidx, (size_t)nn + 1));
+    BVH_TRY(scratch.get(&aff, nn2));
+    BVH_TRY(scratch.get(&arrive, nn2));
+    BVH_CUDA_TRY(cudaMemsetAsync(arrive, 0, sizeof(uint32_t) * nn2, st));
+    survive_kernel<<<(nn + 256) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, nn, rk.R, flag);
+    LAUNCHED(ctx, 1);
+    BVH_TRY(exclusive_sum_u32(scratch, flag, newidx, (size_t)nn + 1, st));
+    Node* nw = nullptr;
+    uint32_t *nstart = nullptr, *nidx = nullptr;
+    Aabb* a_new = nullptr;
+    T* sa_new = nullptr;
+    int rc = dalloc_t(ctx, &nw, nn2);
+    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nstart, nn2);
+    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nidx, m);
+    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &a_new, m);
+    if (rc == BVHGPU_OK && tree->d_sa_base) rc = dalloc_t(ctx, &sa_new, nn2);
+    if (rc != BVHGPU_OK) { dfree(ctx, nw); dfree(ctx, nstart); dfree(ctx, nidx); dfree(ctx, a_new); dfree(ctx, sa_new); return rc; }
+    contract_kernel<T><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, nn, rk.R, newidx, m, rk.Rm, rk.holes,
+                                                          tree->d_sa_base, nw, nstart, nidx, aff, sa_new);
+    permute_shapes_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_rm, n, m, rk.Rm, rk.holes, tree->d_aabb, a_new, nullptr, nullptr, 0u);
+    LAUNCHED(ctx, 2);
+    dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
+    tree->d_nodes = nw; tree->d_node_start = nstart; tree->d_node_index = nidx; tree->d_aabb = a_new; tree->d_sa_base = sa_new;
+    tree->n = m; tree->n_nodes = nn2;
+    drop_caches4(tree);
+    if (nn2 > 1) {
+        climb_affected_kernel<4, T><<<(nn2 + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn2, aff, tree->d_aabb, arrive, nullptr, T(0), nullptr, nullptr,
+                                                                     nullptr, nullptr);
+        LAUNCHED(ctx, 1);
+    }
+    return BVHGPU_OK;
+}
+
+// Bvh::add_shape, batched: the contract of the 3-D add_impl (capi.cu).  The new boxes are checked for NaN before the tree is touched;
+// n == 0: the call is bvhgpu_build_* over the k boxes.  Synchronous (the builder reads one word per level).
+template <class T> static int add4_impl(Tree4<T>* tree, const typename D4<T>::Aabb* aabbs, size_t k, double max_growth, size_t* rebuilt, bool dev_input) {
+    using Aabb = typename D4<T>::Aabb;
+    if (!tree || (k && !aabbs)) { set_error("add_shapes: null argument"); return BVHGPU_ERR_INVALID; }
+    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("add_shapes: max_growth = %g, must be >= 1 (or <= 0 for no rebuild)", max_growth); return BVHGPU_ERR_INVALID; }
+    if (rebuilt) *rebuilt = 0;
+    if ((uint64_t)tree->n + k > (1ull << 30)) { set_error("add_shapes: %u + %zu shapes exceed 2^30 (u32 node indices); the tree was left unchanged", tree->n, k); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (k == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const Aabb* d_in = aabbs;
+    if (!dev_input) {
+        void* d = nullptr;
+        BVH_TRY(upload4(ctx, scratch, aabbs, sizeof(*aabbs) * k, &d));
+        d_in = static_cast<const Aabb*>(d);
+    }
+    BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)k, scratch, "add_shapes"));
+    const uint32_t n = tree->n;
+    if (n == 0) {                                               // an empty tree: exactly bvhgpu_build_*
+        Tree4<T> fresh;
+        fresh.ctx = ctx; fresh.n = (uint32_t)k; fresh.n_nodes = 2 * (uint32_t)k - 1;
+        const int rc = build4<T>(&fresh, d_in, cudaMemcpyDeviceToDevice);
+        if (rc != BVHGPU_OK) { release4<T>(&fresh); return rc; }
+        dfree(ctx, tree->d_sa_base); tree->d_sa_base = nullptr;
+        tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
+        tree->n = fresh.n; tree->n_nodes = fresh.n_nodes;
+        drop_caches4(tree);
+        return BVHGPU_OK;
+    }
+    Aabb* all = nullptr;
+    BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
+    if (cudaMemcpyAsync(all, tree->d_aabb, sizeof(Aabb) * n, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(all + n, d_in, sizeof(Aabb) * k, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+        dfree(ctx, all);
+        set_error("add_shapes: CUDA error while staging the AABBs");
+        return BVHGPU_ERR_CUDA;
+    }
+    size_t shapes = 0;
+    int rc = add_shapes4(tree, all, (uint32_t)k, max_growth, &shapes);
+    if (rc != BVHGPU_OK) {
+        if (tree->d_aabb != all) { dfree(ctx, all); return rc; }    // failed before the tree was touched
+        return failed4(tree, rc, "add_shapes");
+    }
+    if (!dev_input && cudaStreamSynchronize(st) != cudaSuccess) { set_error("add_shapes: CUDA error"); return failed4(tree, BVHGPU_ERR_CUDA, "add_shapes"); }
+    if (rebuilt) *rebuilt = shapes;
+    return BVHGPU_OK;
+}
+
+// Bvh::remove_shape(i, swap_shape = true), batched: the contract of the 3-D remove_impl (capi.cu).  Range and duplicates are checked
+// before the tree is touched.
+template <class T> static int remove4_impl(Tree4<T>* tree, const uint32_t* indices, size_t k, bool dev_input) {
+    if (!tree || (k && !indices)) { set_error("remove_shapes: null argument"); return BVHGPU_ERR_INVALID; }
+    if (k > tree->n) { set_error("remove_shapes: %zu indices for a tree over %u shapes; the tree was left unchanged", k, tree->n); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (k == 0) return BVHGPU_OK;
+    const uint32_t n = tree->n;
+    Scratch scratch(ctx);
+    const uint32_t* d_idx = indices;
+    if (!dev_input) {
+        void* c = nullptr;
+        BVH_TRY(upload4(ctx, scratch, indices, sizeof(uint32_t) * k, &c));
+        d_idx = static_cast<const uint32_t*>(c);
+    }
+    uint32_t *rm = nullptr, *flags = nullptr;
+    BVH_TRY(scratch.get(&rm, (size_t)n + 1));
+    BVH_TRY(scratch.get(&flags, 2));
+    BVH_CUDA_TRY(cudaMemsetAsync(rm, 0, sizeof(uint32_t) * ((size_t)n + 1), st));
+    BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), st));
+    BVH_TRY(remove_check(ctx, d_idx, (uint32_t)k, n, rm, flags));
+    uint32_t* h = ctx->h_pinned + 222;
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    if (h[0]) { set_error("remove_shapes: a shape index is >= %u; the tree was left unchanged", n); return BVHGPU_ERR_INVALID; }
+    if (h[1]) { set_error("remove_shapes: a shape index is listed twice; the tree was left unchanged"); return BVHGPU_ERR_INVALID; }
+    const void* nodes_before = tree->d_nodes;
+    int rc = remove_shapes4(tree, rm, (uint32_t)k);
+    if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(st) != cudaSuccess) { set_error("remove_shapes: CUDA error"); rc = BVHGPU_ERR_CUDA; }
+    if (rc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rc : failed4(tree, rc, "remove_shapes");
     return BVHGPU_OK;
 }
 
@@ -1331,6 +1592,18 @@ struct bvhgpu_tree4d : Tree4<double> {};
     BVH_EXPORT4 int bvhgpu_update_dev_##SUF(TREE* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, \
                                             double max_growth, size_t* rebuilt) {                                         \
         return update4_impl<T>(tree, (const uint32_t*)dev_changed, (const AABB*)dev_changed_aabbs, m, max_growth, rebuilt, true); \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) { \
+        return add4_impl<T>(tree, aabbs, k, max_growth, rebuilt, false);                                                  \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_add_shapes_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt) { \
+        return add4_impl<T>(tree, (const AABB*)dev_aabbs, k, max_growth, rebuilt, true);                                  \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                           \
+        return remove4_impl<T>(tree, indices, k, false);                                                                  \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_remove_shapes_dev_##SUF(TREE* tree, const void* dev_indices, size_t k) {                       \
+        return remove4_impl<T>(tree, (const uint32_t*)dev_indices, k, true);                                              \
     }
 
 DEFINE_API4(float, f32x4, bvhgpu_tree4f, bvh_aabb4f, bvh_ray4f, bvh_node4f, bvh_flat4f)

@@ -51,8 +51,9 @@ struct bvhgpu_ctx {
     int64_t build_subtree = -1;    // exact builder: in-register subtrees for ranges <= 32 shapes (-1 auto, 0 never, 1 always)
     int64_t build_small = -1;      // exact builder: defer ranges <= 16 shapes to the thread-per-range kernel (-1 auto by size, 0 never, 1 always)
     // small pinned read-back area (256 words): 0-25 the ray traversal's scan tail, 64-79 the streamed path's per-chunk values,
-    // 128-129 the stream probe, 200-221 the capi / dynamic checks, 232-235 the 4-D build, CSR_TOTAL_WORD (236-237) the total of
-    // the two-pass CSR walks (csr.cuh), 240-248 the 4-D update checks
+    // 128-129 the stream probe, 200-221 the capi / dynamic checks, 222-225 the 4-D add / remove (index checks, group and seed
+    // counts), 232-235 the 4-D build, CSR_TOTAL_WORD (236-237) the total of the two-pass CSR walks (csr.cuh), 240-248 the 4-D
+    // update checks
     uint32_t* h_pinned = nullptr;
     int64_t profile = 0;           // bracket dominant kernels with events
     cudaEvent_t ev_walk[2] = {nullptr, nullptr};

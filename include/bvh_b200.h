@@ -298,6 +298,30 @@ int bvhgpu_update_f64x4(bvhgpu_tree4d* tree, const uint32_t* changed, const bvh_
 int bvhgpu_update_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
 int bvhgpu_update_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt);
 
+/* ---- D = 2 and D = 4 add / remove shapes (Bvh::add_shape / Bvh::remove_shape, src/bvh/optimization.rs:67-301, generic in D).  The
+ * contract of bvhgpu_add_shapes_f32x3 / bvhgpu_remove_shapes_f32x3 below, with D components: the descent, the grafts (exact-SAH
+ * subtrees over the shapes that chose one insertion point), the growth test and rebuild with max_growth >= 1, the contraction and the
+ * swap renumbering of remove, the checks before the tree is touched (NaN, indices >= n, duplicates, k > n, n + k > 2^30,
+ * 0 < max_growth < 1), *rebuilt = shapes in the subtrees rebuilt by the growth test, k = 0 is a no-op, add to an empty tree is
+ * bvhgpu_build_*, removing every shape leaves the tree of an n = 0 build, a failure after the tree was modified is sticky.  Traversal
+ * records and flat arrays built earlier follow the new tree.  The node index of every shape may change: re-read them with
+ * bvhgpu_tree_nodes_* after every call.
+ * D = 2 runs the 3-D add / remove on the tree embedded in z = [0, 0] (exact, dim2.cu); host pointers only.  D = 4 has its own drivers
+ * (dim4.cu) and builds the group subtrees and the growth rebuilds with the 4-D exact builder; the calls are synchronous (the builder
+ * reads one word per level).  _dev_: inputs on the device (C-ABI layout). */
+int bvhgpu_add_shapes_f32x2(bvhgpu_tree2f* tree, const bvh_aabb2f* aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_f64x2(bvhgpu_tree2d* tree, const bvh_aabb2d* aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_remove_shapes_f32x2(bvhgpu_tree2f* tree, const uint32_t* indices, size_t k);
+int bvhgpu_remove_shapes_f64x2(bvhgpu_tree2d* tree, const uint32_t* indices, size_t k);
+int bvhgpu_add_shapes_f32x4(bvhgpu_tree4f* tree, const bvh_aabb4f* aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_f64x4(bvhgpu_tree4d* tree, const bvh_aabb4d* aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_add_shapes_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt);
+int bvhgpu_remove_shapes_f32x4(bvhgpu_tree4f* tree, const uint32_t* indices, size_t k);
+int bvhgpu_remove_shapes_f64x4(bvhgpu_tree4d* tree, const uint32_t* indices, size_t k);
+int bvhgpu_remove_shapes_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_indices, size_t k);
+int bvhgpu_remove_shapes_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_indices, size_t k);
+
 /* ---- flatten: replaces Bvh::flatten (src/flat_bvh.rs:60-143, 240-251, 312-319) -----
  * Writes the FlatBvh (3n-2 FlatNodes for n >= 2, 1 for n == 1, 0 for n == 0) into `out`
  * (may be NULL to only build the device copy) and its length into *len. */
