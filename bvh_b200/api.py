@@ -456,7 +456,7 @@ def swap_moves(n: int, indices) -> np.ndarray:
 
 class Bvh2:
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays
-    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries and nearest_to.  Rays: structured array with 2-component origin, direction
+    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries, nearest_to, the distance-ordered traversal and the AABB closest hit.  Rays: structured array with 2-component origin, direction
     (normalised), inv_direction."""
 
     _TABLE = BY_PREC_2D
@@ -565,6 +565,37 @@ class Bvh2:
                 best = (shapes[int(s)], d)
         return None if best is None else (best[0], float(np.sqrt(best[1])))
 
+    def traverse_ordered(self, rays, ascending: bool = True):
+        """Batched nearest_traverse_iterator (ascending: by entry distance) / farthest_traverse_iterator (by exit distance,
+        descending): (offsets, hits, dists), the set of traverse_batch(..., TRAVERSE_BVH) perfectly sorted per ray, ties in DFS order,
+        with the slice distance of the child box the tree stores for each leaf.  A short capacity is retried once at the exact total,
+        hits and distances together."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        offsets = np.zeros(n + 1, dtype=np.uint32)
+        cap = max(8 * n, 1024)
+        fn = getattr(capi.lib(), f"bvhgpu_traverse_ordered_{self._d['suffix']}")
+        while True:
+            hits = np.zeros(cap, dtype=np.uint32)
+            dists = np.zeros(cap, dtype=self._d["scalar"])
+            total = C.c_size_t(0)
+            st = fn(self._h, _ptr(rays), n, 1 if ascending else 0, _ptr(offsets), _ptr(hits), _ptr(dists), cap, C.byref(total))
+            if st == capi.ERR_CAPACITY and total.value > cap and total.value <= U32_MAX:
+                cap = total.value
+                continue
+            capi.check(st)
+            return offsets, hits[: total.value], dists[: total.value]
+
+    def closest_hit(self, rays):
+        """Per ray: (shape whose own AABB the ray enters first, key (entry distance, DFS order), or U32_MAX; that entry distance or
+        +inf).  Exact: the head of traverse_ordered(rays, True) on trees whose stored child boxes are tight."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        shape = np.zeros(n, dtype=np.uint32)
+        dist = np.zeros(n, dtype=self._d["scalar"])
+        capi.check(getattr(capi.lib(), f"bvhgpu_closest_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(shape), _ptr(dist)))
+        return shape, dist
+
     def refit(self, aabbs):
         """Bvh::update_shapes' refit (fix_aabbs_ascending) for all shapes: `aabbs` = the new boxes of every shape.  Topology is kept."""
         a = np.ascontiguousarray(aabbs, dtype=self._d["aabb"])
@@ -613,7 +644,7 @@ class Bvh4(Bvh2):
     """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten, batched
     ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction), and the queries and nearest_to
     of Bvh2 with 4 components (refit, update_shapes, add_shapes and remove_shapes included), plus query_dev, refit_dev, update_dev,
-    add_shapes_dev and remove_shapes_dev."""
+    add_shapes_dev, remove_shapes_dev and closest_hit_dev."""
 
     _TABLE = BY_PREC_4D
     _DIM = 4
@@ -637,6 +668,12 @@ class Bvh4(Bvh2):
         capi.check(fn(self._h, mode, kind, C.c_void_p(queries_ptr), n, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
                       C.byref(total) if want_total else None))
         return total.value if want_total else None
+
+    def closest_hit_dev(self, rays_ptr: int, nrays: int, shape_ptr: int, dist_ptr: int):
+        """closest_hit from device pointers: nrays full 4-D rays (12 scalars each) in, u32 shapes and distances out, enqueued on the
+        context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_closest_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, C.c_void_p(shape_ptr),
+                                                                                     C.c_void_p(dist_ptr)))
 
     def refit_dev(self, aabbs_ptr: int, n: int):
         """refit from the new boxes of all n shapes on the device (C-ABI layout), enqueued on the context's stream."""

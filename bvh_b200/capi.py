@@ -138,7 +138,11 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
         getattr(L, f"bvhgpu_add_shapes_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
         getattr(L, f"bvhgpu_remove_shapes_{s}").argtypes = [vp, vp, sz]
+    for s in ("f32x2", "f64x2", "f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_traverse_ordered_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_closest_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
     for s in ("f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
         for f in ("add_shapes", "add_shapes_dev"):
             getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
         for f in ("remove_shapes", "remove_shapes_dev"):

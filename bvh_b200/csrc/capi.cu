@@ -345,10 +345,14 @@ static int nearest_candidates_host_impl(Tree<T>* tree, const T* points, size_t n
     });
 }
 
-template <class T>
-static int ordered_host_impl(Tree<T>* tree, const typename Traits<T>::Ray* rays, size_t nrays, int ascending,
+// D = 3: the C-ABI rays as they are.  D = 2: rays of 6 T lifted on the device (dim2_expand_rays: origin.z = 0, inv_direction.z = +inf)
+// and walked by the 3-D ordered kernel on the embedded tree, whose records span z = [-1, +1]: the z slab is (-inf, +inf) and leaves
+// both the set and the distances of the 2-D slice unchanged (dim2.cu).
+template <class T, int D = 3, class RAY = typename Traits<T>::Ray>
+static int ordered_host_impl(Tree<T>* tree, const RAY* rays, size_t nrays, int ascending,
                              uint32_t* offsets, uint32_t* hits, T* dists, size_t cap, size_t* total) {
     if (!tree || (nrays && !rays) || !offsets || (cap && (!hits || !dists))) { set_error("traverse_ordered: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D != 3 && nrays > 0x7FFFFFFFull) { set_error("traverse_ordered: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
@@ -360,7 +364,13 @@ static int ordered_host_impl(Tree<T>* tree, const typename Traits<T>::Ray* rays,
     BVH_TRY(scratch.get(&d_off, nrays + 1));
     BVH_TRY(scratch.get(&d_hits, cap));
     BVH_TRY(scratch.get(&d_dists, cap));
-    if (nrays) BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    if (nrays && D == 3) BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    if (nrays && D != 3) {
+        T* r6 = nullptr;
+        BVH_TRY(scratch.get(&r6, 6 * nrays));
+        BVH_CUDA_TRY(cudaMemcpyAsync(r6, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+        BVH_TRY(dim2_expand_rays<T>(ctx, r6, (uint32_t)nrays, reinterpret_cast<T*>(d_rays)));
+    }
     size_t tot = 0;
     int rc = traverse_ordered_device<T>(tree, d_rays, nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
     if (total) *total = tot;
@@ -395,6 +405,30 @@ static int closest_host_impl(Tree<T>* tree, const void* rays, uint32_t fmt, size
     BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     if (out_uv) BVH_CUDA_TRY(cudaMemcpyAsync(out_uv, d_uv, sizeof(T) * 2 * nrays, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+
+// 2-D AABB-mode closest hit: the rays of 6 T go straight to closest_aabb_device<2, T>, which tests x and y of the embedded tree.
+template <class T, class RAY2>
+static int closest2_impl(Tree<T>* tree, const RAY2* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {
+    if (!tree || (nrays && (!rays || !out_shape || !out_dist))) { set_error("closest_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("closest_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    T *d_rays = nullptr, *d_d = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(scratch.get(&d_rays, 6 * nrays));
+    BVH_TRY(scratch.get(&d_s, nrays));
+    BVH_TRY(scratch.get(&d_d, nrays));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(RAY2) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    const int rc = closest_aabb_device<2, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, d_rays, nrays, d_s, d_d);
+    if (rc != BVHGPU_OK) return rc;
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return BVHGPU_OK;
 }
@@ -1199,6 +1233,13 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                    size_t cap, size_t* total) {                                            \
         return nearest_candidates_host_impl<T, 2>(tree, points, n, offsets, cand, cap, total);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,     \
+                                                 uint32_t* hits, T* dists, size_t cap, size_t* total) {                   \
+        return ordered_host_impl<T, 2, RAY>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);               \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {  \
+        return closest2_impl<T, RAY>(tree, rays, nrays, out_shape, out_dist);                                              \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit2_impl<T, AABB>(tree, aabbs, n); } \
     BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, \

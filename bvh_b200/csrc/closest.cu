@@ -17,31 +17,13 @@
 //                  G differs from the unpruned minimum W only where W's Moeller-Trumbore distance lies more than 2^-16 in front of
 //                  the slab entry of W's own AABB; then d_W <= d_G, that entry exceeds fl(d_G * (1 + 2^-16)), and W's exact
 //                  intersection lies behind d_G.  G's distance, u and v are always the reference's Moeller-Trumbore result for G.
+// Dimensions: the AABB mode runs in D = 2, 3 and 4 (the same slab_slice over D axes, common.cuh); triangles are 3-D only.
 // The walk needs no stack: nodes carry parent links, a lane remembers which child it comes back from and re-derives the near / far
 // order from the node (same loads, same bits), so any tree depth works (the reference's iterators use a 32-slot stack / a heap).
 #include "internal.h"
+#include "csr.cuh"
 
 namespace bvhb200 {
-
-template <class T> __device__ __forceinline__ T cmin(T a, T b);
-template <> __device__ __forceinline__ float cmin(float a, float b) { return fminf(a, b); }
-template <> __device__ __forceinline__ double cmin(double a, double b) { return fmin(a, b); }
-template <class T> __device__ __forceinline__ T cmax(T a, T b);
-template <> __device__ __forceinline__ float cmax(float a, float b) { return fmaxf(a, b); }
-template <> __device__ __forceinline__ double cmax(double a, double b) { return fmax(a, b); }
-
-// Ray::intersection_slice_for_aabb (src/ray/ray_impl.rs:118-145): entry distance (clamped at 0) or "no intersection".
-template <class T>
-__device__ __forceinline__ bool slice_entry(const T o[3], const T inv[3], const T mn[3], const T mx[3], T& entry) {
-    const T l0 = mul_rn(sub_rn(mn[0], o[0]), inv[0]), r0 = mul_rn(sub_rn(mx[0], o[0]), inv[0]);
-    const T l1 = mul_rn(sub_rn(mn[1], o[1]), inv[1]), r1 = mul_rn(sub_rn(mx[1], o[1]), inv[1]);
-    const T l2 = mul_rn(sub_rn(mn[2], o[2]), inv[2]), r2 = mul_rn(sub_rn(mx[2], o[2]), inv[2]);
-    const bool nan = (l0 != l0) | (r0 != r0) | (l1 != l1) | (r1 != r1) | (l2 != l2) | (r2 != r2);
-    const T tmin = cmax(cmax(cmin(l0, r0), cmin(l1, r1)), cmin(l2, r2));
-    const T tmax = cmin(cmin(cmax(l0, r0), cmax(l1, r1)), cmax(l2, r2));
-    entry = tmin > T(0) ? tmin : T(0);
-    return !nan && !(entry > tmax);
-}
 
 template <class T> __device__ __forceinline__ void cross_rn(const T a[3], const T b[3], T o[3]) {       // nalgebra 3-D cross
     o[0] = sub_rn(mul_rn(a[1], b[2]), mul_rn(a[2], b[1]));
@@ -97,18 +79,27 @@ __global__ void __launch_bounds__(256) fill_nohit_kernel(uint32_t n, uint32_t* _
     if (uv) { uv[2 * (size_t)i] = T(0); uv[2 * (size_t)i + 1] = T(0); }
 }
 
-template <class T, bool TRI>
-__global__ void __launch_bounds__(128) closest_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_shapes,
-                                                      const typename Traits<T>::DAabb* __restrict__ aabb, const DTri<T>* __restrict__ tris,
+// The walk tests D axes of the boxes.  D = 3: the 3-D tree, rays of 9 T (origin, direction, inv_direction) or 6 T (origin,
+// direction).  D = 4: a Tree4's bvh_node4* and ABI boxes, rays of 12 T.  D = 2: the 3-D nodes and boxes a 2-D tree is embedded in
+// (z = [0, 0]), of which only x and y are tested, and the 2-D rays of 6 T as they are.  The lift that serves the other 2-D walks does
+// not work here: on z = [0, 0] the z slab would be (0 - 0) * inf = NaN and reject every box.  Triangles: D = 3 only.
+// (node and box types: ClosestLayout, internal.h)
+
+template <int D, class T, bool TRI>
+__global__ void __launch_bounds__(128) closest_kernel(const typename ClosestLayout<D, T>::Node* __restrict__ nodes, uint32_t n_shapes,
+                                                      const typename ClosestLayout<D, T>::Box* __restrict__ aabb, const DTri<T>* __restrict__ tris,
                                                       const T* __restrict__ rays, uint32_t ray_stride, uint32_t nrays,
                                                       uint32_t* __restrict__ out_shape, T* __restrict__ out_dist, T* __restrict__ out_uv) {
+    static_assert(!TRI || D == 3, "Ray::intersects_triangle is 3-D only");
+    constexpr int BD = D == 4 ? 4 : 3;                         // components of the stored boxes
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= nrays) return;
-    T o[3], dir[3], inv[3];
+    T o[D], dir[D], inv[D];
     {
         const T* p = rays + (size_t)ray_stride * r;
+        const bool full = D != 3 || ray_stride == 9;           // only D = 3 has the compact {origin, direction} layout
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { o[k] = __ldg(p + k); dir[k] = __ldg(p + 3 + k); inv[k] = ray_stride == 9 ? __ldg(p + 6 + k) : div_rn(T(1), dir[k]); }
+        for (int k = 0; k < D; ++k) { o[k] = __ldg(p + k); dir[k] = __ldg(p + D + k); inv[k] = full ? __ldg(p + 2 * D + k) : div_rn(T(1), dir[k]); }
     }
     const T INF = Traits<T>::inf();
     const T margin = TRI ? add_rn(T(1), T(1.0 / 65536.0)) : T(1);
@@ -116,7 +107,7 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename Traits<T>::
     T best_d = INF, bu = T(0), bv = T(0);
 
     auto leaf = [&](uint32_t shape, uint32_t node_idx) {
-        if (TRI) {
+        if constexpr (TRI) {
             const DTri<T>& t = tris[shape];
             T a[3], b[3], c[3];
 #pragma unroll
@@ -125,18 +116,18 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename Traits<T>::
             const T d = moeller_trumbore(o, dir, a, b, c, u, v);
             if (d < best_d || (d == best_d && d < INF && shape < best)) { best = shape; best_d = d; bu = u; bv = v; }
         } else {
-            T mn[3], mx[3], e;
-            load_aabb(aabb + shape, mn, mx);
-            if (slice_entry(o, inv, mn, mx, e)) {
+            T mn[BD], mx[BD], e, x;
+            load_box(aabb + shape, mn, mx);
+            if (slab_slice<D, T>(o, inv, mn, mx, e, x)) {
                 if (best == BVH_INVALID || e < best_d || (e == best_d && node_idx < best_key)) { best = shape; best_d = e; best_key = node_idx; }
             }
         }
     };
 
     if (n_shapes == 1) {                                       // root leaf (bvh_node.rs:314 tests the shape's own AABB)
-        T mn[3], mx[3], e;
-        load_aabb(aabb + nodes[0].shape, mn, mx);
-        if (slice_entry(o, inv, mn, mx, e)) leaf(nodes[0].shape, 0u);
+        T mn[BD], mx[BD], e, x;
+        load_box(aabb + nodes[0].shape, mn, mx);
+        if (slab_slice<D, T>(o, inv, mn, mx, e, x)) leaf(nodes[0].shape, 0u);
     } else {
         uint32_t node = 0, from = BVH_INVALID;                  // from: the child we are coming back from (BVH_INVALID: arriving from the parent)
         for (;;) {
@@ -146,11 +137,11 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename Traits<T>::
                 from = node; node = meta.x;
                 continue;
             }
-            const typename Traits<T>::Node& nd = nodes[node];
-            T lmn[3], lmx[3], rmn[3], rmx[3], el, er;
+            const typename ClosestLayout<D, T>::Node& nd = nodes[node];
+            T lmn[D], lmx[D], rmn[D], rmx[D], el, er, x;
 #pragma unroll
-            for (int k = 0; k < 3; ++k) { lmn[k] = __ldg(&nd.l_aabb.min[k]); lmx[k] = __ldg(&nd.l_aabb.max[k]); rmn[k] = __ldg(&nd.r_aabb.min[k]); rmx[k] = __ldg(&nd.r_aabb.max[k]); }
-            const bool hl = slice_entry(o, inv, lmn, lmx, el), hr = slice_entry(o, inv, rmn, rmx, er);
+            for (int k = 0; k < D; ++k) { lmn[k] = __ldg(&nd.l_aabb.min[k]); lmx[k] = __ldg(&nd.l_aabb.max[k]); rmn[k] = __ldg(&nd.r_aabb.min[k]); rmx[k] = __ldg(&nd.r_aabb.max[k]); }
+            const bool hl = slab_slice<D, T>(o, inv, lmn, lmx, el, x), hr = slab_slice<D, T>(o, inv, rmn, rmx, er, x);
             if (!hl) el = INF;
             if (!hr) er = INF;
             const bool left_first = el <= er;                   // front to back; ties: left (DFS order)
@@ -216,9 +207,21 @@ int closest_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t n
     const unsigned grid = (unsigned)((nrays + 127) / 128);
     const uint32_t stride = fmt == BVHGPU_RAYS_FULL ? 9u : 6u;
     if (use_triangles)
-        closest_kernel<T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv);
+        closest_kernel<3, T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv);
     else
-        closest_kernel<T, false><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, nullptr, reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv);
+        closest_kernel<3, T, false><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, nullptr, reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+template <int D, class T>
+int closest_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes, const typename ClosestLayout<D, T>::Box* aabb,
+                        const T* d_rays, size_t nrays, uint32_t* d_shape, T* d_dist) {
+    cudaStream_t st = ctx->stream;
+    if (nrays == 0) return BVHGPU_OK;
+    if (n_shapes == 0) fill_nohit_kernel<T><<<(unsigned)((nrays + 255) / 256), 256, 0, st>>>((uint32_t)nrays, d_shape, d_dist, nullptr);
+    else closest_kernel<D, T, false><<<(unsigned)((nrays + 127) / 128), 128, 0, st>>>(nodes, n_shapes, aabb, nullptr, d_rays, 3 * D, (uint32_t)nrays, d_shape, d_dist, nullptr);
     ctx->launches++;
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
@@ -228,5 +231,9 @@ template int set_triangles<float>(Tree<float>*, const float*, size_t, bool);
 template int set_triangles<double>(Tree<double>*, const double*, size_t, bool);
 template int closest_hit_device<float>(Tree<float>*, const void*, uint32_t, size_t, int, uint32_t*, float*, float*);
 template int closest_hit_device<double>(Tree<double>*, const void*, uint32_t, size_t, int, uint32_t*, double*, double*);
+template int closest_aabb_device<2, float>(bvhgpu_ctx*, const bvh_node3f*, uint32_t, const DAabbF*, const float*, size_t, uint32_t*, float*);
+template int closest_aabb_device<2, double>(bvhgpu_ctx*, const bvh_node3d*, uint32_t, const DAabbD*, const double*, size_t, uint32_t*, double*);
+template int closest_aabb_device<4, float>(bvhgpu_ctx*, const bvh_node4f*, uint32_t, const bvh_aabb4f*, const float*, size_t, uint32_t*, float*);
+template int closest_aabb_device<4, double>(bvhgpu_ctx*, const bvh_node4d*, uint32_t, const bvh_aabb4d*, const double*, size_t, uint32_t*, double*);
 
 }  // namespace bvhb200

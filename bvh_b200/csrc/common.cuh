@@ -108,6 +108,28 @@ template <class T> __device__ __forceinline__ T surface_area(const T mn[3], cons
     return mul_rn(T(2), add_rn(add_rn(mul_rn(sx, sx), mul_rn(sy, sy)), mul_rn(sz, sz)));
 }
 
+// Ray::intersection_slice_for_aabb (src/ray/ray_impl.rs:118-145) over D axes: (entry clamped at 0, exit), false = no intersection.
+// Per axis l = (min - o) * inv, r = (max - o) * inv; any NaN rejects.  The axes are folded left to right, in the order of the
+// reference's inf / sup over the vector: tmin = max(..max(min(l0, r0), min(l1, r1)).., min(l_{D-1}, r_{D-1})), tmax the
+// same with min / max exchanged.  The distance-ordered traversal and the AABB-mode closest hit of every dimension use this one slice.
+template <int D, class T>
+__device__ __forceinline__ bool slab_slice(const T o[D], const T inv[D], const T mn[D], const T mx[D], T& tmin_out, T& tmax_out) {
+    T l[D], r[D];
+#pragma unroll
+    for (int k = 0; k < D; ++k) { l[k] = mul_rn(sub_rn(mn[k], o[k]), inv[k]); r[k] = mul_rn(sub_rn(mx[k], o[k]), inv[k]); }
+    bool nan = (l[0] != l[0]) | (r[0] != r[0]);
+#pragma unroll
+    for (int k = 1; k < D; ++k) nan = nan | (l[k] != l[k]) | (r[k] != r[k]);
+    T tmin = min_t(l[0], r[0]), tmax = max_t(l[0], r[0]);
+#pragma unroll
+    for (int k = 1; k < D; ++k) tmin = max_t(tmin, min_t(l[k], r[k]));
+#pragma unroll
+    for (int k = 1; k < D; ++k) tmax = min_t(tmax, max_t(l[k], r[k]));
+    tmin_out = tmin > T(0) ? tmin : T(0);                       // fast_max(inf.max(), 0)
+    tmax_out = tmax;
+    return !nan && !(tmin_out > tmax);                          // None iff tmin > tmax or NaN
+}
+
 // ---- coherent (L2) loads/stores for data that other SMs produce during the same kernel ----
 template <class V> __device__ __forceinline__ V ld_cg(const V* p) { return __ldcg(p); }
 template <class V> __device__ __forceinline__ void st_cg(V* p, V v) { __stcg(p, v); }

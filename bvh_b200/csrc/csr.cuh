@@ -1,7 +1,8 @@
 // bvh_b200/csrc/csr.cuh -- the two-pass CSR walk that every batched walk except the 3-D ray traversal produces its hit lists with:
-// the traversal records of D = 3 and D = 4 and their fetch, the record walk generic in D, the count / fill kernel, and the host
-// driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries and nearest_candidates, D = 2 through the z = 0 lift, the
-// ordered traversal) and dim4.cu (D = 4 rays, queries and nearest_candidates).  The 3-D ray kernels of traverse.cu use the same fetch.
+// the traversal records of D = 3 and D = 4 and their fetch, the record walk generic in D, the count / fill kernel, the ordered
+// traversal's kernel, and the host driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries, nearest_candidates and the
+// ordered traversal, D = 2 through the z = 0 lift) and dim4.cu (D = 4 rays, queries, nearest_candidates and the ordered traversal).
+// The 3-D ray kernels of traverse.cu use the same fetch.
 //
 // CSR: offsets[n + 1] (u32, saturated to 0xFFFFFFFF) and the hit list hits[total]; the fill pass stores hits[0 .. cap) only, so a
 // short `cap` leaves a prefix of the full list.
@@ -16,11 +17,12 @@ struct __align__(16) TRec4F { float min[4]; float max[4]; uint32_t skip, shape, 
 struct __align__(16) TRec4D { double min[4]; double max[4]; uint32_t skip, shape, pad[2]; };  // 80 B
 static_assert(sizeof(TRec4F) == 48 && sizeof(TRec4D) == 80, "4-D record size");
 
-// record and shape-box types of the walk in D (3: TNodeF / TNodeD and the padded device boxes; 4: TRec4F / TRec4D and the ABI boxes)
+// record, shape-box and ray types of the walk in D (3: TNodeF / TNodeD, the padded device boxes and bvh_ray3*; 4: TRec4F / TRec4D,
+// the ABI boxes and bvh_ray4*)
 template <int D, class T> struct CsrRecords;
-template <class T> struct CsrRecords<3, T> { using Rec = typename Traits<T>::TNode; using Box = typename Traits<T>::DAabb; };
-template <> struct CsrRecords<4, float> { using Rec = TRec4F; using Box = bvh_aabb4f; };
-template <> struct CsrRecords<4, double> { using Rec = TRec4D; using Box = bvh_aabb4d; };
+template <class T> struct CsrRecords<3, T> { using Rec = typename Traits<T>::TNode; using Box = typename Traits<T>::DAabb; using Ray = typename Traits<T>::Ray; };
+template <> struct CsrRecords<4, float> { using Rec = TRec4F; using Box = bvh_aabb4f; using Ray = bvh_ray4f; };
+template <> struct CsrRecords<4, double> { using Rec = TRec4D; using Box = bvh_aabb4d; using Ray = bvh_ray4d; };
 
 #ifdef __CUDACC__
 // ---- record fetch: 128-bit non-coherent loads (LDG.E.128, the widest global load sm_90a has) ------------
@@ -77,6 +79,23 @@ __device__ __forceinline__ void load_box(const DAabbD* p, double mn[3], double m
 __device__ __forceinline__ void load_box(const bvh_aabb4f* p, float mn[4], float mx[4]) { load4(p, mn, mx); }
 __device__ __forceinline__ void load_box(const bvh_aabb4d* p, double mn[4], double mx[4]) { load4(p, mn, mx); }
 
+// ---- rays of the C ABI: origin and inv_direction (the direction is not needed by a slab test) ----
+template <class T> __device__ __forceinline__ void load_ray3(const T* p, T o[3], T inv[3]) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { o[k] = __ldg(p + k); inv[k] = __ldg(p + 6 + k); }
+}
+__device__ __forceinline__ void load_ray_full(const bvh_ray3f* p, float o[3], float inv[3]) { load_ray3(reinterpret_cast<const float*>(p), o, inv); }
+__device__ __forceinline__ void load_ray_full(const bvh_ray3d* p, double o[3], double inv[3]) { load_ray3(reinterpret_cast<const double*>(p), o, inv); }
+__device__ __forceinline__ void load_ray_full(const bvh_ray4f* p, float o[4], float inv[4]) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 2);
+    o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; inv[0] = b.x; inv[1] = b.y; inv[2] = b.z; inv[3] = b.w;
+}
+__device__ __forceinline__ void load_ray_full(const bvh_ray4d* p, double o[4], double inv[4]) {
+    const double2* q = reinterpret_cast<const double2*>(p);
+    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 4), d = __ldg(q + 5);
+    o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y; inv[0] = c.x; inv[1] = c.y; inv[2] = d.x; inv[3] = d.y;
+}
+
 // ---- the walk: stackless over the preorder records, hit -> next record, miss -> skip, so hits come out in the reference's
 // left-first DFS order.  `probe.hit(mn, mx)` is the predicate; `emit(shape)` is called for every reported shape. ----
 template <int D, class T, bool FLAT, class Rec, class Box, class Probe, class Emit>
@@ -129,9 +148,54 @@ __global__ void __launch_bounds__(256) csr_walk_kernel(const typename CsrRecords
     }
 }
 
+// ---- ordered traversal (SURVEY 8f N3): hits of every ray sorted by AABB entry distance (nearest first) or by exit
+// distance (farthest first), with the distance.  The reference's DistanceTraverseIterator (src/bvh/distance_traverse.rs) is
+// a best-effort heap walk ("not necessarily perfectly sorted", ties in heap order); this returns the same SET, perfectly
+// sorted, ties in the reference's DFS order.  Distances are slab_slice (Ray::intersection_slice_for_aabb) of the record's box:
+// the child box the parent stores for the leaf, or the shape's own box at a root leaf.  D = 3 and D = 4 over their records;
+// D = 2 runs the D = 3 instance on the tree embedded in z = 0 (dim2.cu).  Count pass (FILL = false) and fill pass as
+// csr_walk_kernel, then a stable insertion sort of the ray's list (lists are short).
+template <int D, class T, bool FILL>
+__global__ void __launch_bounds__(256) ordered_kernel(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                                      const typename CsrRecords<D, T>::Ray* __restrict__ rays, uint32_t nrays, int ascending,
+                                                      uint32_t* __restrict__ counts, const uint32_t* __restrict__ local,
+                                                      const unsigned long long* __restrict__ blocksum, const unsigned long long* __restrict__ total,
+                                                      uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits, T* __restrict__ dists, unsigned long long cap) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (FILL && r == 0) { const unsigned long long t = *total; offsets[nrays] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
+    if (r >= nrays) return;
+    T o[D], inv[D];
+    load_ray_full(rays + r, o, inv);
+    unsigned long long base = 0, w = 0;
+    if (FILL) { base = blocksum[r / CSR_SCAN_TILE] + local[r]; offsets[r] = base > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)base; w = base; }
+    uint32_t cnt = 0, i = 0;
+    while (i < n_rec) {
+        T mn[D], mx[D], t0, t1;
+        uint32_t skip, shape;
+        fetch(trec + i, mn, mx, skip, shape);
+        if (slab_slice<D, T>(o, inv, mn, mx, t0, t1)) {
+            if (shape != BVH_INVALID) {
+                if (FILL) { if (w < cap) { hits[w] = shape; dists[w] = ascending ? t0 : t1; } ++w; }
+                ++cnt;
+            }
+            i = i + 1;
+        } else i = skip;
+    }
+    if (!FILL) { counts[r] = cnt; return; }
+    // stable insertion sort of this ray's list: ascending entry distance / descending exit distance
+    const unsigned long long end = w < cap ? w : cap;
+    for (unsigned long long a = base + 1; a < end; ++a) {
+        const T d = dists[a];
+        const uint32_t h = hits[a];
+        unsigned long long b = a;
+        while (b > base && (ascending ? dists[b - 1] > d : dists[b - 1] < d)) { dists[b] = dists[b - 1]; hits[b] = hits[b - 1]; --b; }
+        dists[b] = d; hits[b] = h;
+    }
+}
+
 // ---- host: count -> scan -> fill ----
 // A walk is what the driver launches: walk.count(stream, n, counts) enqueues the count pass, walk.fill(stream, n, local, sums, total,
-// offsets, hits, cap) the fill pass.  CsrWalk is the one of csr_walk_kernel; the ordered traversal has its own (traverse.cu).
+// offsets, hits, cap) the fill pass.  CsrWalk is the one of csr_walk_kernel, OrderedWalk the one of ordered_kernel.
 template <int D, class T, class Probe> struct CsrWalk {
     bool flat;
     const typename CsrRecords<D, T>::Rec* trec;
@@ -147,6 +211,20 @@ template <int D, class T, class Probe> struct CsrWalk {
     void count(cudaStream_t st, uint32_t n, uint32_t* counts) const { launch<false>(st, n, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0); }
     void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
               uint32_t* offsets, uint32_t* hits, size_t cap) const { launch<true>(st, n, nullptr, local, sums, total, offsets, hits, cap); }
+};
+template <int D, class T> struct OrderedWalk {
+    const typename CsrRecords<D, T>::Rec* trec;
+    uint32_t n_rec;
+    const typename CsrRecords<D, T>::Ray* rays;
+    int ascending;
+    T* dists;                                         // written next to the hits, cap entries
+    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const {
+        ordered_kernel<D, T, false><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    }
+    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
+              uint32_t* offsets, uint32_t* hits, size_t cap) const {
+        ordered_kernel<D, T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, nullptr, local, sums, total, offsets, hits, dists, (unsigned long long)cap);
+    }
 };
 
 // One CSR over n items (0 < n <= 2^31 - 1) on the context's stream, in two steps so that a caller can read the total between them.

@@ -8,6 +8,13 @@
 //   traverse  the traversal records (and the shape AABBs the FLAT leaf re-test reads) get z = [-1, +1]; rays get origin.z = 0 and
 //             inv_direction.z = +inf: the z slab is (-1 - 0) * inf = -inf, (1 - 0) * inf = +inf -- never NaN, and max(tmin, -inf),
 //             min(tmax, +inf) are identities, so the 3-D slab test returns exactly what the 2-D one does.
+//   ordered   the distance-ordered traversal walks the same records with the same lifted rays (ordered_kernel<3, T>, csr.cuh).  The z
+//             slab is (-inf, +inf) on every record (an empty child box has z = [+inf, -inf]: (+inf - 0) * inf = +inf and
+//             (-inf - 0) * inf = -inf, again no NaN), z is the last axis of the fold, and max(tmin, -inf) / min(tmax, +inf) are
+//             identities: the 3-D instance returns the 2-D set and the 2-D entry / exit distances bit for bit.
+//   closest   does NOT lift: it slices the node boxes and the shape boxes, which have z = [0, 0], and (0 - 0) * inf = NaN would
+//             reject every box.  closest_kernel<2, T> (closest.cu) walks the embedded 3-D nodes and d_aabb, tests x and y only, and
+//             reads the 2-D rays (6 T) as they are.
 //   queries   Aabb / Point / Ball records and nearest_to points are lifted to z = 0 (lift2_kernel) and run through the 3-D query and
 //             nearest kernels.  Every z term is exactly neutral, so the results are the 2-D ones bit for bit:
 //               - Aabb and Point tests pass on z: the records and the FLAT re-test boxes span z = [-1, +1] and contain 0.

@@ -535,21 +535,12 @@ __device__ __forceinline__ bool slab4(const T o[4], const T inv[4], const T mn[4
     const T tmax = min_t(min_t(hi[0], hi[1]), min_t(hi[2], hi[3]));
     return !nan && tmax >= (tmin > T(0) ? tmin : T(0));
 }
-__device__ __forceinline__ void load_ray4(const bvh_ray4f* p, float o[4], float inv[4]) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 2);
-    o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; inv[0] = b.x; inv[1] = b.y; inv[2] = b.z; inv[3] = b.w;
-}
-__device__ __forceinline__ void load_ray4(const bvh_ray4d* p, double o[4], double inv[4]) {
-    const double2* q = reinterpret_cast<const double2*>(p);
-    const double2 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 4), d = __ldg(q + 5);
-    o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y; inv[0] = c.x; inv[1] = c.y; inv[2] = d.x; inv[3] = d.y;
-}
 
 // The probe of a ray batch for csr_walk_kernel (csr.cuh): load(src, r) reads ray r, hit(mn, mx) is the 4-wide slab test.  Queries
 // use Query<T, KIND, 4> of queries.cuh directly.
 template <class T> struct RayProbe4 {
     T o[4], inv[4];
-    __device__ __forceinline__ void load(const void* src, uint32_t r) { load_ray4(reinterpret_cast<const typename D4<T>::Ray*>(src) + r, o, inv); }
+    __device__ __forceinline__ void load(const void* src, uint32_t r) { load_ray_full(reinterpret_cast<const typename D4<T>::Ray*>(src) + r, o, inv); }
     __device__ __forceinline__ bool hit(const T mn[4], const T mx[4]) const { return slab4(o, inv, mn, mx); }
 };
 
@@ -1090,6 +1081,75 @@ template <class T> static int nearest_candidates4_host_impl(Tree4<T>* tree, cons
     return csr4_host<Query<T, QUERY_WITHIN, 4>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
 }
 
+// ---- distance-ordered traversal and AABB-mode closest hit (the contract of the 3-D calls; DESIGN.md section 4.14) ----
+// ordered_kernel<4, T> of csr.cuh over the records, sorted lists into scratch of `cap` entries, copied back as the 3-D host form does.
+template <class T> static int ordered4_host_impl(Tree4<T>* tree, const typename D4<T>::Ray* rays, size_t nrays, int ascending, uint32_t* offsets,
+                                                 uint32_t* hits, T* dists, size_t cap, size_t* total) {
+    if (!tree || (nrays && !rays) || !offsets || (cap && (!hits || !dists))) { set_error("traverse_ordered: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("traverse_ordered: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nrays == 0 || tree->n == 0) {
+        std::fill(offsets, offsets + nrays + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    Scratch scratch(ctx);
+    void* d_rays = nullptr;
+    uint32_t *d_off = nullptr, *d_hits = nullptr;
+    T* d_dists = nullptr;
+    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
+    BVH_TRY(scratch.get(&d_off, nrays + 1));
+    BVH_TRY(scratch.get(&d_hits, cap));
+    BVH_TRY(scratch.get(&d_dists, cap));
+    BVH_TRY(ensure_trec4(tree));
+    const OrderedWalk<4, T> walk{tree->d_trec, tree->n_trec, reinterpret_cast<const typename D4<T>::Ray*>(d_rays), ascending, d_dists};
+    size_t tot = 0;
+    const int rc = csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_off, d_hits, cap, &tot);
+    if (total) *total = tot;
+    if (rc != BVHGPU_OK && rc != BVHGPU_ERR_CAPACITY) return rc;
+    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, d_off, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, st));
+    const size_t m = std::min(tot, cap);
+    if (m) {
+        BVH_CUDA_TRY(cudaMemcpyAsync(hits, d_hits, sizeof(uint32_t) * m, cudaMemcpyDeviceToHost, st));
+        BVH_CUDA_TRY(cudaMemcpyAsync(dists, d_dists, sizeof(T) * m, cudaMemcpyDeviceToHost, st));
+    }
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    return rc;
+}
+// closest_aabb_device<4, T> (closest.cu) over the 4-D nodes and shape boxes; rays of 12 T.
+template <class T> static int closest4_dev_impl(Tree4<T>* tree, const void* d_rays, size_t nrays, void* d_shape, void* d_dist) {
+    if (!tree || (nrays && (!d_rays || !d_shape || !d_dist))) { set_error("closest_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("closest_hit_dev: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return closest_aabb_device<4, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, (uint32_t*)d_shape, (T*)d_dist);
+}
+template <class T> static int closest4_host_impl(Tree4<T>* tree, const typename D4<T>::Ray* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {
+    if (!tree || (nrays && (!rays || !out_shape || !out_dist))) { set_error("closest_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("closest_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    void* d_rays = nullptr;
+    uint32_t* d_s = nullptr;
+    T* d_d = nullptr;
+    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
+    BVH_TRY(scratch.get(&d_s, nrays));
+    BVH_TRY(scratch.get(&d_d, nrays));
+    const int rc = closest_aabb_device<4, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, d_s, d_d);
+    if (rc != BVHGPU_OK) return rc;
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nrays, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    return BVHGPU_OK;
+}
+
 // ---- refit / update_shapes ----
 // A failure after the tree was modified leaves arrays that no longer agree with each other: sticky, as a failed build.
 template <class T> static int failed4(Tree4<T>* t, int rc, const char* who) {
@@ -1580,6 +1640,16 @@ struct bvhgpu_tree4d : Tree4<double> {};
     BVH_EXPORT4 int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                     size_t cap, size_t* total) {                                          \
         return nearest_candidates4_host_impl<T>(tree, points, n, offsets, cand, cap, total);                              \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,   \
+                                                  uint32_t* hits, T* dists, size_t cap, size_t* total) {                  \
+        return ordered4_host_impl<T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);                     \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t* out_shape, T* out_dist) { \
+        return closest4_host_impl<T>(tree, rays, nrays, out_shape, out_dist);                                             \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_closest_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, void* dev_shape, void* dev_dist) { \
+        return closest4_dev_impl<T>(tree, dev_rays, nrays, dev_shape, dev_dist);                                          \
     }                                                                                                                     \
     BVH_EXPORT4 int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit4_impl<T>(tree, aabbs, n, false); } \
     BVH_EXPORT4 int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) {                                 \

@@ -228,6 +228,14 @@ template <class T, class F2> int dim2_flat_out(Tree<T>* tree, F2* d_out);
 // ---- closest.cu ----
 template <class T> int set_triangles(Tree<T>* tree, const T* tris9, size_t n, bool dev_input);
 template <class T> int closest_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, int use_triangles, uint32_t* d_shape, T* d_dist, T* d_uv);
+// AABB-mode closest hit of a 2-D tree (D = 2: the 3-D nodes and boxes it is embedded in, x and y tested, 2-D rays of 6 T) or a 4-D
+// tree (D = 4: its bvh_node4* and ABI boxes, rays of 12 T); device pointers, on the context's stream, nothing synchronises.  Arguments
+// and the tree's status are checked by the caller.
+template <int D, class T> struct ClosestLayout { using Node = typename Traits<T>::Node; using Box = typename Traits<T>::DAabb; };   // D = 2, 3
+template <> struct ClosestLayout<4, float> { using Node = bvh_node4f; using Box = bvh_aabb4f; };
+template <> struct ClosestLayout<4, double> { using Node = bvh_node4d; using Box = bvh_aabb4d; };
+template <int D, class T> int closest_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes,
+                                                  const typename ClosestLayout<D, T>::Box* aabb, const T* d_rays, size_t nrays, uint32_t* d_shape, T* d_dist);
 template <class T> int rays_new_device(bvhgpu_ctx* ctx, const T* d_origins, const T* d_dirs, size_t n,
                                        typename Traits<T>::Ray* d_rays);
 

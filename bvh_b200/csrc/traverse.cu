@@ -1472,77 +1472,7 @@ template int nearest_device<double>(Tree<double>*, int, const double*, size_t, u
 template int nearest_candidates_device<float>(Tree<float>*, const float*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 template int nearest_candidates_device<double>(Tree<double>*, const double*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 
-// ---- ordered traversal (SURVEY 8f N3): hits of every ray sorted by AABB entry distance (nearest first) or by exit
-// distance (farthest first), with the distance.  The reference's DistanceTraverseIterator (src/bvh/distance_traverse.rs) is
-// a best-effort heap walk ("not necessarily perfectly sorted", ties in heap order); this returns the same SET, perfectly
-// sorted, ties in the reference's DFS order.  Distances follow Ray::intersection_slice_for_aabb (src/ray/ray_impl.rs:118-145).
-template <class T>
-__device__ __forceinline__ bool slab_slice(const T o[3], const T inv[3], const T mn[3], const T mx[3], T& tmin_out, T& tmax_out) {
-    const T l0 = mul_rn(sub_rn(mn[0], o[0]), inv[0]), r0 = mul_rn(sub_rn(mx[0], o[0]), inv[0]);
-    const T l1 = mul_rn(sub_rn(mn[1], o[1]), inv[1]), r1 = mul_rn(sub_rn(mx[1], o[1]), inv[1]);
-    const T l2 = mul_rn(sub_rn(mn[2], o[2]), inv[2]), r2 = mul_rn(sub_rn(mx[2], o[2]), inv[2]);
-    const bool nan = (l0 != l0) | (r0 != r0) | (l1 != l1) | (r1 != r1) | (l2 != l2) | (r2 != r2);
-    const T tmin = tmax2(tmax2(tmin2(l0, r0), tmin2(l1, r1)), tmin2(l2, r2));
-    const T tmax = tmin2(tmin2(tmax2(l0, r0), tmax2(l1, r1)), tmax2(l2, r2));
-    tmin_out = tmin > T(0) ? tmin : T(0);                       // fast_max(inf.max(), 0)
-    tmax_out = tmax;
-    return !nan && !(tmin_out > tmax);                          // None iff tmin > tmax or NaN
-}
-
-template <class T, bool FILL>
-__global__ void __launch_bounds__(256) ordered_kernel(const typename Traits<T>::TNode* __restrict__ trec, uint32_t n_rec,
-                                                      const typename Traits<T>::Ray* __restrict__ rays, uint32_t nrays, int ascending,
-                                                      uint32_t* __restrict__ counts, const uint32_t* __restrict__ local,
-                                                      const unsigned long long* __restrict__ blocksum, const unsigned long long* __restrict__ total,
-                                                      uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits, T* __restrict__ dists, unsigned long long cap) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (FILL && r == 0) { const unsigned long long t = *total; offsets[nrays] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
-    if (r >= nrays) return;
-    T o[3], inv[3];
-    load_ray<T, false>(RaySrc<T>{reinterpret_cast<const T*>(rays), RAYS_FULL}, r, o, inv);
-    unsigned long long base = 0, w = 0;
-    if (FILL) { base = blocksum[r / SCAN_TILE] + local[r]; offsets[r] = base > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)base; w = base; }
-    uint32_t cnt = 0, i = 0;
-    while (i < n_rec) {
-        T mn[3], mx[3], t0, t1;
-        uint32_t skip, shape;
-        fetch(trec + i, mn, mx, skip, shape);
-        if (slab_slice(o, inv, mn, mx, t0, t1)) {
-            if (shape != BVH_INVALID) {
-                if (FILL) { if (w < cap) { hits[w] = shape; dists[w] = ascending ? t0 : t1; } ++w; }
-                ++cnt;
-            }
-            i = i + 1;
-        } else i = skip;
-    }
-    if (!FILL) { counts[r] = cnt; return; }
-    // stable insertion sort of this ray's list (lists are short): ascending entry distance / descending exit distance
-    const unsigned long long end = w < cap ? w : cap;
-    for (unsigned long long a = base + 1; a < end; ++a) {
-        const T d = dists[a];
-        const uint32_t h = hits[a];
-        unsigned long long b = a;
-        while (b > base && (ascending ? dists[b - 1] > d : dists[b - 1] < d)) { dists[b] = dists[b - 1]; hits[b] = hits[b - 1]; --b; }
-        dists[b] = d; hits[b] = h;
-    }
-}
-
-// the two passes of ordered_kernel, launched by the driver of csr.cuh
-template <class T> struct OrderedWalk {
-    const typename Traits<T>::TNode* trec;
-    uint32_t n_rec;
-    const typename Traits<T>::Ray* rays;
-    int ascending;
-    T* dists;
-    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const {
-        ordered_kernel<T, false><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, counts, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
-    }
-    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
-              uint32_t* offsets, uint32_t* hits, size_t cap) const {
-        ordered_kernel<T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, nullptr, local, sums, total, offsets, hits, dists, (unsigned long long)cap);
-    }
-};
-
+// ---- ordered traversal: ordered_kernel<3, T> of csr.cuh over the 3-D records (2-D trees: the lifted rays of dim2_expand_rays) ----
 template <class T>
 int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays, size_t nrays, int ascending,
                             uint32_t* d_offsets, uint32_t* d_hits, T* d_dists, size_t cap, size_t* total) {
@@ -1556,7 +1486,7 @@ int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays
     }
     BVH_TRY(resolve_status(tree));
     if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
-    const OrderedWalk<T> walk{tree->d_tnodes, tree->n_trec, d_rays, ascending, d_dists};
+    const OrderedWalk<3, T> walk{tree->d_tnodes, tree->n_trec, d_rays, ascending, d_dists};
     return csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_offsets, d_hits, cap, total);
 }
 template int traverse_ordered_device<float>(Tree<float>*, const bvh_ray3f*, size_t, int, uint32_t*, uint32_t*, float*, size_t, size_t*);

@@ -322,6 +322,38 @@ int bvhgpu_remove_shapes_f64x4(bvhgpu_tree4d* tree, const uint32_t* indices, siz
 int bvhgpu_remove_shapes_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_indices, size_t k);
 int bvhgpu_remove_shapes_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_indices, size_t k);
 
+/* ---- D = 2 and D = 4 distance-ordered traversal and closest hit (Bvh::nearest_traverse_iterator / farthest_traverse_iterator and
+ * the child variants, src/bvh/bvh_impl.rs:145-220, src/bvh/distance_traverse.rs, child_distance_traverse.rs, over
+ * Ray::intersection_slice_for_aabb, src/ray/ray_impl.rs:118-145, all generic in D).  The contract of bvhgpu_traverse_ordered_f32x3
+ * and of bvhgpu_closest_hit_f32x3 with use_triangles == 0 below, with D components: the set of bvhgpu_traverse_* in BVH semantics
+ * with its offsets, sorted by entry distance ascending (`ascending` != 0) or exit distance descending of the child box the tree stores
+ * for each leaf (empty boxes of "no split wins" nodes: entry 0 / exit +inf), ties in DFS order, that distance in `dists`; closest =
+ * the shape whose own AABB the ray enters first, key (entry distance, DFS order), exact, BVHGPU_INVALID_INDEX / +inf without a hit.
+ * Differences:
+ *   - there is no triangle mode: Ray::intersects_triangle needs a 3-D cross product.
+ *   - a null argument or nrays > 2^31-1: BVHGPU_ERR_INVALID, nothing is read or written.  An empty tree gives all-zero offsets or
+ *     no-hit results; a root leaf (n = 1) is decided by the shape's own box, as in the reference.
+ *   - ordered, host pointers, `cap` entries in hits and dists: there is no fetch call.  When the hits do not fit `cap`, offsets and
+ *     *total are valid and the call returns BVHGPU_ERR_CAPACITY; call again with cap = *total.
+ *   - D = 2: ordered runs the 3-D kernel on the tree embedded in z = 0 (exact, dim2.cu); closest tests x and y of the embedded tree
+ *     and reads the 2-D rays as they are.  Host pointers only.
+ *   - closest_hit_dev (D = 4 only): device pointers, full 4-D rays (12 T), enqueued on the context's stream, no synchronisation.
+ *     A sticky failure of the tree is reported as by the other 4-D calls. */
+int bvhgpu_traverse_ordered_f32x2(bvhgpu_tree2f* tree, const bvh_ray2f* rays, size_t nrays, int ascending,
+                                  uint32_t* offsets, uint32_t* hits, float* dists, size_t cap, size_t* total);
+int bvhgpu_traverse_ordered_f64x2(bvhgpu_tree2d* tree, const bvh_ray2d* rays, size_t nrays, int ascending,
+                                  uint32_t* offsets, uint32_t* hits, double* dists, size_t cap, size_t* total);
+int bvhgpu_traverse_ordered_f32x4(bvhgpu_tree4f* tree, const bvh_ray4f* rays, size_t nrays, int ascending,
+                                  uint32_t* offsets, uint32_t* hits, float* dists, size_t cap, size_t* total);
+int bvhgpu_traverse_ordered_f64x4(bvhgpu_tree4d* tree, const bvh_ray4d* rays, size_t nrays, int ascending,
+                                  uint32_t* offsets, uint32_t* hits, double* dists, size_t cap, size_t* total);
+int bvhgpu_closest_hit_f32x2(bvhgpu_tree2f* tree, const bvh_ray2f* rays, size_t nrays, uint32_t* out_shape, float* out_dist);
+int bvhgpu_closest_hit_f64x2(bvhgpu_tree2d* tree, const bvh_ray2d* rays, size_t nrays, uint32_t* out_shape, double* out_dist);
+int bvhgpu_closest_hit_f32x4(bvhgpu_tree4f* tree, const bvh_ray4f* rays, size_t nrays, uint32_t* out_shape, float* out_dist);
+int bvhgpu_closest_hit_f64x4(bvhgpu_tree4d* tree, const bvh_ray4d* rays, size_t nrays, uint32_t* out_shape, double* out_dist);
+int bvhgpu_closest_hit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_rays, size_t nrays, void* dev_shape, void* dev_dist);
+int bvhgpu_closest_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t nrays, void* dev_shape, void* dev_dist);
+
 /* ---- flatten: replaces Bvh::flatten (src/flat_bvh.rs:60-143, 240-251, 312-319) -----
  * Writes the FlatBvh (3n-2 FlatNodes for n >= 2, 1 for n == 1, 0 for n == 0) into `out`
  * (may be NULL to only build the device copy) and its length into *len. */

@@ -57,7 +57,23 @@ for prec in ("f32", "f64"):
     r2["origin"], r2["direction"], r2["inv_direction"] = o2, d2, 1.0 / d2
     for mode in (capi.TRAVERSE_BVH, capi.TRAVERSE_FLAT):
         b2.traverse_batch(r2, mode=mode)
+    b2.traverse_ordered(r2, True); b2.traverse_ordered(r2, False); b2.closest_hit(r2)
     b2.free()
+# 4-D ordered traversal and closest hit (host and device-pointer forms)
+from bvh_b200.dtypes import BY_PREC_4D
+for prec in ("f32", "f64"):
+    a4 = np.zeros(500, dtype=BY_PREC_4D[prec]["aabb"]); mn = rng.uniform(-100, 100, (500, 4)); a4["min"] = mn; a4["max"] = mn + rng.uniform(0, 5, (500, 4))
+    b4 = api.Bvh4.build(a4, prec=prec)
+    r4 = np.zeros(300, dtype=BY_PREC_4D[prec]["ray"])
+    o4 = rng.uniform(-120, 120, (300, 4)); d4 = rng.normal(0, 1, (300, 4)); d4 /= np.linalg.norm(d4, axis=1, keepdims=True)
+    r4["origin"], r4["direction"], r4["inv_direction"] = o4, d4, 1.0 / d4
+    b4.traverse_ordered(r4, True); b4.traverse_ordered(r4, False); s4, _ = b4.closest_hit(r4)
+    import torch
+    dr = torch.from_numpy(r4.view(np.uint8)).to("cuda:0"); ds = torch.empty(300, dtype=torch.int32, device="cuda:0")
+    dd = torch.empty(300, dtype=torch.float32 if prec == "f32" else torch.float64, device="cuda:0")
+    torch.cuda.synchronize()
+    b4.closest_hit_dev(dr.data_ptr(), 300, ds.data_ptr(), dd.data_ptr()); ctx.synchronize()
+    b4.free()
 # host path on a batch large enough to be chunked (under the sanitizer the library takes the copy-then-walk form; forced streaming too)
 a = scenes.create_n_cubes_aabbs(300)
 b = api.Bvh.build(a)
