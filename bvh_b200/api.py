@@ -295,6 +295,17 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_closest_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, 1 if triangles else 0, _ptr(shape), _ptr(dist), _ptr(uv)))
         return shape, dist, uv
 
+    def any_hit(self, rays: np.ndarray, tmax=None, triangles: bool = False) -> np.ndarray:
+        """Occlusion: per ray a shape hit at distance < tmax (one limit per ray, a scalar for all, or None for +inf), U32_MAX if none.
+        triangles=False: a shape whose own AABB the ray enters before tmax (exact); triangles=True: a triangle (set_triangles) whose
+        Ray::intersects_triangle distance is < tmax.  The walk stops at the first such shape; which one is deterministic."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        shape = np.zeros(n, dtype=np.uint32)
+        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), 1 if triangles else 0, _ptr(shape)))
+        return shape
+
     def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
         """Bvh::traverse with Aabb / Point / Ball queries (IntersectsAabb implementors other than Ray).
         queries: (n, 6) {min,max} for capi.QUERY_AABB, (n, 3) for QUERY_POINT, (n, 4) {center, radius} for QUERY_BALL."""
@@ -456,7 +467,7 @@ def swap_moves(n: int, indices) -> np.ndarray:
 
 class Bvh2:
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays
-    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries, nearest_to, the distance-ordered traversal and the AABB closest hit.  Rays: structured array with 2-component origin, direction
+    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries, nearest_to, the distance-ordered traversal, the AABB closest hit and any hit.  Rays: structured array with 2-component origin, direction
     (normalised), inv_direction."""
 
     _TABLE = BY_PREC_2D
@@ -596,6 +607,16 @@ class Bvh2:
         capi.check(getattr(capi.lib(), f"bvhgpu_closest_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(shape), _ptr(dist)))
         return shape, dist
 
+    def any_hit(self, rays, tmax=None) -> np.ndarray:
+        """Occlusion: per ray a shape whose own AABB the ray enters at a distance < tmax (one limit per ray, a scalar for all, or None
+        for +inf), U32_MAX if none.  Exact: a shape is reported iff closest_hit's distance is < tmax."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        shape = np.zeros(n, dtype=np.uint32)
+        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), _ptr(shape)))
+        return shape
+
     def refit(self, aabbs):
         """Bvh::update_shapes' refit (fix_aabbs_ascending) for all shapes: `aabbs` = the new boxes of every shape.  Topology is kept."""
         a = np.ascontiguousarray(aabbs, dtype=self._d["aabb"])
@@ -644,7 +665,7 @@ class Bvh4(Bvh2):
     """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten, batched
     ray traversal of 4-D AABBs and rays (4-component origin, direction (normalised), inv_direction), and the queries and nearest_to
     of Bvh2 with 4 components (refit, update_shapes, add_shapes and remove_shapes included), plus query_dev, refit_dev, update_dev,
-    add_shapes_dev, remove_shapes_dev and closest_hit_dev."""
+    add_shapes_dev, remove_shapes_dev, closest_hit_dev and any_hit_dev."""
 
     _TABLE = BY_PREC_4D
     _DIM = 4
@@ -674,6 +695,12 @@ class Bvh4(Bvh2):
         context's stream without host synchronisation."""
         capi.check(getattr(capi.lib(), f"bvhgpu_closest_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, C.c_void_p(shape_ptr),
                                                                                      C.c_void_p(dist_ptr)))
+
+    def any_hit_dev(self, rays_ptr: int, nrays: int, tmax_ptr: int, shape_ptr: int):
+        """any_hit from device pointers: nrays full 4-D rays (12 scalars each) and nrays limits (tmax_ptr = 0: +inf for every ray) in,
+        u32 shapes out, enqueued on the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, C.c_void_p(tmax_ptr or None),
+                                                                                 C.c_void_p(shape_ptr)))
 
     def refit_dev(self, aabbs_ptr: int, n: int):
         """refit from the new boxes of all n shapes on the device (C-ABI layout), enqueued on the context's stream."""

@@ -99,6 +99,8 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_tree_set_triangles_dev_{s}").argtypes = [vp, vp, sz]
         getattr(L, f"bvhgpu_closest_hit_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp]
         getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, i32, sz, i32, vp, vp, vp]
+        getattr(L, f"bvhgpu_any_hit_{s}").argtypes = [vp, vp, sz, vp, i32, vp]
+        getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, i32, sz, vp, i32, vp]
         getattr(L, f"bvhgpu_traverse_od_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_traverse_od_dev_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_refit_dev_{s}").argtypes = [vp, vp, sz]
@@ -141,8 +143,10 @@ def lib() -> C.CDLL:
     for s in ("f32x2", "f64x2", "f32x4", "f64x4"):
         getattr(L, f"bvhgpu_traverse_ordered_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_closest_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
+        getattr(L, f"bvhgpu_any_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
     for s in ("f32x4", "f64x4"):
         getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
+        getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
         for f in ("add_shapes", "add_shapes_dev"):
             getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
         for f in ("remove_shapes", "remove_shapes_dev"):

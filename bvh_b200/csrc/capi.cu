@@ -433,6 +433,57 @@ static int closest2_impl(Tree<T>* tree, const RAY2* rays, size_t nrays, uint32_t
     return BVHGPU_OK;
 }
 
+// Any hit, host pointers: rays (9 T) and the optional limits staged as closest_host_impl stages the rays.
+template <class T>
+static int any_hit_host_impl(Tree<T>* tree, const void* rays, size_t nrays, const T* tmax, int use_triangles, uint32_t* out_shape) {
+    if (!tree || (nrays && (!rays || !out_shape))) { set_error("any_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    T *d_rays = nullptr, *d_tmax = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(scratch.get(&d_rays, 9 * nrays));
+    BVH_TRY(scratch.get(&d_s, nrays));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(T) * 9 * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    if (tmax) {
+        BVH_TRY(scratch.get(&d_tmax, nrays));
+        BVH_CUDA_TRY(cudaMemcpyAsync(d_tmax, tmax, sizeof(T) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    BVH_TRY(any_hit_device<T>(tree, d_rays, BVHGPU_RAYS_FULL, nrays, d_tmax, use_triangles, d_s));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+
+// 2-D any hit: the rays of 6 T go straight to any_hit_aabb_device<2, T>, as in closest2_impl.
+template <class T, class RAY2>
+static int any2_impl(Tree<T>* tree, const RAY2* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {
+    if (!tree || (nrays && (!rays || !out_shape))) { set_error("any_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    T *d_rays = nullptr, *d_tmax = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(scratch.get(&d_rays, 6 * nrays));
+    BVH_TRY(scratch.get(&d_s, nrays));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(RAY2) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    if (tmax) {
+        BVH_TRY(scratch.get(&d_tmax, nrays));
+        BVH_CUDA_TRY(cudaMemcpyAsync(d_tmax, tmax, sizeof(T) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    const int rc = any_hit_aabb_device<2, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, d_rays, nrays, d_tmax, d_s);
+    if (rc != BVHGPU_OK) return rc;
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+
 template <class T> static int fetch_impl(Tree<T>* tree, uint32_t* hits, size_t cap) {
     if (!tree || !hits) { set_error("traverse_fetch: null argument"); return BVHGPU_ERR_INVALID; }
     if (cap < tree->last_total) { set_error("traverse_fetch: capacity %zu < %zu hits", cap, tree->last_total); return BVHGPU_ERR_CAPACITY; }
@@ -1161,6 +1212,15 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
         BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
         return closest_hit_device<T>(tree, dev_rays, (uint32_t)ray_layout, nrays, use_triangles, (uint32_t*)dev_shape, (T*)dev_dist, (T*)dev_uv); \
     }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, int use_triangles, uint32_t* out_shape) { \
+        return any_hit_host_impl<T>(tree, rays, nrays, tmax, use_triangles, out_shape);                                   \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax, \
+                                            int use_triangles, void* dev_shape) {                                         \
+        if (!tree || (nrays && (!dev_rays || !dev_shape))) { set_error("any_hit_dev: null argument"); return BVHGPU_ERR_INVALID; } \
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
+        return any_hit_device<T>(tree, dev_rays, (uint32_t)ray_layout, nrays, (const T*)dev_tmax, use_triangles, (uint32_t*)dev_shape); \
+    }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_stats_##SUF(TREE* tree, uint64_t* out2) {                                              \
         if (!tree || !out2) { set_error("traverse_stats: null argument"); return BVHGPU_ERR_INVALID; }                    \
         out2[0] = tree->last_visits; out2[1] = tree->last_total;                                                          \
@@ -1240,6 +1300,9 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {  \
         return closest2_impl<T, RAY>(tree, rays, nrays, out_shape, out_dist);                                              \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {   \
+        return any2_impl<T, RAY>(tree, rays, nrays, tmax, out_shape);                                                      \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit2_impl<T, AABB>(tree, aabbs, n); } \
     BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, \

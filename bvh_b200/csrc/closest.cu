@@ -17,6 +17,11 @@
 //                  G differs from the unpruned minimum W only where W's Moeller-Trumbore distance lies more than 2^-16 in front of
 //                  the slab entry of W's own AABB; then d_W <= d_G, that entry exceeds fl(d_G * (1 + 2^-16)), and W's exact
 //                  intersection lies behind d_G.  G's distance, u and v are always the reference's Moeller-Trumbore result for G.
+// Any hit (ANY = true): the other loop callers write over the same two calls, traverse(..).iter().any(|s| distance < tmax) -- a
+// shadow ray, a line of sight.  The same walk with a per-ray constant bound instead of best * margin: a child is entered while its entry
+// is < tmax (AABB mode; exact, since slab entries are monotone under box containment and every stored box contains the boxes below
+// it) or <= fl(tmax * (1 + 2^-16)) (triangle mode, the margin above), a leaf is accepted when its own box is entered before tmax /
+// its Moeller-Trumbore distance is < tmax, and the first accepted leaf ends the walk.  Only out_shape is written.
 // Dimensions: the AABB mode runs in D = 2, 3 and 4 (the same slab_slice over D axes, common.cuh); triangles are 3-D only.
 // The walk needs no stack: nodes carry parent links, a lane remembers which child it comes back from and re-derives the near / far
 // order from the node (same loads, same bits), so any tree depth works (the reference's iterators use a 32-slot stack / a heap).
@@ -85,11 +90,12 @@ __global__ void __launch_bounds__(256) fill_nohit_kernel(uint32_t n, uint32_t* _
 // not work here: on z = [0, 0] the z slab would be (0 - 0) * inf = NaN and reject every box.  Triangles: D = 3 only.
 // (node and box types: ClosestLayout, internal.h)
 
-template <int D, class T, bool TRI>
+template <int D, class T, bool TRI, bool ANY = false>
 __global__ void __launch_bounds__(128) closest_kernel(const typename ClosestLayout<D, T>::Node* __restrict__ nodes, uint32_t n_shapes,
                                                       const typename ClosestLayout<D, T>::Box* __restrict__ aabb, const DTri<T>* __restrict__ tris,
                                                       const T* __restrict__ rays, uint32_t ray_stride, uint32_t nrays,
-                                                      uint32_t* __restrict__ out_shape, T* __restrict__ out_dist, T* __restrict__ out_uv) {
+                                                      uint32_t* __restrict__ out_shape, T* __restrict__ out_dist, T* __restrict__ out_uv,
+                                                      const T* __restrict__ ray_tmax) {
     static_assert(!TRI || D == 3, "Ray::intersects_triangle is 3-D only");
     constexpr int BD = D == 4 ? 4 : 3;                         // components of the stored boxes
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -105,9 +111,29 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename ClosestLayo
     const T margin = TRI ? add_rn(T(1), T(1.0 / 65536.0)) : T(1);
     uint32_t best = BVH_INVALID, best_key = BVH_INVALID;
     T best_d = INF, bu = T(0), bv = T(0);
+    // any hit: a leaf is accepted when its distance is < tmax; children are entered while entry < tmax (AABB mode) or
+    // entry <= fl(tmax * (1 + 2^-16)) (triangle mode), a per-ray constant instead of best * margin
+    T tmax = INF, any_bound = INF;
+    if constexpr (ANY) {
+        if (ray_tmax) tmax = __ldg(ray_tmax + r);
+        any_bound = mul_rn(tmax, margin);
+    }
 
     auto leaf = [&](uint32_t shape, uint32_t node_idx) {
-        if constexpr (TRI) {
+        if constexpr (ANY) {
+            if constexpr (TRI) {
+                const DTri<T>& t = tris[shape];
+                T a[3], b[3], c[3];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { a[k] = __ldg(&t.a[k]); b[k] = __ldg(&t.b[k]); c[k] = __ldg(&t.c[k]); }
+                T u, v;
+                if (moeller_trumbore(o, dir, a, b, c, u, v) < tmax) best = shape;
+            } else {
+                T mn[BD], mx[BD], e, x;
+                load_box(aabb + shape, mn, mx);
+                if (slab_slice<D, T>(o, inv, mn, mx, e, x) && e < tmax) best = shape;
+            }
+        } else if constexpr (TRI) {
             const DTri<T>& t = tris[shape];
             T a[3], b[3], c[3];
 #pragma unroll
@@ -134,6 +160,9 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename ClosestLayo
             const uint4 meta = __ldg(reinterpret_cast<const uint4*>(nodes + node));      // parent, child_l, child_r, shape / count
             if (meta.y == BVH_INVALID) {
                 leaf(meta.w, node);
+                if constexpr (ANY) {
+                    if (best != BVH_INVALID) break;             // any hit: the first accepted leaf ends the walk
+                }
                 from = node; node = meta.x;
                 continue;
             }
@@ -148,15 +177,29 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename ClosestLayo
             const uint32_t near_i = left_first ? meta.y : meta.z, far_i = left_first ? meta.z : meta.y;
             const T near_e = left_first ? el : er, far_e = left_first ? er : el;
             const bool near_ok = left_first ? hl : hr, far_ok = left_first ? hr : hl;
-            const T bound = mul_rn(best_d, margin);             // inf stays inf
             uint32_t next = BVH_INVALID;
-            if (from == BVH_INVALID) {
-                if (near_ok && near_e <= bound) next = near_i;
-                else from = near_i;                             // skipped: as if we had just come back from it
-            }
-            if (next == BVH_INVALID && from == near_i) {
-                if (far_ok && far_e <= bound) next = far_i;
-                else from = far_i;
+            if constexpr (ANY) {
+                // AABB mode: entry < tmax, exact (a box entered at or beyond tmax holds no accepted leaf); triangles: the margin
+                const bool near_in = near_ok && (TRI ? near_e <= any_bound : near_e < tmax);
+                const bool far_in = far_ok && (TRI ? far_e <= any_bound : far_e < tmax);
+                if (from == BVH_INVALID) {
+                    if (near_in) next = near_i;
+                    else from = near_i;
+                }
+                if (next == BVH_INVALID && from == near_i) {
+                    if (far_in) next = far_i;
+                    else from = far_i;
+                }
+            } else {
+                const T bound = mul_rn(best_d, margin);             // inf stays inf
+                if (from == BVH_INVALID) {
+                    if (near_ok && near_e <= bound) next = near_i;
+                    else from = near_i;                             // skipped: as if we had just come back from it
+                }
+                if (next == BVH_INVALID && from == near_i) {
+                    if (far_ok && far_e <= bound) next = far_i;
+                    else from = far_i;
+                }
             }
             if (next != BVH_INVALID) { node = next; from = BVH_INVALID; continue; }
             if (node == 0) break;                               // back from the far child of the root
@@ -164,8 +207,10 @@ __global__ void __launch_bounds__(128) closest_kernel(const typename ClosestLayo
         }
     }
     out_shape[r] = best;
-    out_dist[r] = best_d;
-    if (out_uv) { out_uv[2 * (size_t)r] = bu; out_uv[2 * (size_t)r + 1] = bv; }
+    if constexpr (!ANY) {
+        out_dist[r] = best_d;
+        if (out_uv) { out_uv[2 * (size_t)r] = bu; out_uv[2 * (size_t)r + 1] = bv; }
+    }
 }
 
 template <class T>
@@ -207,9 +252,9 @@ int closest_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t n
     const unsigned grid = (unsigned)((nrays + 127) / 128);
     const uint32_t stride = fmt == BVHGPU_RAYS_FULL ? 9u : 6u;
     if (use_triangles)
-        closest_kernel<3, T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv);
+        closest_kernel<3, T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv, nullptr);
     else
-        closest_kernel<3, T, false><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, nullptr, reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv);
+        closest_kernel<3, T, false><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, nullptr, reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, d_dist, d_uv, nullptr);
     ctx->launches++;
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
@@ -221,7 +266,48 @@ int closest_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Nod
     cudaStream_t st = ctx->stream;
     if (nrays == 0) return BVHGPU_OK;
     if (n_shapes == 0) fill_nohit_kernel<T><<<(unsigned)((nrays + 255) / 256), 256, 0, st>>>((uint32_t)nrays, d_shape, d_dist, nullptr);
-    else closest_kernel<D, T, false><<<(unsigned)((nrays + 127) / 128), 128, 0, st>>>(nodes, n_shapes, aabb, nullptr, d_rays, 3 * D, (uint32_t)nrays, d_shape, d_dist, nullptr);
+    else closest_kernel<D, T, false><<<(unsigned)((nrays + 127) / 128), 128, 0, st>>>(nodes, n_shapes, aabb, nullptr, d_rays, 3 * D, (uint32_t)nrays, d_shape, d_dist, nullptr, nullptr);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+// Any hit (bvhgpu_any_hit_*): closest_kernel<D, T, TRI, true>, one ray per thread, out_shape only.  d_tmax: nrays limits or
+// nullptr (+inf for every ray).  An empty tree reports no hit for every ray (BVH_INVALID bytes, no kernel).
+template <class T>
+int any_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const T* d_tmax, int use_triangles, uint32_t* d_shape) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: too many rays"); return BVHGPU_ERR_INVALID; }
+    if (fmt != BVHGPU_RAYS_FULL && fmt != BVHGPU_RAYS_OD) { set_error("any_hit: bad ray layout %u", fmt); return BVHGPU_ERR_INVALID; }
+    if (nrays == 0) return BVHGPU_OK;
+    BVH_TRY(resolve_status(tree));
+    if (tree->n == 0) {
+        BVH_CUDA_TRY(cudaMemsetAsync(d_shape, 0xFF, sizeof(uint32_t) * nrays, st));
+        return BVHGPU_OK;
+    }
+    if (use_triangles && !tree->d_tris) { set_error("any_hit: triangle mode needs bvhgpu_tree_set_triangles_* first"); return BVHGPU_ERR_INVALID; }
+    const unsigned grid = (unsigned)((nrays + 127) / 128);
+    const uint32_t stride = fmt == BVHGPU_RAYS_FULL ? 9u : 6u;
+    if (use_triangles)
+        closest_kernel<3, T, true, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, nullptr, nullptr, d_tmax);
+    else
+        closest_kernel<3, T, false, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->n, tree->d_aabb, nullptr, reinterpret_cast<const T*>(d_rays), stride, (uint32_t)nrays, d_shape, nullptr, nullptr, d_tmax);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+template <int D, class T>
+int any_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes, const typename ClosestLayout<D, T>::Box* aabb,
+                        const T* d_rays, size_t nrays, const T* d_tmax, uint32_t* d_shape) {
+    cudaStream_t st = ctx->stream;
+    if (nrays == 0) return BVHGPU_OK;
+    if (n_shapes == 0) {
+        BVH_CUDA_TRY(cudaMemsetAsync(d_shape, 0xFF, sizeof(uint32_t) * nrays, st));
+        return BVHGPU_OK;
+    }
+    closest_kernel<D, T, false, true><<<(unsigned)((nrays + 127) / 128), 128, 0, st>>>(nodes, n_shapes, aabb, nullptr, d_rays, 3 * D, (uint32_t)nrays, d_shape, nullptr, nullptr, d_tmax);
     ctx->launches++;
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
@@ -235,5 +321,12 @@ template int closest_aabb_device<2, float>(bvhgpu_ctx*, const bvh_node3f*, uint3
 template int closest_aabb_device<2, double>(bvhgpu_ctx*, const bvh_node3d*, uint32_t, const DAabbD*, const double*, size_t, uint32_t*, double*);
 template int closest_aabb_device<4, float>(bvhgpu_ctx*, const bvh_node4f*, uint32_t, const bvh_aabb4f*, const float*, size_t, uint32_t*, float*);
 template int closest_aabb_device<4, double>(bvhgpu_ctx*, const bvh_node4d*, uint32_t, const bvh_aabb4d*, const double*, size_t, uint32_t*, double*);
+
+template int any_hit_device<float>(Tree<float>*, const void*, uint32_t, size_t, const float*, int, uint32_t*);
+template int any_hit_device<double>(Tree<double>*, const void*, uint32_t, size_t, const double*, int, uint32_t*);
+template int any_hit_aabb_device<2, float>(bvhgpu_ctx*, const bvh_node3f*, uint32_t, const DAabbF*, const float*, size_t, const float*, uint32_t*);
+template int any_hit_aabb_device<2, double>(bvhgpu_ctx*, const bvh_node3d*, uint32_t, const DAabbD*, const double*, size_t, const double*, uint32_t*);
+template int any_hit_aabb_device<4, float>(bvhgpu_ctx*, const bvh_node4f*, uint32_t, const bvh_aabb4f*, const float*, size_t, const float*, uint32_t*);
+template int any_hit_aabb_device<4, double>(bvhgpu_ctx*, const bvh_node4d*, uint32_t, const bvh_aabb4d*, const double*, size_t, const double*, uint32_t*);
 
 }  // namespace bvhb200

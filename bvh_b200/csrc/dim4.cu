@@ -1150,6 +1150,35 @@ template <class T> static int closest4_host_impl(Tree4<T>* tree, const typename 
     return BVHGPU_OK;
 }
 
+// any_hit_aabb_device<4, T> (closest.cu) over the 4-D nodes and shape boxes; rays of 12 T, limits of 1 T (nullptr: +inf).
+template <class T> static int any4_dev_impl(Tree4<T>* tree, const void* d_rays, size_t nrays, const void* d_tmax, void* d_shape) {
+    if (!tree || (nrays && (!d_rays || !d_shape))) { set_error("any_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("any_hit_dev: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return any_hit_aabb_device<4, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, (const T*)d_tmax, (uint32_t*)d_shape);
+}
+template <class T> static int any4_host_impl(Tree4<T>* tree, const typename D4<T>::Ray* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {
+    if (!tree || (nrays && (!rays || !out_shape))) { set_error("any_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(sticky4(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    void *d_rays = nullptr, *d_tmax = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
+    if (tmax) BVH_TRY(upload4(ctx, scratch, tmax, sizeof(T) * nrays, &d_tmax));
+    BVH_TRY(scratch.get(&d_s, nrays));
+    const int rc = any_hit_aabb_device<4, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, (const T*)d_tmax, d_s);
+    if (rc != BVHGPU_OK) return rc;
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    return BVHGPU_OK;
+}
+
 // ---- refit / update_shapes ----
 // A failure after the tree was modified leaves arrays that no longer agree with each other: sticky, as a failed build.
 template <class T> static int failed4(Tree4<T>* t, int rc, const char* who) {
@@ -1650,6 +1679,12 @@ struct bvhgpu_tree4d : Tree4<double> {};
     }                                                                                                                     \
     BVH_EXPORT4 int bvhgpu_closest_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, void* dev_shape, void* dev_dist) { \
         return closest4_dev_impl<T>(tree, dev_rays, nrays, dev_shape, dev_dist);                                          \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {  \
+        return any4_host_impl<T>(tree, rays, nrays, tmax, out_shape);                                                     \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape) { \
+        return any4_dev_impl<T>(tree, dev_rays, nrays, dev_tmax, dev_shape);                                              \
     }                                                                                                                     \
     BVH_EXPORT4 int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit4_impl<T>(tree, aabbs, n, false); } \
     BVH_EXPORT4 int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) {                                 \

@@ -236,6 +236,12 @@ template <> struct ClosestLayout<4, float> { using Node = bvh_node4f; using Box 
 template <> struct ClosestLayout<4, double> { using Node = bvh_node4d; using Box = bvh_aabb4d; };
 template <int D, class T> int closest_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes,
                                                   const typename ClosestLayout<D, T>::Box* aabb, const T* d_rays, size_t nrays, uint32_t* d_shape, T* d_dist);
+// Any hit (closest.cu): per ray the first leaf the closest walk accepts with distance < tmax (d_tmax: nrays limits, or nullptr for
+// +inf), BVH_INVALID without one; device pointers, on the context's stream.  any_hit_device checks its arguments and the tree's
+// status as closest_hit_device does; any_hit_aabb_device (D = 2, 4) leaves both to the caller, as closest_aabb_device.
+template <class T> int any_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const T* d_tmax, int use_triangles, uint32_t* d_shape);
+template <int D, class T> int any_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes,
+                                                  const typename ClosestLayout<D, T>::Box* aabb, const T* d_rays, size_t nrays, const T* d_tmax, uint32_t* d_shape);
 template <class T> int rays_new_device(bvhgpu_ctx* ctx, const T* d_origins, const T* d_dirs, size_t n,
                                        typename Traits<T>::Ray* d_rays);
 

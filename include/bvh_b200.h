@@ -494,6 +494,39 @@ int bvhgpu_closest_hit_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_rays, int 
 int bvhgpu_closest_hit_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_rays, int ray_layout, size_t nrays, int use_triangles,
                                  void* dev_shape, void* dev_dist, void* dev_uv);
 
+/* ---- any hit (occlusion) with a per-ray distance limit: the other loop callers of the reference write over Bvh::traverse +
+ * Ray::intersects_triangle -- traverse(..).iter().any(|s| ray.intersects_triangle(..).distance < tmax), a shadow ray, a line of sight,
+ * a segment against the scene.  Per ray r, with the limit tmax[r] (`tmax` == NULL: +inf for every ray):
+ *   use_triangles == 0 (D = 2, 3, 4): out_shape[r] = a shape s of Bvh::traverse's set (reached through the stored child boxes, the NaN
+ *       rule applied at every ancestor) whose own AABB the ray enters at e_s < tmax[r], e_s the entry of
+ *       Ray::intersection_slice_for_aabb bit for bit as bvhgpu_closest_hit_* uses it; BVHGPU_INVALID_INDEX exactly when there is none.
+ *       Exact: a hit exists iff the AABB-mode closest_hit distance is < tmax[r].  Slab entries are monotone under box containment and
+ *       every stored child box contains the boxes below it ("no split wins" empty boxes pass at entry 0), so subtrees entered at or
+ *       beyond tmax[r] are never opened without losing a shape.
+ *   use_triangles != 0 (D = 3, triangles from bvhgpu_tree_set_triangles_*): a reported shape always has a Moeller-Trumbore distance
+ *       (the reference's operation order, no FMA) < tmax[r].  A child is entered when its entry <= fl(tmax[r] * (1 + 2^-16)), the
+ *       margin of closest_hit, for the same reason; so "no hit" where the unpruned loop has one happens only in the grazing case:
+ *       every qualifying triangle's Moeller-Trumbore distance lies more than 2^-16 in front of the slab entry of its own AABB (its
+ *       entry then exceeds fl(tmax[r] * (1 + 2^-16)) > its distance).
+ *   Which shape: the first leaf the walk accepts, the closest_hit walk (stackless, near child first by entry, left on ties) with the
+ *       per-ray bound above; deterministic, the same across calls, host and device forms and both 3-D ray layouts.
+ *   tmax[r] <= 0 (-0 included) or NaN: no hit (the comparison is a strict <).  An empty tree: no hit for every ray; n = 1: the shape's
+ *   own box decides, as in the reference.  nrays > 2^31-1, an unknown ray_layout, a null argument, or use_triangles without triangles
+ *   (also after bvhgpu_add_shapes_* dropped them): BVHGPU_ERR_INVALID.  A failed build is reported sticky.  The _dev forms take device
+ *   pointers (dev_tmax may be NULL) and enqueue on the context's stream without synchronising; D = 2 has host pointers only. */
+int bvhgpu_any_hit_f32x3(bvhgpu_tree3f* tree, const bvh_ray3f* rays, size_t nrays, const float* tmax, int use_triangles, uint32_t* out_shape);
+int bvhgpu_any_hit_f64x3(bvhgpu_tree3d* tree, const bvh_ray3d* rays, size_t nrays, const double* tmax, int use_triangles, uint32_t* out_shape);
+int bvhgpu_any_hit_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax,
+                             int use_triangles, void* dev_shape);      /* FULL or OD rays, as bvhgpu_closest_hit_dev_* */
+int bvhgpu_any_hit_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax,
+                             int use_triangles, void* dev_shape);
+int bvhgpu_any_hit_f32x2(bvhgpu_tree2f* tree, const bvh_ray2f* rays, size_t nrays, const float* tmax, uint32_t* out_shape);
+int bvhgpu_any_hit_f64x2(bvhgpu_tree2d* tree, const bvh_ray2d* rays, size_t nrays, const double* tmax, uint32_t* out_shape);
+int bvhgpu_any_hit_f32x4(bvhgpu_tree4f* tree, const bvh_ray4f* rays, size_t nrays, const float* tmax, uint32_t* out_shape);
+int bvhgpu_any_hit_f64x4(bvhgpu_tree4d* tree, const bvh_ray4d* rays, size_t nrays, const double* tmax, uint32_t* out_shape);
+int bvhgpu_any_hit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape);
+int bvhgpu_any_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape);
+
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
  * leaves (user code), so there are two forms.  `points`: 3 T per query point, host pointers.

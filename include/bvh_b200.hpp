@@ -99,6 +99,7 @@ template <> struct Abi<float> {
     static int update(tree* t, const uint32_t* c, const aabb* a, size_t m, double g, size_t* r) { return bvhgpu_update_f32x3(t, c, a, m, g, r); }
     static int set_triangles(tree* t, const float* abc, size_t n) { return bvhgpu_tree_set_triangles_f32x3(t, abc, n); }
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_closest_hit_f32x3(t, r, n, tri, s, d, uv); }
+    static int any(tree* t, const ray* r, size_t n, const float* tm, int tri, uint32_t* s) { return bvhgpu_any_hit_f32x3(t, r, n, tm, tri, s); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f32x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
 };
@@ -116,6 +117,7 @@ template <> struct Abi<double> {
     static int update(tree* t, const uint32_t* c, const aabb* a, size_t m, double g, size_t* r) { return bvhgpu_update_f64x3(t, c, a, m, g, r); }
     static int set_triangles(tree* t, const double* abc, size_t n) { return bvhgpu_tree_set_triangles_f64x3(t, abc, n); }
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_closest_hit_f64x3(t, r, n, tri, s, d, uv); }
+    static int any(tree* t, const ray* r, size_t n, const double* tm, int tri, uint32_t* s) { return bvhgpu_any_hit_f64x3(t, r, n, tm, tri, s); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f64x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
 };
@@ -331,6 +333,14 @@ template <class T> class Bvh {
     void closest_hit(const std::vector<Ray<T>>& rays, bool triangles, std::vector<uint32_t>& shape, std::vector<T>& distance) const {
         shape.assign(rays.size(), 0); distance.assign(rays.size(), T(0));
         check(A::closest(tree_, reinterpret_cast<const typename A::ray*>(rays.data()), rays.size(), triangles ? 1 : 0, shape.data(), distance.data(), nullptr));
+    }
+    // Any hit per ray (occlusion: what callers build as traverse(..).iter().any(|s| ray.intersects_triangle(..).distance < tmax)):
+    // shape[i] = a shape hit at a distance < tmax[i] (tmax empty: +inf for every ray), UINT32_MAX if none.  triangles == false: a shape
+    // whose AABB the ray enters before tmax[i] (exact); true: a triangle whose Moeller-Trumbore distance is < tmax[i].
+    void any_hit(const std::vector<Ray<T>>& rays, const std::vector<T>& tmax, bool triangles, std::vector<uint32_t>& shape) const {
+        if (!tmax.empty() && tmax.size() != rays.size()) throw Error(BVHGPU_ERR_INVALID, "any_hit: one limit per ray, or none");
+        shape.assign(rays.size(), 0);
+        check(A::any(tree_, reinterpret_cast<const typename A::ray*>(rays.data()), rays.size(), tmax.empty() ? nullptr : tmax.data(), triangles ? 1 : 0, shape.data()));
     }
     size_t num_shapes() const { return n_; }
 

@@ -45,6 +45,20 @@ for prec, ncubes in (("f32", 60), ("f32", 700), ("f64", 300)):
     cs2, cd2, _ = b.closest_hit(rays, triangles=False)
     ts_, td_ = b.nearest_triangles_batch(pts[:256])
     b.traverse_ordered(rays[:512], True)
+    # any hit: both modes, host form with and without limits, device form with both ray layouts
+    ah_t, ah_a = b.any_hit(rays, cd, triangles=True), b.any_hit(rays, cd2 * 2)
+    b.any_hit(rays)
+    import ctypes as C, torch
+    sfx = "f32x3" if prec == "f32" else "f64x3"
+    tdt = torch.float32 if prec == "f32" else torch.float64
+    d_tm = torch.from_numpy(np.ascontiguousarray(cd)).to("cuda:0"); d_sh = torch.empty(len(rays), dtype=torch.int32, device="cuda:0")
+    for lay, src in ((capi.RAYS_FULL, rays), (capi.RAYS_OD, np.ascontiguousarray(np.concatenate([rays["origin"], rays["direction"]], axis=1)))):
+        d_r = torch.from_numpy(np.frombuffer(src.tobytes(), dtype=np.uint8).copy()).to("cuda:0"); torch.cuda.synchronize()
+        for tri in (0, 1):
+            capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_dev_{sfx}")(b._h, C.c_void_p(d_r.data_ptr()), lay, len(rays), C.c_void_p(d_tm.data_ptr()), tri,
+                                                                         C.c_void_p(d_sh.data_ptr())))
+        ctx.synchronize()
+    print("  any hit", int((ah_t != 0xFFFFFFFF).sum()), int((ah_a != 0xFFFFFFFF).sum()))
     b.free()
 # D = 2
 from bvh_b200.dtypes import BY_PREC_2D
@@ -57,9 +71,10 @@ for prec in ("f32", "f64"):
     r2["origin"], r2["direction"], r2["inv_direction"] = o2, d2, 1.0 / d2
     for mode in (capi.TRAVERSE_BVH, capi.TRAVERSE_FLAT):
         b2.traverse_batch(r2, mode=mode)
-    b2.traverse_ordered(r2, True); b2.traverse_ordered(r2, False); b2.closest_hit(r2)
+    b2.traverse_ordered(r2, True); b2.traverse_ordered(r2, False); _, c2 = b2.closest_hit(r2)
+    b2.any_hit(r2); b2.any_hit(r2, np.nextafter(c2, np.inf))
     b2.free()
-# 4-D ordered traversal and closest hit (host and device-pointer forms)
+# 4-D ordered traversal, closest hit and any hit (host and device-pointer forms)
 from bvh_b200.dtypes import BY_PREC_4D
 for prec in ("f32", "f64"):
     a4 = np.zeros(500, dtype=BY_PREC_4D[prec]["aabb"]); mn = rng.uniform(-100, 100, (500, 4)); a4["min"] = mn; a4["max"] = mn + rng.uniform(0, 5, (500, 4))
@@ -73,6 +88,8 @@ for prec in ("f32", "f64"):
     dd = torch.empty(300, dtype=torch.float32 if prec == "f32" else torch.float64, device="cuda:0")
     torch.cuda.synchronize()
     b4.closest_hit_dev(dr.data_ptr(), 300, ds.data_ptr(), dd.data_ptr()); ctx.synchronize()
+    b4.any_hit(r4); b4.any_hit(r4, np.full(300, 50.0))
+    b4.any_hit_dev(dr.data_ptr(), 300, dd.data_ptr(), ds.data_ptr()); b4.any_hit_dev(dr.data_ptr(), 300, 0, ds.data_ptr()); ctx.synchronize()
     b4.free()
 # host path on a batch large enough to be chunked (under the sanitizer the library takes the copy-then-walk form; forced streaming too)
 a = scenes.create_n_cubes_aabbs(300)
