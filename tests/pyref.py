@@ -34,8 +34,10 @@ def _grow(a, p):
     return ([x if x <= y else y for x, y in zip(a[0], p)], [x if x >= y else y for x, y in zip(a[1], p)])
 
 
-def build(aabbs, F=np.float32):
-    """Returns (nodes, node_index): nodes[i] = ('leaf', parent, shape) | ('node', parent, cl, cr, laabb, raabb)."""
+def build(aabbs, F=np.float32, root_aabb=None):
+    """Returns (nodes, node_index): nodes[i] = ('leaf', parent, shape) | ('node', parent, cl, cr, laabb, raabb).
+    root_aabb = (min, max): the box the root's split costs are divided by, instead of the joint box of the shapes (Bvh::build's).
+    The device's in-place rebuild of a subtree takes the join of the root's two stored child boxes there (tests/rebuildref.py)."""
     n = len(aabbs)
     if n == 0:
         return [], []
@@ -57,6 +59,8 @@ def build(aabbs, F=np.float32):
         return ab, cb
 
     ab, cb = joint(range(n))
+    if root_aabb is not None:
+        ab = ([F(v) for v in root_aabb[0]], [F(v) for v in root_aabb[1]])
     stack = [(list(range(n)), 0, 0, ab, cb)]
     with np.errstate(all="ignore"):
         while stack:

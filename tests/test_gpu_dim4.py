@@ -119,7 +119,8 @@ def _check_against_pyref(api, a, prec, rng, m=200):
 
 @pytest.mark.parametrize("prec", ["f32", "f64"])
 @pytest.mark.parametrize("kind,n", [("random", 0), ("random", 1), ("random", 2), ("random", 33), ("random", 700), ("coincident", 300),
-                                    ("axis0", 200), ("axis1", 200), ("axis2", 200), ("axis3", 200), ("peel", 300), ("overflow", 400)])
+                                    ("axis0", 200), ("axis1", 200), ("axis2", 200), ("axis3", 200), ("peel", 300), ("overflow", 400),
+                                    ("random", 257), ("random", 513), ("random", 16385), ("coincident", 5000)])
 def test_four_dimensional_bvh_matches_the_4d_restatement(api, kind, n, prec):
     rng = np.random.default_rng(n * 11 + len(kind))
     a = _scene4(kind, n, prec, rng)
