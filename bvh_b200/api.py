@@ -306,6 +306,19 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), 1 if triangles else 0, _ptr(shape)))
         return shape
 
+    def knn(self, points, k: int, max_dist=None):
+        """The k nearest shapes of every point: (shape (n, k) u32, dist (n, k)).  Row i lists the shapes in ascending
+        (Aabb::min_distance_squared of the shape's own box, index) order with their distances; with `max_dist` (a scalar for all points,
+        one limit per point, or None for no limit) only shapes at squared distance <= fl(r * r) qualify (r < 0 or NaN: none).  Slots
+        past the qualifying shapes hold U32_MAX and +inf.  Exact: the head of a stable brute-force sort.  1 <= k <= 64."""
+        return _knn_call(self, points, 3, k, max_dist)
+
+    def knn_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int):
+        """knn from device pointers: n points (3 scalars each) and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes and
+        distances out, enqueued on the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_dev_{self._d['suffix']}")(self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None),
+                                                                             C.c_void_p(shape_ptr), C.c_void_p(dist_ptr)))
+
     def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
         """Bvh::traverse with Aabb / Point / Ball queries (IntersectsAabb implementors other than Ray).
         queries: (n, 6) {min,max} for capi.QUERY_AABB, (n, 3) for QUERY_POINT, (n, 4) {center, radius} for QUERY_BALL."""
@@ -454,6 +467,18 @@ class Bvh:
         return swap_moves(n, idx)
 
 
+def _knn_call(bvh, points, D: int, k: int, max_dist):
+    """bvhgpu_knn_<suffix> on host arrays: points (n, D), max_dist None, a scalar or (n,)."""
+    p = np.ascontiguousarray(points, dtype=bvh._d["scalar"]).reshape(-1, D)
+    n = len(p)
+    r = None if max_dist is None else np.ascontiguousarray(np.broadcast_to(np.asarray(max_dist, dtype=bvh._d["scalar"]), (n,)))
+    kk = max(int(k), 0)
+    shape = np.zeros((n, kk), dtype=np.uint32)
+    dist = np.zeros((n, kk), dtype=bvh._d["scalar"])
+    capi.check(getattr(capi.lib(), f"bvhgpu_knn_{bvh._d['suffix']}")(bvh._h, _ptr(p), n, int(k) & 0xFFFFFFFF, _ptr(r), _ptr(shape), _ptr(dist)))
+    return shape, dist
+
+
 def swap_moves(n: int, indices) -> np.ndarray:
     """The renumbering of Bvh.remove_shapes: (m, 2) rows (new index, old index) of the survivors that move.  Survivors with index
     >= n-k take the vacated indices < n-k, smallest hole first (for k = 1: remove_shape(i, true) followed by pop())."""
@@ -575,6 +600,10 @@ class Bvh2:
             if best is None or d < best[1]:
                 best = (shapes[int(s)], d)
         return None if best is None else (best[0], float(np.sqrt(best[1])))
+
+    def knn(self, points, k: int, max_dist=None):
+        """The k nearest shapes of every point (points (n, D)), with the contract of Bvh.knn: (shape (n, k) u32, dist (n, k))."""
+        return _knn_call(self, points, self._DIM, k, max_dist)
 
     def traverse_ordered(self, rays, ascending: bool = True):
         """Batched nearest_traverse_iterator (ascending: by entry distance) / farthest_traverse_iterator (by exit distance,
@@ -701,6 +730,12 @@ class Bvh4(Bvh2):
         u32 shapes out, enqueued on the context's stream without host synchronisation."""
         capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, C.c_void_p(tmax_ptr or None),
                                                                                  C.c_void_p(shape_ptr)))
+
+    def knn_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int):
+        """knn from device pointers: n points (4 scalars each) and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes and
+        distances out, enqueued on the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_dev_{self._d['suffix']}")(self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None),
+                                                                             C.c_void_p(shape_ptr), C.c_void_p(dist_ptr)))
 
     def refit_dev(self, aabbs_ptr: int, n: int):
         """refit from the new boxes of all n shapes on the device (C-ABI layout), enqueued on the context's stream."""

@@ -144,6 +144,10 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_traverse_ordered_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp, sz, szp]
         getattr(L, f"bvhgpu_closest_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
         getattr(L, f"bvhgpu_any_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
+    for s in ("f32x2", "f64x2", "f32x3", "f64x3", "f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_knn_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
+    for s in ("f32x3", "f64x3", "f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_knn_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
     for s in ("f32x4", "f64x4"):
         getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
         getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]

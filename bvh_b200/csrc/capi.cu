@@ -330,6 +330,33 @@ static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n,
     return rc;
 }
 
+// k nearest shapes, host pointers: D = 3 points as they are, D = 2 points lifted to z = 0 (dim2.cu); n * k results copied back.
+template <class T, int D = 3>
+static int knn_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("knn: null argument"); return BVHGPU_ERR_INVALID; }
+    if (n > 0x7FFFFFFFull) { set_error("knn: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (n == 0) return BVHGPU_OK;
+    T *d_p = nullptr, *d_r = nullptr, *d_d = nullptr;
+    uint32_t* d_s = nullptr;
+    Scratch scratch(ctx);
+    BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
+    if (max_dist) {
+        BVH_TRY(scratch.get(&d_r, n));
+        BVH_CUDA_TRY(cudaMemcpyAsync(d_r, max_dist, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    BVH_TRY(scratch.get(&d_s, n * k));
+    BVH_TRY(scratch.get(&d_d, n * k));
+    BVH_TRY(knn_device<T>(tree, d_p, n, k, d_r, d_s, d_d));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n * k, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n * k, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+
 template <class T, int D = 3>
 static int nearest_candidates_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
     if (!tree || (n && !points) || !offsets) { set_error("nearest_candidates: null argument"); return BVHGPU_ERR_INVALID; }
@@ -1192,6 +1219,15 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
                                                  uint32_t* hits, T* dists, size_t cap, size_t* total) {                  \
         return ordered_host_impl<T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);                      \
     }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
+        return knn_host_impl<T>(tree, points, n, k, max_dist, out_shape, out_dist);                                      \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_knn_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist,  \
+                                        void* dev_shape, void* dev_dist) {                                                \
+        if (!tree || (n && (!dev_points || !dev_shape || !dev_dist))) { set_error("knn_dev: null argument"); return BVHGPU_ERR_INVALID; } \
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
+        return knn_device<T>(tree, (const T*)dev_points, n, k, (const T*)dev_max_dist, (uint32_t*)dev_shape, (T*)dev_dist); \
+    }                                                                                                                     \
     BVH_EXPORT int bvhgpu_tree_set_triangles_##SUF(TREE* tree, const T* triangles, size_t n) {                            \
         if (!tree || (n && !triangles)) { set_error("set_triangles: null argument"); return BVHGPU_ERR_INVALID; }         \
         BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
@@ -1293,6 +1329,9 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                    size_t cap, size_t* total) {                                            \
         return nearest_candidates_host_impl<T, 2>(tree, points, n, offsets, cand, cap, total);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
+        return knn_host_impl<T, 2>(tree, points, n, k, max_dist, out_shape, out_dist);                                     \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,     \
                                                  uint32_t* hits, T* dists, size_t cap, size_t* total) {                   \

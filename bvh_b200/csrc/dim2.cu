@@ -23,6 +23,10 @@
 //                 = 0; on an empty child box (z = [+inf, -inf]) the centre is NaN and o_z = 0 as well (NaN.max(0) = 0, as in Rust).
 //               - the QUERY_WITHIN lower bound on a record: max(-1 - 0, 0 - 1) = -1 -> 0; the farthest-corner bound on a shape: |0 - 0| = 0.
 //               - adding +0 to a non-negative sum is exact, and the squares are summed left to right, so z comes last.
+//   knn       the k nearest shapes: points lifted to z = 0 (lift2_kernel, nvec = 1), knn_kernel<T, K> (traverse.cu) on the embedded
+//             tree.  The keys are aabb_min_d2 of d_aabb (z = [0, 0]: o_z = 0, as above); the pruning bound box_lower_d2 of a node box
+//             with z = [0, 0] has a z gap of max(0 - 0, 0 - 0) = 0 minus a positive slack, clamped to 0; empty child boxes fall under
+//             the always-entered rule.  Every z term is +0 added last, so keys, bounds and rows are the 2-D ones bit for bit.
 // The 2-D PODs are converted on the device (expand on the way in, drop z on the way out).
 #include "internal.h"
 

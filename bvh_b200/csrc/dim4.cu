@@ -561,6 +561,19 @@ __global__ void __launch_bounds__(128) nearest4_kernel(const typename D4<T>::Nod
     out_shape[i] = best;
     out_dist[i] = sqrt_rn(best_d);                          // bvh_impl.rs:237
 }
+// k nearest shapes: knn_walk<4, T, K> (queries.cuh) over the 4-D nodes, keys from the shapes' own boxes; one thread per point
+template <class T, int K>
+__global__ void __launch_bounds__(128) knn4_kernel(const typename D4<T>::Node* __restrict__ nodes, uint32_t n_shapes, const typename D4<T>::Aabb* __restrict__ aabb,
+                                                   const T* __restrict__ points, const T* __restrict__ max_dist, uint32_t nq, uint32_t k,
+                                                   uint32_t* __restrict__ out_shape, T* __restrict__ out_dist) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    T p[4];
+    for (int c = 0; c < 4; ++c) p[c] = points[4 * (size_t)i + c];
+    auto leaf = [&](uint32_t shape) { T mn[4], mx[4]; load4(aabb + shape, mn, mx); return aabb_min_d2<4>(p, mn, mx); };
+    knn_point<4, T, K>(nodes, n_shapes, p, max_dist != nullptr, max_dist ? max_dist[i] : T(0), k, out_shape + (size_t)i * k,
+                       out_dist + (size_t)i * k, leaf);
+}
 // nearest_candidates, first pass: the farthest-corner bound U of every point (as nearest_bound_kernel), records {p, U} for QUERY_WITHIN
 template <class T>
 __global__ void __launch_bounds__(128) nearest_bound4_kernel(const typename D4<T>::Node* __restrict__ nodes, const typename D4<T>::Aabb* __restrict__ aabb,
@@ -1179,6 +1192,50 @@ template <class T> static int any4_host_impl(Tree4<T>* tree, const typename D4<T
     return BVHGPU_OK;
 }
 
+// ---- k nearest shapes: 4 T per point, n limits (nullptr: none), n * k results ----
+template <class T> static int knn4_check(Tree4<T>* tree, size_t n, uint32_t k, const char* what) {
+    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("%s: k = %u outside 1 .. %d", what, k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    return sticky4(tree);
+}
+template <class T> static int knn4_launch(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    knn_bucket(k, [&](auto kb) {
+        knn4_kernel<T, decltype(kb)::value><<<grid, 128, 0, ctx->stream>>>(tree->d_nodes, tree->n, tree->d_aabb, d_points, d_max_dist, (uint32_t)n, k, d_shape, d_dist);
+    });
+    LAUNCHED(ctx, 1);
+    return BVHGPU_OK;
+}
+template <class T> static int knn4_dev_impl(Tree4<T>* tree, const void* d_points, size_t n, uint32_t k, const void* d_max_dist, void* d_shape, void* d_dist) {
+    if (!tree || (n && (!d_points || !d_shape || !d_dist))) { set_error("knn_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(knn4_check(tree, n, k, "knn_dev"));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    if (n == 0) return BVHGPU_OK;
+    return knn4_launch<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist);
+}
+template <class T> static int knn4_host_impl(Tree4<T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("knn: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(knn4_check(tree, n, k, "knn"));
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    void *d_p = nullptr, *d_r = nullptr;
+    uint32_t* d_s = nullptr;
+    T* d_d = nullptr;
+    BVH_TRY(upload4(ctx, scratch, points, sizeof(T) * 4 * n, &d_p));
+    if (max_dist) BVH_TRY(upload4(ctx, scratch, max_dist, sizeof(T) * n, &d_r));
+    BVH_TRY(scratch.get(&d_s, n * k));
+    BVH_TRY(scratch.get(&d_d, n * k));
+    BVH_TRY(knn4_launch<T>(tree, (const T*)d_p, n, k, (const T*)d_r, d_s, d_d));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n * k, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n * k, cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    return BVHGPU_OK;
+}
+
 // ---- refit / update_shapes ----
 // A failure after the tree was modified leaves arrays that no longer agree with each other: sticky, as a failed build.
 template <class T> static int failed4(Tree4<T>* t, int rc, const char* who) {
@@ -1685,6 +1742,13 @@ struct bvhgpu_tree4d : Tree4<double> {};
     }                                                                                                                     \
     BVH_EXPORT4 int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape) { \
         return any4_dev_impl<T>(tree, dev_rays, nrays, dev_tmax, dev_shape);                                              \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
+        return knn4_host_impl<T>(tree, points, n, k, max_dist, out_shape, out_dist);                                      \
+    }                                                                                                                     \
+    BVH_EXPORT4 int bvhgpu_knn_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, \
+                                         void* dev_shape, void* dev_dist) {                                               \
+        return knn4_dev_impl<T>(tree, dev_points, n, k, dev_max_dist, dev_shape, dev_dist);                               \
     }                                                                                                                     \
     BVH_EXPORT4 int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit4_impl<T>(tree, aabbs, n, false); } \
     BVH_EXPORT4 int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) {                                 \

@@ -207,6 +207,9 @@ template <class T> int query_device(Tree<T>* tree, int mode, int kind, const T* 
 // nearest_to for a batch of points (device pointers): exact reference walk for AABB-distance shapes; candidate lists for any shape
 template <class T> int nearest_device(Tree<T>* tree, int mode, const T* d_points, size_t nq, uint32_t* d_shape, T* d_dist, int use_triangles = 0);
 template <class T> int nearest_candidates_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t* d_offsets, uint32_t* d_cand, size_t cap, size_t* total);
+// k nearest shapes of every point (device pointers: 3 T per point, nq limits or nullptr, nq * k outputs), on the context's stream.
+// Checks nq, k and the tree's status; the pointers are checked by the caller.
+template <class T> int knn_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
 // CSR scan of per-item counts (traverse.cu), launched by the count -> scan -> fill driver of csr.cuh (CsrPasses) for every two-pass
 // walk: scan_local_kernel runs CSR_SCAN_THREADS threads per block over CSR_SCAN_TILE counts and leaves local exclusive offsets and
 // block totals; scan_blocks_kernel (one block of 1024 threads) turns the block totals into exclusive 64-bit block offsets and adds the

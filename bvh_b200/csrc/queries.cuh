@@ -3,6 +3,7 @@
 // left to right in T without FMA, so the instantiation for D = 3 performs exactly the operations the 3-D kernels always did.
 #pragma once
 #include "common.cuh"
+#include <type_traits>
 
 namespace bvhb200 {
 
@@ -188,6 +189,93 @@ __device__ __forceinline__ void nearest_walk(const Node* __restrict__ nodes, con
         if (node == 0) return;                              // back from the farther child of the root
         from = node; node = meta.x;
     }
+}
+
+// ---- k nearest shapes (bvhgpu_knn_*): the parent-link walk of nearest_walk<D, T, false> keeping the K best keys ----
+// The key of shape s is (d2, s) in lexicographic order, d2 = leaf(s) (aabb_min_d2 of the shape's own current box, never NaN).  The
+// list d[0 .. K) / s[0 .. K) is sorted DESCENDING.  Slots 0 .. k-1 start as (+inf, BVH_INVALID), worse than every real key; slots
+// k .. K-1 hold (-inf, BVH_INVALID) sentinels that no key passes.  So d[0], s[0] is the current k-th key for any k <= K, the insertion
+// shifts towards slot 0, and every array index is a compile-time constant: the list stays in registers when it fits.
+// A child is entered when its box is empty or box_lower_d2 <= min(d[0], r2): every shape below it has a key >= that bound (the bound
+// is monotone under containment and stays below the rounded distance of the shape's own box, see Query<T, QUERY_WITHIN, D>), so a
+// pruned subtree holds no shape that could still enter the list or qualify.  Ties are entered, so an equal key with a lower index is
+// never lost, and the result is the brute-force order whatever the visiting order.
+template <class T> __device__ __forceinline__ bool key_less(T a, uint32_t ia, T b, uint32_t ib) { return a < b || (a == b && ia < ib); }
+template <class T, int K> __device__ __forceinline__ void knn_insert(T (&d)[K], uint32_t (&s)[K], T key, uint32_t id) {
+    bool moving = true;                                     // slot 0 (the k-th key) is dropped; (key, id) goes where it belongs
+#pragma unroll
+    for (int j = 0; j + 1 < K; ++j) {
+        const bool shift = moving && key_less(key, id, d[j + 1], s[j + 1]);
+        if (moving) { d[j] = shift ? d[j + 1] : key; s[j] = shift ? s[j + 1] : id; }
+        moving = shift;
+    }
+    if (moving) { d[K - 1] = key; s[K - 1] = id; }
+}
+template <int D, class T, int K, class Node, class Leaf>
+__device__ __forceinline__ void knn_walk(const Node* __restrict__ nodes, const T p[D], T r2, T (&d)[K], uint32_t (&s)[K], Leaf leaf) {
+    uint32_t node = 0, from = BVH_INVALID;
+    for (;;) {
+        const uint4 meta = __ldg(reinterpret_cast<const uint4*>(nodes + node));      // parent, child_l, child_r, shape
+        if (meta.y == BVH_INVALID) {
+            const T key = leaf(meta.w);
+            if (key <= r2 && key_less(key, meta.w, d[0], s[0])) knn_insert(d, s, key, meta.w);
+            if (node == 0) return;
+            from = node; node = meta.x;
+            continue;
+        }
+        const Node& nd = nodes[node];
+        T lmn[D], lmx[D], rmn[D], rmx[D];
+        bool el = false, er = false;
+#pragma unroll
+        for (int k = 0; k < D; ++k) {
+            lmn[k] = __ldg(&nd.l_aabb.min[k]); lmx[k] = __ldg(&nd.l_aabb.max[k]); rmn[k] = __ldg(&nd.r_aabb.min[k]); rmx[k] = __ldg(&nd.r_aabb.max[k]);
+            el |= lmn[k] > lmx[k]; er |= rmn[k] > rmx[k];
+        }
+        const T dl = box_lower_d2<D>(p, lmn, lmx), dr = box_lower_d2<D>(p, rmn, rmx);
+        const bool swap = dl > dr;
+        const uint32_t near_i = swap ? meta.z : meta.y, far_i = swap ? meta.y : meta.z;
+        const T near_d = swap ? dr : dl, far_d = swap ? dl : dr;
+        const bool near_e = swap ? er : el, far_e = swap ? el : er;
+        uint32_t next = BVH_INVALID;
+        if (from == BVH_INVALID) {                          // first visit: the nearer child
+            if (near_e || (near_d <= d[0] && near_d <= r2)) next = near_i;
+            else from = near_i;                             // skipped: as if we had just returned from it
+        }
+        if (next == BVH_INVALID && from == near_i) {        // back from (or past) the nearer child: the farther one, against the new k-th key
+            if (far_e || (far_d <= d[0] && far_d <= r2)) next = far_i;
+            else from = far_i;
+        }
+        if (next != BVH_INVALID) { node = next; from = BVH_INVALID; continue; }
+        if (node == 0) return;
+        from = node; node = meta.x;
+    }
+}
+// One point of a knn batch: limit r (has_limit) qualifies the shapes with d2 <= fl(r * r) (Ball::intersects_aabb's comparison); r < 0
+// or NaN qualifies none (-0 >= 0 holds); an empty tree (n_shapes == 0) none.  Row i*k .. i*k+k-1 of the outputs gets the list in
+// ascending order, sqrt of each key as the distance, (BVH_INVALID, +inf) past the qualifying shapes.
+template <int D, class T, int K, class Node, class Leaf>
+__device__ __forceinline__ void knn_point(const Node* __restrict__ nodes, uint32_t n_shapes, const T p[D], bool has_limit, T r, uint32_t k,
+                                          uint32_t* __restrict__ out_shape, T* __restrict__ out_dist, Leaf leaf) {
+    T d[K];
+    uint32_t s[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) { d[j] = j < (int)k ? Traits<T>::inf() : -Traits<T>::inf(); s[j] = BVH_INVALID; }
+    const T r2 = has_limit ? mul_rn(r, r) : Traits<T>::inf();
+    if (n_shapes != 0 && (!has_limit || r >= T(0))) knn_walk<D, T, K>(nodes, p, r2, d, s, leaf);
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+        if (j < (int)k) { out_shape[k - 1 - j] = s[j]; out_dist[k - 1 - j] = d[j]; }
+    // the square roots in a loop of its own: one call site of sqrt's slow path instead of K, none with the list live (no spills)
+#pragma unroll 1
+    for (uint32_t j = 0; j < k; ++j) out_dist[j] = sqrt_rn(out_dist[j]);
+}
+// The K bucket of knn_walk for 1 <= k <= BVHGPU_KNN_MAX_K: launch(std::integral_constant<int, K>{}).
+template <class Launch> inline void knn_bucket(uint32_t k, Launch launch) {
+    if (k <= 4) launch(std::integral_constant<int, 4>{});
+    else if (k <= 8) launch(std::integral_constant<int, 8>{});
+    else if (k <= 16) launch(std::integral_constant<int, 16>{});
+    else if (k <= 32) launch(std::integral_constant<int, 32>{});
+    else launch(std::integral_constant<int, 64>{});
 }
 
 // FlatBvh::nearest_to (flat_bvh.rs:513-562) over the reference FlatNode array.  Flat: a bvh_flat{D}{f,d} POD.

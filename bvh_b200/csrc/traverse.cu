@@ -1469,6 +1469,39 @@ int nearest_candidates_device(Tree<T>* tree, const T* d_points, size_t nq, uint3
 }
 template int nearest_device<float>(Tree<float>*, int, const float*, size_t, uint32_t*, float*, int);
 template int nearest_device<double>(Tree<double>*, int, const double*, size_t, uint32_t*, double*, int);
+
+// ---- k nearest shapes: knn_walk<3, T, K> (queries.cuh) over the node array, keys from the shapes' own boxes (d_aabb); one thread per
+// point.  A 2-D tree runs here on points lifted to z = 0 (dim2.cu). ----
+template <class T, int K>
+__global__ void __launch_bounds__(128) knn_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_shapes,
+                                                  const typename Traits<T>::DAabb* __restrict__ aabb, const T* __restrict__ points,
+                                                  const T* __restrict__ max_dist, uint32_t nq, uint32_t k, uint32_t* __restrict__ out_shape,
+                                                  T* __restrict__ out_dist) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    T p[3];
+    for (int c = 0; c < 3; ++c) p[c] = points[3 * (size_t)i + c];
+    auto leaf = [&](uint32_t shape) { T mn[3], mx[3]; load_aabb(aabb + shape, mn, mx); return aabb_min_d2<3>(p, mn, mx); };
+    knn_point<3, T, K>(nodes, n_shapes, p, max_dist != nullptr, max_dist ? max_dist[i] : T(0), k, out_shape + (size_t)i * k,
+                       out_dist + (size_t)i * k, leaf);
+}
+template <class T>
+int knn_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist) {
+    if (nq > 0x7FFFFFFFull) { set_error("knn: n = %zu exceeds 2^31-1", nq); return BVHGPU_ERR_INVALID; }
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(resolve_status(tree));
+    if (nq == 0) return BVHGPU_OK;
+    bvhgpu_ctx* ctx = tree->ctx;
+    const unsigned grid = (unsigned)((nq + 127) / 128);
+    knn_bucket(k, [&](auto kb) {
+        knn_kernel<T, decltype(kb)::value><<<grid, 128, 0, ctx->stream>>>(tree->d_nodes, tree->n, tree->d_aabb, d_points, d_max_dist, (uint32_t)nq, k, d_shape, d_dist);
+    });
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+template int knn_device<float>(Tree<float>*, const float*, size_t, uint32_t, const float*, uint32_t*, float*);
+template int knn_device<double>(Tree<double>*, const double*, size_t, uint32_t, const double*, uint32_t*, double*);
 template int nearest_candidates_device<float>(Tree<float>*, const float*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 template int nearest_candidates_device<double>(Tree<double>*, const double*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 

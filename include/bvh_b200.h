@@ -527,6 +527,36 @@ int bvhgpu_any_hit_f64x4(bvhgpu_tree4d* tree, const bvh_ray4d* rays, size_t nray
 int bvhgpu_any_hit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape);
 int bvhgpu_any_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape);
 
+/* ---- k nearest shapes with an optional per-point radius: the query of point-cloud, neighbour-search and collision code that the
+ * reference leaves to a loop over Bvh::traverse with a guessed Ball and a sort.  `points`: D T per point (D = 2, 3, 4).  For point i
+ * the key of shape s is d2_s = Aabb::min_distance_squared(p_i) of the shape's OWN CURRENT AABB (after refit, update, add and remove;
+ * src/aabb/aabb_impl.rs:618-629, the reference's operation order, no FMA; the clamp maps NaN to 0, so no key is NaN).
+ * Shape s qualifies when `max_dist` is NULL, or when max_dist[i] >= 0 (-0 included) and d2_s <= fl(max_dist[i] * max_dist[i]), the
+ * comparison of Ball::intersects_aabb.  max_dist[i] < 0 or NaN: nothing qualifies; +inf: everything does.
+ * Output, row-major, k slots per point: out_shape[i*k + j] is the j-th qualifying shape in ascending (d2_s, s) order and
+ * out_dist[i*k + j] = fl(sqrt(d2_s)), the distance bvhgpu_nearest_* returns; slots past the qualifying shapes hold
+ * BVHGPU_INVALID_INDEX and +inf.  Exact: every row is the first min(k, #qualifying) entries of a stable brute-force sort, for every
+ * input (points with NaN or infinite coordinates included).  Pruning uses a lower bound of the distance (rounding slack per axis,
+ * monotone under box containment) with ties entered, and empty child boxes ("no split wins" nodes) are always entered.
+ *   k = 1 is NOT bvhgpu_nearest_*: Bvh::nearest_to prunes with the rounded reference distance, which is not monotone, and on large
+ *   coordinates can return a shape that brute force does not pick.  k = 1 is the brute-force minimum of min_distance_squared, ties
+ *   to the lower index.
+ *   Distances are the AABB's (the UnitBox PointDistance of bvhgpu_nearest_*); there is no triangle form.
+ * 1 <= k <= BVHGPU_KNN_MAX_K.  k out of range, a null argument or n > 2^31-1: BVHGPU_ERR_INVALID, nothing written.  n = 0: no-op.
+ * An empty tree: rows of padding.  A failed build is reported sticky.  The _dev forms take device pointers (dev_max_dist may be
+ * NULL), check k and the pointers on the host and enqueue on the context's stream without synchronising; D = 2 has host pointers only. */
+#define BVHGPU_KNN_MAX_K 64
+int bvhgpu_knn_f32x3(bvhgpu_tree3f* tree, const float* points, size_t n, uint32_t k, const float* max_dist, uint32_t* out_shape, float* out_dist);
+int bvhgpu_knn_f64x3(bvhgpu_tree3d* tree, const double* points, size_t n, uint32_t k, const double* max_dist, uint32_t* out_shape, double* out_dist);
+int bvhgpu_knn_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, void* dev_shape, void* dev_dist);
+int bvhgpu_knn_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, void* dev_shape, void* dev_dist);
+int bvhgpu_knn_f32x2(bvhgpu_tree2f* tree, const float* points, size_t n, uint32_t k, const float* max_dist, uint32_t* out_shape, float* out_dist);
+int bvhgpu_knn_f64x2(bvhgpu_tree2d* tree, const double* points, size_t n, uint32_t k, const double* max_dist, uint32_t* out_shape, double* out_dist);
+int bvhgpu_knn_f32x4(bvhgpu_tree4f* tree, const float* points, size_t n, uint32_t k, const float* max_dist, uint32_t* out_shape, float* out_dist);
+int bvhgpu_knn_f64x4(bvhgpu_tree4d* tree, const double* points, size_t n, uint32_t k, const double* max_dist, uint32_t* out_shape, double* out_dist);
+int bvhgpu_knn_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, void* dev_shape, void* dev_dist);
+int bvhgpu_knn_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, void* dev_shape, void* dev_dist);
+
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
  * leaves (user code), so there are two forms.  `points`: 3 T per query point, host pointers.
