@@ -45,8 +45,13 @@ __global__ void __launch_bounds__(256) morton_kernel(const typename Traits<T>::D
     for (int k = 0; k < 3; ++k) {
         const double lo = (double)key2f(rootkeys[6 + k]), hi = (double)key2f(rootkeys[9 + k]);
         const double c = (double)center1(mn[k], mx[k]);
-        double u = hi > lo ? (c - lo) / (hi - lo) : 0.0;
-        u = u < 0.0 ? 0.0 : (u > 1.0 ? 1.0 : u);
+        double num = c - lo, den = hi - lo;
+        if (den == __longlong_as_double(0x7ff0000000000000ll)) {    // f64 extent beyond DBL_MAX: quantise with both operands halved
+            num = c * 0.5 - lo * 0.5;
+            den = hi * 0.5 - lo * 0.5;
+        }
+        double u = hi > lo ? num / den : 0.0;
+        u = u >= 0.0 ? (u > 1.0 ? 1.0 : u) : 0.0;                  // NaN -> 0: never convert a NaN to an integer
         unsigned long long q = (unsigned long long)(u * 2097151.0);
         if (q > 2097151ull) q = 2097151ull;
         code |= expand21(q) << (2 - k);
@@ -140,10 +145,10 @@ __global__ void __launch_bounds__(256) box_up_kernel(const typename Traits<T>::D
         const uint32_t sib = left[par] == v ? right[par] : left[par];
         const T* sb = boxes + 12ull * sib;
 #pragma unroll
-        for (int k = 0; k < 12; ++k) {
+        for (int k = 0; k < 12; ++k) {                         // min_t / max_t: order-free, -0 below +0 (whichever thread arrives second)
             const T o = __ldcg(sb + k);
             const bool isMin = (k % 6) < 3;
-            b[k] = isMin ? (o < b[k] ? o : b[k]) : (o > b[k] ? o : b[k]);
+            b[k] = isMin ? min_t(o, b[k]) : max_t(o, b[k]);
         }
         v = par;
         T* d = boxes + 12ull * v;
