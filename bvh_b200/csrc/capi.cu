@@ -7,10 +7,12 @@
 #include <algorithm>
 #include <cctype>
 #include <sched.h>
+#include <type_traits>
 
 namespace bvhb200 {
 
 static thread_local std::string g_last_error;
+const char* last_error() { return g_last_error.c_str(); }
 
 void set_error(const char* fmt, ...) {
     char buf[1024];
@@ -32,9 +34,8 @@ void dfree(bvhgpu_ctx* ctx, void* p) {
 }
 
 // Resolve the deferred device status of a build (synchronises the stream once).
-// A failure is STICKY: the node arrays of a tree whose build / refit / optimize failed are uninitialised or half rewritten,
-// so every later entry point on that tree reports the same status again (the reference panicked at this point and the
-// Bvh never existed); only bvhgpu_tree_free_* is meaningful afterwards.
+// A failure is STICKY (mark_failed): the node arrays of a tree whose build / refit / optimize failed are uninitialised or half
+// rewritten (the reference panicked at this point and the Bvh never existed).
 template <class T> int resolve_status(Tree<T>* tree) {
     if (tree->failed_status != BVHGPU_OK) { set_error("%s", tree->failed_message.c_str()); return tree->failed_status; }
     if (!tree->status_pending) return BVHGPU_OK;
@@ -48,8 +49,7 @@ template <class T> int resolve_status(Tree<T>* tree) {
     if (h.nan_found) { snprintf(msg, sizeof msg, "build: NaN coordinate in an input AABB (the reference panics here, src/bvh/bvh_node.rs:214-217); the tree is unusable"); rc = BVHGPU_ERR_NAN; }
     else if (h.error == BVHGPU_ERR_TIMEOUT) { snprintf(msg, sizeof msg, "build: device watchdog fired (tickets=%u leaves=%u/%u); the tree is unusable", h.tickets, h.leaves_done, tree->n); rc = BVHGPU_ERR_TIMEOUT; }
     else if (h.error) { snprintf(msg, sizeof msg, "build: device reported status %u (tickets=%u leaves=%u/%u); the tree is unusable", h.error, h.tickets, h.leaves_done, tree->n); rc = (int)h.error; }
-    if (rc != BVHGPU_OK) { tree->failed_status = rc; tree->failed_message = msg; set_error("%s", msg); }
-    return rc;
+    return rc == BVHGPU_OK ? rc : mark_failed(tree, rc, nullptr, msg);
 }
 
 template int resolve_status<float>(Tree<float>*);
@@ -62,6 +62,14 @@ template <class T> static void tree_release(Tree<T>* t) {
         dfree(ctx, t->d_aabb); dfree(ctx, t->d_aabb_trav); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
         dfree(ctx, t->d_tris); dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad); dfree(ctx, t->d_tnodes); dfree(ctx, t->d_top); dfree(ctx, t->d_flat); dfree(ctx, t->d_status); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
     }
+}
+
+template <class T> static void tree_release(Tree4<T>* t) {
+    if (!t || !t->ctx) return;
+    bvhgpu_ctx* ctx = t->ctx;
+    dfree(ctx, t->d_aabb); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
+    dfree(ctx, t->d_trec); dfree(ctx, t->d_flat); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
+    dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad);
 }
 
 template <class T, class TreeT>
@@ -195,21 +203,81 @@ template <class T> static int flatten_impl(Tree<T>* tree, typename Traits<T>::Fl
     return BVHGPU_OK;
 }
 
-template <class T> static int ensure_result_buffers(Tree<T>* tree, size_t nrays, size_t hits_cap) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    if (tree->offsets_cap < nrays + 1) {
-        dfree(ctx, tree->d_offsets); tree->d_offsets = nullptr; tree->offsets_cap = 0;
-        BVH_TRY(dalloc_t(ctx, &tree->d_offsets, nrays + 1));
-        tree->offsets_cap = nrays + 1;
+// ---- D = 4 (dim4.cu): exact SAH build only, synchronous; node and flat arrays in the ABI layout already ----
+template <class T, class TreeT> static int build4_impl(bvhgpu_ctx* ctx, const typename D4<T>::Aabb* aabbs, size_t n, int mode, TreeT** out) {
+    if (!ctx || !out || (n && !aabbs)) { set_error("build: null argument"); return BVHGPU_ERR_INVALID; }
+    *out = nullptr;
+    if (n > (1ull << 30)) { set_error("build: n = %zu exceeds 2^30 shapes", n); return BVHGPU_ERR_INVALID; }
+    if (mode == BVHGPU_BUILD_LBVH || mode == BVHGPU_BUILD_LBVH_TREELET) {
+        set_error("build: D = 4 has the exact SAH build only (BVHGPU_BUILD_EXACT_SAH); the LBVH modes are not implemented for D = 4");
+        return BVHGPU_ERR_UNSUPPORTED;
     }
-    if (tree->hits_cap < hits_cap) {
-        dfree(ctx, tree->d_hits); tree->d_hits = nullptr; tree->hits_cap = 0;
-        BVH_TRY(dalloc_t(ctx, &tree->d_hits, hits_cap));
-        tree->hits_cap = hits_cap;
+    if (mode != BVHGPU_BUILD_EXACT_SAH) { set_error("build: unknown mode %d", mode); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    TreeT* tree = new (std::nothrow) TreeT();
+    if (!tree) { set_error("build: out of host memory"); return BVHGPU_ERR_INTERNAL; }
+    tree->ctx = ctx;
+    tree->n = (uint32_t)n;
+    tree->n_nodes = n ? 2 * (uint32_t)n - 1 : 0;
+    const int rc = n ? build4<T>(tree, aabbs, cudaMemcpyHostToDevice) : (int)BVHGPU_OK;
+    if (rc != BVHGPU_OK) { tree_release<T>(tree); delete tree; return rc; }
+    *out = tree;
+    return BVHGPU_OK;
+}
+template <class T> static int tree_nodes_impl(Tree4<T>* tree, typename D4<T>::Node* out_nodes, uint32_t* out_node_index) {
+    if (!tree) { set_error("tree_nodes: null tree"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(resolve_status(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (tree->n == 0) return BVHGPU_OK;
+    if (out_nodes) BVH_CUDA_TRY(cudaMemcpyAsync(out_nodes, tree->d_nodes, sizeof(*out_nodes) * tree->n_nodes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_node_index) BVH_CUDA_TRY(cudaMemcpyAsync(out_node_index, tree->d_node_index, sizeof(uint32_t) * tree->n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T> static int flatten_impl(Tree4<T>* tree, typename D4<T>::Flat* out, size_t cap, size_t* len) {
+    if (!tree) { set_error("flatten: null tree"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(resolve_status(tree));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(build_flat4(tree));
+    if (len) *len = tree->n_flat;
+    if (out) {
+        if (cap < tree->n_flat) { set_error("flatten: capacity %zu < %zu flat nodes", cap, tree->n_flat); return BVHGPU_ERR_CAPACITY; }
+        if (tree->n_flat) BVH_CUDA_TRY(cudaMemcpyAsync(out, tree->d_flat, sizeof(*out) * tree->n_flat, cudaMemcpyDeviceToHost, ctx->stream));
+        BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     }
     return BVHGPU_OK;
 }
 
+// The size guard of the batched calls: n must fit the kernels' u32 item indices.
+static int check_n(const char* what, size_t n) {
+    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+
+// The tree type of dimension D: Bvh<T,2> lives embedded in the 3-D tree (dim2.cu), Bvh<T,4> has its own (dim4.cu).
+template <int D, class T> using TreeOf = typename std::conditional<D == 4, Tree4<T>, Tree<T>>::type;
+
+// A host batch staged on the device.  D = 3, 4: the C-ABI records as they are.  D = 2: records of 2-vectors (a Bvh<T,2> embedded in
+// z = 0), lifted on the device before they reach the 3-D kernels: nvec 2-vectors and nscal scalars per record (dim2_lift), or
+// RAY_RECORD: rays of 6 T (dim2_expand_rays, 9 T), or AABB_RECORD: boxes of 4 T (dim2_expand_aabbs, 6 T).  There is no fetch
+// call for D = 2, so a short `cap` is answered with "call again with cap = *total" and the retained buffers are re-used by that call.
+constexpr int RAY_RECORD = -1, AABB_RECORD = -2;
+template <int D, class T> static int upload_records(bvhgpu_ctx* ctx, Scratch& scratch, const void* h, size_t n, int nvec, int nscal, T** d_out) {
+    const size_t in_w = nvec == RAY_RECORD ? 3 * D : nvec == AABB_RECORD ? 2 * D : (size_t)D * nvec + nscal;
+    T* d_in = nullptr;
+    BVH_TRY(scratch.get(&d_in, n * in_w));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_in, h, sizeof(T) * n * in_w, cudaMemcpyHostToDevice, ctx->stream));
+    if (D != 2) { *d_out = d_in; return BVHGPU_OK; }
+    T* d_lift = nullptr;
+    BVH_TRY(scratch.get(&d_lift, n * (nvec == RAY_RECORD ? 9 : nvec == AABB_RECORD ? 6 : 3 * (size_t)nvec + nscal)));
+    if (nvec == RAY_RECORD) BVH_TRY(dim2_expand_rays<T>(ctx, d_in, (uint32_t)n, d_lift));
+    else if (nvec == AABB_RECORD) BVH_TRY(dim2_expand_aabbs<T>(ctx, d_in, (uint32_t)n, d_lift));
+    else BVH_TRY(dim2_lift<T>(ctx, d_in, (uint32_t)n, nvec, nscal, d_lift));
+    *d_out = d_lift;
+    return BVHGPU_OK;
+}
 // The host-pointer CSR calls of a 3-D (or lifted 2-D) tree run into the tree's retained buffers, which bvhgpu_traverse_fetch_*
 // reads later.  The hit buffer starts at max(hits_cap, per_item * n, 1024).  When run(d_offsets, d_hits, cap, &tot) reports
 // BVHGPU_ERR_CAPACITY with a total the u32 offsets can hold, the buffer grows to that total and the call runs once more.
@@ -243,74 +311,119 @@ static int retained_to_host(Tree<T>* tree, const char* what, size_t n, size_t pe
     return ret;
 }
 
-template <class T>
-static int traverse_host_impl(Tree<T>* tree, int mode, const void* rays, uint32_t fmt, size_t nrays,
+// Ray traversal, host pointers.  D = 3: the streamed host traversal.  D = 2: rays of 6 T lifted on the device (dim2_expand_rays)
+// and walked by traverse_device.  D = 4: rays of 12 T through csr4_host.
+template <int D, class T>
+static int traverse_host_impl(TreeOf<D, T>* tree, int mode, const void* rays, uint32_t fmt, size_t nrays,
                               uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D != 2) BVH_TRY(check_n("traverse", nrays));
+    if (D == 4 && mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
-    if (nrays == 0 || tree->n == 0) {                            // nothing to pipeline
-        size_t tot0 = 0;
-        BVH_TRY(ensure_result_buffers(tree, nrays, 1024));
-        BVH_TRY(traverse_device<T>(tree, mode, nullptr, fmt, nrays, tree->d_offsets, tree->d_hits, tree->hits_cap, &tot0));
-        BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, ctx->stream));
-        BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        if (total) *total = 0;
+    if (D == 2) BVH_TRY(check_n("traverse", nrays));            // a 2-D tree reports a sticky failure first
+    Scratch scratch(ctx);
+    T* d_rays = nullptr;
+    if constexpr (D == 4) {
+        if (nrays && tree->n) BVH_TRY(upload_records<D>(ctx, scratch, rays, nrays, RAY_RECORD, 0, &d_rays));
+        return csr4_host<T>(tree, PROBE_RAYS4, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, offsets, hits, cap, total, "traverse");
+    } else if constexpr (D == 2) {
+        if (nrays) BVH_TRY(upload_records<D>(ctx, scratch, rays, nrays, RAY_RECORD, 0, &d_rays));
+        return retained_to_host<D>(tree, "traverse", nrays, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+            return traverse_device<T>(tree, mode, d_rays, BVHGPU_RAYS_FULL, nrays, d_off, d_hits, hcap, t);
+        });
+    } else {
+        if (nrays == 0 || tree->n == 0) {                            // nothing to pipeline
+            size_t tot0 = 0;
+            BVH_TRY(ensure_result_buffers(tree, nrays, 1024));
+            BVH_TRY(traverse_device<T>(tree, mode, nullptr, fmt, nrays, tree->d_offsets, tree->d_hits, tree->hits_cap, &tot0));
+            BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, ctx->stream));
+            BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+            if (total) *total = 0;
+            return BVHGPU_OK;
+        }
+        size_t tot = 0;
+        const int rc = run_retained(tree, nrays, 4, &tot, [&](uint32_t*, uint32_t*, size_t, size_t* t) {   // copies back for itself
+            return traverse_host_pipelined<T>(tree, mode, rays, fmt, nrays, offsets, hits, cap, t);
+        });
+        if (total) *total = tot;
+        if (rc != BVHGPU_OK) return rc;
+        if (tot > cap) {
+            set_error("traverse: %zu hits do not fit the caller's capacity %zu (use bvhgpu_traverse_fetch_*)", tot, cap);
+            return BVHGPU_ERR_CAPACITY;
+        }
         return BVHGPU_OK;
     }
-    size_t tot = 0;
-    const int rc = run_retained(tree, nrays, 4, &tot, [&](uint32_t*, uint32_t*, size_t, size_t* t) {   // copies back for itself
-        return traverse_host_pipelined<T>(tree, mode, rays, fmt, nrays, offsets, hits, cap, t);
-    });
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK) return rc;
-    if (tot > cap) {
-        set_error("traverse: %zu hits do not fit the caller's capacity %zu (use bvhgpu_traverse_fetch_*)", tot, cap);
-        return BVHGPU_ERR_CAPACITY;
+}
+// Ray traversal, device pointers (D = 3, 4): enqueued on the context's stream; synchronises only to return *total.
+template <int D, class T>
+static int traverse_dev_impl(TreeOf<D, T>* tree, int mode, const void* d_rays, uint32_t fmt, size_t nrays, uint32_t* d_offsets, uint32_t* d_hits,
+                             size_t cap, size_t* total, const char* what) {
+    if (!tree || !d_offsets || (nrays && !d_rays)) { set_error("%s: null argument", what); return BVHGPU_ERR_INVALID; }
+    if constexpr (D == 4) {
+        BVH_TRY(check_n("traverse", nrays));
+        if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+        BVH_TRY(resolve_status(tree));
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+        return csr4_device<T>(tree, PROBE_RAYS4, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, d_offsets, d_hits, cap, total, "traverse");
+    } else {
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+        return traverse_device<T>(tree, mode, d_rays, fmt, nrays, d_offsets, d_hits, cap, total);
     }
-    return BVHGPU_OK;
 }
 
-// D = 3: the C-ABI records as they are.  D = 2: records of 2-vectors (a Bvh<T,2> embedded in z = 0), lifted on the device
-// (dim2_lift) before they reach the 3-D kernels; there is no fetch call for D = 2, so a short `cap` is answered with
-// "call again with cap = *total" and the retained buffers are re-used by that call.
-template <int D, class T> static int upload_records(Tree<T>* tree, Scratch& scratch, const T* h, size_t n, int nvec, int nscal, T** d_out) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    const size_t in_w = (size_t)D * nvec + nscal;
-    T* d_in = nullptr;
-    BVH_TRY(scratch.get(&d_in, n * in_w));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_in, h, sizeof(T) * n * in_w, cudaMemcpyHostToDevice, ctx->stream));
-    if (D == 3) { *d_out = d_in; return BVHGPU_OK; }
-    T* d_lift = nullptr;
-    BVH_TRY(scratch.get(&d_lift, n * (3 * (size_t)nvec + nscal)));
-    BVH_TRY(dim2_lift<T>(ctx, d_in, (uint32_t)n, nvec, nscal, d_lift));
-    *d_out = d_lift;
-    return BVHGPU_OK;
-}
-template <class T, int D = 3>
-static int query_host_impl(Tree<T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+static bool bad_mode(int mode) { return mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT; }
+
+// Aabb / Point / Ball queries, host pointers: records of 2D / D / D + 1 T.  The mode of a 3-D call is checked by query_device.
+template <int D, class T>
+static int query_host_impl(TreeOf<D, T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || (n && !queries) || !offsets) { set_error("query: null argument"); return BVHGPU_ERR_INVALID; }
     if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
-    if (D != 3 && n > 0x7FFFFFFFull) { set_error("query: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
-    if (D != 3 && mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("query: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("query", n));
+    if (D != 3 && bad_mode(mode)) { set_error("query: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
     const int nvec = kind == BVHGPU_QUERY_AABB ? 2 : 1, nscal = kind == BVHGPU_QUERY_BALL ? 1 : 0;
     T* d_q = nullptr;
     Scratch scratch(ctx);                                           // released on every return path
-    if (n) BVH_TRY(upload_records<D>(tree, scratch, queries, n, nvec, nscal, &d_q));
-    return retained_to_host<D>(tree, "query", n, 16, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-        return query_device<T>(tree, mode, kind, d_q, n, d_off, d_hits, hcap, t);
-    });
+    if (n) BVH_TRY(upload_records<D>(ctx, scratch, queries, n, nvec, nscal, &d_q));
+    if constexpr (D == 4) {
+        return csr4_host<T>(tree, kind, mode == BVHGPU_TRAVERSE_FLAT, d_q, n, offsets, hits, cap, total, "query");
+    } else {
+        return retained_to_host<D>(tree, "query", n, 16, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+            return query_device<T>(tree, mode, kind, d_q, n, d_off, d_hits, hcap, t);
+        });
+    }
+}
+// Queries, device pointers (D = 3, 4).  query_device also serves the library's internal kinds (nearest_candidates): only the public
+// ones get through here.  With `total` given the call synchronises, and the CSR is complete when it returns.
+template <int D, class T>
+static int query_dev_impl(TreeOf<D, T>* tree, int mode, int kind, const void* d_queries, size_t n, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
+    if (!tree || !d_offsets || (n && !d_queries)) { set_error("query_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
+    int rc;
+    if constexpr (D == 4) {
+        BVH_TRY(check_n("query_dev", n));
+        if (bad_mode(mode)) { set_error("query_dev: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+        BVH_TRY(resolve_status(tree));
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+        rc = csr4_device<T>(tree, kind, mode == BVHGPU_TRAVERSE_FLAT, d_queries, n, d_offsets, d_hits, cap, total, "query_dev");
+    } else {
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+        rc = query_device<T>(tree, mode, kind, (const T*)d_queries, n, d_offsets, d_hits, cap, total);
+    }
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
+    return rc;
 }
 
-template <class T, int D = 3>
-static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist, int use_triangles = 0) {
+// nearest_to, host pointers: D T per point.  The mode of a 3-D call is checked by nearest_device.
+template <int D, class T>
+static int nearest_host_impl(TreeOf<D, T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist, int use_triangles = 0) {
     if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("nearest: null argument"); return BVHGPU_ERR_INVALID; }
-    if (D != 3 && n > 0x7FFFFFFFull) { set_error("nearest: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
-    if (D != 3 && mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("nearest: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("nearest", n));
+    if (D != 3 && bad_mode(mode)) { set_error("nearest: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
@@ -318,10 +431,12 @@ static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n,
     T *d_p = nullptr, *d_d = nullptr;
     uint32_t* d_s = nullptr;
     Scratch scratch(ctx);
-    BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
+    BVH_TRY(upload_records<D>(ctx, scratch, points, n, 1, 0, &d_p));
     BVH_TRY(scratch.get(&d_d, n));
     BVH_TRY(scratch.get(&d_s, n));
-    int rc = nearest_device<T>(tree, mode, d_p, n, d_s, d_d, use_triangles);
+    int rc;
+    if constexpr (D == 4) rc = nearest4_device<T>(tree, mode, d_p, n, d_s, d_d);
+    else rc = nearest_device<T>(tree, mode, d_p, n, d_s, d_d, use_triangles);
     if (rc == BVHGPU_OK) {
         BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
         BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -330,11 +445,11 @@ static int nearest_host_impl(Tree<T>* tree, int mode, const T* points, size_t n,
     return rc;
 }
 
-// k nearest shapes, host pointers: D = 3 points as they are, D = 2 points lifted to z = 0 (dim2.cu); n * k results copied back.
-template <class T, int D = 3>
-static int knn_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) {
+// k nearest shapes, host pointers: D T per point (D = 2 lifted to z = 0, dim2.cu), n optional limits; n * k results copied back.
+template <int D, class T>
+static int knn_host_impl(TreeOf<D, T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) {
     if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("knn: null argument"); return BVHGPU_ERR_INVALID; }
-    if (n > 0x7FFFFFFFull) { set_error("knn: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("knn", n));
     if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
@@ -343,63 +458,71 @@ static int knn_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t k, c
     T *d_p = nullptr, *d_r = nullptr, *d_d = nullptr;
     uint32_t* d_s = nullptr;
     Scratch scratch(ctx);
-    BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
+    BVH_TRY(upload_records<D>(ctx, scratch, points, n, 1, 0, &d_p));
     if (max_dist) {
         BVH_TRY(scratch.get(&d_r, n));
         BVH_CUDA_TRY(cudaMemcpyAsync(d_r, max_dist, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
     }
     BVH_TRY(scratch.get(&d_s, n * k));
     BVH_TRY(scratch.get(&d_d, n * k));
-    BVH_TRY(knn_device<T>(tree, d_p, n, k, d_r, d_s, d_d));
+    if constexpr (D == 4) BVH_TRY(knn4_device<T>(tree, d_p, n, k, d_r, d_s, d_d));
+    else BVH_TRY(knn_device<T>(tree, d_p, n, k, d_r, d_s, d_d));
     BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n * k, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n * k, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return BVHGPU_OK;
 }
+// k nearest shapes, device pointers (D = 3, 4): the device driver checks n, k and the tree's status.
+template <int D, class T>
+static int knn_dev_impl(TreeOf<D, T>* tree, const void* d_points, size_t n, uint32_t k, const void* d_max_dist, void* d_shape, void* d_dist) {
+    if (!tree || (n && (!d_points || !d_shape || !d_dist))) { set_error("knn_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    if constexpr (D == 4) return knn4_device<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist);
+    else return knn_device<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist);
+}
 
-template <class T, int D = 3>
-static int nearest_candidates_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
+template <int D, class T>
+static int nearest_candidates_host_impl(TreeOf<D, T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
     if (!tree || (n && !points) || !offsets) { set_error("nearest_candidates: null argument"); return BVHGPU_ERR_INVALID; }
-    if (D != 3 && n > 0x7FFFFFFFull) { set_error("nearest_candidates: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("nearest_candidates", n));
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
     T* d_p = nullptr;
     Scratch scratch(ctx);
-    if (n) BVH_TRY(upload_records<D>(tree, scratch, points, n, 1, 0, &d_p));
-    return retained_to_host<D>(tree, "nearest_candidates", n, 16, offsets, cand, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-        return nearest_candidates_device<T>(tree, d_p, n, d_off, d_hits, hcap, t);
-    });
+    if (n) BVH_TRY(upload_records<D>(ctx, scratch, points, n, 1, 0, &d_p));
+    if constexpr (D == 4) {
+        return nearest_candidates4<T>(tree, d_p, n, offsets, cand, cap, total);
+    } else {
+        return retained_to_host<D>(tree, "nearest_candidates", n, 16, offsets, cand, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+            return nearest_candidates_device<T>(tree, d_p, n, d_off, d_hits, hcap, t);
+        });
+    }
 }
 
-// D = 3: the C-ABI rays as they are.  D = 2: rays of 6 T lifted on the device (dim2_expand_rays: origin.z = 0, inv_direction.z = +inf)
-// and walked by the 3-D ordered kernel on the embedded tree, whose records span z = [-1, +1]: the z slab is (-inf, +inf) and leaves
-// both the set and the distances of the 2-D slice unchanged (dim2.cu).
-template <class T, int D = 3, class RAY = typename Traits<T>::Ray>
-static int ordered_host_impl(Tree<T>* tree, const RAY* rays, size_t nrays, int ascending,
+// Distance-ordered traversal, host pointers.  D = 3, 4: the C-ABI rays as they are.  D = 2: rays of 6 T lifted on the device
+// (dim2_expand_rays: origin.z = 0, inv_direction.z = +inf) and walked by the 3-D ordered kernel on the embedded tree, whose records
+// span z = [-1, +1]: the z slab is (-inf, +inf) and leaves both the set and the distances of the 2-D slice unchanged (dim2.cu).
+template <int D, class T>
+static int ordered_host_impl(TreeOf<D, T>* tree, const void* rays, size_t nrays, int ascending,
                              uint32_t* offsets, uint32_t* hits, T* dists, size_t cap, size_t* total) {
     if (!tree || (nrays && !rays) || !offsets || (cap && (!hits || !dists))) { set_error("traverse_ordered: null argument"); return BVHGPU_ERR_INVALID; }
-    if (D != 3 && nrays > 0x7FFFFFFFull) { set_error("traverse_ordered: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("traverse_ordered", nrays));
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
-    typename Traits<T>::Ray* d_rays = nullptr;
+    T* d_rays = nullptr;
     uint32_t *d_off = nullptr, *d_hits = nullptr;
     T* d_dists = nullptr;
     Scratch scratch(ctx);
-    BVH_TRY(scratch.get(&d_rays, nrays));
+    if (nrays) BVH_TRY(upload_records<D>(ctx, scratch, rays, nrays, RAY_RECORD, 0, &d_rays));
     BVH_TRY(scratch.get(&d_off, nrays + 1));
     BVH_TRY(scratch.get(&d_hits, cap));
     BVH_TRY(scratch.get(&d_dists, cap));
-    if (nrays && D == 3) BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, ctx->stream));
-    if (nrays && D != 3) {
-        T* r6 = nullptr;
-        BVH_TRY(scratch.get(&r6, 6 * nrays));
-        BVH_CUDA_TRY(cudaMemcpyAsync(r6, rays, sizeof(*rays) * nrays, cudaMemcpyHostToDevice, ctx->stream));
-        BVH_TRY(dim2_expand_rays<T>(ctx, r6, (uint32_t)nrays, reinterpret_cast<T*>(d_rays)));
-    }
     size_t tot = 0;
-    int rc = traverse_ordered_device<T>(tree, d_rays, nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
+    int rc;
+    if constexpr (D == 4) rc = ordered4_device<T>(tree, d_rays, nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
+    else rc = traverse_ordered_device<T>(tree, reinterpret_cast<const typename Traits<T>::Ray*>(d_rays), nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
     if (total) *total = tot;
     if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) {
         cudaMemcpyAsync(offsets, d_off, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, ctx->stream);
@@ -411,15 +534,30 @@ static int ordered_host_impl(Tree<T>* tree, const RAY* rays, size_t nrays, int a
     return rc;
 }
 
-template <class T>
-static int closest_host_impl(Tree<T>* tree, const void* rays, uint32_t fmt, size_t nrays, int use_triangles, uint32_t* out_shape, T* out_dist, T* out_uv) {
+// Closest hit / any hit on the device.  D = 3: closest_hit_device / any_hit_device (rays of 9 or 6 T, AABB or triangle mode; they
+// check n, the layout and the tree's status).  D = 2, 4: AABB mode, rays of 3D T straight to closest_aabb_device<D, T> /
+// any_hit_aabb_device<D, T> (D = 2 tests x and y of the embedded tree), which leave the checks to the caller.
+template <int D, class T>
+static int closest_driver(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, int use_triangles, uint32_t* d_shape, T* d_dist, T* d_uv) {
+    if constexpr (D == 3) return closest_hit_device<T>(tree, d_rays, fmt, nrays, use_triangles, d_shape, d_dist, d_uv);
+    else return closest_aabb_device<D, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, d_shape, d_dist);
+}
+template <int D, class T>
+static int any_hit_driver(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const T* d_tmax, int use_triangles, uint32_t* d_shape) {
+    if constexpr (D == 3) return any_hit_device<T>(tree, d_rays, fmt, nrays, d_tmax, use_triangles, d_shape);
+    else return any_hit_aabb_device<D, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, d_tmax, d_shape);
+}
+
+template <int D, class T>
+static int closest_host_impl(TreeOf<D, T>* tree, const void* rays, uint32_t fmt, size_t nrays, int use_triangles, uint32_t* out_shape, T* out_dist, T* out_uv) {
     if (!tree || (nrays && (!rays || !out_shape || !out_dist))) { set_error("closest_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("closest_hit", nrays));
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
     if (nrays == 0) return BVHGPU_OK;
     Scratch scratch(ctx);
-    const size_t ray_bytes = (fmt == BVHGPU_RAYS_FULL ? 9 : 6) * sizeof(T);
+    const size_t ray_bytes = (D != 3 ? 3 * D : fmt == BVHGPU_RAYS_FULL ? 9 : 6) * sizeof(T);
     unsigned char* d_rays = nullptr;
     uint32_t* d_s = nullptr;
     T *d_d = nullptr, *d_uv = nullptr;
@@ -428,87 +566,54 @@ static int closest_host_impl(Tree<T>* tree, const void* rays, uint32_t fmt, size
     BVH_TRY(scratch.get(&d_d, nrays));
     if (out_uv) BVH_TRY(scratch.get(&d_uv, 2 * nrays));
     BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, ray_bytes * nrays, cudaMemcpyHostToDevice, ctx->stream));
-    BVH_TRY(closest_hit_device<T>(tree, d_rays, fmt, nrays, use_triangles, d_s, d_d, d_uv));
+    BVH_TRY((closest_driver<D, T>(tree, d_rays, fmt, nrays, use_triangles, d_s, d_d, d_uv)));
     BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     if (out_uv) BVH_CUDA_TRY(cudaMemcpyAsync(out_uv, d_uv, sizeof(T) * 2 * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return BVHGPU_OK;
 }
-
-// 2-D AABB-mode closest hit: the rays of 6 T go straight to closest_aabb_device<2, T>, which tests x and y of the embedded tree.
-template <class T, class RAY2>
-static int closest2_impl(Tree<T>* tree, const RAY2* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {
-    if (!tree || (nrays && (!rays || !out_shape || !out_dist))) { set_error("closest_hit: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("closest_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    if (nrays == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    T *d_rays = nullptr, *d_d = nullptr;
-    uint32_t* d_s = nullptr;
-    BVH_TRY(scratch.get(&d_rays, 6 * nrays));
-    BVH_TRY(scratch.get(&d_s, nrays));
-    BVH_TRY(scratch.get(&d_d, nrays));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(RAY2) * nrays, cudaMemcpyHostToDevice, ctx->stream));
-    const int rc = closest_aabb_device<2, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, d_rays, nrays, d_s, d_d);
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return BVHGPU_OK;
+template <int D, class T>
+static int closest_dev_impl(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, int use_triangles, void* d_shape, void* d_dist, void* d_uv) {
+    if (!tree || (nrays && (!d_rays || !d_shape || !d_dist))) { set_error("closest_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D == 4) BVH_TRY(check_n("closest_hit_dev", nrays));
+    if (D == 4) BVH_TRY(resolve_status(tree));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return closest_driver<D, T>(tree, d_rays, fmt, nrays, use_triangles, (uint32_t*)d_shape, (T*)d_dist, (T*)d_uv);
 }
 
-// Any hit, host pointers: rays (9 T) and the optional limits staged as closest_host_impl stages the rays.
-template <class T>
-static int any_hit_host_impl(Tree<T>* tree, const void* rays, size_t nrays, const T* tmax, int use_triangles, uint32_t* out_shape) {
+// Any hit, host pointers: rays and the optional limits (nullptr: +inf) staged as closest_host_impl stages the rays.
+template <int D, class T>
+static int any_hit_host_impl(TreeOf<D, T>* tree, const void* rays, size_t nrays, const T* tmax, int use_triangles, uint32_t* out_shape) {
     if (!tree || (nrays && (!rays || !out_shape))) { set_error("any_hit: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("any_hit", nrays));
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
     if (nrays == 0) return BVHGPU_OK;
     Scratch scratch(ctx);
+    const size_t ray_w = 3 * D;
     T *d_rays = nullptr, *d_tmax = nullptr;
     uint32_t* d_s = nullptr;
-    BVH_TRY(scratch.get(&d_rays, 9 * nrays));
+    BVH_TRY(scratch.get(&d_rays, ray_w * nrays));
     BVH_TRY(scratch.get(&d_s, nrays));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(T) * 9 * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(T) * ray_w * nrays, cudaMemcpyHostToDevice, ctx->stream));
     if (tmax) {
         BVH_TRY(scratch.get(&d_tmax, nrays));
         BVH_CUDA_TRY(cudaMemcpyAsync(d_tmax, tmax, sizeof(T) * nrays, cudaMemcpyHostToDevice, ctx->stream));
     }
-    BVH_TRY(any_hit_device<T>(tree, d_rays, BVHGPU_RAYS_FULL, nrays, d_tmax, use_triangles, d_s));
+    BVH_TRY((any_hit_driver<D, T>(tree, d_rays, BVHGPU_RAYS_FULL, nrays, d_tmax, use_triangles, d_s)));
     BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return BVHGPU_OK;
 }
-
-// 2-D any hit: the rays of 6 T go straight to any_hit_aabb_device<2, T>, as in closest2_impl.
-template <class T, class RAY2>
-static int any2_impl(Tree<T>* tree, const RAY2* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {
-    if (!tree || (nrays && (!rays || !out_shape))) { set_error("any_hit: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    if (nrays == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    T *d_rays = nullptr, *d_tmax = nullptr;
-    uint32_t* d_s = nullptr;
-    BVH_TRY(scratch.get(&d_rays, 6 * nrays));
-    BVH_TRY(scratch.get(&d_s, nrays));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(RAY2) * nrays, cudaMemcpyHostToDevice, ctx->stream));
-    if (tmax) {
-        BVH_TRY(scratch.get(&d_tmax, nrays));
-        BVH_CUDA_TRY(cudaMemcpyAsync(d_tmax, tmax, sizeof(T) * nrays, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    const int rc = any_hit_aabb_device<2, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, d_rays, nrays, d_tmax, d_s);
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return BVHGPU_OK;
+template <int D, class T>
+static int any_hit_dev_impl(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const void* d_tmax, int use_triangles, void* d_shape) {
+    if (!tree || (nrays && (!d_rays || !d_shape))) { set_error("any_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D == 4) BVH_TRY(check_n("any_hit_dev", nrays));
+    if (D == 4) BVH_TRY(resolve_status(tree));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return any_hit_driver<D, T>(tree, d_rays, fmt, nrays, (const T*)d_tmax, use_triangles, (uint32_t*)d_shape);
 }
 
 template <class T> static int fetch_impl(Tree<T>* tree, uint32_t* hits, size_t cap) {
@@ -552,20 +657,40 @@ static int stage_new_aabbs(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs,
     return BVHGPU_OK;
 }
 
-template <class T>
-static int refit_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size_t n, bool dev_input) {
+// Refit from n new shape boxes (ABI layout of D).  D = 2 (host pointers): the 2-D boxes are lifted to z = [0, 0] on the device.
+// Surface areas with z = [0, 0] are exact and largest_axis never picks z (dim2.cu), so the 3-D refit, growth test and rebuild are the
+// 2-D ones.  D = 4: the boxes are checked (check4), copied into the tree and refit4 runs; synchronous for host pointers.
+template <int D, class T>
+static int refit_impl(TreeOf<D, T>* tree, const void* aabbs, size_t n, bool dev_input) {
     if (!tree || (n && !aabbs)) { set_error("refit: null argument"); return BVHGPU_ERR_INVALID; }
+    if (D == 4) BVH_TRY(resolve_status(tree));                     // a 4-D tree reports a sticky failure before the size
     if (n != tree->n) { set_error("refit: %zu AABBs for a tree over %u shapes", n, tree->n); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
+    if (D != 4) BVH_TRY(resolve_status(tree));
     if (n == 0) return BVHGPU_OK;
-    BVH_TRY(stage_new_aabbs<T>(tree, aabbs, n, dev_input, "refit"));
-    if (tree->dims == 2) BVH_TRY(dim2_finish_build<T>(tree));          // the FLAT leaf boxes follow d_aabb before the records are rebuilt
-    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
-    BVH_TRY(refit(tree));
-    tree->status_pending = true;
-    return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+    Scratch scratch(ctx);
+    if (D != 3 && !dev_input) {
+        T* staged = nullptr;
+        BVH_TRY(upload_records<D>(ctx, scratch, aabbs, n, AABB_RECORD, 0, &staged));
+        aabbs = staged;
+    }
+    if constexpr (D == 4) {
+        using Aabb = typename D4<T>::Aabb;
+        const Aabb* d_in = static_cast<const Aabb*>(aabbs);
+        BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)n, scratch, "refit"));
+        int rc = cudaMemcpyAsync(tree->d_aabb, d_in, sizeof(*d_in) * n, cudaMemcpyDeviceToDevice, ctx->stream) == cudaSuccess ? (int)BVHGPU_OK : (int)BVHGPU_ERR_CUDA;
+        if (rc == BVHGPU_OK) rc = refit4(tree);
+        if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("refit: CUDA error"); rc = BVHGPU_ERR_CUDA; }
+        return rc == BVHGPU_OK ? rc : mark_failed(tree, rc, "refit");
+    } else {
+        BVH_TRY(stage_new_aabbs<T>(tree, static_cast<const typename Traits<T>::Aabb*>(aabbs), n, dev_input || D == 2, "refit"));
+        if (tree->dims == 2) BVH_TRY(dim2_finish_build<T>(tree));      // the FLAT leaf boxes follow d_aabb before the records are rebuilt
+        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
+        BVH_TRY(refit(tree));
+        tree->status_pending = true;
+        return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+    }
 }
 
 template <class T>
@@ -598,13 +723,8 @@ static int build2_impl(bvhgpu_ctx* ctx, const AABB2* aabbs, size_t n, int mode, 
     if (n > (1ull << 30)) { set_error("build: n = %zu exceeds 2^30 shapes", n); return BVHGPU_ERR_INVALID; }
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     Scratch scratch(ctx);
-    T *in4 = nullptr, *in6 = nullptr;
-    if (n) {
-        BVH_TRY(scratch.get(&in4, 4 * n));
-        BVH_TRY(scratch.get(&in6, 6 * n));
-        BVH_CUDA_TRY(cudaMemcpyAsync(in4, aabbs, sizeof(AABB2) * n, cudaMemcpyHostToDevice, ctx->stream));
-        BVH_TRY(dim2_expand_aabbs<T>(ctx, in4, (uint32_t)n, in6));
-    }
+    T* in6 = nullptr;
+    if (n) BVH_TRY(upload_records<2>(ctx, scratch, aabbs, n, AABB_RECORD, 0, &in6));
     TREE2* tree = nullptr;
     BVH_TRY((build_impl<T, TREE2>(ctx, reinterpret_cast<const typename Traits<T>::Aabb*>(in6), n, mode, false, &tree)));
     int rc = dim2_finish_build<T>(tree);
@@ -652,30 +772,10 @@ static int flatten2_impl(Tree<T>* tree, F2* out, size_t cap, size_t* len) {
     }
     return BVHGPU_OK;
 }
-template <class T, class RAY2>
-static int traverse2_impl(Tree<T>* tree, int mode, const RAY2* rays, size_t nrays, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
-    if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    if (nrays > 0x7FFFFFFFull) { set_error("traverse: too many rays"); return BVHGPU_ERR_INVALID; }
-    Scratch scratch(ctx);
-    T *r6 = nullptr, *r9 = nullptr;
-    if (nrays) {
-        BVH_TRY(scratch.get(&r6, 6 * nrays));
-        BVH_TRY(scratch.get(&r9, 9 * nrays));
-        BVH_CUDA_TRY(cudaMemcpyAsync(r6, rays, sizeof(RAY2) * nrays, cudaMemcpyHostToDevice, ctx->stream));
-        BVH_TRY(dim2_expand_rays<T>(ctx, r6, (uint32_t)nrays, r9));
-    }
-    return retained_to_host<2>(tree, "traverse", nrays, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-        return traverse_device<T>(tree, mode, r9, BVHGPU_RAYS_FULL, nrays, d_off, d_hits, hcap, t);
-    });
-}
-
 // Bvh::update_shapes(changed_shape_indices, shapes): only the m changed shapes cross the boundary.  The tree is touched only after
 // the new AABBs passed the NaN / index check.  max_growth <= 0: refit only (topology kept).
-template <class T>
-static int update_impl(Tree<T>* tree, const uint32_t* changed, const typename Traits<T>::Aabb* fresh, size_t m, double max_growth, size_t* rebuilt, bool dev_input) {
+template <int D, class T>
+static int update_impl(TreeOf<D, T>* tree, const uint32_t* changed, const void* fresh, size_t m, double max_growth, size_t* rebuilt, bool dev_input) {
     if (!tree || (m && (!changed || !fresh))) { set_error("update: null argument"); return BVHGPU_ERR_INVALID; }
     if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("update: max_growth = %g, must be >= 1 (or <= 0 for a pure refit)", max_growth); return BVHGPU_ERR_INVALID; }
     if (m > 0xFFFFFFFFull) { set_error("update: too many changed shapes"); return BVHGPU_ERR_INVALID; }
@@ -686,16 +786,26 @@ static int update_impl(Tree<T>* tree, const uint32_t* changed, const typename Tr
     if (m == 0 || tree->n == 0) return BVHGPU_OK;
     Scratch scratch(ctx);
     const uint32_t* d_changed = changed;
-    const typename Traits<T>::Aabb* d_fresh = fresh;
     if (!dev_input) {
         uint32_t* c = nullptr;
-        typename Traits<T>::Aabb* f = nullptr;
+        T* f = nullptr;
         BVH_TRY(scratch.get(&c, m));
-        BVH_TRY(scratch.get(&f, m));
         BVH_CUDA_TRY(cudaMemcpyAsync(c, changed, sizeof(uint32_t) * m, cudaMemcpyHostToDevice, ctx->stream));
-        BVH_CUDA_TRY(cudaMemcpyAsync(f, fresh, sizeof(*fresh) * m, cudaMemcpyHostToDevice, ctx->stream));
-        d_changed = c; d_fresh = f;
+        BVH_TRY(upload_records<D>(ctx, scratch, fresh, m, AABB_RECORD, 0, &f));
+        d_changed = c; fresh = f;
     }
+    if constexpr (D == 4) {                                             // checked, scattered and climbed by the 4-D drivers; synchronous
+        const typename D4<T>::Aabb* d_fresh = static_cast<const typename D4<T>::Aabb*>(fresh);
+        BVH_TRY(check4(tree, d_changed, d_fresh, (uint32_t)m, scratch, "update"));
+        size_t shapes = 0;
+        int rc = put4(tree, d_changed, d_fresh, (uint32_t)m);
+        if (rc == BVHGPU_OK) rc = update4(tree, d_changed, (uint32_t)m, max_growth, &shapes);     // touches the root paths of the changed leaves only
+        if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("update: CUDA error"); rc = BVHGPU_ERR_CUDA; }
+        if (rc != BVHGPU_OK) return mark_failed(tree, rc, "update");
+        if (rebuilt) *rebuilt = shapes;
+        return BVHGPU_OK;
+    } else {
+    const typename Traits<T>::Aabb* d_fresh = static_cast<const typename Traits<T>::Aabb*>(fresh);
     uint32_t* flags = nullptr;
     BVH_TRY(scratch.get(&flags, 2));
     BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), ctx->stream));
@@ -716,71 +826,13 @@ static int update_impl(Tree<T>* tree, const uint32_t* changed, const typename Tr
     BVH_TRY(resolve_status(tree));
     if (rebuilt) *rebuilt = hs.rebuilt;
     return BVHGPU_OK;
-}
-
-// D = 2 refit / update_shapes: the 2-D boxes are lifted to z = [0, 0] on the device and run through refit_impl / update_impl above.
-// Surface areas with z = [0, 0] are exact and largest_axis never picks z (dim2.cu), so the 3-D refit, growth test and rebuild are the
-// 2-D ones.  Host pointers; synchronous.
-template <class T, class AABB2>
-static int lift2_aabbs(Tree<T>* tree, Scratch& scratch, const AABB2* aabbs, size_t n, const typename Traits<T>::Aabb** d_out) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    T *in4 = nullptr, *in6 = nullptr;
-    BVH_TRY(scratch.get(&in4, 4 * n));
-    BVH_TRY(scratch.get(&in6, 6 * n));
-    BVH_CUDA_TRY(cudaMemcpyAsync(in4, aabbs, sizeof(AABB2) * n, cudaMemcpyHostToDevice, ctx->stream));
-    BVH_TRY(dim2_expand_aabbs<T>(ctx, in4, (uint32_t)n, in6));
-    *d_out = reinterpret_cast<const typename Traits<T>::Aabb*>(in6);
-    return BVHGPU_OK;
-}
-template <class T, class AABB2>
-static int refit2_impl(Tree<T>* tree, const AABB2* aabbs, size_t n) {
-    if (!tree || (n && !aabbs)) { set_error("refit: null argument"); return BVHGPU_ERR_INVALID; }
-    if (n != tree->n) { set_error("refit: %zu AABBs for a tree over %u shapes", n, tree->n); return BVHGPU_ERR_INVALID; }
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    if (n == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    const typename Traits<T>::Aabb* d6 = nullptr;
-    BVH_TRY((lift2_aabbs<T, AABB2>(tree, scratch, aabbs, n, &d6)));
-    BVH_TRY(refit_impl<T>(tree, d6, n, true));
-    return resolve_status(tree);
-}
-template <class T, class AABB2>
-static int update2_impl(Tree<T>* tree, const uint32_t* changed, const AABB2* fresh, size_t m, double max_growth, size_t* rebuilt) {
-    if (!tree || (m && (!changed || !fresh))) { set_error("update: null argument"); return BVHGPU_ERR_INVALID; }
-    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("update: max_growth = %g, must be >= 1 (or <= 0 for a pure refit)", max_growth); return BVHGPU_ERR_INVALID; }
-    if (m > 0xFFFFFFFFull) { set_error("update: too many changed shapes"); return BVHGPU_ERR_INVALID; }
-    if (rebuilt) *rebuilt = 0;
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    if (m == 0 || tree->n == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    uint32_t* d_changed = nullptr;
-    BVH_TRY(scratch.get(&d_changed, m));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d_changed, changed, sizeof(uint32_t) * m, cudaMemcpyHostToDevice, ctx->stream));
-    const typename Traits<T>::Aabb* d6 = nullptr;
-    BVH_TRY((lift2_aabbs<T, AABB2>(tree, scratch, fresh, m, &d6)));
-    size_t r = 0;
-    BVH_TRY(update_impl<T>(tree, d_changed, d6, m, max_growth, &r, true));   // with `rebuilt` given, the call synchronises
-    if (rebuilt) *rebuilt = r;
-    return BVHGPU_OK;
-}
-
-// A relocation that failed half-way leaves arrays that no longer agree with each other: the failure is sticky, as a failed build's.
-template <class T> static int mark_failed(Tree<T>* tree, int rc, const char* who) {
-    char msg[1200];
-    snprintf(msg, sizeof msg, "%s failed after the tree was modified (%s); the tree is unusable", who, g_last_error.c_str());
-    tree->failed_status = rc; tree->failed_message = msg;
-    set_error("%s", msg);
-    return rc;
+    }
 }
 
 // Bvh::add_shape, batched: the k new shapes get indices n .. n+k-1.  The AABBs are staged next to the tree's own and checked for NaN
 // before the tree is touched.  n == 0: the call is bvhgpu_build_* over the k AABBs.
-template <class T>
-static int add_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size_t k, double max_growth, size_t* rebuilt, bool dev_input) {
+template <int D, class T>
+static int add_impl(TreeOf<D, T>* tree, const void* aabbs, size_t k, double max_growth, size_t* rebuilt, bool dev_input) {
     if (!tree || (k && !aabbs)) { set_error("add_shapes: null argument"); return BVHGPU_ERR_INVALID; }
     if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("add_shapes: max_growth = %g, must be >= 1 (or <= 0 for no rebuild)", max_growth); return BVHGPU_ERR_INVALID; }
     if (rebuilt) *rebuilt = 0;
@@ -790,14 +842,46 @@ static int add_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size_t
     BVH_TRY(resolve_status(tree));
     if (k == 0) return BVHGPU_OK;
     Scratch scratch(ctx);
-    const typename Traits<T>::Aabb* d_in = aabbs;
     if (!dev_input) {
-        typename Traits<T>::Aabb* staged = nullptr;
-        BVH_TRY(scratch.get(&staged, k));
-        BVH_CUDA_TRY(cudaMemcpyAsync(staged, aabbs, k * sizeof(*aabbs), cudaMemcpyHostToDevice, ctx->stream));
-        d_in = staged;
+        T* staged = nullptr;
+        BVH_TRY(upload_records<D>(ctx, scratch, aabbs, k, AABB_RECORD, 0, &staged));
+        aabbs = staged;
     }
     const uint32_t n = tree->n;
+    if constexpr (D == 4) {                                             // the 4-D drivers: synchronous (the builder reads one word per level)
+        using Aabb = typename D4<T>::Aabb;
+        const Aabb* d_in = static_cast<const Aabb*>(aabbs);
+        BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)k, scratch, "add_shapes"));
+        if (n == 0) {                                                   // an empty tree: exactly bvhgpu_build_*
+            Tree4<T> fresh;
+            fresh.ctx = ctx; fresh.n = (uint32_t)k; fresh.n_nodes = 2 * (uint32_t)k - 1;
+            const int rc = build4<T>(&fresh, d_in, cudaMemcpyDeviceToDevice);
+            if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
+            dfree(ctx, tree->d_sa_base); tree->d_sa_base = nullptr;
+            tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
+            tree->n = fresh.n; tree->n_nodes = fresh.n_nodes;
+            drop_caches4(tree);
+            return BVHGPU_OK;
+        }
+        Aabb* all = nullptr;
+        BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
+        if (cudaMemcpyAsync(all, tree->d_aabb, sizeof(Aabb) * n, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess ||
+            cudaMemcpyAsync(all + n, d_in, sizeof(Aabb) * k, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) {
+            dfree(ctx, all);
+            set_error("add_shapes: CUDA error while staging the AABBs");
+            return BVHGPU_ERR_CUDA;
+        }
+        size_t shapes = 0;
+        const int rc = add_shapes4(tree, all, (uint32_t)k, max_growth, &shapes);
+        if (rc != BVHGPU_OK) {
+            if (tree->d_aabb != all) { dfree(ctx, all); return rc; }    // failed before the tree was touched
+            return mark_failed(tree, rc, "add_shapes");
+        }
+        if (!dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("add_shapes: CUDA error"); return mark_failed(tree, BVHGPU_ERR_CUDA, "add_shapes"); }
+        if (rebuilt) *rebuilt = shapes;
+        return BVHGPU_OK;
+    } else {
+    const typename Traits<T>::Aabb* d_in = static_cast<const typename Traits<T>::Aabb*>(aabbs);
     if (n == 0) {                                                       // an empty tree: exactly bvhgpu_build_*
         Tree<T> fresh;
         int rc = build_exact_sah<T>(ctx, d_in, (uint32_t)k, &fresh);
@@ -841,12 +925,13 @@ static int add_impl(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs, size_t
     BVH_TRY(resolve_status(tree));
     if (rebuilt && max_growth > 0.0) *rebuilt = hs.rebuilt;
     return BVHGPU_OK;
+    }
 }
 
 // Bvh::remove_shape(i, swap_shape = true), batched: `indices` are distinct shape indices before the call; survivors >= n-k take the
 // vacated indices < n-k, smallest hole first.  Checked (range, duplicates) before the tree is touched.
-template <class T>
-static int remove_impl(Tree<T>* tree, const uint32_t* indices, size_t k, bool dev_input) {
+template <int D, class T>
+static int remove_impl(TreeOf<D, T>* tree, const uint32_t* indices, size_t k, bool dev_input) {
     if (!tree || (k && !indices)) { set_error("remove_shapes: null argument"); return BVHGPU_ERR_INVALID; }
     if (k > tree->n) { set_error("remove_shapes: %zu indices for a tree over %u shapes; the tree was left unchanged", k, tree->n); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
@@ -873,36 +958,19 @@ static int remove_impl(Tree<T>* tree, const uint32_t* indices, size_t k, bool de
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (h[0]) { set_error("remove_shapes: a shape index is >= %u; the tree was left unchanged", n); return BVHGPU_ERR_INVALID; }
     if (h[1]) { set_error("remove_shapes: a shape index is listed twice; the tree was left unchanged"); return BVHGPU_ERR_INVALID; }
-    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
     const void* nodes_before = tree->d_nodes;
-    const int rrc = remove_shapes<T>(tree, rm, (uint32_t)k);
-    if (rrc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rrc : mark_failed(tree, rrc, "remove_shapes");
-    tree->status_pending = true;
-    return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
-}
-
-// D = 2 add_shapes: the new 2-D boxes are lifted to z = [0, 0] and run through add_impl above; the descent's surface areas and the
-// exact builder of the group subtrees see z = [0, 0] only (exact, dim2.cu).  remove_shapes is remove_impl itself.  finish_relayout
-// (dynamic.cu) rebuilds the z = [-1, +1] boxes of the FLAT leaf re-test at the new n before the traversal records.  Host pointers;
-// synchronous.
-template <class T, class AABB2>
-static int add2_impl(Tree<T>* tree, const AABB2* aabbs, size_t k, double max_growth, size_t* rebuilt) {
-    if (!tree || (k && !aabbs)) { set_error("add_shapes: null argument"); return BVHGPU_ERR_INVALID; }
-    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("add_shapes: max_growth = %g, must be >= 1 (or <= 0 for no rebuild)", max_growth); return BVHGPU_ERR_INVALID; }
-    if (rebuilt) *rebuilt = 0;
-    if ((uint64_t)tree->n + k > (1ull << 30)) { set_error("add_shapes: %u + %zu shapes exceed 2^30 (u32 node indices); the tree was left unchanged", tree->n, k); return BVHGPU_ERR_INVALID; }
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    if (k == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    const typename Traits<T>::Aabb* d6 = nullptr;
-    BVH_TRY((lift2_aabbs<T, AABB2>(tree, scratch, aabbs, k, &d6)));
-    size_t r = 0;
-    BVH_TRY(add_impl<T>(tree, d6, k, max_growth, &r, true));
-    BVH_TRY(resolve_status(tree));
-    if (rebuilt) *rebuilt = r;
-    return BVHGPU_OK;
+    if constexpr (D == 4) {                                             // synchronous for host pointers
+        int rc = remove_shapes4(tree, rm, (uint32_t)k);
+        if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("remove_shapes: CUDA error"); rc = BVHGPU_ERR_CUDA; }
+        if (rc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rc : mark_failed(tree, rc, "remove_shapes");
+        return BVHGPU_OK;
+    } else {
+        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
+        const int rrc = remove_shapes<T>(tree, rm, (uint32_t)k);
+        if (rrc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rrc : mark_failed(tree, rrc, "remove_shapes");
+        tree->status_pending = true;
+        return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+    }
 }
 
 }  // namespace bvhb200
@@ -1162,24 +1230,20 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_##SUF(TREE* tree, int mode, const RAY* rays, size_t nrays, uint32_t* offsets,          \
                                          uint32_t* hits, size_t cap, size_t* total) {                                     \
-        return traverse_host_impl<T>(tree, mode, rays, BVHGPU_RAYS_FULL, nrays, offsets, hits, cap, total);               \
+        return traverse_host_impl<3, T>(tree, mode, rays, BVHGPU_RAYS_FULL, nrays, offsets, hits, cap, total);               \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_od_##SUF(TREE* tree, int mode, const T* origin_dir, size_t nrays, uint32_t* offsets,   \
                                             uint32_t* hits, size_t cap, size_t* total) {                                  \
-        return traverse_host_impl<T>(tree, mode, origin_dir, BVHGPU_RAYS_OD, nrays, offsets, hits, cap, total);           \
+        return traverse_host_impl<3, T>(tree, mode, origin_dir, BVHGPU_RAYS_OD, nrays, offsets, hits, cap, total);           \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_fetch_##SUF(TREE* tree, uint32_t* hits, size_t cap) { return fetch_impl<T>(tree, hits, cap); } \
     BVH_EXPORT int bvhgpu_traverse_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, void* dev_offsets, \
                                              void* dev_hits, size_t cap, size_t* total) {                                 \
-        if (!tree || !dev_offsets || (nrays && !dev_rays)) { set_error("traverse_dev: null argument"); return BVHGPU_ERR_INVALID; } \
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        return traverse_device<T>(tree, mode, dev_rays, BVHGPU_RAYS_FULL, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+        return traverse_dev_impl<3, T>(tree, mode, dev_rays, BVHGPU_RAYS_FULL, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total, "traverse_dev"); \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_od_dev_##SUF(TREE* tree, int mode, const void* dev_origin_dir, size_t nrays, void* dev_offsets, \
                                                 void* dev_hits, size_t cap, size_t* total) {                              \
-        if (!tree || !dev_offsets || (nrays && !dev_origin_dir)) { set_error("traverse_od_dev: null argument"); return BVHGPU_ERR_INVALID; } \
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        return traverse_device<T>(tree, mode, dev_origin_dir, BVHGPU_RAYS_OD, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+        return traverse_dev_impl<3, T>(tree, mode, dev_origin_dir, BVHGPU_RAYS_OD, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total, "traverse_od_dev"); \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_sharded_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, const bvhgpu_shard* shard) { \
         if (!tree || !shard || (nrays && !dev_rays)) { set_error("traverse_sharded: null argument"); return BVHGPU_ERR_INVALID; } \
@@ -1192,41 +1256,32 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, \
                                       size_t cap, size_t* total) {                                                       \
-        return query_host_impl<T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                              \
+        return query_host_impl<3, T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                           \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_query_dev_##SUF(TREE* tree, int mode, int kind, const void* dev_queries, size_t n, void* dev_offsets, \
                                           void* dev_hits, size_t cap, size_t* total) {                                    \
-        if (!tree || !dev_offsets || (n && !dev_queries)) { set_error("query_dev: null argument"); return BVHGPU_ERR_INVALID; } \
-        /* query_device also serves the library's internal kinds (nearest_candidates): only the public ones get through here */ \
-        if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; } \
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        const int rc = query_device<T>(tree, mode, kind, (const T*)dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
-        /* with `total` given the call synchronises, and the CSR is complete when it returns */                         \
-        if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream)); \
-        return rc;                                                                                                        \
+        return query_dev_impl<3, T>(tree, mode, kind, dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
-        return nearest_host_impl<T>(tree, mode, points, n, out_shape, out_dist);                                         \
+        return nearest_host_impl<3, T>(tree, mode, points, n, out_shape, out_dist);                                         \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_triangles_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
-        return nearest_host_impl<T>(tree, mode, points, n, out_shape, out_dist, 1);                                      \
+        return nearest_host_impl<3, T>(tree, mode, points, n, out_shape, out_dist, 1);                                      \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                    size_t cap, size_t* total) {                                           \
-        return nearest_candidates_host_impl<T>(tree, points, n, offsets, cand, cap, total);                               \
+        return nearest_candidates_host_impl<3, T>(tree, points, n, offsets, cand, cap, total);                               \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,      \
                                                  uint32_t* hits, T* dists, size_t cap, size_t* total) {                  \
-        return ordered_host_impl<T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);                      \
+        return ordered_host_impl<3, T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);                      \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
-        return knn_host_impl<T>(tree, points, n, k, max_dist, out_shape, out_dist);                                      \
+        return knn_host_impl<3, T>(tree, points, n, k, max_dist, out_shape, out_dist);                                      \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_knn_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist,  \
                                         void* dev_shape, void* dev_dist) {                                                \
-        if (!tree || (n && (!dev_points || !dev_shape || !dev_dist))) { set_error("knn_dev: null argument"); return BVHGPU_ERR_INVALID; } \
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        return knn_device<T>(tree, (const T*)dev_points, n, k, (const T*)dev_max_dist, (uint32_t*)dev_shape, (T*)dev_dist); \
+        return knn_dev_impl<3, T>(tree, dev_points, n, k, dev_max_dist, dev_shape, dev_dist);                             \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_tree_set_triangles_##SUF(TREE* tree, const T* triangles, size_t n) {                            \
         if (!tree || (n && !triangles)) { set_error("set_triangles: null argument"); return BVHGPU_ERR_INVALID; }         \
@@ -1240,22 +1295,18 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, int use_triangles, uint32_t* out_shape, \
                                             T* out_dist, T* out_uv) {                                                     \
-        return closest_host_impl<T>(tree, rays, BVHGPU_RAYS_FULL, nrays, use_triangles, out_shape, out_dist, out_uv);     \
+        return closest_host_impl<3, T>(tree, rays, BVHGPU_RAYS_FULL, nrays, use_triangles, out_shape, out_dist, out_uv);     \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_closest_hit_dev_##SUF(TREE* tree, const void* dev_rays, int ray_layout, size_t nrays, int use_triangles, \
                                                 void* dev_shape, void* dev_dist, void* dev_uv) {                          \
-        if (!tree || (nrays && (!dev_rays || !dev_shape || !dev_dist))) { set_error("closest_hit_dev: null argument"); return BVHGPU_ERR_INVALID; } \
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        return closest_hit_device<T>(tree, dev_rays, (uint32_t)ray_layout, nrays, use_triangles, (uint32_t*)dev_shape, (T*)dev_dist, (T*)dev_uv); \
+        return closest_dev_impl<3, T>(tree, dev_rays, (uint32_t)ray_layout, nrays, use_triangles, dev_shape, dev_dist, dev_uv); \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, int use_triangles, uint32_t* out_shape) { \
-        return any_hit_host_impl<T>(tree, rays, nrays, tmax, use_triangles, out_shape);                                   \
+        return any_hit_host_impl<3, T>(tree, rays, nrays, tmax, use_triangles, out_shape);                                   \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax, \
                                             int use_triangles, void* dev_shape) {                                         \
-        if (!tree || (nrays && (!dev_rays || !dev_shape))) { set_error("any_hit_dev: null argument"); return BVHGPU_ERR_INVALID; } \
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        return any_hit_device<T>(tree, dev_rays, (uint32_t)ray_layout, nrays, (const T*)dev_tmax, use_triangles, (uint32_t*)dev_shape); \
+        return any_hit_dev_impl<3, T>(tree, dev_rays, (uint32_t)ray_layout, nrays, dev_tmax, use_triangles, dev_shape);    \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_stats_##SUF(TREE* tree, uint64_t* out2) {                                              \
         if (!tree || !out2) { set_error("traverse_stats: null argument"); return BVHGPU_ERR_INVALID; }                    \
@@ -1273,8 +1324,8 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
         BVH_TRY(resolve_status<T>(tree));                                                                                 \
         return sah_cost<T>(tree, out2);                                                                                   \
     }                                                                                                                     \
-    BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit_impl<T>(tree, aabbs, n, false); } \
-    BVH_EXPORT int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) { return refit_impl<T>(tree, (const AABB*)dev_aabbs, n, true); } \
+    BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit_impl<3, T>(tree, aabbs, n, false); } \
+    BVH_EXPORT int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) { return refit_impl<3, T>(tree, dev_aabbs, n, true); } \
     BVH_EXPORT int bvhgpu_optimize_##SUF(TREE* tree, const AABB* aabbs, size_t n, double max_growth, size_t* rebuilt) { \
         return optimize_impl<T>(tree, aabbs, n, max_growth, rebuilt, false);                                           \
     }                                                                                                                     \
@@ -1282,22 +1333,22 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
         return optimize_impl<T>(tree, (const AABB*)dev_aabbs, n, max_growth, rebuilt, true);                            \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, size_t* rebuilt) { \
-        return update_impl<T>(tree, changed, changed_aabbs, m, max_growth, rebuilt, false);                              \
+        return update_impl<3, T>(tree, changed, changed_aabbs, m, max_growth, rebuilt, false);                              \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_update_dev_##SUF(TREE* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, double max_growth, size_t* rebuilt) { \
-        return update_impl<T>(tree, (const uint32_t*)dev_changed, (const AABB*)dev_changed_aabbs, m, max_growth, rebuilt, true); \
+        return update_impl<3, T>(tree, (const uint32_t*)dev_changed, dev_changed_aabbs, m, max_growth, rebuilt, true); \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) { \
-        return add_impl<T>(tree, aabbs, k, max_growth, rebuilt, false);                                                   \
+        return add_impl<3, T>(tree, aabbs, k, max_growth, rebuilt, false);                                                   \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_add_shapes_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt) { \
-        return add_impl<T>(tree, (const AABB*)dev_aabbs, k, max_growth, rebuilt, true);                                   \
+        return add_impl<3, T>(tree, dev_aabbs, k, max_growth, rebuilt, true);                                   \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                            \
-        return remove_impl<T>(tree, indices, k, false);                                                                   \
+        return remove_impl<3, T>(tree, indices, k, false);                                                                \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_remove_shapes_dev_##SUF(TREE* tree, const void* dev_indices, size_t k) {                        \
-        return remove_impl<T>(tree, (const uint32_t*)dev_indices, k, true);                                               \
+        return remove_impl<3, T>(tree, (const uint32_t*)dev_indices, k, true);                                            \
     }
 
 #define DEFINE_API2(T, SUF, TREE, AABB, RAY, NODE, FLAT)                                                                   \
@@ -1317,45 +1368,131 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_flatten_##SUF(TREE* tree, FLAT* out, size_t cap, size_t* len) { return flatten2_impl<T, FLAT>(tree, out, cap, len); } \
     BVH_EXPORT int bvhgpu_traverse_##SUF(TREE* tree, int mode, const RAY* rays, size_t nrays, uint32_t* offsets, uint32_t* hits, \
                                          size_t cap, size_t* total) {                                                      \
-        return traverse2_impl<T, RAY>(tree, mode, rays, nrays, offsets, hits, cap, total);                                 \
+        return traverse_host_impl<2, T>(tree, mode, rays, BVHGPU_RAYS_FULL, nrays, offsets, hits, cap, total);                                 \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, \
                                       size_t cap, size_t* total) {                                                        \
-        return query_host_impl<T, 2>(tree, mode, kind, queries, n, offsets, hits, cap, total);                             \
+        return query_host_impl<2, T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                             \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
-        return nearest_host_impl<T, 2>(tree, mode, points, n, out_shape, out_dist);                                        \
+        return nearest_host_impl<2, T>(tree, mode, points, n, out_shape, out_dist);                                        \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
                                                    size_t cap, size_t* total) {                                            \
-        return nearest_candidates_host_impl<T, 2>(tree, points, n, offsets, cand, cap, total);                             \
+        return nearest_candidates_host_impl<2, T>(tree, points, n, offsets, cand, cap, total);                             \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
-        return knn_host_impl<T, 2>(tree, points, n, k, max_dist, out_shape, out_dist);                                     \
+        return knn_host_impl<2, T>(tree, points, n, k, max_dist, out_shape, out_dist);                                     \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,     \
                                                  uint32_t* hits, T* dists, size_t cap, size_t* total) {                   \
-        return ordered_host_impl<T, 2, RAY>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);               \
+        return ordered_host_impl<2, T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);               \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {  \
-        return closest2_impl<T, RAY>(tree, rays, nrays, out_shape, out_dist);                                              \
+        return closest_host_impl<2, T>(tree, rays, BVHGPU_RAYS_FULL, nrays, 0, out_shape, out_dist, nullptr);                                              \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {   \
-        return any2_impl<T, RAY>(tree, rays, nrays, tmax, out_shape);                                                      \
+        return any_hit_host_impl<2, T>(tree, rays, nrays, tmax, 0, out_shape);                                                      \
     }                                                                                                                      \
-    BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit2_impl<T, AABB>(tree, aabbs, n); } \
+    BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit_impl<2, T>(tree, aabbs, n, false); } \
     BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, \
                                        size_t* rebuilt) {                                                                  \
-        return update2_impl<T, AABB>(tree, changed, changed_aabbs, m, max_growth, rebuilt);                                \
+        return update_impl<2, T>(tree, changed, changed_aabbs, m, max_growth, rebuilt, false);                                \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) {  \
-        return add2_impl<T, AABB>(tree, aabbs, k, max_growth, rebuilt);                                                    \
+        return add_impl<2, T>(tree, aabbs, k, max_growth, rebuilt, false);                                                    \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                             \
-        return remove_impl<T>(tree, indices, k, false);                                                                    \
+        return remove_impl<2, T>(tree, indices, k, false);                                                                 \
+    }
+
+#define DEFINE_API4(T, SUF, TREE, AABB, RAY, NODE, FLAT)                                                                   \
+    BVH_EXPORT int bvhgpu_build_##SUF(bvhgpu_ctx* ctx, const AABB* aabbs, size_t n, int mode, TREE** out) {               \
+        return build4_impl<T, TREE>(ctx, aabbs, n, mode, out);                                                             \
+    }                                                                                                                      \
+    BVH_EXPORT void bvhgpu_tree_free_##SUF(TREE* tree) {                                                                   \
+        if (!tree) return;                                                                                                 \
+        if (tree->ctx) cudaSetDevice(tree->ctx->device);                                                                   \
+        tree_release<T>(tree);                                                                                             \
+        delete tree;                                                                                                       \
+    }                                                                                                                      \
+    BVH_EXPORT size_t bvhgpu_tree_num_shapes_##SUF(const TREE* tree) { return tree ? tree->n : 0; }                        \
+    BVH_EXPORT int bvhgpu_tree_nodes_##SUF(TREE* tree, NODE* out_nodes, uint32_t* out_node_index) {                        \
+        return tree_nodes_impl<T>(tree, out_nodes, out_node_index);                                                        \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_flatten_##SUF(TREE* tree, FLAT* out, size_t cap, size_t* len) { return flatten_impl<T>(tree, out, cap, len); } \
+    BVH_EXPORT int bvhgpu_traverse_##SUF(TREE* tree, int mode, const RAY* rays, size_t nrays, uint32_t* offsets, uint32_t* hits, \
+                                         size_t cap, size_t* total) {                                                      \
+        return traverse_host_impl<4, T>(tree, mode, rays, BVHGPU_RAYS_FULL, nrays, offsets, hits, cap, total);             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_traverse_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, void* dev_offsets,  \
+                                             void* dev_hits, size_t cap, size_t* total) {                                  \
+        return traverse_dev_impl<4, T>(tree, mode, dev_rays, BVHGPU_RAYS_FULL, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total, "traverse_dev"); \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets,      \
+                                      uint32_t* hits, size_t cap, size_t* total) {                                        \
+        return query_host_impl<4, T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_query_dev_##SUF(TREE* tree, int mode, int kind, const void* dev_queries, size_t n,              \
+                                          void* dev_offsets, void* dev_hits, size_t cap, size_t* total) {                 \
+        return query_dev_impl<4, T>(tree, mode, kind, dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
+        return nearest_host_impl<4, T>(tree, mode, points, n, out_shape, out_dist);                                        \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
+                                                   size_t cap, size_t* total) {                                            \
+        return nearest_candidates_host_impl<4, T>(tree, points, n, offsets, cand, cap, total);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,    \
+                                                 uint32_t* hits, T* dists, size_t cap, size_t* total) {                   \
+        return ordered_host_impl<4, T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);                    \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {  \
+        return closest_host_impl<4, T>(tree, rays, BVHGPU_RAYS_FULL, nrays, 0, out_shape, out_dist, nullptr);              \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_closest_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, void* dev_shape, void* dev_dist) { \
+        return closest_dev_impl<4, T>(tree, dev_rays, BVHGPU_RAYS_FULL, nrays, 0, dev_shape, dev_dist, nullptr);           \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {   \
+        return any_hit_host_impl<4, T>(tree, rays, nrays, tmax, 0, out_shape);                                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape) { \
+        return any_hit_dev_impl<4, T>(tree, dev_rays, BVHGPU_RAYS_FULL, nrays, dev_tmax, 0, dev_shape);                    \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
+        return knn_host_impl<4, T>(tree, points, n, k, max_dist, out_shape, out_dist);                                     \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_knn_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, \
+                                        void* dev_shape, void* dev_dist) {                                                 \
+        return knn_dev_impl<4, T>(tree, dev_points, n, k, dev_max_dist, dev_shape, dev_dist);                              \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit_impl<4, T>(tree, aabbs, n, false); } \
+    BVH_EXPORT int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) { return refit_impl<4, T>(tree, dev_aabbs, n, true); } \
+    BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m,           \
+                                       double max_growth, size_t* rebuilt) {                                               \
+        return update_impl<4, T>(tree, changed, changed_aabbs, m, max_growth, rebuilt, false);                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_update_dev_##SUF(TREE* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m,   \
+                                           double max_growth, size_t* rebuilt) {                                           \
+        return update_impl<4, T>(tree, (const uint32_t*)dev_changed, dev_changed_aabbs, m, max_growth, rebuilt, true);     \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) {  \
+        return add_impl<4, T>(tree, aabbs, k, max_growth, rebuilt, false);                                                 \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_add_shapes_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt) { \
+        return add_impl<4, T>(tree, dev_aabbs, k, max_growth, rebuilt, true);                                              \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                             \
+        return remove_impl<4, T>(tree, indices, k, false);                                                                 \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_remove_shapes_dev_##SUF(TREE* tree, const void* dev_indices, size_t k) {                         \
+        return remove_impl<4, T>(tree, (const uint32_t*)dev_indices, k, true);                                             \
     }
 
 DEFINE_API2(float, f32x2, bvhgpu_tree2f, bvh_aabb2f, bvh_ray2f, bvh_node2f, bvh_flat2f)
 DEFINE_API2(double, f64x2, bvhgpu_tree2d, bvh_aabb2d, bvh_ray2d, bvh_node2d, bvh_flat2d)
 DEFINE_API(float, f32x3, bvhgpu_tree3f, bvh_aabb3f, bvh_ray3f, bvh_node3f, bvh_flat3f)
 DEFINE_API(double, f64x3, bvhgpu_tree3d, bvh_aabb3d, bvh_ray3d, bvh_node3d, bvh_flat3d)
+DEFINE_API4(float, f32x4, bvhgpu_tree4f, bvh_aabb4f, bvh_ray4f, bvh_node4f, bvh_flat4f)
+DEFINE_API4(double, f64x4, bvhgpu_tree4d, bvh_aabb4d, bvh_ray4d, bvh_node4d, bvh_flat4d)

@@ -11,12 +11,6 @@
 
 namespace bvhb200 {
 
-// ---- 4-D traversal record: the AABB the node has in its parent, `skip` (first record behind the subtree) and the shape index of a
-// leaf.  Sized in whole 16-byte granules so that a record is fetched with 128-bit non-coherent loads only: 3 for f32, 5 for f64.
-struct __align__(16) TRec4F { float min[4]; float max[4]; uint32_t skip, shape, pad[2]; };    // 48 B
-struct __align__(16) TRec4D { double min[4]; double max[4]; uint32_t skip, shape, pad[2]; };  // 80 B
-static_assert(sizeof(TRec4F) == 48 && sizeof(TRec4D) == 80, "4-D record size");
-
 // record, shape-box and ray types of the walk in D (3: TNodeF / TNodeD, the padded device boxes and bvh_ray3*; 4: TRec4F / TRec4D,
 // the ABI boxes and bvh_ray4*)
 template <int D, class T> struct CsrRecords;

@@ -5,6 +5,8 @@
 // D = 2 hides in z = 0 (dim2.cu): surface areas, largest_axis and the slab test all see it.  So D = 4 has its own pipeline here, with
 // its own node types and its own Tree4<T>; it shares the exact-arithmetic helpers and keys of common.cuh, Scratch, the records,
 // walk and count -> scan -> fill driver of csr.cuh, and the predicates of queries.cuh.  DESIGN.md section 4.11 describes the design.
+// This file holds the kernels and the device-side drivers declared in internal.h; the bvhgpu_*_f32x4 / _f64x4 entry points are the
+// D = 4 instances of the host layer in capi.cu, which checks the arguments and the tree's status and stages the batch.
 //
 // Builder (bit-identical to Bvh::build in the sense of DESIGN.md section 2):
 //   ranges of more than SMALL4 shapes: level-synchronous.  Per level: prep (tile numbering, bucket identities), bin (one warp per
@@ -25,34 +27,7 @@
 
 namespace bvhb200 {
 
-// ---- device layouts (the traversal records TRec4F / TRec4D are in csr.cuh) ------------------------------------------------------
-static_assert(sizeof(bvh_aabb4f) == 32 && sizeof(bvh_aabb4d) == 64 && sizeof(bvh_ray4f) == 48 && sizeof(bvh_ray4d) == 96, "4-D POD size");
-static_assert(sizeof(bvh_node4f) == 80 && sizeof(bvh_node4d) == 144 && sizeof(bvh_flat4f) == 44 && sizeof(bvh_flat4d) == 80, "4-D POD size");
-
-template <class T> struct D4;
-template <> struct D4<float> { using Aabb = bvh_aabb4f; using Ray = bvh_ray4f; using Node = bvh_node4f; using Flat = bvh_flat4f; using Rec = TRec4F; };
-template <> struct D4<double> { using Aabb = bvh_aabb4d; using Ray = bvh_ray4d; using Node = bvh_node4d; using Flat = bvh_flat4d; using Rec = TRec4D; };
-
-template <class T> struct Tree4 {
-    using Aabb = typename D4<T>::Aabb; using Node = typename D4<T>::Node; using Flat = typename D4<T>::Flat; using Rec = typename D4<T>::Rec;
-    bvhgpu_ctx* ctx = nullptr;
-    uint32_t n = 0, n_nodes = 0;
-    Aabb* d_aabb = nullptr;            // [n]      shape AABBs (ABI layout: already whole sectors)
-    Node* d_nodes = nullptr;           // [2n-1]   Bvh.nodes, reference preorder layout
-    uint32_t* d_node_index = nullptr;  // [n]      leaf node of every shape
-    uint32_t* d_node_start = nullptr;  // [2n-1]   first position of the node's shape range (== leaves before it)
-    Rec* d_trec = nullptr;             // [n_trec] traversal records (built on first use)
-    uint32_t n_trec = 0;
-    Flat* d_flat = nullptr;            // [n_flat] FlatBvh (built on demand)
-    size_t n_flat = 0;
-    int failed_status = 0;             // sticky (DESIGN.md section 1)
-    std::string failed_message;
-    uint32_t* d_offsets = nullptr; size_t offsets_cap = 0;   // result buffers of the host-pointer traversal
-    uint32_t* d_hits = nullptr;    size_t hits_cap = 0;
-    T* d_sa_base = nullptr;            // [2n-1] surface area of every inner node when it was last (re)built: baseline of update (first update)
-    uint32_t* d_arrive = nullptr;      // [2n-1] arrival counters of the incremental update (all zero between calls)
-    uint8_t* d_bad = nullptr;          // [2n-1] growth flags of the incremental update (all zero between calls)
-};
+// The node / record types D4<T>, the tree Tree4<T> and the records TRec4F / TRec4D are in internal.h.
 
 constexpr uint32_t SMALL4 = 256;     // ranges this small are finished by one warp (depth-first, shared-memory stack)
 constexpr uint32_t TILE4 = 512;      // shapes per warp tile of a large range
@@ -729,23 +704,6 @@ __global__ void __launch_bounds__(256) root_seed4_kernel(const typename D4<T>::N
 // ================================================================================================================================
 #define LAUNCHED(ctx, k) do { (ctx)->launches += (k); BVH_CUDA_TRY(cudaGetLastError()); } while (0)
 
-template <class T> static void release4(Tree4<T>* t) {
-    if (!t || !t->ctx) return;
-    bvhgpu_ctx* ctx = t->ctx;
-    dfree(ctx, t->d_aabb); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
-    dfree(ctx, t->d_trec); dfree(ctx, t->d_flat); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
-    dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad);
-}
-template <class T> static int sticky4(const Tree4<T>* t) {
-    if (t->failed_status != BVHGPU_OK) set_error("%s", t->failed_message.c_str());
-    return t->failed_status;
-}
-template <class T> static int fail4(Tree4<T>* t, int rc, const char* msg) {
-    t->failed_status = rc; t->failed_message = msg;
-    set_error("%s", msg);
-    return rc;
-}
-
 // Buffers of the level loop, sized for n shapes: at most max_tasks disjoint ranges of > SMALL4 shapes on one level.
 template <class T> struct Levels4 {
     Task4<T>* tasks = nullptr;                   // [2 max_tasks]: this level's ranges, the next level's
@@ -787,7 +745,7 @@ template <class T> static int run_levels4(Tree4<T>* tree, const BuildArgs4& A, c
         LAUNCHED(ctx, 4);
         BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
         BVH_CUDA_TRY(cudaStreamSynchronize(st));
-        if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], err.c_str());
+        if (h[CTL_ERROR]) return mark_failed(tree, (int)h[CTL_ERROR], who, err.c_str());
         m = h[CTL_NEXT];
         n_small = h[CTL_SMALL];
         cur ^= 1;
@@ -798,12 +756,12 @@ template <class T> static int run_levels4(Tree4<T>* tree, const BuildArgs4& A, c
     }
     BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (h[CTL_ERROR]) return fail4(tree, (int)h[CTL_ERROR], err.c_str());
+    if (h[CTL_ERROR]) return mark_failed(tree, (int)h[CTL_ERROR], who, err.c_str());
     return BVHGPU_OK;
 }
 
 // The exact SAH build.  h_aabbs: host pointer (device pointer with kind = cudaMemcpyDeviceToDevice).  Synchronous (the host learns the range count of every level anyway).
-template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb* h_aabbs, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
+template <class T> int build4(Tree4<T>* tree, const typename D4<T>::Aabb* h_aabbs, cudaMemcpyKind kind) {
     using Key = typename Traits<T>::Key;
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
@@ -832,7 +790,7 @@ template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb*
     uint32_t* h = ctx->h_pinned + 232;
     BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (h[CTL_NAN]) return fail4(tree, BVHGPU_ERR_NAN, "build: NaN coordinate in an input AABB (the reference panics here, src/bvh/bvh_node.rs:214-217)");
+    if (h[CTL_NAN]) return mark_failed(tree, BVHGPU_ERR_NAN, "build", "build: NaN coordinate in an input AABB (the reference panics here, src/bvh/bvh_node.rs:214-217)");
 
     Levels4<T> L;
     if (n > SMALL4) {                                          // one root task: the level list, or the small list
@@ -845,55 +803,14 @@ template <class T> static int build4(Tree4<T>* tree, const typename D4<T>::Aabb*
     return run_levels4(tree, A, L, n > SMALL4 ? 1u : 0u, n > SMALL4 ? 0u : 1u, "build");
 }
 
-template <class T, class TreeT> static int build4_impl(bvhgpu_ctx* ctx, const typename D4<T>::Aabb* aabbs, size_t n, int mode, TreeT** out) {
-    if (!ctx || !out || (n && !aabbs)) { set_error("build: null argument"); return BVHGPU_ERR_INVALID; }
-    *out = nullptr;
-    if (n > (1ull << 30)) { set_error("build: n = %zu exceeds 2^30 shapes", n); return BVHGPU_ERR_INVALID; }
-    if (mode == BVHGPU_BUILD_LBVH || mode == BVHGPU_BUILD_LBVH_TREELET) {
-        set_error("build: D = 4 has the exact SAH build only (BVHGPU_BUILD_EXACT_SAH); the LBVH modes are not implemented for D = 4");
-        return BVHGPU_ERR_UNSUPPORTED;
-    }
-    if (mode != BVHGPU_BUILD_EXACT_SAH) { set_error("build: unknown mode %d", mode); return BVHGPU_ERR_INVALID; }
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    TreeT* tree = new (std::nothrow) TreeT();
-    if (!tree) { set_error("build: out of host memory"); return BVHGPU_ERR_INTERNAL; }
-    tree->ctx = ctx;
-    tree->n = (uint32_t)n;
-    tree->n_nodes = n ? 2 * (uint32_t)n - 1 : 0;
-    const int rc = n ? build4<T>(tree, aabbs) : (int)BVHGPU_OK;
-    if (rc != BVHGPU_OK) { release4<T>(tree); delete tree; return rc; }
-    *out = tree;
-    return BVHGPU_OK;
-}
-
-template <class T> static int nodes4_impl(Tree4<T>* tree, typename D4<T>::Node* out_nodes, uint32_t* out_node_index) {
-    if (!tree) { set_error("tree_nodes: null tree"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
+// The FlatBvh, built once (3n - 2 nodes for n >= 2, 1 for n == 1, 0 for n == 0).
+template <class T> int build_flat4(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (tree->n == 0) return BVHGPU_OK;
-    if (out_nodes) BVH_CUDA_TRY(cudaMemcpyAsync(out_nodes, tree->d_nodes, sizeof(*out_nodes) * tree->n_nodes, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_node_index) BVH_CUDA_TRY(cudaMemcpyAsync(out_node_index, tree->d_node_index, sizeof(uint32_t) * tree->n, cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return BVHGPU_OK;
-}
-
-template <class T> static int flatten4_impl(Tree4<T>* tree, typename D4<T>::Flat* out, size_t cap, size_t* len) {
-    if (!tree) { set_error("flatten: null tree"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     tree->n_flat = tree->n == 0 ? 0 : (tree->n == 1 ? 1 : 3 * (size_t)tree->n - 2);
-    if (len) *len = tree->n_flat;
     if (tree->n && !tree->d_flat) {
         BVH_TRY(dalloc_t(ctx, &tree->d_flat, tree->n_flat));
         flat4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_start, tree->n_nodes, tree->d_flat);
         LAUNCHED(ctx, 1);
-    }
-    if (out) {
-        if (cap < tree->n_flat) { set_error("flatten: capacity %zu < %zu flat nodes", cap, tree->n_flat); return BVHGPU_ERR_CAPACITY; }
-        if (tree->n_flat) BVH_CUDA_TRY(cudaMemcpyAsync(out, tree->d_flat, sizeof(*out) * tree->n_flat, cudaMemcpyDeviceToHost, ctx->stream));
-        BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     }
     return BVHGPU_OK;
 }
@@ -907,18 +824,6 @@ template <class T> static int ensure_trec4(Tree4<T>* tree) {
     trec4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec);
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
-}
-
-// `what` names the entry point in error messages
-template <class T> static int check_batch_args(Tree4<T>* tree, int mode, size_t n, const char* what) {
-    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
-    if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("%s: bad mode %d", what, mode); return BVHGPU_ERR_INVALID; }
-    return sticky4(tree);
-}
-static bool public_query_kind(int kind) { return kind >= BVHGPU_QUERY_AABB && kind <= BVHGPU_QUERY_BALL; }
-template <class T> static size_t query_stride4(int kind) {
-    return kind == BVHGPU_QUERY_AABB ? Query<T, BVHGPU_QUERY_AABB, 4>::STRIDE : kind == BVHGPU_QUERY_POINT ? Query<T, BVHGPU_QUERY_POINT, 4>::STRIDE
-                                                                            : Query<T, BVHGPU_QUERY_BALL, 4>::STRIDE;
 }
 
 // Device pointers, enqueued on the context's stream; synchronises only to return *total.  Arguments checked by the caller.
@@ -939,10 +844,15 @@ template <class P, class T> static int csr4_dev(Tree4<T>* tree, bool flat, const
 // Host CSR out of a batch already on the device (d_src, n > 0, tree->n > 0): count, read the total, size the retained hit buffer
 // exactly, fill, copy back.  Hits that do not fit `cap` are not copied; offsets and *total are, and the call returns
 // BVHGPU_ERR_CAPACITY -- the caller's second call with cap = *total is the only extra walk.
-template <class P, class T> static int csr4_host(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
-                                                 size_t cap, size_t* total, const char* what) {
+template <class P, class T> static int csr4_host_p(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
+                                                   size_t cap, size_t* total, const char* what) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
+    if (n == 0 || tree->n == 0) {                                  // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
+        std::fill(offsets, offsets + n + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
     BVH_TRY(ensure_trec4(tree));
     const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
     CsrPasses passes(ctx, (uint32_t)n);
@@ -951,17 +861,8 @@ template <class P, class T> static int csr4_host(Tree4<T>* tree, bool flat, cons
     const int rc = passes.total(what, nullptr, 0, &tot);
     if (total) *total = tot;
     if (rc != BVHGPU_OK) return rc;
-    if (tree->offsets_cap < n + 1) {
-        dfree(ctx, tree->d_offsets); tree->d_offsets = nullptr; tree->offsets_cap = 0;
-        BVH_TRY(dalloc_t(ctx, &tree->d_offsets, n + 1));
-        tree->offsets_cap = n + 1;
-    }
     const bool fits = hits && tot <= cap;
-    if (fits && tree->hits_cap < tot) {
-        dfree(ctx, tree->d_hits); tree->d_hits = nullptr; tree->hits_cap = 0;
-        BVH_TRY(dalloc_t(ctx, &tree->d_hits, tot));
-        tree->hits_cap = tot;
-    }
+    BVH_TRY(ensure_result_buffers(tree, n, fits ? tot : 0));
     BVH_TRY(passes.fill(walk, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
     BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
     if (fits && tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, st));
@@ -970,235 +871,77 @@ template <class P, class T> static int csr4_host(Tree4<T>* tree, bool flat, cons
     return BVHGPU_OK;
 }
 
-// host batch -> device scratch (n items of `bytes` each)
-static int upload4(bvhgpu_ctx* ctx, Scratch& scratch, const void* h_src, size_t bytes, void** d_out) {
-    char* d = nullptr;
-    BVH_TRY(scratch.get(&d, bytes));
-    BVH_CUDA_TRY(cudaMemcpyAsync(d, h_src, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    *d_out = d;
-    return BVHGPU_OK;
-}
-
-// ---- rays ----
-template <class T> static int traverse4_dev_impl(Tree4<T>* tree, int mode, const void* d_rays, size_t nrays, uint32_t* d_offsets, uint32_t* d_hits,
-                                                 size_t cap, size_t* total) {
-    if (!tree || !d_offsets || (nrays && !d_rays)) { set_error("traverse_dev: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_batch_args(tree, mode, nrays, "traverse"));
-    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-    return csr4_dev<RayProbe4<T>>(tree, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, d_offsets, d_hits, cap, total, "traverse");
-}
-template <class T> static int traverse4_host_impl(Tree4<T>* tree, int mode, const typename D4<T>::Ray* rays, size_t nrays, uint32_t* offsets,
-                                                  uint32_t* hits, size_t cap, size_t* total) {
-    if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_batch_args(tree, mode, nrays, "traverse"));
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (nrays == 0 || tree->n == 0) {
-        std::fill(offsets, offsets + nrays + 1, 0u);
-        if (total) *total = 0;
-        return BVHGPU_OK;
+// The probe of a CSR walk: rays, or one of the public query kinds.
+template <class T, class F> static int with_probe4(int probe, F f) {
+    switch (probe) {
+    case PROBE_RAYS4: return f(RayProbe4<T>{});
+    case BVHGPU_QUERY_AABB: return f(Query<T, BVHGPU_QUERY_AABB, 4>{});
+    case BVHGPU_QUERY_POINT: return f(Query<T, BVHGPU_QUERY_POINT, 4>{});
+    default: return f(Query<T, BVHGPU_QUERY_BALL, 4>{});
     }
-    Scratch scratch(ctx);
-    void* d_rays = nullptr;
-    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
-    return csr4_host<RayProbe4<T>>(tree, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, offsets, hits, cap, total, "traverse");
 }
-
-// ---- Aabb / Point / Ball queries: records of 8 / 4 / 5 T ----
-template <class T> static int query4_dev_impl(Tree4<T>* tree, int mode, int kind, const void* d_queries, size_t n, uint32_t* d_offsets,
-                                              uint32_t* d_hits, size_t cap, size_t* total) {
-    if (!tree || !d_offsets || (n && !d_queries)) { set_error("query_dev: null argument"); return BVHGPU_ERR_INVALID; }
-    if (!public_query_kind(kind)) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_batch_args(tree, mode, n, "query_dev"));
-    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    const int rc = kind == BVHGPU_QUERY_AABB  ? csr4_dev<Query<T, BVHGPU_QUERY_AABB, 4>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
-                 : kind == BVHGPU_QUERY_POINT ? csr4_dev<Query<T, BVHGPU_QUERY_POINT, 4>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev")
-                                              : csr4_dev<Query<T, BVHGPU_QUERY_BALL, 4>>(tree, flat, d_queries, n, d_offsets, d_hits, cap, total, "query_dev");
-    // as bvhgpu_query_dev_f32x3: with `total` given the call synchronises, and the CSR is complete when it returns
-    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
-    return rc;
+template <class T> int csr4_device(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* d_offsets, uint32_t* d_hits,
+                                   size_t cap, size_t* total, const char* what) {
+    return with_probe4<T>(probe, [&](auto p) { return csr4_dev<decltype(p)>(tree, flat, d_src, n, d_offsets, d_hits, cap, total, what); });
 }
-template <class T> static int query4_host_impl(Tree4<T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits,
-                                               size_t cap, size_t* total) {
-    if (!tree || (n && !queries) || !offsets) { set_error("query: null argument"); return BVHGPU_ERR_INVALID; }
-    if (!public_query_kind(kind)) { set_error("query: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_batch_args(tree, mode, n, "query"));
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (n == 0 || tree->n == 0) {
-        std::fill(offsets, offsets + n + 1, 0u);
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    Scratch scratch(ctx);
-    void* d_q = nullptr;
-    BVH_TRY(upload4(ctx, scratch, queries, sizeof(T) * query_stride4<T>(kind) * n, &d_q));
-    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    return kind == BVHGPU_QUERY_AABB  ? csr4_host<Query<T, BVHGPU_QUERY_AABB, 4>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
-         : kind == BVHGPU_QUERY_POINT ? csr4_host<Query<T, BVHGPU_QUERY_POINT, 4>>(tree, flat, d_q, n, offsets, hits, cap, total, "query")
-                                      : csr4_host<Query<T, BVHGPU_QUERY_BALL, 4>>(tree, flat, d_q, n, offsets, hits, cap, total, "query");
+template <class T> int csr4_host(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
+                                 size_t cap, size_t* total, const char* what) {
+    return with_probe4<T>(probe, [&](auto p) { return csr4_host_p<decltype(p)>(tree, flat, d_src, n, offsets, hits, cap, total, what); });
 }
 
 // ---- nearest_to: 4 T per point ----
-template <class T> static int nearest4_host_impl(Tree4<T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) {
-    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("nearest: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_batch_args(tree, mode, n, "nearest"));
+template <class T> int nearest4_device(Tree4<T>* tree, int mode, const T* d_points, size_t n, uint32_t* d_shape, T* d_dist) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     if (n == 0) return BVHGPU_OK;
     if (tree->n == 0) {                                            // empty tree: None (bvh_impl.rs:229-231)
-        std::fill(out_shape, out_shape + n, BVH_INVALID);
-        std::fill(out_dist, out_dist + n, T(0));
+        BVH_CUDA_TRY(cudaMemsetAsync(d_shape, 0xFF, sizeof(uint32_t) * n, st));
+        BVH_CUDA_TRY(cudaMemsetAsync(d_dist, 0, sizeof(T) * n, st));
         return BVHGPU_OK;
     }
-    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    if (flat) BVH_TRY(flatten4_impl(tree, nullptr, 0, nullptr));    // builds d_flat once
-    Scratch scratch(ctx);
-    void* d_p = nullptr;
-    uint32_t* d_s = nullptr;
-    T* d_d = nullptr;
-    BVH_TRY(upload4(ctx, scratch, points, sizeof(T) * 4 * n, &d_p));
-    BVH_TRY(scratch.get(&d_s, n));
-    BVH_TRY(scratch.get(&d_d, n));
     const unsigned grid = (unsigned)((n + 127) / 128);
-    if (flat) nearest4_kernel<T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->d_flat, (uint32_t)tree->n_flat, tree->d_aabb, (const T*)d_p, (uint32_t)n, d_s, d_d);
-    else      nearest4_kernel<T, false><<<grid, 128, 0, st>>>(tree->d_nodes, nullptr, 0u, tree->d_aabb, (const T*)d_p, (uint32_t)n, d_s, d_d);
+    if (mode == BVHGPU_TRAVERSE_FLAT) {
+        BVH_TRY(build_flat4(tree));
+        nearest4_kernel<T, true><<<grid, 128, 0, st>>>(tree->d_nodes, tree->d_flat, (uint32_t)tree->n_flat, tree->d_aabb, d_points, (uint32_t)n, d_shape, d_dist);
+    } else {
+        nearest4_kernel<T, false><<<grid, 128, 0, st>>>(tree->d_nodes, nullptr, 0u, tree->d_aabb, d_points, (uint32_t)n, d_shape, d_dist);
+    }
     LAUNCHED(ctx, 1);
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
     return BVHGPU_OK;
 }
 // Candidate lists that contain the nearest shape of every point, for shapes with their own distance (bvh_b200.h): the bound walk,
 // then a QUERY_WITHIN pass over the records in FLAT semantics (leaves re-test the shape's own AABB).
-template <class T> static int nearest_candidates4_host_impl(Tree4<T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand,
-                                                            size_t cap, size_t* total) {
-    if (!tree || (n && !points) || !offsets) { set_error("nearest_candidates: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(check_batch_args(tree, BVHGPU_TRAVERSE_FLAT, n, "nearest_candidates"));
+template <class T> int nearest_candidates4(Tree4<T>* tree, const T* d_points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
     bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (n == 0 || tree->n == 0) {
-        std::fill(offsets, offsets + n + 1, 0u);
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
+    if (n == 0 || tree->n == 0) return csr4_host_p<Query<T, QUERY_WITHIN, 4>>(tree, true, nullptr, n, offsets, cand, cap, total, "nearest_candidates");
     Scratch scratch(ctx);
-    void* d_p = nullptr;
     T* rec = nullptr;
-    BVH_TRY(upload4(ctx, scratch, points, sizeof(T) * 4 * n, &d_p));
     BVH_TRY(scratch.get(&rec, 5 * n));
-    nearest_bound4_kernel<T><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, (const T*)d_p, (uint32_t)n, rec);
+    nearest_bound4_kernel<T><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, d_points, (uint32_t)n, rec);
     LAUNCHED(ctx, 1);
-    return csr4_host<Query<T, QUERY_WITHIN, 4>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
+    return csr4_host_p<Query<T, QUERY_WITHIN, 4>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
 }
 
-// ---- distance-ordered traversal and AABB-mode closest hit (the contract of the 3-D calls; DESIGN.md section 4.14) ----
-// ordered_kernel<4, T> of csr.cuh over the records, sorted lists into scratch of `cap` entries, copied back as the 3-D host form does.
-template <class T> static int ordered4_host_impl(Tree4<T>* tree, const typename D4<T>::Ray* rays, size_t nrays, int ascending, uint32_t* offsets,
-                                                 uint32_t* hits, T* dists, size_t cap, size_t* total) {
-    if (!tree || (nrays && !rays) || !offsets || (cap && (!hits || !dists))) { set_error("traverse_ordered: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("traverse_ordered: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
+// ---- distance-ordered traversal (the contract of the 3-D calls; DESIGN.md section 4.14): ordered_kernel<4, T> of csr.cuh ----
+template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_t nrays, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
+                                       T* d_dists, size_t cap, size_t* total) {
     bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     if (nrays == 0 || tree->n == 0) {
-        std::fill(offsets, offsets + nrays + 1, 0u);
+        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (nrays + 1), ctx->stream));
         if (total) *total = 0;
         return BVHGPU_OK;
     }
-    Scratch scratch(ctx);
-    void* d_rays = nullptr;
-    uint32_t *d_off = nullptr, *d_hits = nullptr;
-    T* d_dists = nullptr;
-    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
-    BVH_TRY(scratch.get(&d_off, nrays + 1));
-    BVH_TRY(scratch.get(&d_hits, cap));
-    BVH_TRY(scratch.get(&d_dists, cap));
     BVH_TRY(ensure_trec4(tree));
     const OrderedWalk<4, T> walk{tree->d_trec, tree->n_trec, reinterpret_cast<const typename D4<T>::Ray*>(d_rays), ascending, d_dists};
-    size_t tot = 0;
-    const int rc = csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_off, d_hits, cap, &tot);
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK && rc != BVHGPU_ERR_CAPACITY) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, d_off, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, st));
-    const size_t m = std::min(tot, cap);
-    if (m) {
-        BVH_CUDA_TRY(cudaMemcpyAsync(hits, d_hits, sizeof(uint32_t) * m, cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaMemcpyAsync(dists, d_dists, sizeof(T) * m, cudaMemcpyDeviceToHost, st));
-    }
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    return rc;
-}
-// closest_aabb_device<4, T> (closest.cu) over the 4-D nodes and shape boxes; rays of 12 T.
-template <class T> static int closest4_dev_impl(Tree4<T>* tree, const void* d_rays, size_t nrays, void* d_shape, void* d_dist) {
-    if (!tree || (nrays && (!d_rays || !d_shape || !d_dist))) { set_error("closest_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("closest_hit_dev: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-    return closest_aabb_device<4, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, (uint32_t*)d_shape, (T*)d_dist);
-}
-template <class T> static int closest4_host_impl(Tree4<T>* tree, const typename D4<T>::Ray* rays, size_t nrays, uint32_t* out_shape, T* out_dist) {
-    if (!tree || (nrays && (!rays || !out_shape || !out_dist))) { set_error("closest_hit: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("closest_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (nrays == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    void* d_rays = nullptr;
-    uint32_t* d_s = nullptr;
-    T* d_d = nullptr;
-    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
-    BVH_TRY(scratch.get(&d_s, nrays));
-    BVH_TRY(scratch.get(&d_d, nrays));
-    const int rc = closest_aabb_device<4, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, d_s, d_d);
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nrays, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    return BVHGPU_OK;
-}
-
-// any_hit_aabb_device<4, T> (closest.cu) over the 4-D nodes and shape boxes; rays of 12 T, limits of 1 T (nullptr: +inf).
-template <class T> static int any4_dev_impl(Tree4<T>* tree, const void* d_rays, size_t nrays, const void* d_tmax, void* d_shape) {
-    if (!tree || (nrays && (!d_rays || !d_shape))) { set_error("any_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("any_hit_dev: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-    return any_hit_aabb_device<4, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, (const T*)d_tmax, (uint32_t*)d_shape);
-}
-template <class T> static int any4_host_impl(Tree4<T>* tree, const typename D4<T>::Ray* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {
-    if (!tree || (nrays && (!rays || !out_shape))) { set_error("any_hit: null argument"); return BVHGPU_ERR_INVALID; }
-    if (nrays > 0x7FFFFFFFull) { set_error("any_hit: n = %zu exceeds 2^31-1", nrays); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (nrays == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    void *d_rays = nullptr, *d_tmax = nullptr;
-    uint32_t* d_s = nullptr;
-    BVH_TRY(upload4(ctx, scratch, rays, sizeof(*rays) * nrays, &d_rays));
-    if (tmax) BVH_TRY(upload4(ctx, scratch, tmax, sizeof(T) * nrays, &d_tmax));
-    BVH_TRY(scratch.get(&d_s, nrays));
-    const int rc = any_hit_aabb_device<4, T>(ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, (const T*)d_tmax, d_s);
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    return BVHGPU_OK;
+    return csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_offsets, d_hits, cap, total);
 }
 
 // ---- k nearest shapes: 4 T per point, n limits (nullptr: none), n * k results ----
-template <class T> static int knn4_check(Tree4<T>* tree, size_t n, uint32_t k, const char* what) {
-    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
-    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("%s: k = %u outside 1 .. %d", what, k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
-    return sticky4(tree);
-}
-template <class T> static int knn4_launch(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist) {
+template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist) {
+    if (n > 0x7FFFFFFFull) { set_error("knn: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(resolve_status(tree));
+    if (n == 0) return BVHGPU_OK;
     bvhgpu_ctx* ctx = tree->ctx;
     const unsigned grid = (unsigned)((n + 127) / 128);
     knn_bucket(k, [&](auto kb) {
@@ -1207,43 +950,8 @@ template <class T> static int knn4_launch(Tree4<T>* tree, const T* d_points, siz
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
 }
-template <class T> static int knn4_dev_impl(Tree4<T>* tree, const void* d_points, size_t n, uint32_t k, const void* d_max_dist, void* d_shape, void* d_dist) {
-    if (!tree || (n && (!d_points || !d_shape || !d_dist))) { set_error("knn_dev: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(knn4_check(tree, n, k, "knn_dev"));
-    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-    if (n == 0) return BVHGPU_OK;
-    return knn4_launch<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist);
-}
-template <class T> static int knn4_host_impl(Tree4<T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) {
-    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("knn: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(knn4_check(tree, n, k, "knn"));
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (n == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    void *d_p = nullptr, *d_r = nullptr;
-    uint32_t* d_s = nullptr;
-    T* d_d = nullptr;
-    BVH_TRY(upload4(ctx, scratch, points, sizeof(T) * 4 * n, &d_p));
-    if (max_dist) BVH_TRY(upload4(ctx, scratch, max_dist, sizeof(T) * n, &d_r));
-    BVH_TRY(scratch.get(&d_s, n * k));
-    BVH_TRY(scratch.get(&d_d, n * k));
-    BVH_TRY(knn4_launch<T>(tree, (const T*)d_p, n, k, (const T*)d_r, d_s, d_d));
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n * k, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n * k, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    return BVHGPU_OK;
-}
 
 // ---- refit / update_shapes ----
-// A failure after the tree was modified leaves arrays that no longer agree with each other: sticky, as a failed build.
-template <class T> static int failed4(Tree4<T>* t, int rc, const char* who) {
-    if (t->failed_status != BVHGPU_OK) return t->failed_status;               // already sticky (run_levels4)
-    char msg[1200];
-    snprintf(msg, sizeof msg, "%s failed after the tree was modified (%s); the tree is unusable", who, bvhgpu_last_error());
-    return fail4(t, rc, msg);
-}
 
 // The traversal records and the flat array, if they were built, are rewritten in place from the new boxes (their sizes do not change);
 // otherwise traverse, query, flatten and FLAT nearest_to would keep using the old boxes.
@@ -1257,7 +965,7 @@ template <class T> static int refresh_caches4(Tree4<T>* tree) {
 
 // m new boxes (and their shape indices, when `d_changed` is given) are checked on the device and the verdict is read back before the
 // tree is touched.
-template <class T> static int check4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m, Scratch& scratch,
+template <class T> int check4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m, Scratch& scratch,
                                      const char* who) {
     bvhgpu_ctx* ctx = tree->ctx;
     uint32_t* flags = nullptr;
@@ -1265,7 +973,7 @@ template <class T> static int check4(Tree4<T>* tree, const uint32_t* d_changed, 
     BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), ctx->stream));
     check4_kernel<T><<<(m + 255) / 256, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->n, flags);
     LAUNCHED(ctx, 1);
-    uint32_t* h = ctx->h_pinned + 240;
+    uint32_t* h = ctx->h_pinned + 208;
     BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (h[1]) { set_error("%s: a changed shape index is >= %u; the tree was left unchanged", who, tree->n); return BVHGPU_ERR_INVALID; }
@@ -1274,7 +982,7 @@ template <class T> static int check4(Tree4<T>* tree, const uint32_t* d_changed, 
 }
 
 // Bottom-up refit of every node from tree->d_aabb.
-template <class T> static int refit4(Tree4<T>* tree) {
+template <class T> int refit4(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
     if (tree->n >= 2) {
         Scratch scratch(ctx);
@@ -1334,7 +1042,7 @@ template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* 
 
 // The shapes d_changed[0 .. m) already carry their new boxes in tree->d_aabb.  max_growth <= 0: boxes only.  The same steps as the 3-D
 // update_incremental (flatten.cu) with the shared kernels of update.cuh.
-template <class T> static int update4(Tree4<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt) {
+template <class T> int update4(Tree4<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt) {
     using Node = typename D4<T>::Node;
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
@@ -1368,56 +1076,10 @@ template <class T> static int update4(Tree4<T>* tree, const uint32_t* d_changed,
     return refresh_caches4(tree);
 }
 
-template <class T> static int refit4_impl(Tree4<T>* tree, const typename D4<T>::Aabb* aabbs, size_t n, bool dev_input) {
-    if (!tree || (n && !aabbs)) { set_error("refit: null argument"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    if (n != tree->n) { set_error("refit: %zu AABBs for a tree over %u shapes", n, tree->n); return BVHGPU_ERR_INVALID; }
+template <class T> int put4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m) {
     bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (n == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    const typename D4<T>::Aabb* d_in = aabbs;
-    if (!dev_input) {
-        void* d = nullptr;
-        BVH_TRY(upload4(ctx, scratch, aabbs, sizeof(*aabbs) * n, &d));
-        d_in = static_cast<const typename D4<T>::Aabb*>(d);
-    }
-    BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)n, scratch, "refit"));
-    int rc = cudaMemcpyAsync(tree->d_aabb, d_in, sizeof(*d_in) * n, cudaMemcpyDeviceToDevice, ctx->stream) == cudaSuccess ? (int)BVHGPU_OK : (int)BVHGPU_ERR_CUDA;
-    if (rc == BVHGPU_OK) rc = refit4(tree);
-    if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("refit: CUDA error"); rc = BVHGPU_ERR_CUDA; }
-    return rc == BVHGPU_OK ? rc : failed4(tree, rc, "refit");
-}
-
-// Bvh::update_shapes(changed_shape_indices, shapes): only the m changed shapes cross the boundary.
-template <class T> static int update4_impl(Tree4<T>* tree, const uint32_t* changed, const typename D4<T>::Aabb* fresh, size_t m, double max_growth,
-                                           size_t* rebuilt, bool dev_input) {
-    if (!tree || (m && (!changed || !fresh))) { set_error("update: null argument"); return BVHGPU_ERR_INVALID; }
-    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("update: max_growth = %g, must be >= 1 (or <= 0 for a pure refit)", max_growth); return BVHGPU_ERR_INVALID; }
-    if (m > 0xFFFFFFFFull) { set_error("update: too many changed shapes"); return BVHGPU_ERR_INVALID; }
-    if (rebuilt) *rebuilt = 0;
-    BVH_TRY(sticky4(tree));
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (m == 0 || tree->n == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    const uint32_t* d_changed = changed;
-    const typename D4<T>::Aabb* d_fresh = fresh;
-    if (!dev_input) {
-        void *c = nullptr, *f = nullptr;
-        BVH_TRY(upload4(ctx, scratch, changed, sizeof(uint32_t) * m, &c));
-        BVH_TRY(upload4(ctx, scratch, fresh, sizeof(*fresh) * m, &f));
-        d_changed = static_cast<const uint32_t*>(c); d_fresh = static_cast<const typename D4<T>::Aabb*>(f);
-    }
-    BVH_TRY(check4(tree, d_changed, d_fresh, (uint32_t)m, scratch, "update"));
-    put4_kernel<T><<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(d_changed, d_fresh, (uint32_t)m, tree->d_aabb);
-    ctx->launches++;
-    size_t shapes = 0;
-    int rc = cudaGetLastError() == cudaSuccess ? (int)BVHGPU_OK : (int)BVHGPU_ERR_CUDA;
-    if (rc == BVHGPU_OK) rc = update4(tree, d_changed, (uint32_t)m, max_growth, &shapes);     // touches the root paths of the changed leaves only
-    if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("update: CUDA error"); rc = BVHGPU_ERR_CUDA; }
-    if (rc != BVHGPU_OK) return failed4(tree, rc, "update");
-    if (rebuilt) *rebuilt = shapes;
+    put4_kernel<T><<<(m + 255) / 256, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->d_aabb);
+    LAUNCHED(ctx, 1);
     return BVHGPU_OK;
 }
 
@@ -1428,7 +1090,7 @@ template <class T> static int update4_impl(Tree4<T>* tree, const uint32_t* chang
 // Arrays that depend on the node count or the shape numbering, after a relocation: the traversal records and the flat array are
 // rebuilt at the new size on first use (refresh_caches4 rewrites them in place and assumes the node count did not change); the
 // update's arrival counters and growth flags are reallocated by the next update.
-template <class T> static void drop_caches4(Tree4<T>* tree) {
+template <class T> void drop_caches4(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
     dfree(ctx, tree->d_trec); tree->d_trec = nullptr;
     dfree(ctx, tree->d_flat); tree->d_flat = nullptr;
@@ -1441,7 +1103,7 @@ template <class T> static void drop_caches4(Tree4<T>* tree) {
 // aabb_all: [n + k] shape boxes (the tree's n followed by the k new ones, checked for NaN); becomes tree->d_aabb.  *rebuilt = shapes in
 // the subtrees rebuilt by the growth test (the group subtrees are not counted).  A failure with tree->d_aabb != aabb_all left the tree
 // untouched.
-template <class T> static int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* aabb_all, uint32_t k, double max_growth, size_t* rebuilt) {
+template <class T> int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* aabb_all, uint32_t k, double max_growth, size_t* rebuilt) {
     using Node = typename D4<T>::Node;
     using Key = typename Traits<T>::Key;
     bvhgpu_ctx* ctx = tree->ctx;
@@ -1541,7 +1203,7 @@ template <class T> static int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* 
 
 // d_rm: [n + 1] removed flag of every shape (0 / 1, the last word 0), 1 <= k <= n.  A failure with tree->d_nodes unchanged left the
 // tree untouched.
-template <class T> static int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint32_t k) {
+template <class T> int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint32_t k) {
     using Node = typename D4<T>::Node;
     using Aabb = typename D4<T>::Aabb;
     bvhgpu_ctx* ctx = tree->ctx;
@@ -1593,187 +1255,24 @@ template <class T> static int remove_shapes4(Tree4<T>* tree, const uint32_t* d_r
     return BVHGPU_OK;
 }
 
-// Bvh::add_shape, batched: the contract of the 3-D add_impl (capi.cu).  The new boxes are checked for NaN before the tree is touched;
-// n == 0: the call is bvhgpu_build_* over the k boxes.  Synchronous (the builder reads one word per level).
-template <class T> static int add4_impl(Tree4<T>* tree, const typename D4<T>::Aabb* aabbs, size_t k, double max_growth, size_t* rebuilt, bool dev_input) {
-    using Aabb = typename D4<T>::Aabb;
-    if (!tree || (k && !aabbs)) { set_error("add_shapes: null argument"); return BVHGPU_ERR_INVALID; }
-    if (max_growth > 0.0 && !(max_growth >= 1.0)) { set_error("add_shapes: max_growth = %g, must be >= 1 (or <= 0 for no rebuild)", max_growth); return BVHGPU_ERR_INVALID; }
-    if (rebuilt) *rebuilt = 0;
-    if ((uint64_t)tree->n + k > (1ull << 30)) { set_error("add_shapes: %u + %zu shapes exceed 2^30 (u32 node indices); the tree was left unchanged", tree->n, k); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (k == 0) return BVHGPU_OK;
-    Scratch scratch(ctx);
-    const Aabb* d_in = aabbs;
-    if (!dev_input) {
-        void* d = nullptr;
-        BVH_TRY(upload4(ctx, scratch, aabbs, sizeof(*aabbs) * k, &d));
-        d_in = static_cast<const Aabb*>(d);
-    }
-    BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)k, scratch, "add_shapes"));
-    const uint32_t n = tree->n;
-    if (n == 0) {                                               // an empty tree: exactly bvhgpu_build_*
-        Tree4<T> fresh;
-        fresh.ctx = ctx; fresh.n = (uint32_t)k; fresh.n_nodes = 2 * (uint32_t)k - 1;
-        const int rc = build4<T>(&fresh, d_in, cudaMemcpyDeviceToDevice);
-        if (rc != BVHGPU_OK) { release4<T>(&fresh); return rc; }
-        dfree(ctx, tree->d_sa_base); tree->d_sa_base = nullptr;
-        tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
-        tree->n = fresh.n; tree->n_nodes = fresh.n_nodes;
-        drop_caches4(tree);
-        return BVHGPU_OK;
-    }
-    Aabb* all = nullptr;
-    BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
-    if (cudaMemcpyAsync(all, tree->d_aabb, sizeof(Aabb) * n, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(all + n, d_in, sizeof(Aabb) * k, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-        dfree(ctx, all);
-        set_error("add_shapes: CUDA error while staging the AABBs");
-        return BVHGPU_ERR_CUDA;
-    }
-    size_t shapes = 0;
-    int rc = add_shapes4(tree, all, (uint32_t)k, max_growth, &shapes);
-    if (rc != BVHGPU_OK) {
-        if (tree->d_aabb != all) { dfree(ctx, all); return rc; }    // failed before the tree was touched
-        return failed4(tree, rc, "add_shapes");
-    }
-    if (!dev_input && cudaStreamSynchronize(st) != cudaSuccess) { set_error("add_shapes: CUDA error"); return failed4(tree, BVHGPU_ERR_CUDA, "add_shapes"); }
-    if (rebuilt) *rebuilt = shapes;
-    return BVHGPU_OK;
-}
-
-// Bvh::remove_shape(i, swap_shape = true), batched: the contract of the 3-D remove_impl (capi.cu).  Range and duplicates are checked
-// before the tree is touched.
-template <class T> static int remove4_impl(Tree4<T>* tree, const uint32_t* indices, size_t k, bool dev_input) {
-    if (!tree || (k && !indices)) { set_error("remove_shapes: null argument"); return BVHGPU_ERR_INVALID; }
-    if (k > tree->n) { set_error("remove_shapes: %zu indices for a tree over %u shapes; the tree was left unchanged", k, tree->n); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(sticky4(tree));
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    if (k == 0) return BVHGPU_OK;
-    const uint32_t n = tree->n;
-    Scratch scratch(ctx);
-    const uint32_t* d_idx = indices;
-    if (!dev_input) {
-        void* c = nullptr;
-        BVH_TRY(upload4(ctx, scratch, indices, sizeof(uint32_t) * k, &c));
-        d_idx = static_cast<const uint32_t*>(c);
-    }
-    uint32_t *rm = nullptr, *flags = nullptr;
-    BVH_TRY(scratch.get(&rm, (size_t)n + 1));
-    BVH_TRY(scratch.get(&flags, 2));
-    BVH_CUDA_TRY(cudaMemsetAsync(rm, 0, sizeof(uint32_t) * ((size_t)n + 1), st));
-    BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), st));
-    BVH_TRY(remove_check(ctx, d_idx, (uint32_t)k, n, rm, flags));
-    uint32_t* h = ctx->h_pinned + 222;
-    BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (h[0]) { set_error("remove_shapes: a shape index is >= %u; the tree was left unchanged", n); return BVHGPU_ERR_INVALID; }
-    if (h[1]) { set_error("remove_shapes: a shape index is listed twice; the tree was left unchanged"); return BVHGPU_ERR_INVALID; }
-    const void* nodes_before = tree->d_nodes;
-    int rc = remove_shapes4(tree, rm, (uint32_t)k);
-    if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(st) != cudaSuccess) { set_error("remove_shapes: CUDA error"); rc = BVHGPU_ERR_CUDA; }
-    if (rc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rc : failed4(tree, rc, "remove_shapes");
-    return BVHGPU_OK;
-}
+#define INSTANTIATE4(T)                                                                                                              \
+    template int build4<T>(Tree4<T>*, const D4<T>::Aabb*, cudaMemcpyKind);                                                          \
+    template int build_flat4<T>(Tree4<T>*);                                                                                         \
+    template int csr4_device<T>(Tree4<T>*, int, bool, const void*, size_t, uint32_t*, uint32_t*, size_t, size_t*, const char*);     \
+    template int csr4_host<T>(Tree4<T>*, int, bool, const void*, size_t, uint32_t*, uint32_t*, size_t, size_t*, const char*);       \
+    template int nearest_candidates4<T>(Tree4<T>*, const T*, size_t, uint32_t*, uint32_t*, size_t, size_t*);                        \
+    template int nearest4_device<T>(Tree4<T>*, int, const T*, size_t, uint32_t*, T*);                                               \
+    template int ordered4_device<T>(Tree4<T>*, const void*, size_t, int, uint32_t*, uint32_t*, T*, size_t, size_t*);               \
+    template int knn4_device<T>(Tree4<T>*, const T*, size_t, uint32_t, const T*, uint32_t*, T*);                                    \
+    template int check4<T>(Tree4<T>*, const uint32_t*, const D4<T>::Aabb*, uint32_t, Scratch&, const char*);                        \
+    template int put4<T>(Tree4<T>*, const uint32_t*, const D4<T>::Aabb*, uint32_t);                                                 \
+    template int refit4<T>(Tree4<T>*);                                                                                              \
+    template int update4<T>(Tree4<T>*, const uint32_t*, uint32_t, double, size_t*);                                                 \
+    template int add_shapes4<T>(Tree4<T>*, D4<T>::Aabb*, uint32_t, double, size_t*);                                                \
+    template int remove_shapes4<T>(Tree4<T>*, const uint32_t*, uint32_t);                                                           \
+    template void drop_caches4<T>(Tree4<T>*);
+INSTANTIATE4(float)
+INSTANTIATE4(double)
+#undef INSTANTIATE4
 
 }  // namespace bvhb200
-
-using namespace bvhb200;
-
-struct bvhgpu_tree4f : Tree4<float> {};
-struct bvhgpu_tree4d : Tree4<double> {};
-
-#define BVH_EXPORT4 extern "C" __attribute__((visibility("default")))
-#define DEFINE_API4(T, SUF, TREE, AABB, RAY, NODE, FLAT)                                                                   \
-    BVH_EXPORT4 int bvhgpu_build_##SUF(bvhgpu_ctx* ctx, const AABB* aabbs, size_t n, int mode, TREE** out) {              \
-        return build4_impl<T, TREE>(ctx, aabbs, n, mode, out);                                                            \
-    }                                                                                                                     \
-    BVH_EXPORT4 void bvhgpu_tree_free_##SUF(TREE* tree) {                                                                 \
-        if (!tree) return;                                                                                                \
-        if (tree->ctx) cudaSetDevice(tree->ctx->device);                                                                  \
-        release4<T>(tree);                                                                                                \
-        delete tree;                                                                                                      \
-    }                                                                                                                     \
-    BVH_EXPORT4 size_t bvhgpu_tree_num_shapes_##SUF(const TREE* tree) { return tree ? tree->n : 0; }                      \
-    BVH_EXPORT4 int bvhgpu_tree_nodes_##SUF(TREE* tree, NODE* out_nodes, uint32_t* out_node_index) {                      \
-        return nodes4_impl<T>(tree, out_nodes, out_node_index);                                                           \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_flatten_##SUF(TREE* tree, FLAT* out, size_t cap, size_t* len) { return flatten4_impl<T>(tree, out, cap, len); } \
-    BVH_EXPORT4 int bvhgpu_traverse_##SUF(TREE* tree, int mode, const RAY* rays, size_t nrays, uint32_t* offsets, uint32_t* hits, \
-                                          size_t cap, size_t* total) {                                                    \
-        return traverse4_host_impl<T>(tree, mode, rays, nrays, offsets, hits, cap, total);                                \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_traverse_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, void* dev_offsets, \
-                                              void* dev_hits, size_t cap, size_t* total) {                                \
-        return traverse4_dev_impl<T>(tree, mode, dev_rays, nrays, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets,     \
-                                       uint32_t* hits, size_t cap, size_t* total) {                                       \
-        return query4_host_impl<T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                              \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_query_dev_##SUF(TREE* tree, int mode, int kind, const void* dev_queries, size_t n,             \
-                                           void* dev_offsets, void* dev_hits, size_t cap, size_t* total) {                \
-        return query4_dev_impl<T>(tree, mode, kind, dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
-        return nearest4_host_impl<T>(tree, mode, points, n, out_shape, out_dist);                                         \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_nearest_candidates_##SUF(TREE* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, \
-                                                    size_t cap, size_t* total) {                                          \
-        return nearest_candidates4_host_impl<T>(tree, points, n, offsets, cand, cap, total);                              \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_traverse_ordered_##SUF(TREE* tree, const RAY* rays, size_t nrays, int ascending, uint32_t* offsets,   \
-                                                  uint32_t* hits, T* dists, size_t cap, size_t* total) {                  \
-        return ordered4_host_impl<T>(tree, rays, nrays, ascending, offsets, hits, dists, cap, total);                     \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_closest_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t* out_shape, T* out_dist) { \
-        return closest4_host_impl<T>(tree, rays, nrays, out_shape, out_dist);                                             \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_closest_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, void* dev_shape, void* dev_dist) { \
-        return closest4_dev_impl<T>(tree, dev_rays, nrays, dev_shape, dev_dist);                                          \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {  \
-        return any4_host_impl<T>(tree, rays, nrays, tmax, out_shape);                                                     \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape) { \
-        return any4_dev_impl<T>(tree, dev_rays, nrays, dev_tmax, dev_shape);                                              \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
-        return knn4_host_impl<T>(tree, points, n, k, max_dist, out_shape, out_dist);                                      \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_knn_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, \
-                                         void* dev_shape, void* dev_dist) {                                               \
-        return knn4_dev_impl<T>(tree, dev_points, n, k, dev_max_dist, dev_shape, dev_dist);                               \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit4_impl<T>(tree, aabbs, n, false); } \
-    BVH_EXPORT4 int bvhgpu_refit_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t n) {                                 \
-        return refit4_impl<T>(tree, (const AABB*)dev_aabbs, n, true);                                                     \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m,         \
-                                        double max_growth, size_t* rebuilt) {                                             \
-        return update4_impl<T>(tree, changed, changed_aabbs, m, max_growth, rebuilt, false);                              \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_update_dev_##SUF(TREE* tree, const void* dev_changed, const void* dev_changed_aabbs, size_t m, \
-                                            double max_growth, size_t* rebuilt) {                                         \
-        return update4_impl<T>(tree, (const uint32_t*)dev_changed, (const AABB*)dev_changed_aabbs, m, max_growth, rebuilt, true); \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_add_shapes_##SUF(TREE* tree, const AABB* aabbs, size_t k, double max_growth, size_t* rebuilt) { \
-        return add4_impl<T>(tree, aabbs, k, max_growth, rebuilt, false);                                                  \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_add_shapes_dev_##SUF(TREE* tree, const void* dev_aabbs, size_t k, double max_growth, size_t* rebuilt) { \
-        return add4_impl<T>(tree, (const AABB*)dev_aabbs, k, max_growth, rebuilt, true);                                  \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                           \
-        return remove4_impl<T>(tree, indices, k, false);                                                                  \
-    }                                                                                                                     \
-    BVH_EXPORT4 int bvhgpu_remove_shapes_dev_##SUF(TREE* tree, const void* dev_indices, size_t k) {                       \
-        return remove4_impl<T>(tree, (const uint32_t*)dev_indices, k, true);                                              \
-    }
-
-DEFINE_API4(float, f32x4, bvhgpu_tree4f, bvh_aabb4f, bvh_ray4f, bvh_node4f, bvh_flat4f)
-DEFINE_API4(double, f64x4, bvhgpu_tree4d, bvh_aabb4d, bvh_ray4d, bvh_node4d, bvh_flat4d)

@@ -51,9 +51,9 @@ struct bvhgpu_ctx {
     int64_t build_subtree = -1;    // exact builder: in-register subtrees for ranges <= 32 shapes (-1 auto, 0 never, 1 always)
     int64_t build_small = -1;      // exact builder: defer ranges <= 16 shapes to the thread-per-range kernel (-1 auto by size, 0 never, 1 always)
     // small pinned read-back area (256 words): 0-25 the ray traversal's scan tail, 64-79 the streamed path's per-chunk values,
-    // 128-129 the stream probe, 200-221 the capi / dynamic checks, 222-225 the 4-D add / remove (index checks, group and seed
-    // counts), 232-235 the 4-D build, CSR_TOTAL_WORD (236-237) the total of the two-pass CSR walks (csr.cuh), 240-248 the 4-D
-    // update checks
+    // 128-129 the stream probe, 200-217 the entry points' checks (200 staged boxes, 204 synchronize, 208-209 changed boxes, 212 added
+    // boxes, 216-217 removal lists), 220 / 224 the group counts of the 3-D / 4-D add, 232-235 the 4-D build, CSR_TOTAL_WORD (236-237) the total of the
+    // two-pass CSR walks (csr.cuh), 244-248 the 4-D rebuild seeds
     uint32_t* h_pinned = nullptr;
     int64_t profile = 0;           // bracket dominant kernels with events
     cudaEvent_t ev_walk[2] = {nullptr, nullptr};
@@ -121,10 +121,43 @@ template <class T> struct Tree {
 // Resolve the deferred device status of a build / refit (synchronises the stream once).
 template <class T> int resolve_status(Tree<T>* tree);
 
+// The message of the last failed call on this thread (bvhgpu_last_error).
+const char* last_error();
+// A failure that leaves a tree's arrays inconsistent (a build, refit, rebuild or relocation that failed half-way) is STICKY: every
+// later entry point on that tree reports the same status again, and only bvhgpu_tree_free_* is meaningful afterwards.  `msg` is the
+// message as it is; without one it reads "<who> failed after the tree was modified (<last error>)".  A tree that has failed already
+// keeps its first failure.  Serves Tree<T> and Tree4<T> (dim4.cu).
+template <class TreeT> int mark_failed(TreeT* tree, int rc, const char* who, const char* msg = nullptr) {
+    if (tree->failed_status != BVHGPU_OK) return tree->failed_status;
+    char buf[1200];
+    if (!msg) { snprintf(buf, sizeof buf, "%s failed after the tree was modified (%s); the tree is unusable", who, last_error()); msg = buf; }
+    tree->failed_status = rc; tree->failed_message = msg;
+    set_error("%s", msg);
+    return rc;
+}
+
 // ---- memory (stream-ordered pool) ----
 int dalloc(bvhgpu_ctx* ctx, void** p, size_t bytes);
 void dfree(bvhgpu_ctx* ctx, void* p);
 template <class P> inline int dalloc_t(bvhgpu_ctx* ctx, P** p, size_t count) { return dalloc(ctx, (void**)p, count * sizeof(P)); }
+// The result buffers a tree retains for its host-pointer CSR calls (d_offsets / d_hits), grown to at least n + 1 offsets and hits_cap
+// hits; they are never shrunk.  Serves Tree<T> and Tree4<T>.
+template <class TreeT> int ensure_result_buffers(TreeT* tree, size_t n, size_t hits_cap) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    if (tree->offsets_cap < n + 1) {
+        dfree(ctx, tree->d_offsets); tree->d_offsets = nullptr; tree->offsets_cap = 0;
+        const int rc = dalloc_t(ctx, &tree->d_offsets, n + 1);
+        if (rc != BVHGPU_OK) return rc;
+        tree->offsets_cap = n + 1;
+    }
+    if (tree->hits_cap < hits_cap) {
+        dfree(ctx, tree->d_hits); tree->d_hits = nullptr; tree->hits_cap = 0;
+        const int rc = dalloc_t(ctx, &tree->d_hits, hits_cap);
+        if (rc != BVHGPU_OK) return rc;
+        tree->hits_cap = hits_cap;
+    }
+    return BVHGPU_OK;
+}
 // Scratch that is released (stream-ordered) when the scope ends, on every return path.
 struct Scratch {
     bvhgpu_ctx* ctx;
@@ -248,9 +281,84 @@ template <int D, class T> int any_hit_aabb_device(bvhgpu_ctx* ctx, const typenam
 template <class T> int rays_new_device(bvhgpu_ctx* ctx, const T* d_origins, const T* d_dirs, size_t n,
                                        typename Traits<T>::Ray* d_rays);
 
+// ---- dim4.cu: D = 4 ----
+// Traversal record: the AABB the node has in its parent, `skip` (first record behind the subtree) and the shape index of a leaf.
+// Sized in whole 16-byte granules so that a record is fetched with 128-bit non-coherent loads only: 3 for f32, 5 for f64.
+struct __align__(16) TRec4F { float min[4]; float max[4]; uint32_t skip, shape, pad[2]; };    // 48 B
+struct __align__(16) TRec4D { double min[4]; double max[4]; uint32_t skip, shape, pad[2]; };  // 80 B
+static_assert(sizeof(TRec4F) == 48 && sizeof(TRec4D) == 80, "4-D record size");
+static_assert(sizeof(bvh_aabb4f) == 32 && sizeof(bvh_aabb4d) == 64 && sizeof(bvh_ray4f) == 48 && sizeof(bvh_ray4d) == 96, "4-D POD size");
+static_assert(sizeof(bvh_node4f) == 80 && sizeof(bvh_node4d) == 144 && sizeof(bvh_flat4f) == 44 && sizeof(bvh_flat4d) == 80, "4-D POD size");
+
+template <class T> struct D4;
+template <> struct D4<float> { using Aabb = bvh_aabb4f; using Ray = bvh_ray4f; using Node = bvh_node4f; using Flat = bvh_flat4f; using Rec = TRec4F; };
+template <> struct D4<double> { using Aabb = bvh_aabb4d; using Ray = bvh_ray4d; using Node = bvh_node4d; using Flat = bvh_flat4d; using Rec = TRec4D; };
+
+// Bvh<T,4>: its own node types and pipeline (a fourth axis cannot hide in the 3-D kernels the way D = 2 hides in z = 0).
+template <class T> struct Tree4 {
+    using Aabb = typename D4<T>::Aabb; using Node = typename D4<T>::Node; using Flat = typename D4<T>::Flat; using Rec = typename D4<T>::Rec;
+    bvhgpu_ctx* ctx = nullptr;
+    uint32_t n = 0, n_nodes = 0;
+    Aabb* d_aabb = nullptr;            // [n]      shape AABBs (ABI layout: already whole sectors)
+    Node* d_nodes = nullptr;           // [2n-1]   Bvh.nodes, reference preorder layout
+    uint32_t* d_node_index = nullptr;  // [n]      leaf node of every shape
+    uint32_t* d_node_start = nullptr;  // [2n-1]   first position of the node's shape range (== leaves before it)
+    Rec* d_trec = nullptr;             // [n_trec] traversal records (built on first use)
+    uint32_t n_trec = 0;
+    Flat* d_flat = nullptr;            // [n_flat] FlatBvh (built on demand)
+    size_t n_flat = 0;
+    int failed_status = 0;             // sticky (mark_failed)
+    std::string failed_message;
+    uint32_t* d_offsets = nullptr; size_t offsets_cap = 0;   // result buffers of the host-pointer traversal
+    uint32_t* d_hits = nullptr;    size_t hits_cap = 0;
+    T* d_sa_base = nullptr;            // [2n-1] surface area of every inner node when it was last (re)built: baseline of update (first update)
+    uint32_t* d_arrive = nullptr;      // [2n-1] arrival counters of the incremental update (all zero between calls)
+    uint8_t* d_bad = nullptr;          // [2n-1] growth flags of the incremental update (all zero between calls)
+};
+// The status check of a 4-D tree: its build is synchronous, so only a sticky failure (mark_failed) is left to report.
+template <class T> inline int resolve_status(const Tree4<T>* t) {
+    if (t->failed_status != BVHGPU_OK) set_error("%s", t->failed_message.c_str());
+    return t->failed_status;
+}
+// The device-side drivers of dim4.cu.  Arguments and the tree's status are checked by the caller unless said otherwise; everything
+// runs on the context's stream.
+// Exact SAH build of tree->n shapes (tree->n, n_nodes set, n >= 1) from `aabbs` (kind: the direction of that copy).  Synchronous.
+template <class T> int build4(Tree4<T>* tree, const typename D4<T>::Aabb* aabbs, cudaMemcpyKind kind);
+template <class T> int build_flat4(Tree4<T>* tree);                 // tree->n_flat; d_flat built once
+// The CSR walks over the traversal records: probe 0 (PROBE_RAYS4) walks rays, BVHGPU_QUERY_AABB / POINT / BALL the queries.
+// csr4_device: device pointers, synchronises only to return *total; n = 0 or an empty tree give all-zero offsets.  csr4_host: a batch
+// already on the device, host CSR out through the tree's retained buffers (count, read the total, fill, copy back; hits that do not
+// fit `cap` are not copied and the call returns BVHGPU_ERR_CAPACITY); n = 0 or an empty tree give all-zero offsets with no device work.
+constexpr int PROBE_RAYS4 = 0;
+template <class T> int csr4_device(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* d_offsets, uint32_t* d_hits,
+                                   size_t cap, size_t* total, const char* what);
+template <class T> int csr4_host(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
+                                 size_t cap, size_t* total, const char* what);
+// nearest_candidates: the bound walk, then the QUERY_WITHIN CSR of csr4_host.
+template <class T> int nearest_candidates4(Tree4<T>* tree, const T* d_points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total);
+// nearest_to (4 T per point); an empty tree gives BVH_INVALID and 0 for every point.
+template <class T> int nearest4_device(Tree4<T>* tree, int mode, const T* d_points, size_t n, uint32_t* d_shape, T* d_dist);
+// distance-ordered traversal (rays of 12 T); n = 0 or an empty tree give all-zero offsets.
+template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_t nrays, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
+                                       T* d_dists, size_t cap, size_t* total);
+// k nearest shapes: checks n, k and the tree's status, as knn_device does.
+template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
+// m new boxes (and their shape indices, when d_changed is given) checked for NaN / range; the verdict is read back (synchronises).
+template <class T> int check4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m, Scratch& scratch, const char* who);
+template <class T> int put4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m);   // scatter into d_aabb
+template <class T> int refit4(Tree4<T>* tree);                      // bottom-up refit of every node from d_aabb
+template <class T> int update4(Tree4<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt);
+// aabb_all: [n + k] boxes (checked), becomes d_aabb; a failure with tree->d_aabb != aabb_all left the tree untouched.
+template <class T> int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* aabb_all, uint32_t k, double max_growth, size_t* rebuilt);
+// d_rm: [n + 1] removed flags, 1 <= k <= n; a failure with tree->d_nodes unchanged left the tree untouched.
+template <class T> int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint32_t k);
+template <class T> void drop_caches4(Tree4<T>* tree);              // after a relocation: records, flat array, update buffers
+
 }  // namespace bvhb200
 
 struct bvhgpu_tree3f : bvhb200::Tree<float> {};
 struct bvhgpu_tree3d : bvhb200::Tree<double> {};
 struct bvhgpu_tree2f : bvhb200::Tree<float> {};
 struct bvhgpu_tree2d : bvhb200::Tree<double> {};
+struct bvhgpu_tree4f : bvhb200::Tree4<float> {};
+struct bvhgpu_tree4d : bvhb200::Tree4<double> {};
