@@ -319,6 +319,29 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_knn_dev_{self._d['suffix']}")(self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None),
                                                                              C.c_void_p(shape_ptr), C.c_void_p(dist_ptr)))
 
+    def knn_triangles(self, points, k: int, max_dist=None, closest: bool = False):
+        """The k nearest triangles (set_triangles) of every point: (shape (n, k) u32, dist (n, k)), plus closest (n, k, 3) with
+        closest=True.  Keys are Triangle::distance_squared (testbase.rs:353-443), the distance of nearest_triangles_batch; NaN keys never
+        qualify; `max_dist` as in knn.  Slots past the qualifying triangles hold U32_MAX, +inf and NaN closest points.  Equal to a
+        stable brute-force sort wherever every qualifying triangle's key is at least its own box's pruning bound (DESIGN.md 4.17)."""
+        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        n = len(p)
+        r = None if max_dist is None else np.ascontiguousarray(np.broadcast_to(np.asarray(max_dist, dtype=self._d["scalar"]), (n,)))
+        kk = max(int(k), 0)
+        shape = np.zeros((n, kk), dtype=np.uint32)
+        dist = np.zeros((n, kk), dtype=self._d["scalar"])
+        q = np.zeros((n, kk, 3), dtype=self._d["scalar"]) if closest else None
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_triangles_{self._d['suffix']}")(self._h, _ptr(p), n, int(k) & 0xFFFFFFFF, _ptr(r), _ptr(shape),
+                                                                                   _ptr(dist), _ptr(q)))
+        return (shape, dist, q) if closest else (shape, dist)
+
+    def knn_triangles_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int, closest_ptr: int = 0):
+        """knn_triangles from device pointers: n points and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes, distances and
+        (closest_ptr != 0) n * k * 3 closest-point coordinates out, enqueued on the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_triangles_dev_{self._d['suffix']}")(
+            self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None), C.c_void_p(shape_ptr), C.c_void_p(dist_ptr),
+            C.c_void_p(closest_ptr or None)))
+
     def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
         """Bvh::traverse with Aabb / Point / Ball queries (IntersectsAabb implementors other than Ray).
         queries: (n, 6) {min,max} for capi.QUERY_AABB, (n, 3) for QUERY_POINT, (n, 4) {center, radius} for QUERY_BALL."""

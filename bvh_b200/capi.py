@@ -148,6 +148,9 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_knn_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
     for s in ("f32x3", "f64x3", "f32x4", "f64x4"):
         getattr(L, f"bvhgpu_knn_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
+    for s in ("f32x3", "f64x3"):
+        getattr(L, f"bvhgpu_knn_triangles_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
+        getattr(L, f"bvhgpu_knn_triangles_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
     for s in ("f32x4", "f64x4"):
         getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
         getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]

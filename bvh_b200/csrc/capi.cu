@@ -480,6 +480,42 @@ static int knn_dev_impl(TreeOf<D, T>* tree, const void* d_points, size_t n, uint
     if constexpr (D == 4) return knn4_device<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist);
     else return knn_device<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist);
 }
+// k nearest triangles (D = 3), host pointers: as knn_host_impl, plus n * k * 3 closest-point coordinates when out_closest is given.
+// Every check (pointers, n, k, triangles, status) runs in knn_tri_device or before it, so a refused call writes nothing.
+template <class T>
+static int knn_tri_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist, T* out_closest) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("knn_triangles: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("knn_triangles", n));
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn_triangles: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return knn_tri_device<T>(tree, nullptr, 0, k, nullptr, nullptr, nullptr, nullptr);      // the triangle and status checks
+    T *d_p = nullptr, *d_r = nullptr, *d_d = nullptr, *d_q = nullptr;
+    uint32_t* d_s = nullptr;
+    Scratch scratch(ctx);
+    BVH_TRY(upload_records<3>(ctx, scratch, points, n, 1, 0, &d_p));
+    if (max_dist) {
+        BVH_TRY(scratch.get(&d_r, n));
+        BVH_CUDA_TRY(cudaMemcpyAsync(d_r, max_dist, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    const size_t nk = n * k;
+    BVH_TRY(scratch.get(&d_s, nk));
+    BVH_TRY(scratch.get(&d_d, nk));
+    if (out_closest) BVH_TRY(scratch.get(&d_q, 3 * nk));
+    BVH_TRY(knn_tri_device<T>(tree, d_p, n, k, d_r, d_s, d_d, d_q));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nk, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nk, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_closest) BVH_CUDA_TRY(cudaMemcpyAsync(out_closest, d_q, sizeof(T) * 3 * nk, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+// k nearest triangles, device pointers: knn_tri_device checks n, k, the triangles and the tree's status.
+template <class T>
+static int knn_tri_dev_impl(Tree<T>* tree, const void* d_points, size_t n, uint32_t k, const void* d_max_dist, void* d_shape, void* d_dist, void* d_closest) {
+    if (!tree || (n && (!d_points || !d_shape || !d_dist))) { set_error("knn_triangles_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return knn_tri_device<T>(tree, (const T*)d_points, n, k, (const T*)d_max_dist, (uint32_t*)d_shape, (T*)d_dist, (T*)d_closest);
+}
 
 template <int D, class T>
 static int nearest_candidates_host_impl(TreeOf<D, T>* tree, const T* points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
@@ -1282,6 +1318,14 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_knn_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist,  \
                                         void* dev_shape, void* dev_dist) {                                                \
         return knn_dev_impl<3, T>(tree, dev_points, n, k, dev_max_dist, dev_shape, dev_dist);                             \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_knn_triangles_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, \
+                                              T* out_dist, T* out_closest) {                                              \
+        return knn_tri_host_impl<T>(tree, points, n, k, max_dist, out_shape, out_dist, out_closest);                       \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_knn_triangles_dev_##SUF(TREE* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, \
+                                                  void* dev_shape, void* dev_dist, void* dev_closest) {                   \
+        return knn_tri_dev_impl<T>(tree, dev_points, n, k, dev_max_dist, dev_shape, dev_dist, dev_closest);                \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_tree_set_triangles_##SUF(TREE* tree, const T* triangles, size_t n) {                            \
         if (!tree || (n && !triangles)) { set_error("set_triangles: null argument"); return BVHGPU_ERR_INVALID; }         \

@@ -243,6 +243,10 @@ template <class T> int nearest_candidates_device(Tree<T>* tree, const T* d_point
 // k nearest shapes of every point (device pointers: 3 T per point, nq limits or nullptr, nq * k outputs), on the context's stream.
 // Checks nq, k and the tree's status; the pointers are checked by the caller.
 template <class T> int knn_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
+// k nearest triangles (bvhgpu_tree_set_triangles_*), as knn_device with Triangle::distance_squared keys; d_closest (nq * k * 3 T) may be
+// nullptr.  Also refuses a non-empty tree without triangles.
+template <class T> int knn_tri_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist,
+                                      T* d_closest);
 // CSR scan of per-item counts (traverse.cu), launched by the count -> scan -> fill driver of csr.cuh (CsrPasses) for every two-pass
 // walk: scan_local_kernel runs CSR_SCAN_THREADS threads per block over CSR_SCAN_TILE counts and leaves local exclusive offsets and
 // block totals; scan_blocks_kernel (one block of 1024 threads) turns the block totals into exclusive 64-bit block offsets and adds the

@@ -1353,8 +1353,9 @@ template <class T> __device__ __forceinline__ void closest_on_segment(const T p[
 #pragma unroll
     for (int k = 0; k < 3; ++k) out[k] = add_rn(a[k], mul_rn(s, ab[k]));
 }
-template <class T> __device__ __forceinline__ T triangle_distance_squared(const T p[3], const T* __restrict__ tri) {
-    T a[3], b[3], c[3], q[3];
+// closest_point_triangle: the point q of triangle tri that the reference's Triangle::distance_squared measures p against.
+template <class T> __device__ __forceinline__ void triangle_closest_point(const T p[3], const T* __restrict__ tri, T q[3]) {
+    T a[3], b[3], c[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) { a[k] = __ldg(tri + k); b[k] = __ldg(tri + 4 + k); c[k] = __ldg(tri + 8 + k); }
     const bool e_ab = a[0] == b[0] && a[1] == b[1] && a[2] == b[2], e_bc = b[0] == c[0] && b[1] == c[1] && b[2] == c[2], e_ac = a[0] == c[0] && a[1] == c[1] && a[2] == c[2];
@@ -1383,6 +1384,10 @@ template <class T> __device__ __forceinline__ T triangle_distance_squared(const 
             for (int k = 0; k < 3; ++k) q[k] = add_rn(add_rn(a[k], mul_rn(v, ab[k])), mul_rn(w, ac[k]));
         }
     }
+}
+template <class T> __device__ __forceinline__ T triangle_distance_squared(const T p[3], const T* __restrict__ tri) {
+    T q[3];
+    triangle_closest_point(p, tri, q);
     T d[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) d[k] = sub_rn(p[k], q[k]);
@@ -1502,6 +1507,56 @@ int knn_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T*
 }
 template int knn_device<float>(Tree<float>*, const float*, size_t, uint32_t, const float*, uint32_t*, float*);
 template int knn_device<double>(Tree<double>*, const double*, size_t, uint32_t, const double*, uint32_t*, double*);
+
+// ---- k nearest triangles: the same walk with Triangle::distance_squared (triangle_distance_squared, bit for bit the key of
+// nearest_kernel's triangle mode) at the leaves.  A NaN key fails knn_walk's `key <= r2` and never enters the list.  The closest points
+// are recomputed for the k final slots after the walk, in a loop of their own as the square roots are: the list carries no 3 K extra
+// values, and the recomputation performs the same operations on the same inputs, so q is the point the key was measured against. ----
+template <class T> __device__ __forceinline__ T quiet_nan();                                      // the padding of out_closest
+template <> __device__ __forceinline__ float quiet_nan<float>() { return __int_as_float(0x7fc00000); }
+template <> __device__ __forceinline__ double quiet_nan<double>() { return __longlong_as_double(0x7ff8000000000000ll); }
+template <class T, int K>
+__global__ void __launch_bounds__(128) knn_tri_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_shapes,
+                                                      const T* __restrict__ tris, const T* __restrict__ points, const T* __restrict__ max_dist,
+                                                      uint32_t nq, uint32_t k, uint32_t* __restrict__ out_shape, T* __restrict__ out_dist,
+                                                      T* __restrict__ out_closest) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    T p[3];
+    for (int c = 0; c < 3; ++c) p[c] = points[3 * (size_t)i + c];
+    auto leaf = [&](uint32_t shape) { return triangle_distance_squared(p, tris + 12 * (size_t)shape); };
+    knn_point<3, T, K>(nodes, n_shapes, p, max_dist != nullptr, max_dist ? max_dist[i] : T(0), k, out_shape + (size_t)i * k,
+                       out_dist + (size_t)i * k, leaf);
+    if (!out_closest) return;
+#pragma unroll 1
+    for (uint32_t j = 0; j < k; ++j) {
+        const uint32_t s = out_shape[(size_t)i * k + j];
+        T q[3] = {quiet_nan<T>(), quiet_nan<T>(), quiet_nan<T>()};
+        if (s != BVH_INVALID) triangle_closest_point(p, tris + 12 * (size_t)s, q);
+        T* o = out_closest + 3 * ((size_t)i * k + j);
+        for (int c = 0; c < 3; ++c) o[c] = q[c];
+    }
+}
+template <class T>
+int knn_tri_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist, T* d_closest) {
+    if (nq > 0x7FFFFFFFull) { set_error("knn_triangles: n = %zu exceeds 2^31-1", nq); return BVHGPU_ERR_INVALID; }
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn_triangles: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(resolve_status(tree));
+    if (!tree->d_tris && tree->n) { set_error("knn_triangles: triangle distances need bvhgpu_tree_set_triangles_* first"); return BVHGPU_ERR_INVALID; }
+    if (nq == 0) return BVHGPU_OK;
+    bvhgpu_ctx* ctx = tree->ctx;
+    const unsigned grid = (unsigned)((nq + 127) / 128);
+    const T* tris = reinterpret_cast<const T*>(tree->d_tris);
+    knn_bucket(k, [&](auto kb) {
+        knn_tri_kernel<T, decltype(kb)::value><<<grid, 128, 0, ctx->stream>>>(tree->d_nodes, tree->n, tris, d_points, d_max_dist, (uint32_t)nq, k,
+                                                                            d_shape, d_dist, d_closest);
+    });
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+template int knn_tri_device<float>(Tree<float>*, const float*, size_t, uint32_t, const float*, uint32_t*, float*, float*);
+template int knn_tri_device<double>(Tree<double>*, const double*, size_t, uint32_t, const double*, uint32_t*, double*, double*);
 template int nearest_candidates_device<float>(Tree<float>*, const float*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 template int nearest_candidates_device<double>(Tree<double>*, const double*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 

@@ -69,6 +69,24 @@ def create_n_cubes_aabbs(n_cubes: int, prec: str = "f32", bounds=None) -> np.nda
     return out.reshape(-1)
 
 
+_TFR, _TBR, _TBL, _TFL = (1, 1, 0), (1, 1, 1), (0, 1, 1), (0, 1, 0)       # push_cube's corners: 1 = pos + 0.5, 0 = pos - 0.5 per axis
+_BFR, _BBR, _BBL, _BFL = (1, 0, 0), (1, 0, 1), (0, 0, 1), (0, 0, 0)
+_CUBE_TRIS = [(_TBR, _TFR, _TFL), (_TFL, _TBL, _TBR), (_BFL, _BFR, _BBR), (_BBR, _BBL, _BFL), (_TBL, _TFL, _BFL), (_BFL, _BBL, _TBL),
+              (_BFR, _TFR, _TBR), (_TBR, _BBR, _BFR), (_TFL, _TFR, _BFR), (_BFR, _BFL, _TFL), (_BBR, _TBR, _TBL), (_TBL, _BBL, _BBR)]
+
+
+def create_n_cubes_tris(n_cubes: int, prec: str = "f32", bounds=None) -> np.ndarray:
+    """The (12n, 3, 3) triangle vertices of create_n_cubes (push_cube, :490-555), in the order of create_n_cubes_aabbs."""
+    F = BY_PREC[prec]["scalar"]
+    bmin, bmax = bounds if bounds is not None else default_bounds(prec)
+    pos = _next_point3(_splitmix_outputs(0, n_cubes), bmin, bmax, F)
+    side = np.stack([(pos + F(-0.5)).astype(F), (pos + F(0.5)).astype(F)])                # [0 / 1, cube, axis]
+    sel = np.array(_CUBE_TRIS)                                                           # (12, 3 vertices, 3 axes) of 0 / 1
+    ax = np.arange(3)
+    out = side[sel[None, :, :, :], np.arange(n_cubes)[:, None, None, None], ax[None, None, None, :]]
+    return np.ascontiguousarray(out.reshape(-1, 3, 3), dtype=F)
+
+
 def ray_endpoints(n: int, first_ray: int = 0, prec: str = "f32", bounds=None):
     """Origins and (un-normalised) directions of rays first_ray .. first_ray+n-1 of the create_ray chain
     started from seed 0 (two splitmix calls per ray); Ray::new normalises them (on the device)."""

@@ -541,7 +541,7 @@ int bvhgpu_any_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t n
  *   k = 1 is NOT bvhgpu_nearest_*: Bvh::nearest_to prunes with the rounded reference distance, which is not monotone, and on large
  *   coordinates can return a shape that brute force does not pick.  k = 1 is the brute-force minimum of min_distance_squared, ties
  *   to the lower index.
- *   Distances are the AABB's (the UnitBox PointDistance of bvhgpu_nearest_*); there is no triangle form.
+ *   Distances are the AABB's (the UnitBox PointDistance of bvhgpu_nearest_*); bvhgpu_knn_triangles_* below is the triangle form.
  * 1 <= k <= BVHGPU_KNN_MAX_K.  k out of range, a null argument or n > 2^31-1: BVHGPU_ERR_INVALID, nothing written.  n = 0: no-op.
  * An empty tree: rows of padding.  A failed build is reported sticky.  The _dev forms take device pointers (dev_max_dist may be
  * NULL), check k and the pointers on the host and enqueue on the context's stream without synchronising; D = 2 has host pointers only. */
@@ -556,6 +556,38 @@ int bvhgpu_knn_f32x4(bvhgpu_tree4f* tree, const float* points, size_t n, uint32_
 int bvhgpu_knn_f64x4(bvhgpu_tree4d* tree, const double* points, size_t n, uint32_t k, const double* max_dist, uint32_t* out_shape, double* out_dist);
 int bvhgpu_knn_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, void* dev_shape, void* dev_dist);
 int bvhgpu_knn_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist, void* dev_shape, void* dev_dist);
+
+/* ---- k nearest triangles with an optional per-point radius (D = 3): point-to-mesh distance, signed-distance fields, ICP, contact
+ * generation.  The triangles are those of bvhgpu_tree_set_triangles_*; a non-empty tree without them (never set, or dropped by
+ * bvhgpu_add_shapes_*) gives BVHGPU_ERR_INVALID.  After bvhgpu_remove_shapes_* the triangles follow their shapes.
+ *   Key: key_s = Triangle::distance_squared(p_i, tri_s) (closest_point_triangle, src/testbase.rs:353-443, the reference's operation
+ *   order, no FMA), bit for bit the distance bvhgpu_nearest_triangles_* evaluates.  Shape s qualifies when key_s is not NaN and either
+ *   `max_dist` is NULL or max_dist[i] >= 0 (-0 included) and key_s <= fl(max_dist[i] * max_dist[i]).  A NaN key (overflow-scale
+ *   coordinates, a 0 * inf in the interior branch, a point with a NaN coordinate) never qualifies.
+ *   Row i, k slots (arguments and refusals as bvhgpu_knn_*x3): the first min(k, #qualifying) triangles of a stable sort by (key_s, s),
+ *   out_dist = fl(sqrt(key_s)) and out_closest (may be NULL; 3 T per slot, row-major n * k * 3) = the point q that
+ *   closest_point_triangle computed for that key.  Padding slots: BVHGPU_INVALID_INDEX, +inf, NaN x 3.
+ *   Guarantee: the walk prunes with the lower bound of bvhgpu_knn_* on the stored child boxes, so a triangle can be lost only where its
+ *   rounded key lies below box_lower_d2(p, AABB_s) of its own current box; call it bounded at p when it does not.  Where every
+ *   qualifying triangle is bounded, the row is the brute-force row exactly (shapes, distances and closest points bit for bit).
+ *   Elsewhere every entry is a real (s, key_s) in ascending order, every bounded qualifying triangle that sorts before the row's last
+ *   entry is in it, and a row that is not full holds every bounded qualifying triangle.  A triangle inside its box is proven bounded
+ *   in every branch of closest_point_triangle except the interior branch of a near-degenerate triangle, where no counterexample is
+ *   known (DESIGN.md section 4.17); a triangle outside its box (a stale triangle after a refit) need not be bounded.
+ *   A refused call (k outside 1 .. BVHGPU_KNN_MAX_K, a null argument, n > 2^31-1, missing triangles) writes nothing; n = 0 is a no-op
+ *   and an empty tree gives rows of padding.  A failed build is reported sticky, before missing triangles.
+ *   k = 1 is the brute-force minimum of key_s over the bounded triangles, not bvhgpu_nearest_triangles_*, which replays
+ *   Bvh::nearest_to's pruning with the reference's rounded, non-monotone box distance.
+ * The _dev forms take device pointers (dev_max_dist and dev_closest may be NULL) and enqueue on the context's stream without
+ * synchronising. */
+int bvhgpu_knn_triangles_f32x3(bvhgpu_tree3f* tree, const float* points, size_t n, uint32_t k, const float* max_dist, uint32_t* out_shape,
+                               float* out_dist, float* out_closest);
+int bvhgpu_knn_triangles_f64x3(bvhgpu_tree3d* tree, const double* points, size_t n, uint32_t k, const double* max_dist, uint32_t* out_shape,
+                               double* out_dist, double* out_closest);
+int bvhgpu_knn_triangles_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist,
+                                   void* dev_shape, void* dev_dist, void* dev_closest);
+int bvhgpu_knn_triangles_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist,
+                                   void* dev_shape, void* dev_dist, void* dev_closest);
 
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
