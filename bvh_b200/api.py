@@ -306,6 +306,32 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), 1 if triangles else 0, _ptr(shape)))
         return shape
 
+    def multi_hit(self, rays: np.ndarray, k: int, tmax=None, triangles: bool = False, uv: bool = False):
+        """The first k hits along every ray: (shape (n, k) u32, dist (n, k), uv (n, k, 2) with uv=True else None).  Row r is the head
+        of a stable sort of the qualifying hits by key; slots past them hold U32_MAX, +inf and uv (0, 0).  tmax: one limit per ray, a
+        scalar for all, or None for none; a hit qualifies only at a distance < tmax.  triangles=False: key (entry of the shape's own
+        AABB, DFS order), exact; triangles=True: key (Ray::intersects_triangle distance, shape) over the triangles of set_triangles,
+        equal to the unpruned sort wherever its triangles are bounded (DESIGN.md 4.18).  k = 1 without tmax is closest_hit."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        kk = max(int(k), 0)
+        shape = np.zeros((n, kk), dtype=np.uint32)
+        dist = np.zeros((n, kk), dtype=self._d["scalar"])
+        u = np.zeros((n, kk, 2), dtype=self._d["scalar"]) if uv else None
+        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, int(k) & 0xFFFFFFFF, _ptr(tm),
+                                                                                1 if triangles else 0, _ptr(shape), _ptr(dist), _ptr(u)))
+        return shape, dist, u
+
+    def multi_hit_dev(self, rays_ptr: int, nrays: int, k: int, tmax_ptr: int, shape_ptr: int, dist_ptr: int, uv_ptr: int = 0,
+                      triangles: bool = False, layout: int = capi.RAYS_FULL):
+        """multi_hit from device pointers: nrays rays (layout RAYS_FULL: the Ray structs, RAYS_OD: origin + direction) and nrays
+        limits (tmax_ptr = 0: none) in, nrays * k u32 shapes, distances and (uv_ptr != 0) 2 * nrays * k uv out, enqueued on the
+        context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_dev_{self._d['suffix']}")(
+            self._h, C.c_void_p(rays_ptr), layout, nrays, k, C.c_void_p(tmax_ptr or None), 1 if triangles else 0, C.c_void_p(shape_ptr),
+            C.c_void_p(dist_ptr), C.c_void_p(uv_ptr or None)))
+
     def knn(self, points, k: int, max_dist=None):
         """The k nearest shapes of every point: (shape (n, k) u32, dist (n, k)).  Row i lists the shapes in ascending
         (Aabb::min_distance_squared of the shape's own box, index) order with their distances; with `max_dist` (a scalar for all points,
@@ -669,6 +695,19 @@ class Bvh2:
         capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), _ptr(shape)))
         return shape
 
+    def multi_hit(self, rays, k: int, tmax=None):
+        """The first k hits along every ray in AABB mode, with the contract of Bvh.multi_hit: (shape (n, k) u32, dist (n, k), None).
+        Exact: the head of a stable sort by (entry of the shape's own AABB, DFS order) over the hits with distance < tmax."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        kk = max(int(k), 0)
+        shape = np.zeros((n, kk), dtype=np.uint32)
+        dist = np.zeros((n, kk), dtype=self._d["scalar"])
+        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, int(k) & 0xFFFFFFFF, _ptr(tm),
+                                                                                _ptr(shape), _ptr(dist)))
+        return shape, dist, None
+
     def refit(self, aabbs):
         """Bvh::update_shapes' refit (fix_aabbs_ascending) for all shapes: `aabbs` = the new boxes of every shape.  Topology is kept."""
         a = np.ascontiguousarray(aabbs, dtype=self._d["aabb"])
@@ -753,6 +792,13 @@ class Bvh4(Bvh2):
         u32 shapes out, enqueued on the context's stream without host synchronisation."""
         capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, C.c_void_p(tmax_ptr or None),
                                                                                  C.c_void_p(shape_ptr)))
+
+    def multi_hit_dev(self, rays_ptr: int, nrays: int, k: int, tmax_ptr: int, shape_ptr: int, dist_ptr: int):
+        """multi_hit from device pointers: nrays full 4-D rays (12 scalars each) and nrays limits (tmax_ptr = 0: none) in, nrays * k
+        u32 shapes and distances out, enqueued on the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, k,
+                                                                                    C.c_void_p(tmax_ptr or None), C.c_void_p(shape_ptr),
+                                                                                    C.c_void_p(dist_ptr)))
 
     def knn_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int):
         """knn from device pointers: n points (4 scalars each) and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes and

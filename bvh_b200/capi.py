@@ -151,7 +151,12 @@ def lib() -> C.CDLL:
     for s in ("f32x3", "f64x3"):
         getattr(L, f"bvhgpu_knn_triangles_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
         getattr(L, f"bvhgpu_knn_triangles_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
+        getattr(L, f"bvhgpu_multi_hit_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, i32, vp, vp, vp]
+        getattr(L, f"bvhgpu_multi_hit_dev_{s}").argtypes = [vp, vp, i32, sz, C.c_uint32, vp, i32, vp, vp, vp]
+    for s in ("f32x2", "f64x2", "f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_multi_hit_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
     for s in ("f32x4", "f64x4"):
+        getattr(L, f"bvhgpu_multi_hit_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
         getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
         getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
         for f in ("add_shapes", "add_shapes_dev"):

@@ -652,6 +652,61 @@ static int any_hit_dev_impl(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt
     return any_hit_driver<D, T>(tree, d_rays, fmt, nrays, (const T*)d_tmax, use_triangles, (uint32_t*)d_shape);
 }
 
+// Multi hit: the first k hits per ray, rows of k slots.  D = 3: multi_hit_device (checks n, the layout, the status and the triangles);
+// D = 2, 4: multi_hit_aabb_device, as any_hit_driver.
+template <int D, class T>
+static int multi_hit_driver(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, uint32_t k, const T* d_tmax, int use_triangles,
+                            uint32_t* d_shape, T* d_dist, T* d_uv) {
+    if constexpr (D == 3) return multi_hit_device<T>(tree, d_rays, fmt, nrays, k, d_tmax, use_triangles, d_shape, d_dist, d_uv);
+    else return multi_hit_aabb_device<D, T>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, (const T*)d_rays, nrays, k, d_tmax, d_shape, d_dist);
+}
+static int check_k(const char* what, uint32_t k) {
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("%s: k = %u outside 1 .. %d", what, k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+// Multi hit, host pointers: rays and the optional limits staged as any_hit_host_impl stages them, nrays * k slots copied back.  Every
+// refusal happens before the first copy to the caller's buffers.
+template <int D, class T>
+static int multi_hit_host_impl(TreeOf<D, T>* tree, const void* rays, size_t nrays, uint32_t k, const T* tmax, int use_triangles, uint32_t* out_shape,
+                               T* out_dist, T* out_uv) {
+    if (!tree || (nrays && (!rays || !out_shape || !out_dist))) { set_error("multi_hit: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("multi_hit", nrays));
+    BVH_TRY(check_k("multi_hit", k));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    const size_t ray_w = 3 * D, slots = nrays * k;
+    T *d_rays = nullptr, *d_tmax = nullptr, *d_d = nullptr, *d_uv = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(scratch.get(&d_rays, ray_w * nrays));
+    BVH_TRY(scratch.get(&d_s, slots));
+    BVH_TRY(scratch.get(&d_d, slots));
+    if (out_uv) BVH_TRY(scratch.get(&d_uv, 2 * slots));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(T) * ray_w * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    if (tmax) {
+        BVH_TRY(scratch.get(&d_tmax, nrays));
+        BVH_CUDA_TRY(cudaMemcpyAsync(d_tmax, tmax, sizeof(T) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    BVH_TRY((multi_hit_driver<D, T>(tree, d_rays, BVHGPU_RAYS_FULL, nrays, k, d_tmax, use_triangles, d_s, d_d, d_uv)));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * slots, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * slots, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_uv) BVH_CUDA_TRY(cudaMemcpyAsync(out_uv, d_uv, sizeof(T) * 2 * slots, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <int D, class T>
+static int multi_hit_dev_impl(TreeOf<D, T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, uint32_t k, const void* d_tmax, int use_triangles,
+                              void* d_shape, void* d_dist, void* d_uv) {
+    if (!tree || (nrays && (!d_rays || !d_shape || !d_dist))) { set_error("multi_hit_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_k("multi_hit_dev", k));
+    if (D == 4) BVH_TRY(check_n("multi_hit_dev", nrays));
+    if (D == 4) BVH_TRY(resolve_status(tree));
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return multi_hit_driver<D, T>(tree, d_rays, fmt, nrays, k, (const T*)d_tmax, use_triangles, (uint32_t*)d_shape, (T*)d_dist, (T*)d_uv);
+}
+
 template <class T> static int fetch_impl(Tree<T>* tree, uint32_t* hits, size_t cap) {
     if (!tree || !hits) { set_error("traverse_fetch: null argument"); return BVHGPU_ERR_INVALID; }
     if (cap < tree->last_total) { set_error("traverse_fetch: capacity %zu < %zu hits", cap, tree->last_total); return BVHGPU_ERR_CAPACITY; }
@@ -1352,6 +1407,16 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
                                             int use_triangles, void* dev_shape) {                                         \
         return any_hit_dev_impl<3, T>(tree, dev_rays, (uint32_t)ray_layout, nrays, dev_tmax, use_triangles, dev_shape);    \
     }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_multi_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t k, const T* tmax, int use_triangles, \
+                                          uint32_t* out_shape, T* out_dist, T* out_uv) {                                  \
+        return multi_hit_host_impl<3, T>(tree, rays, nrays, k, tmax, use_triangles, out_shape, out_dist, out_uv);          \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_multi_hit_dev_##SUF(TREE* tree, const void* dev_rays, int ray_layout, size_t nrays, uint32_t k,  \
+                                              const void* dev_tmax, int use_triangles, void* dev_shape, void* dev_dist,   \
+                                              void* dev_uv) {                                                             \
+        return multi_hit_dev_impl<3, T>(tree, dev_rays, (uint32_t)ray_layout, nrays, k, dev_tmax, use_triangles, dev_shape, \
+                                        dev_dist, dev_uv);                                                                \
+    }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_stats_##SUF(TREE* tree, uint64_t* out2) {                                              \
         if (!tree || !out2) { set_error("traverse_stats: null argument"); return BVHGPU_ERR_INVALID; }                    \
         out2[0] = tree->last_visits; out2[1] = tree->last_total;                                                          \
@@ -1438,6 +1503,10 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_any_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_shape) {   \
         return any_hit_host_impl<2, T>(tree, rays, nrays, tmax, 0, out_shape);                                                      \
     }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_multi_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t k, const T* tmax, uint32_t* out_shape, \
+                                          T* out_dist) {                                                                   \
+        return multi_hit_host_impl<2, T>(tree, rays, nrays, k, tmax, 0, out_shape, out_dist, nullptr);                     \
+    }                                                                                                                      \
     BVH_EXPORT int bvhgpu_refit_##SUF(TREE* tree, const AABB* aabbs, size_t n) { return refit_impl<2, T>(tree, aabbs, n, false); } \
     BVH_EXPORT int bvhgpu_update_##SUF(TREE* tree, const uint32_t* changed, const AABB* changed_aabbs, size_t m, double max_growth, \
                                        size_t* rebuilt) {                                                                  \
@@ -1503,6 +1572,14 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_any_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, const void* dev_tmax, void* dev_shape) { \
         return any_hit_dev_impl<4, T>(tree, dev_rays, BVHGPU_RAYS_FULL, nrays, dev_tmax, 0, dev_shape);                    \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_multi_hit_##SUF(TREE* tree, const RAY* rays, size_t nrays, uint32_t k, const T* tmax, uint32_t* out_shape, \
+                                          T* out_dist) {                                                                   \
+        return multi_hit_host_impl<4, T>(tree, rays, nrays, k, tmax, 0, out_shape, out_dist, nullptr);                     \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_multi_hit_dev_##SUF(TREE* tree, const void* dev_rays, size_t nrays, uint32_t k, const void* dev_tmax, \
+                                              void* dev_shape, void* dev_dist) {                                           \
+        return multi_hit_dev_impl<4, T>(tree, dev_rays, BVHGPU_RAYS_FULL, nrays, k, dev_tmax, 0, dev_shape, dev_dist, nullptr); \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_knn_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist) { \
         return knn_host_impl<4, T>(tree, points, n, k, max_dist, out_shape, out_dist);                                     \

@@ -25,8 +25,11 @@
 // Dimensions: the AABB mode runs in D = 2, 3 and 4 (the same slab_slice over D axes, common.cuh); triangles are 3-D only.
 // The walk needs no stack: nodes carry parent links, a lane remembers which child it comes back from and re-derives the near / far
 // order from the node (same loads, same bits), so any tree depth works (the reference's iterators use a 32-slot stack / a heap).
+// Multi hit (multi_hit_kernel): the first k hits along the ray, the same walk and ray loading with the sorted register list of the k
+// nearest shapes (key_less / knn_insert of queries.cuh) in place of the one best hit; see the comment above the kernel.
 #include "internal.h"
 #include "csr.cuh"
+#include "queries.cuh"
 
 namespace bvhb200 {
 
@@ -313,6 +316,187 @@ int any_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Nod
     return BVHGPU_OK;
 }
 
+// ---- multi hit (bvhgpu_multi_hit_*): the first k hits along each ray, one ray per thread ----
+// The walk, the near / far order and the ray loading are closest_kernel's.  The one best hit becomes the K-slot list of knn_walk
+// (queries.cuh): sorted DESCENDING, slots 0 .. k-1 start as (+inf, BVH_INVALID), slots k .. K-1 hold (-inf, BVH_INVALID) sentinels, so
+// (d[0], s[0]) is the current k-th key and every index is a compile-time constant.  Keys, in key_less order:
+//   AABB mode      (entry of the shape's own box, the leaf's node index): the DFS tie rule of closest_kernel.  The list holds node
+//                  indices; they are mapped to shapes when the row is written.  A leaf qualifies when its own box passes the slab test
+//                  (and, with a limit, entry < tmax).  A child is entered when its slab test passes, its entry <= d[0] (ties entered)
+//                  and, with a limit, its entry < tmax: exact, since slab entries are monotone under box containment.
+//   triangle mode  (Moeller-Trumbore distance, shape): a triangle qualifies when its distance is < tmax (+inf without a limit, so a
+//                  miss never qualifies).  A child is entered when its slab test passes and entry <= fl(d[0] * (1 + 2^-16)) and
+//                  entry <= fl(tmax * (1 + 2^-16)): closest_kernel's and the any-hit walk's margins.  u and v are recomputed for the
+//                  k final triangles after the walk (the same function on the same inputs), so the list carries only (key, id).
+// With k = 1 and no limit the bounds are closest_kernel's, so the row is closest_hit's; while the list is empty they are the any-hit
+// walk's, so a row is empty exactly where any_hit reports no hit.  Rows start at (size_t)r * k: n * k passes 2^32 from n = 2^26.
+template <int D, class T, bool TRI, int K>
+__global__ void __launch_bounds__(128) multi_hit_kernel(const typename ClosestLayout<D, T>::Node* __restrict__ nodes, uint32_t n_shapes,
+                                                        const typename ClosestLayout<D, T>::Box* __restrict__ aabb, const DTri<T>* __restrict__ tris,
+                                                        const T* __restrict__ rays, uint32_t ray_stride, uint32_t nrays, uint32_t k,
+                                                        const T* __restrict__ ray_tmax, uint32_t* __restrict__ out_shape, T* __restrict__ out_dist,
+                                                        T* __restrict__ out_uv) {
+    static_assert(!TRI || D == 3, "Ray::intersects_triangle is 3-D only");
+    constexpr int BD = D == 4 ? 4 : 3;
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nrays) return;
+    T o[D], dir[D], inv[D];
+    {
+        const T* p = rays + (size_t)ray_stride * r;
+        const bool full = D != 3 || ray_stride == 9;
+#pragma unroll
+        for (int c = 0; c < D; ++c) { o[c] = __ldg(p + c); dir[c] = __ldg(p + D + c); inv[c] = full ? __ldg(p + 2 * D + c) : div_rn(T(1), dir[c]); }
+    }
+    const T INF = Traits<T>::inf();
+    const T margin = TRI ? add_rn(T(1), T(1.0 / 65536.0)) : T(1);
+    const bool has_limit = ray_tmax != nullptr;
+    const T tmax = has_limit ? __ldg(ray_tmax + r) : INF;
+    const T tmax_bound = mul_rn(tmax, margin);                  // triangle mode; inf stays inf, NaN stays NaN
+    T d[K];
+    uint32_t s[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) { d[j] = j < (int)k ? INF : -INF; s[j] = BVH_INVALID; }
+
+    auto leaf = [&](uint32_t shape, uint32_t node_idx) {
+        T key;
+        uint32_t id;
+        bool ok;
+        if constexpr (TRI) {
+            const DTri<T>& t = tris[shape];
+            T a[3], b[3], c[3];
+#pragma unroll
+            for (int q = 0; q < 3; ++q) { a[q] = __ldg(&t.a[q]); b[q] = __ldg(&t.b[q]); c[q] = __ldg(&t.c[q]); }
+            T u, v;
+            key = moeller_trumbore(o, dir, a, b, c, u, v);
+            id = shape;
+            ok = key < tmax;
+        } else {
+            T mn[BD], mx[BD], x;
+            load_box(aabb + shape, mn, mx);
+            ok = slab_slice<D, T>(o, inv, mn, mx, key, x) && (!has_limit || key < tmax);
+            id = node_idx;
+        }
+        if (ok && key_less(key, id, d[0], s[0])) knn_insert(d, s, key, id);
+    };
+    auto enter = [&](bool hit, T e) {
+        if constexpr (TRI) return hit && e <= mul_rn(d[0], margin) && e <= tmax_bound;
+        else return hit && e <= d[0] && (!has_limit || e < tmax);
+    };
+
+    if (n_shapes == 1) {                                       // root leaf (bvh_node.rs:314 tests the shape's own AABB)
+        T mn[BD], mx[BD], e, x;
+        load_box(aabb + nodes[0].shape, mn, mx);
+        if (slab_slice<D, T>(o, inv, mn, mx, e, x)) leaf(nodes[0].shape, 0u);
+    } else {
+        uint32_t node = 0, from = BVH_INVALID;
+        for (;;) {
+            const uint4 meta = __ldg(reinterpret_cast<const uint4*>(nodes + node));      // parent, child_l, child_r, shape / count
+            if (meta.y == BVH_INVALID) {
+                leaf(meta.w, node);
+                from = node; node = meta.x;
+                continue;
+            }
+            const typename ClosestLayout<D, T>::Node& nd = nodes[node];
+            T lmn[D], lmx[D], rmn[D], rmx[D], el, er, x;
+#pragma unroll
+            for (int c = 0; c < D; ++c) { lmn[c] = __ldg(&nd.l_aabb.min[c]); lmx[c] = __ldg(&nd.l_aabb.max[c]); rmn[c] = __ldg(&nd.r_aabb.min[c]); rmx[c] = __ldg(&nd.r_aabb.max[c]); }
+            const bool hl = slab_slice<D, T>(o, inv, lmn, lmx, el, x), hr = slab_slice<D, T>(o, inv, rmn, rmx, er, x);
+            if (!hl) el = INF;
+            if (!hr) er = INF;
+            const bool left_first = el <= er;
+            const uint32_t near_i = left_first ? meta.y : meta.z, far_i = left_first ? meta.z : meta.y;
+            const T near_e = left_first ? el : er, far_e = left_first ? er : el;
+            const bool near_ok = left_first ? hl : hr, far_ok = left_first ? hr : hl;
+            uint32_t next = BVH_INVALID;
+            if (from == BVH_INVALID) {
+                if (enter(near_ok, near_e)) next = near_i;
+                else from = near_i;                             // skipped: as if we had just come back from it
+            }
+            if (next == BVH_INVALID && from == near_i) {        // the far child, against the k-th key as it is now
+                if (enter(far_ok, far_e)) next = far_i;
+                else from = far_i;
+            }
+            if (next != BVH_INVALID) { node = next; from = BVH_INVALID; continue; }
+            if (node == 0) break;
+            from = node; node = meta.x;
+        }
+    }
+    const size_t base = (size_t)r * k;
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+        if (j < (int)k) { out_shape[base + k - 1 - j] = s[j]; out_dist[base + k - 1 - j] = d[j]; }
+    // node indices -> shapes, and u, v, in loops of their own after the list is dead (no spills, one call site of moeller_trumbore)
+#pragma unroll 1
+    for (uint32_t j = 0; j < k; ++j) {
+        const uint32_t id = out_shape[base + j];
+        T u = T(0), v = T(0);
+        if constexpr (TRI) {
+            if (id != BVH_INVALID && out_uv) {
+                const DTri<T>& t = tris[id];
+                T a[3], b[3], c[3];
+#pragma unroll
+                for (int q = 0; q < 3; ++q) { a[q] = __ldg(&t.a[q]); b[q] = __ldg(&t.b[q]); c[q] = __ldg(&t.c[q]); }
+                moeller_trumbore(o, dir, a, b, c, u, v);
+            }
+        } else if (id != BVH_INVALID) {
+            out_shape[base + j] = __ldg(&reinterpret_cast<const uint4*>(nodes + id)->w);
+        }
+        if (out_uv) { out_uv[2 * (base + j)] = u; out_uv[2 * (base + j) + 1] = v; }
+    }
+}
+
+template <class T>
+__global__ void __launch_bounds__(256) fill_multi_pad_kernel(size_t n, uint32_t* __restrict__ shape, T* __restrict__ dist, T* __restrict__ uv) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        shape[i] = BVH_INVALID; dist[i] = Traits<T>::inf();
+        if (uv) { uv[2 * i] = T(0); uv[2 * i + 1] = T(0); }
+    }
+}
+
+// One launch of multi_hit_kernel in the K bucket of k (knn_bucket), or rows of padding for an empty tree.
+template <int D, class T, bool TRI>
+static int multi_hit_launch(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes, const typename ClosestLayout<D, T>::Box* aabb,
+                            const DTri<T>* tris, const T* d_rays, uint32_t stride, size_t nrays, uint32_t k, const T* d_tmax, uint32_t* d_shape,
+                            T* d_dist, T* d_uv) {
+    cudaStream_t st = ctx->stream;
+    if (n_shapes == 0) {
+        const size_t slots = nrays * k;
+        fill_multi_pad_kernel<T><<<(unsigned)std::min<size_t>((slots + 255) / 256, 65535), 256, 0, st>>>(slots, d_shape, d_dist, d_uv);
+    } else {
+        const unsigned grid = (unsigned)((nrays + 127) / 128);
+        knn_bucket(k, [&](auto kb) {
+            multi_hit_kernel<D, T, TRI, decltype(kb)::value><<<grid, 128, 0, st>>>(nodes, n_shapes, aabb, tris, d_rays, stride, (uint32_t)nrays, k, d_tmax,
+                                                                              d_shape, d_dist, d_uv);
+        });
+    }
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+template <class T>
+int multi_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, uint32_t k, const T* d_tmax, int use_triangles,
+                     uint32_t* d_shape, T* d_dist, T* d_uv) {
+    if (nrays > 0x7FFFFFFFull) { set_error("multi_hit: too many rays"); return BVHGPU_ERR_INVALID; }
+    if (fmt != BVHGPU_RAYS_FULL && fmt != BVHGPU_RAYS_OD) { set_error("multi_hit: bad ray layout %u", fmt); return BVHGPU_ERR_INVALID; }
+    if (nrays == 0) return BVHGPU_OK;
+    BVH_TRY(resolve_status(tree));
+    if (use_triangles && tree->n && !tree->d_tris) { set_error("multi_hit: triangle mode needs bvhgpu_tree_set_triangles_* first"); return BVHGPU_ERR_INVALID; }
+    const uint32_t stride = fmt == BVHGPU_RAYS_FULL ? 9u : 6u;
+    const T* rays = reinterpret_cast<const T*>(d_rays);
+    if (use_triangles)
+        return multi_hit_launch<3, T, true>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), rays, stride,
+                                            nrays, k, d_tmax, d_shape, d_dist, d_uv);
+    return multi_hit_launch<3, T, false>(tree->ctx, tree->d_nodes, tree->n, tree->d_aabb, nullptr, rays, stride, nrays, k, d_tmax, d_shape, d_dist, d_uv);
+}
+
+template <int D, class T>
+int multi_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes, const typename ClosestLayout<D, T>::Box* aabb,
+                          const T* d_rays, size_t nrays, uint32_t k, const T* d_tmax, uint32_t* d_shape, T* d_dist) {
+    if (nrays == 0) return BVHGPU_OK;
+    return multi_hit_launch<D, T, false>(ctx, nodes, n_shapes, aabb, nullptr, d_rays, 3 * D, nrays, k, d_tmax, d_shape, d_dist, nullptr);
+}
+
 template int set_triangles<float>(Tree<float>*, const float*, size_t, bool);
 template int set_triangles<double>(Tree<double>*, const double*, size_t, bool);
 template int closest_hit_device<float>(Tree<float>*, const void*, uint32_t, size_t, int, uint32_t*, float*, float*);
@@ -328,5 +512,12 @@ template int any_hit_aabb_device<2, float>(bvhgpu_ctx*, const bvh_node3f*, uint3
 template int any_hit_aabb_device<2, double>(bvhgpu_ctx*, const bvh_node3d*, uint32_t, const DAabbD*, const double*, size_t, const double*, uint32_t*);
 template int any_hit_aabb_device<4, float>(bvhgpu_ctx*, const bvh_node4f*, uint32_t, const bvh_aabb4f*, const float*, size_t, const float*, uint32_t*);
 template int any_hit_aabb_device<4, double>(bvhgpu_ctx*, const bvh_node4d*, uint32_t, const bvh_aabb4d*, const double*, size_t, const double*, uint32_t*);
+
+template int multi_hit_device<float>(Tree<float>*, const void*, uint32_t, size_t, uint32_t, const float*, int, uint32_t*, float*, float*);
+template int multi_hit_device<double>(Tree<double>*, const void*, uint32_t, size_t, uint32_t, const double*, int, uint32_t*, double*, double*);
+template int multi_hit_aabb_device<2, float>(bvhgpu_ctx*, const bvh_node3f*, uint32_t, const DAabbF*, const float*, size_t, uint32_t, const float*, uint32_t*, float*);
+template int multi_hit_aabb_device<2, double>(bvhgpu_ctx*, const bvh_node3d*, uint32_t, const DAabbD*, const double*, size_t, uint32_t, const double*, uint32_t*, double*);
+template int multi_hit_aabb_device<4, float>(bvhgpu_ctx*, const bvh_node4f*, uint32_t, const bvh_aabb4f*, const float*, size_t, uint32_t, const float*, uint32_t*, float*);
+template int multi_hit_aabb_device<4, double>(bvhgpu_ctx*, const bvh_node4d*, uint32_t, const bvh_aabb4d*, const double*, size_t, uint32_t, const double*, uint32_t*, double*);
 
 }  // namespace bvhb200

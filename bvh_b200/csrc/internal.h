@@ -282,6 +282,15 @@ template <int D, class T> int closest_aabb_device(bvhgpu_ctx* ctx, const typenam
 template <class T> int any_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const T* d_tmax, int use_triangles, uint32_t* d_shape);
 template <int D, class T> int any_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes,
                                                   const typename ClosestLayout<D, T>::Box* aabb, const T* d_rays, size_t nrays, const T* d_tmax, uint32_t* d_shape);
+// Multi hit (closest.cu): per ray the first k hits of the closest walk's keys with distance < tmax (d_tmax: nrays limits or nullptr
+// for no limit), rows of k slots (nrays * k outputs, d_uv: 2 T per slot or nullptr), padded with (BVH_INVALID, +inf, 0, 0); device
+// pointers, on the context's stream.  1 <= k <= BVHGPU_KNN_MAX_K is checked by the caller.  multi_hit_device checks the other
+// arguments and the tree's status as any_hit_device does; multi_hit_aabb_device (D = 2, 4) leaves them to the caller.
+template <class T> int multi_hit_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, uint32_t k, const T* d_tmax, int use_triangles,
+                                        uint32_t* d_shape, T* d_dist, T* d_uv);
+template <int D, class T> int multi_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes,
+                                                    const typename ClosestLayout<D, T>::Box* aabb, const T* d_rays, size_t nrays, uint32_t k,
+                                                    const T* d_tmax, uint32_t* d_shape, T* d_dist);
 template <class T> int rays_new_device(bvhgpu_ctx* ctx, const T* d_origins, const T* d_dirs, size_t n,
                                        typename Traits<T>::Ray* d_rays);
 

@@ -589,6 +589,54 @@ int bvhgpu_knn_triangles_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_points, 
 int bvhgpu_knn_triangles_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_points, size_t n, uint32_t k, const void* dev_max_dist,
                                    void* dev_shape, void* dev_dist, void* dev_closest);
 
+/* ---- multi hit: the first k hits along each ray, with an optional per-ray distance limit (transparency and layered surfaces, LiDAR
+ * with several returns, entry plus exit for wall thickness, inside / outside counting).  The closest_hit walk keeping a sorted list of
+ * k keys instead of one.  Output, row-major, k slots per ray: row r is the first min(k, #qualifying) entries of a stable sort of the
+ * qualifying set by key; slots past them hold BVHGPU_INVALID_INDEX, +inf and uv (0, 0) (what closest_hit writes for no hit).
+ * Limit: `tmax` NULL: none (no comparison, as closest_hit).  Otherwise an entry qualifies only if its distance is < tmax[r], the strict
+ * comparison of any_hit, so tmax[r] <= 0 (-0 included) or NaN gives an empty row.
+ *   use_triangles == 0 (D = 2, 3, 4): the candidates are the shapes of Bvh::traverse's set (BVH semantics); s qualifies when the slab
+ *       test of its own AABB passes.  Key (e_s, the leaf's node index): e_s the entry of Ray::intersection_slice_for_aabb bit for bit as
+ *       closest_hit computes it, ties in DFS order (closest_hit's rule).  out_dist = e_s; out_uv, if given, zeros.  EXACT for every
+ *       input: a child is pruned only when its slab test fails, its entry exceeds the current k-th key or (with a limit) its entry is
+ *       >= tmax[r]; slab entries are monotone under box containment ("no split wins" empty boxes pass at entry 0).  On a built tree
+ *       without "no split wins" nodes and with tmax NULL, a row is the head of bvhgpu_traverse_ordered_* (ascending).
+ *   use_triangles != 0 (D = 3, triangles from bvhgpu_tree_set_triangles_*): key (d_s, s), d_s = Ray::intersects_triangle
+ *       (Moeller-Trumbore with backface culling, the reference's operation order, no FMA; the function of closest_hit); s qualifies
+ *       when d_s is finite.  out_uv (may be NULL) = the u, v of that evaluation.  Leaves are reached through their stored boxes only; a
+ *       child is entered when its slab test passes and entry <= min(fl(kth * (1 + 2^-16)), fl(tmax[r] * (1 + 2^-16))), kth = +inf
+ *       until the list is full: the margins of closest_hit / any_hit.  Call s bounded on ray r when the box its parent stores for it
+ *       passes the slab test with entry <= fl(d_s * (1 + 2^-16)).  Where every triangle of the unpruned row (the stable sort of the loop
+ *       over Bvh::traverse with intersects_triangle) is bounded, the row equals it bit for bit: shapes, distances and uv.  Elsewhere (the
+ *       grazing hits closest_hit documents) every entry is still a real qualifying (s, d_s), in ascending order.
+ *   Identities: k = 1 with tmax NULL is closest_hit (shape, distance, uv) in both modes and every D; with tmax given, a row is empty
+ *   exactly where any_hit with the same tmax reports no hit.
+ *   1 <= k <= BVHGPU_KNN_MAX_K.  k out of range, a null argument, nrays > 2^31-1, an unknown ray_layout, or use_triangles without
+ *   triangles (never set, or dropped by bvhgpu_add_shapes_*): BVHGPU_ERR_INVALID, nothing written.  nrays = 0: no-op.  An empty tree:
+ *   rows of padding; n = 1: the shape's own box decides.  A failed build is reported sticky, before missing triangles.  After
+ *   bvhgpu_remove_shapes_* the triangles follow their shapes.  The _dev forms take device pointers (dev_tmax and dev_uv may be NULL),
+ *   check k and the pointers on the host and enqueue on the context's stream without synchronising; D = 2 has host pointers only. */
+int bvhgpu_multi_hit_f32x3(bvhgpu_tree3f* tree, const bvh_ray3f* rays, size_t nrays, uint32_t k, const float* tmax, int use_triangles,
+                           uint32_t* out_shape, float* out_dist, float* out_uv);
+int bvhgpu_multi_hit_f64x3(bvhgpu_tree3d* tree, const bvh_ray3d* rays, size_t nrays, uint32_t k, const double* tmax, int use_triangles,
+                           uint32_t* out_shape, double* out_dist, double* out_uv);
+int bvhgpu_multi_hit_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_rays, int ray_layout, size_t nrays, uint32_t k, const void* dev_tmax,
+                               int use_triangles, void* dev_shape, void* dev_dist, void* dev_uv);   /* FULL or OD rays */
+int bvhgpu_multi_hit_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_rays, int ray_layout, size_t nrays, uint32_t k, const void* dev_tmax,
+                               int use_triangles, void* dev_shape, void* dev_dist, void* dev_uv);
+int bvhgpu_multi_hit_f32x2(bvhgpu_tree2f* tree, const bvh_ray2f* rays, size_t nrays, uint32_t k, const float* tmax, uint32_t* out_shape,
+                           float* out_dist);
+int bvhgpu_multi_hit_f64x2(bvhgpu_tree2d* tree, const bvh_ray2d* rays, size_t nrays, uint32_t k, const double* tmax, uint32_t* out_shape,
+                           double* out_dist);
+int bvhgpu_multi_hit_f32x4(bvhgpu_tree4f* tree, const bvh_ray4f* rays, size_t nrays, uint32_t k, const float* tmax, uint32_t* out_shape,
+                           float* out_dist);
+int bvhgpu_multi_hit_f64x4(bvhgpu_tree4d* tree, const bvh_ray4d* rays, size_t nrays, uint32_t k, const double* tmax, uint32_t* out_shape,
+                           double* out_dist);
+int bvhgpu_multi_hit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_rays, size_t nrays, uint32_t k, const void* dev_tmax, void* dev_shape,
+                               void* dev_dist);
+int bvhgpu_multi_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t nrays, uint32_t k, const void* dev_tmax, void* dev_shape,
+                               void* dev_dist);
+
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
  * leaves (user code), so there are two forms.  `points`: 3 T per query point, host pointers.

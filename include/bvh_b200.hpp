@@ -100,6 +100,7 @@ template <> struct Abi<float> {
     static int set_triangles(tree* t, const float* abc, size_t n) { return bvhgpu_tree_set_triangles_f32x3(t, abc, n); }
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_closest_hit_f32x3(t, r, n, tri, s, d, uv); }
     static int any(tree* t, const ray* r, size_t n, const float* tm, int tri, uint32_t* s) { return bvhgpu_any_hit_f32x3(t, r, n, tm, tri, s); }
+    static int multi(tree* t, const ray* r, size_t n, uint32_t k, const float* tm, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_multi_hit_f32x3(t, r, n, k, tm, tri, s, d, uv); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f32x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
 };
@@ -118,6 +119,7 @@ template <> struct Abi<double> {
     static int set_triangles(tree* t, const double* abc, size_t n) { return bvhgpu_tree_set_triangles_f64x3(t, abc, n); }
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_closest_hit_f64x3(t, r, n, tri, s, d, uv); }
     static int any(tree* t, const ray* r, size_t n, const double* tm, int tri, uint32_t* s) { return bvhgpu_any_hit_f64x3(t, r, n, tm, tri, s); }
+    static int multi(tree* t, const ray* r, size_t n, uint32_t k, const double* tm, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_multi_hit_f64x3(t, r, n, k, tm, tri, s, d, uv); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f64x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
 };
@@ -341,6 +343,18 @@ template <class T> class Bvh {
         if (!tmax.empty() && tmax.size() != rays.size()) throw Error(BVHGPU_ERR_INVALID, "any_hit: one limit per ray, or none");
         shape.assign(rays.size(), 0);
         check(A::any(tree_, reinterpret_cast<const typename A::ray*>(rays.data()), rays.size(), tmax.empty() ? nullptr : tmax.data(), triangles ? 1 : 0, shape.data()));
+    }
+    // The first k hits per ray (transparency, several LiDAR returns, entry and exit of a wall): row i of shape / distance (k slots each,
+    // row-major) lists the hits at a distance < tmax[i] (tmax empty: no limit) in ascending (distance, tie) order, then UINT32_MAX and
+    // +inf.  triangle == false: the shapes whose own AABB the ray enters, by entry (exact); true: Moeller-Trumbore hits of the triangles
+    // of set_triangles, with u, v in uv (2 per slot) when it is given.  k = 1 without a limit is closest_hit.  1 <= k <= 64.
+    void multi_hit(const std::vector<Ray<T>>& rays, uint32_t k, const std::vector<T>& tmax, bool triangles, std::vector<uint32_t>& shape,
+                   std::vector<T>& distance, std::vector<T>* uv = nullptr) const {
+        if (!tmax.empty() && tmax.size() != rays.size()) throw Error(BVHGPU_ERR_INVALID, "multi_hit: one limit per ray, or none");
+        shape.assign(rays.size() * k, 0); distance.assign(rays.size() * k, T(0));
+        if (uv) uv->assign(2 * rays.size() * k, T(0));
+        check(A::multi(tree_, reinterpret_cast<const typename A::ray*>(rays.data()), rays.size(), k, tmax.empty() ? nullptr : tmax.data(),
+                       triangles ? 1 : 0, shape.data(), distance.data(), uv ? uv->data() : nullptr));
     }
     size_t num_shapes() const { return n_; }
 

@@ -59,6 +59,12 @@ for prec, ncubes in (("f32", 60), ("f32", 700), ("f64", 300)):
                                                                          C.c_void_p(d_sh.data_ptr())))
         ctx.synchronize()
     print("  any hit", int((ah_t != 0xFFFFFFFF).sum()), int((ah_a != 0xFFFFFFFF).sum()))
+    # multi hit: both modes, every K bucket, with and without limits, host form with uv and the device form with OD rays
+    for k in (1, 5, 9, 17, 33):
+        b.multi_hit(rays, k, cd, triangles=True, uv=True); b.multi_hit(rays, k, triangles=False)
+    d_ms = torch.empty(len(rays) * 7, dtype=torch.int32, device="cuda:0"); d_md = torch.empty(len(rays) * 7, dtype=tdt, device="cuda:0")
+    b.multi_hit_dev(d_r.data_ptr(), len(rays), 7, d_tm.data_ptr(), d_ms.data_ptr(), d_md.data_ptr(), triangles=True, layout=capi.RAYS_OD)
+    ctx.synchronize()
     b.free()
 # D = 2
 from bvh_b200.dtypes import BY_PREC_2D
@@ -73,6 +79,7 @@ for prec in ("f32", "f64"):
         b2.traverse_batch(r2, mode=mode)
     b2.traverse_ordered(r2, True); b2.traverse_ordered(r2, False); _, c2 = b2.closest_hit(r2)
     b2.any_hit(r2); b2.any_hit(r2, np.nextafter(c2, np.inf))
+    b2.multi_hit(r2, 3); b2.multi_hit(r2, 40, np.nextafter(c2, np.inf))
     b2.free()
 # 4-D ordered traversal, closest hit and any hit (host and device-pointer forms)
 from bvh_b200.dtypes import BY_PREC_4D
@@ -90,6 +97,7 @@ for prec in ("f32", "f64"):
     b4.closest_hit_dev(dr.data_ptr(), 300, ds.data_ptr(), dd.data_ptr()); ctx.synchronize()
     b4.any_hit(r4); b4.any_hit(r4, np.full(300, 50.0))
     b4.any_hit_dev(dr.data_ptr(), 300, dd.data_ptr(), ds.data_ptr()); b4.any_hit_dev(dr.data_ptr(), 300, 0, ds.data_ptr()); ctx.synchronize()
+    b4.multi_hit(r4, 3); b4.multi_hit(r4, 40, np.full(300, 50.0)); b4.multi_hit_dev(dr.data_ptr(), 300, 1, 0, ds.data_ptr(), dd.data_ptr()); ctx.synchronize()
     b4.free()
 # host path on a batch large enough to be chunked (under the sanitizer the library takes the copy-then-walk form; forced streaming too)
 a = scenes.create_n_cubes_aabbs(300)
