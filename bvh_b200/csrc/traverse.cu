@@ -72,6 +72,21 @@ __device__ __forceinline__ bool slab_hit(const T o[3], const T inv[3], const T m
     const T lo = tmin > T(0) ? tmin : T(0);                     // fast_max(tmin, 0), utils.rs:52-54
     return !nan && tmax >= lo;                                  // :35
 }
+// f32: the folds propagate NaN (min.NaN / max.NaN, one FMNMX.NAN each) and the six NaN tests go.  Every product enters both the
+// tmin and the tmax fold, so a NaN anywhere makes tmax NaN and `tmax >= lo` false: a miss, as above.  Without a NaN both forms
+// give the same values up to the sign of a zero, which neither the clamp nor the comparison can see (DESIGN §2).
+__device__ __forceinline__ float fmin_nan(float a, float b) { float r; asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+__device__ __forceinline__ float fmax_nan(float a, float b) { float r; asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+template <>
+__device__ __forceinline__ bool slab_hit<float>(const float o[3], const float inv[3], const float mn[3], const float mx[3]) {
+    const float l0 = mul_rn(sub_rn(mn[0], o[0]), inv[0]), r0 = mul_rn(sub_rn(mx[0], o[0]), inv[0]);
+    const float l1 = mul_rn(sub_rn(mn[1], o[1]), inv[1]), r1 = mul_rn(sub_rn(mx[1], o[1]), inv[1]);
+    const float l2 = mul_rn(sub_rn(mn[2], o[2]), inv[2]), r2 = mul_rn(sub_rn(mx[2], o[2]), inv[2]);
+    const float tmin = fmax_nan(fmax_nan(fmin_nan(l0, r0), fmin_nan(l1, r1)), fmin_nan(l2, r2));
+    const float tmax = fmin_nan(fmin_nan(fmax_nan(l0, r0), fmax_nan(l1, r1)), fmax_nan(l2, r2));
+    const float lo = tmin > 0.f ? tmin : 0.f;
+    return tmax >= lo;
+}
 
 // The walk.  `emit(shape)` is called for every reported shape in reference order.
 template <class T, bool FLAT, class Emit>
@@ -310,17 +325,20 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
     const uint32_t n_top = reinterpret_cast<const uint32_t*>(top)[0];      // header {n_top, C}, then lo[n_top], hi[n_top]
     for (uint32_t k = threadIdx.x; k < 2 * n_top; k += blockDim.x) s_top[k] = top[2 + k];
     __syncthreads();
-    uint32_t s_lo;                                                   // opaque: keeps ptxas from re-deriving the window address every visit
+    uint32_t s_lo, s_hi;                                             // opaque: keeps ptxas from re-deriving the window addresses every visit
     asm volatile("mov.u32 %0, %1;" : "=r"(s_lo) : "r"((uint32_t)__cvta_generic_to_shared(s_top)));
-    const uint32_t s_hi = s_lo + 16u * n_top;
+    asm volatile("mov.u32 %0, %1;" : "=r"(s_hi) : "r"(s_lo + 16u * n_top));
     constexpr uint32_t NONE = 0xFFFFFFFFu;
     const uint32_t FULL = 0xffffffffu;
     const uint32_t lane = lane_id(), lt = lanemask_lt();
     // Lane state: r ray, j next top entry (the resume point while below the top), [g, gend) global records left to walk in the
-    // current fringe subtree -- empty (gend = 0) while the lane is in the top.  STREAM: `loaded` as in walk_persistent_kernel.
-    uint32_t r = NONE, j = 0, g = 0, gend = 0, cnt = 0, visits = 0;
+    // current fringe subtree -- empty (g >= gend) while the lane is in the top.  The lane walks while g < gend || j < n_top: a
+    // lane without a ray, with a ray still in flight (STREAM: `loaded` as in walk_persistent_kernel) or with a finished ray has
+    // j = NONE or j >= n_top and an empty range, so the visit needs no other test of the lane.
+    uint32_t r = NONE, j = NONE, g = 0, gend = 0, cnt = 0, visits = 0;
     bool loaded = false;
     float o[3] = {0.f, 0.f, 0.f}, inv[3] = {0.f, 0.f, 0.f};
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;              // the record being visited: {min, w3}, {max, w7}
     bool exhausted = false;
     for (;;) {
         const uint32_t need = __ballot_sync(FULL, r == NONE);
@@ -332,9 +350,9 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
             const uint32_t mine = base + __popc(need & lt);
             // (no top records -- a degenerate tree whose first histogram bin already exceeds the budget: everything is "below")
             if (r == NONE && mine < nrays) {
-                r = mine; j = 0; cnt = 0; g = 0; gend = n_top ? 0u : n_rec;
-                if (STREAM) loaded = false;
-                else load_ray<float, false>(rays, mine, o, inv);
+                r = mine; cnt = 0; g = 0;
+                if (STREAM) { loaded = false; j = NONE; gend = 0; }         // pending: does not walk until its ray is loaded
+                else { j = 0; gend = n_top ? 0u : n_rec; load_ray<float, false>(rays, mine, o, inv); }
             }
         }
         if (STREAM) {                                                // see walk_persistent_kernel: pending lanes never block walking lanes
@@ -364,7 +382,10 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
                     if (r != NONE && !loaded) r = NONE;
                 } else if (__ballot_sync(FULL, r != NONE && !loaded && r < rd)) {
                     __threadfence();
-                    if (r != NONE && !loaded && r < rd) { load_ray<float, true>(rays, r, o, inv); loaded = true; }
+                    if (r != NONE && !loaded && r < rd) {
+                        load_ray<float, true>(rays, r, o, inv); loaded = true;
+                        j = 0; gend = n_top ? 0u : n_rec;
+                    }
                 }
             }
         }
@@ -373,23 +394,24 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
         // One warp step = VPC visits per lane, then one vote on the idle lanes: the vote, its population count and the loop branch
         // are paid once per VPC visits.  A lane whose ray ends inside a step idles for the rest of it, and the warp goes back for
         // tickets up to VPC - 1 visits later: cheap where a visit is a shared-memory or L1/L2 hit, not where visits wait on DRAM.
-        auto visit = [&]() {
+        // VPC = 1 (trees beyond L2, visits wait on DRAM): the visit branches between the top and the global records and ends the
+        // ray itself; the predicated visit below was 2 % slower there (DESIGN §4.3).
+        auto visit_branchy = [&]() {
             if (r != NONE && (!STREAM || loaded)) {
                 float mn[3], mx[3];
                 uint32_t w3, w7;
                 const bool below = g < gend;
                 if (!below) {
-                    float4 a, b;                                      // explicit shared-window addresses: two LDS.128, no per-visit cvta
-                    asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w) : "r"(s_lo + 16u * j));
-                    asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "r"(s_hi + 16u * j));
-                    mn[0] = a.x; mn[1] = a.y; mn[2] = a.z; w3 = __float_as_uint(a.w);
-                    mx[0] = b.x; mx[1] = b.y; mx[2] = b.z; w7 = __float_as_uint(b.w);
+                    float4 lo4, hi4;                                  // explicit shared-window addresses: two LDS.128, no per-visit cvta
+                    asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(lo4.x), "=f"(lo4.y), "=f"(lo4.z), "=f"(lo4.w) : "r"(s_lo + 16u * j));
+                    asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(hi4.x), "=f"(hi4.y), "=f"(hi4.z), "=f"(hi4.w) : "r"(s_hi + 16u * j));
+                    mn[0] = lo4.x; mn[1] = lo4.y; mn[2] = lo4.z; w3 = __float_as_uint(lo4.w);
+                    mx[0] = hi4.x; mx[1] = hi4.y; mx[2] = hi4.z; w7 = __float_as_uint(hi4.w);
                 } else {
                     fetch(trec + g, mn, mx, w3, w7);
                 }
                 ++visits;
-                // One select chain for both index spaces (no divergence between lanes in the top and lanes below it):
-                //   top entry: w7 = ~0 top-internal | 0x80000000+first global record (fringe inner, w3 = end of that range) | shape
+                // One select chain for both index spaces (no divergence between lanes in the top and lanes below it).
                 const bool hit = slab_hit(o, inv, mn, mx);
                 const bool fringe = !below && (w7 + 0x80000000u) < 0x7FFFFFFFu;
                 const uint32_t cur = below ? g : j;
@@ -409,10 +431,51 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
                 if (g >= gend && j >= n_top) { counts[r] = cnt; r = NONE; }
             }
         };
+        // VPC > 1: a visit is straight-line code for every lane: the record comes from a predicated LDS pair (top) or LDG pair
+        // (below) into the same registers, and the lane state moves by predicated selects.  Only a reached leaf branches.
+        auto visit = [&]() {
+            const bool below = g < gend;
+            const bool top = !below && j < n_top;
+            const bool walking = below || top;
+            const TNodeF* gp = trec + g;
+            asm("{\n\t.reg .pred pt, pb;\n\t"
+                "setp.ne.u32 pt, %10, 0;\n\tsetp.ne.u32 pb, %11, 0;\n\t"
+                "@pt ld.shared.v4.f32 {%0,%1,%2,%3}, [%8];\n\t"
+                "@pt ld.shared.v4.f32 {%4,%5,%6,%7}, [%9];\n\t"
+                "@pb ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%12];\n\t"
+                "@pb ld.global.nc.v4.f32 {%4,%5,%6,%7}, [%12+16];\n\t}"
+                : "+f"(a.x), "+f"(a.y), "+f"(a.z), "+f"(a.w), "+f"(b.x), "+f"(b.y), "+f"(b.z), "+f"(b.w)
+                : "r"(s_lo + 16u * j), "r"(s_hi + 16u * j), "r"((uint32_t)top), "r"((uint32_t)below), "l"(gp));
+            const float mn[3] = {a.x, a.y, a.z}, mx[3] = {b.x, b.y, b.z};
+            const uint32_t w3 = __float_as_uint(a.w), w7 = __float_as_uint(b.w);
+            visits += walking;
+            //   top entry: w7 = ~0 top-internal | 0x80000000+first global record (fringe inner, w3 = end of that range) | shape;
+            //   global record: w7 = shape | ~0, never in the fringe range, so `fringe` needs no test of `below`.
+            const bool hit = walking & slab_hit(o, inv, mn, mx);      // `&`: no branch around the test
+            const bool fringe = (int32_t)w7 < -1;
+            const bool adv = hit || fringe;                           // next record, else the skip link w3
+            if (hit && (int32_t)w7 >= 0) {                           // a leaf
+                bool report = true;
+                if (FLAT) {
+                    float smn[3], smx[3];
+                    load_aabb(aabb + w7, smn, smx);
+                    report = slab_hit(o, inv, smn, smx);
+                }
+                if (report) { if (cnt < K) slots[(size_t)cnt * nrays + r] = w7; ++cnt; }
+            }
+            if (top) j = adv ? j + 1 : w3;
+            if (below) g = adv ? g + 1 : w3;
+            if (hit && fringe) { g = w7 & 0x7FFFFFFFu; gend = w3; }     // enter the subtree's global records [g, gend)
+        };
         uint32_t rounds = 0;
         for (;;) {
+            if constexpr (VPC == 1) {
+                visit_branchy();
+            } else {
 #pragma unroll
-            for (int u = 0; u < VPC; ++u) visit();
+                for (int u = 0; u < VPC; ++u) visit();
+                if (r != NONE && (!STREAM || loaded) && g >= gend && j >= n_top) { counts[r] = cnt; r = NONE; }   // the ray ended in this step
+            }
             const uint32_t idle_mask = __ballot_sync(FULL, r == NONE);
             if (__popc(idle_mask) >= leave) break;
             if (STREAM) {                                            // look for arrivals every 16 visits, at once if nobody walks
