@@ -748,9 +748,44 @@ static int stage_new_aabbs(Tree<T>* tree, const typename Traits<T>::Aabb* aabbs,
     return BVHGPU_OK;
 }
 
+// 4-D: the boxes are checked (the tree is left untouched if that fails), then copied into the tree: the ABI box is the device layout.
+template <class T>
+static int stage_new_aabbs(Tree4<T>* tree, const typename D4<T>::Aabb* d_in, size_t n, bool, const char* who) {
+    Scratch scratch(tree->ctx);
+    BVH_TRY(check_boxes(tree, nullptr, d_in, (uint32_t)n, scratch, who));
+    if (cudaMemcpyAsync(tree->d_aabb, d_in, sizeof(*d_in) * n, cudaMemcpyDeviceToDevice, tree->ctx->stream) != cudaSuccess)
+        return mark_failed(tree, BVHGPU_ERR_CUDA, who);
+    return BVHGPU_OK;
+}
+
+// A 3-D tree's deferred build status is cleared before a call enqueues builder work; a 4-D tree reports its errors synchronously.
+template <class T> static int reset_status(Tree<T>* tree) {
+    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), tree->ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T> static int reset_status(Tree4<T>*) { return BVHGPU_OK; }
+
+// The end of a call that changed the tree.  Tree<T>: the status stays pending for device pointers unless the caller asked for the
+// rebuilt count, and is resolved otherwise; the status counts the rebuilt shapes.  Tree4<T>: host pointers synchronise, and the
+// count is the driver's `shapes`.
+template <class T> static int complete(Tree<T>* tree, bool dev_input, size_t* rebuilt, size_t, const char*) {
+    tree->status_pending = true;
+    if (!rebuilt) return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+    BuildStatus hs;
+    BVH_CUDA_TRY(cudaMemcpyAsync(&hs, tree->d_status, sizeof(hs), cudaMemcpyDeviceToHost, tree->ctx->stream));
+    BVH_TRY(resolve_status(tree));                                      // synchronises
+    *rebuilt = hs.rebuilt;
+    return BVHGPU_OK;
+}
+template <class T> static int complete(Tree4<T>* tree, bool dev_input, size_t* rebuilt, size_t shapes, const char* who) {
+    if (!dev_input && cudaStreamSynchronize(tree->ctx->stream) != cudaSuccess) { set_error("%s: CUDA error", who); return mark_failed(tree, BVHGPU_ERR_CUDA, who); }
+    if (rebuilt) *rebuilt = shapes;
+    return BVHGPU_OK;
+}
+
 // Refit from n new shape boxes (ABI layout of D).  D = 2 (host pointers): the 2-D boxes are lifted to z = [0, 0] on the device.
 // Surface areas with z = [0, 0] are exact and largest_axis never picks z (dim2.cu), so the 3-D refit, growth test and rebuild are the
-// 2-D ones.  D = 4: the boxes are checked (check4), copied into the tree and refit4 runs; synchronous for host pointers.
+// 2-D ones.  The boxes are checked before the tree is touched; a refit that fails after that leaves the tree failed.
 template <int D, class T>
 static int refit_impl(TreeOf<D, T>* tree, const void* aabbs, size_t n, bool dev_input) {
     if (!tree || (n && !aabbs)) { set_error("refit: null argument"); return BVHGPU_ERR_INVALID; }
@@ -766,22 +801,11 @@ static int refit_impl(TreeOf<D, T>* tree, const void* aabbs, size_t n, bool dev_
         BVH_TRY(upload_records<D>(ctx, scratch, aabbs, n, AABB_RECORD, 0, &staged));
         aabbs = staged;
     }
-    if constexpr (D == 4) {
-        using Aabb = typename D4<T>::Aabb;
-        const Aabb* d_in = static_cast<const Aabb*>(aabbs);
-        BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)n, scratch, "refit"));
-        int rc = cudaMemcpyAsync(tree->d_aabb, d_in, sizeof(*d_in) * n, cudaMemcpyDeviceToDevice, ctx->stream) == cudaSuccess ? (int)BVHGPU_OK : (int)BVHGPU_ERR_CUDA;
-        if (rc == BVHGPU_OK) rc = refit4(tree);
-        if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("refit: CUDA error"); rc = BVHGPU_ERR_CUDA; }
-        return rc == BVHGPU_OK ? rc : mark_failed(tree, rc, "refit");
-    } else {
-        BVH_TRY(stage_new_aabbs<T>(tree, static_cast<const typename Traits<T>::Aabb*>(aabbs), n, dev_input || D == 2, "refit"));
-        if (tree->dims == 2) BVH_TRY(dim2_finish_build<T>(tree));      // the FLAT leaf boxes follow d_aabb before the records are rebuilt
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
-        BVH_TRY(refit(tree));
-        tree->status_pending = true;
-        return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
-    }
+    BVH_TRY(stage_new_aabbs<T>(tree, static_cast<const typename TreeOf<D, T>::Aabb*>(aabbs), n, dev_input || D != 3, "refit"));
+    int rc = reset_status(tree);
+    if (rc == BVHGPU_OK) rc = refit(tree);
+    if (rc != BVHGPU_OK) return mark_failed(tree, rc, "refit");
+    return complete(tree, dev_input, nullptr, 0, "refit");
 }
 
 template <class T>
@@ -885,39 +909,91 @@ static int update_impl(TreeOf<D, T>* tree, const uint32_t* changed, const void* 
         BVH_TRY(upload_records<D>(ctx, scratch, fresh, m, AABB_RECORD, 0, &f));
         d_changed = c; fresh = f;
     }
-    if constexpr (D == 4) {                                             // checked, scattered and climbed by the 4-D drivers; synchronous
-        const typename D4<T>::Aabb* d_fresh = static_cast<const typename D4<T>::Aabb*>(fresh);
-        BVH_TRY(check4(tree, d_changed, d_fresh, (uint32_t)m, scratch, "update"));
-        size_t shapes = 0;
-        int rc = put4(tree, d_changed, d_fresh, (uint32_t)m);
-        if (rc == BVHGPU_OK) rc = update4(tree, d_changed, (uint32_t)m, max_growth, &shapes);     // touches the root paths of the changed leaves only
-        if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("update: CUDA error"); rc = BVHGPU_ERR_CUDA; }
-        if (rc != BVHGPU_OK) return mark_failed(tree, rc, "update");
-        if (rebuilt) *rebuilt = shapes;
-        return BVHGPU_OK;
-    } else {
-    const typename Traits<T>::Aabb* d_fresh = static_cast<const typename Traits<T>::Aabb*>(fresh);
-    uint32_t* flags = nullptr;
-    BVH_TRY(scratch.get(&flags, 2));
-    BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), ctx->stream));
-    BVH_TRY(update_changed<T>(tree, d_changed, d_fresh, (uint32_t)m, flags));
-    uint32_t* h = ctx->h_pinned + 208;
-    BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    if (h[1]) { set_error("update: a changed shape index is >= %u; the tree was left unchanged", tree->n); return BVHGPU_ERR_INVALID; }
-    if (h[0]) { set_error("update: NaN coordinate in a new AABB; the tree was left unchanged"); return BVHGPU_ERR_NAN; }
-    BVH_TRY(update_scatter<T>(tree, d_changed, d_fresh, (uint32_t)m));
-    if (tree->dims == 2) BVH_TRY(dim2_finish_build<T>(tree));          // the FLAT leaf boxes follow d_aabb before the records are rebuilt
-    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
-    BVH_TRY(update_incremental<T>(tree, d_changed, (uint32_t)m, max_growth));      // touches the root paths of the changed leaves only
-    tree->status_pending = true;
-    if (dev_input && !rebuilt) return BVHGPU_OK;                        // asynchronous from here on
-    BuildStatus hs;
-    BVH_CUDA_TRY(cudaMemcpyAsync(&hs, tree->d_status, sizeof(hs), cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_TRY(resolve_status(tree));
-    if (rebuilt) *rebuilt = hs.rebuilt;
-    return BVHGPU_OK;
+    const auto* d_fresh = static_cast<const typename TreeOf<D, T>::Aabb*>(fresh);
+    BVH_TRY(check_boxes(tree, d_changed, d_fresh, (uint32_t)m, scratch, "update"));
+    BVH_TRY(reset_status(tree));
+    size_t shapes = 0;
+    int rc = scatter_boxes(tree, d_changed, d_fresh, (uint32_t)m);
+    if (rc == BVHGPU_OK) rc = update_incremental(tree, d_changed, (uint32_t)m, max_growth, &shapes);   // touches the root paths of the changed leaves only
+    if (rc != BVHGPU_OK) return mark_failed(tree, rc, "update");
+    return complete(tree, dev_input, rebuilt, shapes, "update");
+}
+
+// Adding to an empty tree is exactly bvhgpu_build_* over the k boxes (device pointers), which replaces the tree's arrays.
+template <class T> static int build_into_empty(Tree<T>* tree, const typename Traits<T>::Aabb* d_in, uint32_t k, bool dev_input) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    Tree<T> fresh;
+    int rc = build_exact_sah<T>(ctx, d_in, k, &fresh);
+    if (rc == BVHGPU_OK) rc = resolve_status(&fresh);
+    if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
+    dfree(ctx, tree->d_status); dfree(ctx, tree->d_sa_base); dfree(ctx, tree->d_tris);
+    tree->d_sa_base = nullptr; tree->d_tris = nullptr;
+    tree->n = fresh.n; tree->n_nodes = fresh.n_nodes; tree->d_status = fresh.d_status;
+    tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
+    if (tree->dims == 2) {                                              // the FLAT leaf boxes, read by the records, at the new n
+        dfree(ctx, tree->d_aabb_trav); tree->d_aabb_trav = nullptr;
+        BVH_TRY(dim2_finish_build<T>(tree));
     }
+    BVH_TRY(build_traversal_records(tree));
+    if (tree->have_flat) BVH_TRY(build_flat(tree));
+    tree->status_pending = true;
+    return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
+}
+template <class T> static int build_into_empty(Tree4<T>* tree, const typename D4<T>::Aabb* d_in, uint32_t k, bool) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    {
+        Scratch scratch(ctx);
+        BVH_TRY(check_boxes(tree, nullptr, d_in, k, scratch, "add_shapes"));
+    }
+    Tree4<T> fresh;
+    fresh.ctx = ctx; fresh.n = k; fresh.n_nodes = 2 * k - 1;
+    const int rc = build4<T>(&fresh, d_in, cudaMemcpyDeviceToDevice);  // synchronous
+    if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
+    dfree(ctx, tree->d_sa_base); tree->d_sa_base = nullptr;
+    tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
+    tree->n = fresh.n; tree->n_nodes = fresh.n_nodes;
+    return finish_relayout(tree);
+}
+
+// The tree's n boxes followed by the k new ones, in a new device array, checked for NaN before the tree is touched.  3-D: the new
+// boxes are converted to the padded device layout; 4-D: checked, then copied as they are.
+template <class T> static int stage_added(Tree<T>* tree, const typename Traits<T>::Aabb* d_in, uint32_t k, typename Traits<T>::DAabb** out) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    const uint32_t n = tree->n;
+    Scratch scratch(ctx);
+    typename Traits<T>::DAabb* all = nullptr;
+    uint32_t* flag = nullptr;
+    BVH_TRY(scratch.get(&flag, 1));
+    BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
+    int rc = cudaMemsetAsync(flag, 0, sizeof(uint32_t), ctx->stream) == cudaSuccess ? BVHGPU_OK : BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK && cudaMemcpyAsync(all, tree->d_aabb, sizeof(*all) * n, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) rc = BVHGPU_ERR_CUDA;
+    if (rc == BVHGPU_OK) rc = convert_aabbs<T>(ctx, d_in, k, all + n, flag);
+    uint32_t* h = ctx->h_pinned + 212;
+    if (rc == BVHGPU_OK && (cudaMemcpyAsync(h, flag, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+                            cudaStreamSynchronize(ctx->stream) != cudaSuccess)) { set_error("add_shapes: CUDA error while staging the AABBs"); rc = BVHGPU_ERR_CUDA; }
+    if (rc == BVHGPU_OK && *h) { set_error("add_shapes: NaN coordinate in a new AABB; the tree was left unchanged"); rc = BVHGPU_ERR_NAN; }
+    if (rc != BVHGPU_OK) { dfree(ctx, all); return rc; }
+    *out = all;
+    return BVHGPU_OK;
+}
+template <class T> static int stage_added(Tree4<T>* tree, const typename D4<T>::Aabb* d_in, uint32_t k, typename D4<T>::Aabb** out) {
+    using Aabb = typename D4<T>::Aabb;
+    bvhgpu_ctx* ctx = tree->ctx;
+    const uint32_t n = tree->n;
+    {
+        Scratch scratch(ctx);
+        BVH_TRY(check_boxes(tree, nullptr, d_in, k, scratch, "add_shapes"));
+    }
+    Aabb* all = nullptr;
+    BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
+    if (cudaMemcpyAsync(all, tree->d_aabb, sizeof(Aabb) * n, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess ||
+        cudaMemcpyAsync(all + n, d_in, sizeof(Aabb) * k, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) {
+        dfree(ctx, all);
+        set_error("add_shapes: CUDA error while staging the AABBs");
+        return BVHGPU_ERR_CUDA;
+    }
+    *out = all;
+    return BVHGPU_OK;
 }
 
 // Bvh::add_shape, batched: the k new shapes get indices n .. n+k-1.  The AABBs are staged next to the tree's own and checked for NaN
@@ -938,85 +1014,18 @@ static int add_impl(TreeOf<D, T>* tree, const void* aabbs, size_t k, double max_
         BVH_TRY(upload_records<D>(ctx, scratch, aabbs, k, AABB_RECORD, 0, &staged));
         aabbs = staged;
     }
-    const uint32_t n = tree->n;
-    if constexpr (D == 4) {                                             // the 4-D drivers: synchronous (the builder reads one word per level)
-        using Aabb = typename D4<T>::Aabb;
-        const Aabb* d_in = static_cast<const Aabb*>(aabbs);
-        BVH_TRY(check4(tree, nullptr, d_in, (uint32_t)k, scratch, "add_shapes"));
-        if (n == 0) {                                                   // an empty tree: exactly bvhgpu_build_*
-            Tree4<T> fresh;
-            fresh.ctx = ctx; fresh.n = (uint32_t)k; fresh.n_nodes = 2 * (uint32_t)k - 1;
-            const int rc = build4<T>(&fresh, d_in, cudaMemcpyDeviceToDevice);
-            if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
-            dfree(ctx, tree->d_sa_base); tree->d_sa_base = nullptr;
-            tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
-            tree->n = fresh.n; tree->n_nodes = fresh.n_nodes;
-            drop_caches4(tree);
-            return BVHGPU_OK;
-        }
-        Aabb* all = nullptr;
-        BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
-        if (cudaMemcpyAsync(all, tree->d_aabb, sizeof(Aabb) * n, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(all + n, d_in, sizeof(Aabb) * k, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) {
-            dfree(ctx, all);
-            set_error("add_shapes: CUDA error while staging the AABBs");
-            return BVHGPU_ERR_CUDA;
-        }
-        size_t shapes = 0;
-        const int rc = add_shapes4(tree, all, (uint32_t)k, max_growth, &shapes);
-        if (rc != BVHGPU_OK) {
-            if (tree->d_aabb != all) { dfree(ctx, all); return rc; }    // failed before the tree was touched
-            return mark_failed(tree, rc, "add_shapes");
-        }
-        if (!dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("add_shapes: CUDA error"); return mark_failed(tree, BVHGPU_ERR_CUDA, "add_shapes"); }
-        if (rebuilt) *rebuilt = shapes;
-        return BVHGPU_OK;
-    } else {
-    const typename Traits<T>::Aabb* d_in = static_cast<const typename Traits<T>::Aabb*>(aabbs);
-    if (n == 0) {                                                       // an empty tree: exactly bvhgpu_build_*
-        Tree<T> fresh;
-        int rc = build_exact_sah<T>(ctx, d_in, (uint32_t)k, &fresh);
-        if (rc == BVHGPU_OK) rc = resolve_status(&fresh);
-        if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
-        dfree(ctx, tree->d_status); dfree(ctx, tree->d_sa_base); dfree(ctx, tree->d_tris);
-        tree->d_sa_base = nullptr; tree->d_tris = nullptr;
-        tree->n = fresh.n; tree->n_nodes = fresh.n_nodes; tree->d_status = fresh.d_status;
-        tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
-        if (tree->dims == 2) {                                          // the FLAT leaf boxes, read by the records, at the new n
-            dfree(ctx, tree->d_aabb_trav); tree->d_aabb_trav = nullptr;
-            BVH_TRY(dim2_finish_build<T>(tree));
-        }
-        BVH_TRY(build_traversal_records(tree));
-        if (tree->have_flat) BVH_TRY(build_flat(tree));
-        tree->status_pending = true;
-        return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
-    }
-    typename Traits<T>::DAabb* all = nullptr;
-    uint32_t* flag = nullptr;
-    BVH_TRY(scratch.get(&flag, 1));
-    BVH_TRY(dalloc_t(ctx, &all, (size_t)n + k));
-    int rc = cudaMemsetAsync(flag, 0, sizeof(uint32_t), ctx->stream) == cudaSuccess ? BVHGPU_OK : BVHGPU_ERR_CUDA;
-    if (rc == BVHGPU_OK && cudaMemcpyAsync(all, tree->d_aabb, sizeof(*all) * n, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) rc = BVHGPU_ERR_CUDA;
-    if (rc == BVHGPU_OK) rc = convert_aabbs<T>(ctx, d_in, (uint32_t)k, all + n, flag);
-    uint32_t* h = ctx->h_pinned + 212;
-    if (rc == BVHGPU_OK && (cudaMemcpyAsync(h, flag, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-                            cudaStreamSynchronize(ctx->stream) != cudaSuccess)) { set_error("add_shapes: CUDA error while staging the AABBs"); rc = BVHGPU_ERR_CUDA; }
-    if (rc == BVHGPU_OK && *h) { set_error("add_shapes: NaN coordinate in a new AABB; the tree was left unchanged"); rc = BVHGPU_ERR_NAN; }
-    if (rc != BVHGPU_OK) { dfree(ctx, all); return rc; }
-    BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
-    rc = add_shapes<T>(tree, all, (uint32_t)k, max_growth);
+    const auto* d_in = static_cast<const typename TreeOf<D, T>::Aabb*>(aabbs);
+    if (tree->n == 0) return build_into_empty(tree, d_in, (uint32_t)k, dev_input);
+    typename TreeOf<D, T>::Box* all = nullptr;
+    BVH_TRY(stage_added(tree, d_in, (uint32_t)k, &all));
+    size_t shapes = 0;
+    int rc = reset_status(tree);
+    if (rc == BVHGPU_OK) rc = add_shapes(tree, all, (uint32_t)k, max_growth, &shapes);
     if (rc != BVHGPU_OK) {
         if (tree->d_aabb != all) { dfree(ctx, all); return rc; }            // failed before the tree was touched
         return mark_failed(tree, rc, "add_shapes");
     }
-    tree->status_pending = true;
-    if (dev_input && !rebuilt) return BVHGPU_OK;                        // asynchronous from here on
-    BuildStatus hs;
-    BVH_CUDA_TRY(cudaMemcpyAsync(&hs, tree->d_status, sizeof(hs), cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_TRY(resolve_status(tree));
-    if (rebuilt && max_growth > 0.0) *rebuilt = hs.rebuilt;
-    return BVHGPU_OK;
-    }
+    return complete(tree, dev_input, rebuilt, shapes, "add_shapes");
 }
 
 // Bvh::remove_shape(i, swap_shape = true), batched: `indices` are distinct shape indices before the call; survivors >= n-k take the
@@ -1050,18 +1059,10 @@ static int remove_impl(TreeOf<D, T>* tree, const uint32_t* indices, size_t k, bo
     if (h[0]) { set_error("remove_shapes: a shape index is >= %u; the tree was left unchanged", n); return BVHGPU_ERR_INVALID; }
     if (h[1]) { set_error("remove_shapes: a shape index is listed twice; the tree was left unchanged"); return BVHGPU_ERR_INVALID; }
     const void* nodes_before = tree->d_nodes;
-    if constexpr (D == 4) {                                             // synchronous for host pointers
-        int rc = remove_shapes4(tree, rm, (uint32_t)k);
-        if (rc == BVHGPU_OK && !dev_input && cudaStreamSynchronize(ctx->stream) != cudaSuccess) { set_error("remove_shapes: CUDA error"); rc = BVHGPU_ERR_CUDA; }
-        if (rc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rc : mark_failed(tree, rc, "remove_shapes");
-        return BVHGPU_OK;
-    } else {
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_status, 0, sizeof(BuildStatus), ctx->stream));
-        const int rrc = remove_shapes<T>(tree, rm, (uint32_t)k);
-        if (rrc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rrc : mark_failed(tree, rrc, "remove_shapes");
-        tree->status_pending = true;
-        return dev_input ? (int)BVHGPU_OK : resolve_status(tree);
-    }
+    BVH_TRY(reset_status(tree));
+    const int rc = remove_shapes(tree, rm, (uint32_t)k);
+    if (rc != BVHGPU_OK) return tree->d_nodes == nodes_before ? rc : mark_failed(tree, rc, "remove_shapes");
+    return complete(tree, dev_input, nullptr, 0, "remove_shapes");
 }
 
 }  // namespace bvhb200

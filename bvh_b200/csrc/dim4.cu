@@ -6,7 +6,9 @@
 // its own node types and its own Tree4<T>; it shares the exact-arithmetic helpers and keys of common.cuh, Scratch, the records,
 // walk and count -> scan -> fill driver of csr.cuh, and the predicates of queries.cuh.  DESIGN.md section 4.11 describes the design.
 // This file holds the kernels and the device-side drivers declared in internal.h; the bvhgpu_*_f32x4 / _f64x4 entry points are the
-// D = 4 instances of the host layer in capi.cu, which checks the arguments and the tree's status and stages the batch.
+// D = 4 instances of the host layer in capi.cu, which checks the arguments and the tree's status and stages the batch.  Refit,
+// update_shapes, add_shapes and remove_shapes run the drivers of dynamic.cu; the 4-D steps they call (the builder seeded from
+// subtree roots, the growth rebuild, the caches) are at the end of this file.
 //
 // Builder (bit-identical to Bvh::build in the sense of DESIGN.md section 2):
 //   ranges of more than SMALL4 shapes: level-synchronous.  Per level: prep (tile numbering, bucket identities), bin (one warp per
@@ -21,7 +23,6 @@
 #include "csr.cuh"
 #include "queries.cuh"
 #include "update.cuh"
-#include "dynamic.cuh"
 #include <algorithm>
 #include <new>
 
@@ -566,52 +567,7 @@ __global__ void __launch_bounds__(128) nearest_bound4_kernel(const typename D4<T
     records[5 * (size_t)i + 4] = u;
 }
 
-// ---- refit and update_shapes (Bvh::update_shapes, src/bvh/optimization.rs:304-351; DESIGN.md section 4.12) ----
-// refit: one thread per shape climbs from its leaf and writes its box into the parent's child slot; the second thread to reach a node
-// joins the two slots and carries on (flatten.cu: refit_kernel).  Topology, node_index and node_start are kept; leaves keep their
-// Aabb::empty() child boxes.
-template <class T>
-__global__ void __launch_bounds__(256) refit4_kernel(typename D4<T>::Node* nodes, const uint32_t* __restrict__ node_index,
-                                                     const typename D4<T>::Aabb* __restrict__ aabb, uint32_t n, uint32_t* arrivals) {
-    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    T mn[4], mx[4];
-    load4(aabb + s, mn, mx);
-    uint32_t node = node_index[s];
-    while (node != 0) {
-        const uint32_t p = __ldcg(&nodes[node].parent);
-        typename D4<T>::Node* pn = nodes + p;
-        const bool is_left = __ldcg(&pn->child_l) == node;
-        auto* dst = is_left ? &pn->l_aabb : &pn->r_aabb;
-        for (int k = 0; k < 4; ++k) { __stcg(&dst->min[k], mn[k]); __stcg(&dst->max[k], mx[k]); }
-        __threadfence();
-        if (atomicAdd(arrivals + p, 1u) == 0u) return;      // sibling subtree not finished yet
-        __threadfence();
-        const auto* sib = is_left ? &pn->r_aabb : &pn->l_aabb;
-        for (int k = 0; k < 4; ++k) { mn[k] = min_t(__ldcg(&sib->min[k]), mn[k]); mx[k] = max_t(__ldcg(&sib->max[k]), mx[k]); }
-        node = p;
-    }
-}
-// New boxes, checked before anything is written: flags[0] NaN, flags[1] an index >= n (changed == nullptr: box i belongs to shape i).
-template <class T>
-__global__ void __launch_bounds__(256) check4_kernel(const uint32_t* __restrict__ changed, const typename D4<T>::Aabb* __restrict__ fresh,
-                                                     uint32_t m, uint32_t n, uint32_t* __restrict__ flags) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    if (changed && changed[i] >= n) atomicExch(flags + 1, 1u);
-    const T* p = reinterpret_cast<const T*>(fresh + i);
-    bool nan = false;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) nan |= p[c] != p[c];
-    if (nan) atomicExch(flags, 1u);
-}
-template <class T>
-__global__ void __launch_bounds__(256) put4_kernel(const uint32_t* __restrict__ changed, const typename D4<T>::Aabb* __restrict__ fresh, uint32_t m,
-                                                   typename D4<T>::Aabb* __restrict__ aabb) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < m) aabb[changed[i]] = fresh[i];                  // an index listed twice: one of its boxes wins
-}
-
+// ---- the growth rebuild of update_shapes / add_shapes and the group subtrees of add_shapes (DESIGN.md sections 4.12, 4.13) ----
 // Seeding the builder from the rebuild roots roots[0 .. *n_roots) (disjoint inner nodes).  The subtree of root r with c shapes is the
 // node range [r, r + 2c - 1) over the leaf positions [node_start[r], node_start[r] + c).  Its nodes are cut into tiles of TILE4, so
 // that a root that holds every shape (global motion) is reduced by many warps, as level_bin4 does.
@@ -951,11 +907,10 @@ template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, 
     return BVHGPU_OK;
 }
 
-// ---- refit / update_shapes ----
-
+// ---- the 4-D steps of the dynamic drivers (dynamic.cu) ----
 // The traversal records and the flat array, if they were built, are rewritten in place from the new boxes (their sizes do not change);
 // otherwise traverse, query, flatten and FLAT nearest_to would keep using the old boxes.
-template <class T> static int refresh_caches4(Tree4<T>* tree) {
+template <class T> int refresh_caches(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
     const unsigned g = (tree->n_nodes + 255) / 256;
     if (tree->d_trec) { trec4_kernel<T><<<g, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec); LAUNCHED(ctx, 1); }
@@ -963,42 +918,24 @@ template <class T> static int refresh_caches4(Tree4<T>* tree) {
     return BVHGPU_OK;
 }
 
-// m new boxes (and their shape indices, when `d_changed` is given) are checked on the device and the verdict is read back before the
-// tree is touched.
-template <class T> int check4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m, Scratch& scratch,
-                                     const char* who) {
+// Arrays that depend on the node count or the shape numbering, after a relocation: the traversal records and the flat array are
+// rebuilt at the new size on first use (refresh_caches rewrites them in place and assumes the node count did not change); the
+// update's arrival counters and growth flags are reallocated by the next update.
+template <class T> int finish_relayout(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
-    uint32_t* flags = nullptr;
-    BVH_TRY(scratch.get(&flags, 2));
-    BVH_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(uint32_t), ctx->stream));
-    check4_kernel<T><<<(m + 255) / 256, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->n, flags);
-    LAUNCHED(ctx, 1);
-    uint32_t* h = ctx->h_pinned + 208;
-    BVH_CUDA_TRY(cudaMemcpyAsync(h, flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    if (h[1]) { set_error("%s: a changed shape index is >= %u; the tree was left unchanged", who, tree->n); return BVHGPU_ERR_INVALID; }
-    if (h[0]) { set_error("%s: NaN coordinate in a new AABB; the tree was left unchanged", who); return BVHGPU_ERR_NAN; }
+    dfree(ctx, tree->d_trec); tree->d_trec = nullptr;
+    dfree(ctx, tree->d_flat); tree->d_flat = nullptr;
+    dfree(ctx, tree->d_arrive); tree->d_arrive = nullptr;
+    dfree(ctx, tree->d_bad); tree->d_bad = nullptr;
+    tree->n_trec = tree->n == 0 ? 0u : (tree->n == 1 ? 1u : tree->n_nodes - 1);
+    tree->n_flat = tree->n == 0 ? 0 : (tree->n == 1 ? 1 : 3 * (size_t)tree->n - 2);
     return BVHGPU_OK;
-}
-
-// Bottom-up refit of every node from tree->d_aabb.
-template <class T> int refit4(Tree4<T>* tree) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    if (tree->n >= 2) {
-        Scratch scratch(ctx);
-        uint32_t* arrivals = nullptr;
-        BVH_TRY(scratch.get(&arrivals, tree->n_nodes));
-        BVH_CUDA_TRY(cudaMemsetAsync(arrivals, 0, sizeof(uint32_t) * tree->n_nodes, ctx->stream));
-        refit4_kernel<T><<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, tree->n, arrivals);
-        LAUNCHED(ctx, 1);
-    }
-    return refresh_caches4(tree);                               // n = 1: the root record holds the shape's own box
 }
 
 // dirty[0 .. cnts[0]) = the nodes whose box changed, tree->d_bad = their growth flags.  Rebuilds in place, with the level loop and
 // small4_kernel of the build, the outermost degraded subtrees (cnts[1], zero on entry, counts them), gives their nodes fresh baselines
 // and clears the flags.  *rebuilt = shapes in the rebuilt subtrees.  `who` names the caller in error messages.
-template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* dirty, uint32_t* cnts, size_t* rebuilt, const char* who) {
+template <class T> int rebuild_degraded(Tree4<T>* tree, const uint32_t* dirty, uint32_t* cnts, size_t* rebuilt, const char* who) {
     using Key = typename Traits<T>::Key;
     using Node = typename D4<T>::Node;
     bvhgpu_ctx* ctx = tree->ctx;
@@ -1040,219 +977,30 @@ template <class T> static int rebuild_degraded4(Tree4<T>* tree, const uint32_t* 
     return BVHGPU_OK;
 }
 
-// The shapes d_changed[0 .. m) already carry their new boxes in tree->d_aabb.  max_growth <= 0: boxes only.  The same steps as the 3-D
-// update_incremental (flatten.cu) with the shared kernels of update.cuh.
-template <class T> int update4(Tree4<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt) {
-    using Node = typename D4<T>::Node;
+// The group subtrees of an add: one task per root (root_seed4_kernel) into the level loop and small4_kernel of the build.
+template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* roots, const uint32_t* n_roots, uint32_t max_roots,
+                                      const typename Traits<T>::Key* keys, uint32_t* idx, const char* who) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
-    const uint32_t nn = tree->n_nodes;
-    const bool rebuild = max_growth > 0.0;
-    if (tree->n < 3) return refit4(tree);                       // one or two shapes: nothing a rebuild could change
-    if (!tree->d_arrive) {
-        BVH_TRY(dalloc_t(ctx, &tree->d_arrive, nn));
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_arrive, 0, sizeof(uint32_t) * nn, st));
-    }
-    if (rebuild && !tree->d_bad) {
-        BVH_TRY(dalloc_t(ctx, &tree->d_bad, nn));
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_bad, 0, nn, st));
-    }
-    if (rebuild && !tree->d_sa_base) {                          // first update on this tree: the baseline is the tree before the motion
-        BVH_TRY(dalloc_t(ctx, &tree->d_sa_base, nn));
-        node_sa_kernel<4, T, Node><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn, tree->d_sa_base);
-        LAUNCHED(ctx, 1);
-    }
-    Scratch scratch(ctx);
-    uint32_t *dirty = nullptr, *cnts = nullptr;
-    BVH_TRY(scratch.get(&dirty, nn));
-    BVH_TRY(scratch.get(&cnts, 2));                             // [0] dirty nodes, [1] rebuild roots
-    BVH_CUDA_TRY(cudaMemsetAsync(cnts, 0, 2 * sizeof(uint32_t), st));
-    const unsigned gm = (m + 255) / 256;
-    mark_paths_kernel<Node><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, d_changed, m, tree->d_arrive);
-    climb_paths_kernel<4, T, Node, typename D4<T>::Aabb><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
-                                                                              tree->d_sa_base, (T)max_growth, rebuild ? tree->d_bad : nullptr, dirty, cnts);
-    LAUNCHED(ctx, 2);
-    if (rebuild) BVH_TRY(rebuild_degraded4(tree, dirty, cnts, rebuilt, "update"));
-    return refresh_caches4(tree);
-}
-
-template <class T> int put4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    put4_kernel<T><<<(m + 255) / 256, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->d_aabb);
-    LAUNCHED(ctx, 1);
-    return BVHGPU_OK;
-}
-
-// ---- add_shapes / remove_shapes (Bvh::add_shape / Bvh::remove_shape, src/bvh/optimization.rs:67-301; DESIGN.md section 4.13) ----
-// The relocation, grafting, contraction and climb of the 3-D drivers (dynamic.cu) with the kernels of dynamic.cuh at D = 4.  The group
-// subtrees and the growth rebuilds are built by the level loop and small4_kernel of the build, seeded with one task per root.
-
-// Arrays that depend on the node count or the shape numbering, after a relocation: the traversal records and the flat array are
-// rebuilt at the new size on first use (refresh_caches4 rewrites them in place and assumes the node count did not change); the
-// update's arrival counters and growth flags are reallocated by the next update.
-template <class T> void drop_caches4(Tree4<T>* tree) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    dfree(ctx, tree->d_trec); tree->d_trec = nullptr;
-    dfree(ctx, tree->d_flat); tree->d_flat = nullptr;
-    dfree(ctx, tree->d_arrive); tree->d_arrive = nullptr;
-    dfree(ctx, tree->d_bad); tree->d_bad = nullptr;
-    tree->n_trec = tree->n == 0 ? 0u : (tree->n == 1 ? 1u : tree->n_nodes - 1);
-    tree->n_flat = tree->n == 0 ? 0 : (tree->n == 1 ? 1 : 3 * (size_t)tree->n - 2);
-}
-
-// aabb_all: [n + k] shape boxes (the tree's n followed by the k new ones, checked for NaN); becomes tree->d_aabb.  *rebuilt = shapes in
-// the subtrees rebuilt by the growth test (the group subtrees are not counted).  A failure with tree->d_aabb != aabb_all left the tree
-// untouched.
-template <class T> int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* aabb_all, uint32_t k, double max_growth, size_t* rebuilt) {
-    using Node = typename D4<T>::Node;
-    using Key = typename Traits<T>::Key;
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = tree->n, nn = tree->n_nodes, nn2 = nn + 2 * k, N = n + k;
-    const bool rebuild = max_growth > 0.0;
+    const uint32_t N = tree->n;
     const int wave = std::max(ctx->sm_count, 1) * 8;
-    if (rebuild && !tree->d_sa_base) {                          // the baseline is the tree before the call
-        BVH_TRY(dalloc_t(ctx, &tree->d_sa_base, nn));
-        node_sa_kernel<4, T, Node><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn, tree->d_sa_base);
-        LAUNCHED(ctx, 1);
-    }
-    T* sa_old = tree->d_sa_base;
     Scratch scratch(ctx);
-    uint32_t *point = nullptr, *ng = nullptr;
-    BVH_TRY(scratch.get(&point, k));
-    // [0] groups, [1] group subtrees to build, [2] dirty nodes, [3] growth rebuild roots, [4] unused, [5] nodes that failed the growth test
-    BVH_TRY(scratch.get(&ng, 6));
-    BVH_CUDA_TRY(cudaMemsetAsync(ng, 0, 6 * sizeof(uint32_t), st));
-    descend_kernel<4, T><<<(k + 255) / 256, 256, 0, st>>>(tree->d_nodes, aabb_all, n, k, point);
+    BuildArgs4 A{};
+    Task4<T>* small = nullptr;
+    Levels4<T> L;
+    BVH_TRY(scratch.get(&A.bkt, N));
+    BVH_TRY(scratch.get(&A.ctl, 8));
+    BVH_TRY(scratch.get(&small, N));
+    BVH_TRY(levels4_alloc(scratch, N, &L));
+    A.idx[0] = idx; A.idx[1] = idx + N; A.small = small;
+    BVH_CUDA_TRY(cudaMemsetAsync(A.ctl, 0, 8 * sizeof(uint32_t), st));
+    root_seed4_kernel<T><<<std::min<uint32_t>((max_roots + 255) / 256, (uint32_t)wave), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, roots, n_roots,
+                                                                                                       keys, L.tasks, A);
     LAUNCHED(ctx, 1);
-    Groups G;
-    BVH_TRY(group_insertions(ctx, scratch, point, k, nn, ng, &G));
-    Scratch scratch2(ctx);
-    uint32_t *idx = nullptr, *roots = nullptr, *gbase = nullptr, *arrive = nullptr, *dirty = nullptr;
-    uint8_t* aff = nullptr;
-    Key* keys = nullptr;
-    BVH_TRY(scratch2.get(&aff, nn2));
-    BVH_TRY(scratch2.get(&idx, 2 * (size_t)N));               // the builder's two index buffers; the groups' shapes go into the first
-    BVH_TRY(scratch2.get(&roots, k));
-    BVH_TRY(scratch2.get(&gbase, k));
-    BVH_TRY(scratch2.get(&keys, 8 * (size_t)k));
-    BVH_TRY(scratch2.get(&arrive, nn2));
-    BVH_TRY(scratch2.get(&dirty, nn2));
-    Node* nw = nullptr;
-    uint32_t *nstart = nullptr, *nidx = nullptr;
-    T* sa_new = nullptr;
-    int rc = dalloc_t(ctx, &nw, nn2);
-    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nstart, nn2);
-    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nidx, N);
-    if (rc == BVHGPU_OK && sa_old) rc = dalloc_t(ctx, &sa_new, nn2);
-    if (rc == BVHGPU_OK && cudaMemsetAsync(aff, 0, nn2, st) != cudaSuccess) rc = BVHGPU_ERR_CUDA;
-    if (rc == BVHGPU_OK) {
-        graft_relayout_kernel<4, T><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, sa_old, nn, G.a, G.S, nw, nstart, nidx, aff, sa_new);
-        graft_groups_kernel<4, T><<<wave, 256, 0, st>>>(G.uniq, G.cnt, G.goff, ng, G.sshape, tree->d_node_start, G.S, aabb_all, n,
-                                                        nw, nstart, nidx, idx, roots, ng + 1, keys, gbase);
-        ctx->launches += 2;
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { set_error("add_shapes: %s", cudaGetErrorString(e)); rc = BVHGPU_ERR_CUDA; }
-    }
-    if (rc != BVHGPU_OK) { dfree(ctx, nw); dfree(ctx, nstart); dfree(ctx, nidx); dfree(ctx, sa_new); return rc; }
-    // the tree now is the new one (its boxes on the affected paths are still to be recomputed); from here on a failure leaves it
-    // half-done, and the caller marks it failed
-    dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
-    tree->d_nodes = nw; tree->d_node_start = nstart; tree->d_node_index = nidx; tree->d_aabb = aabb_all; tree->d_sa_base = sa_new;
-    tree->n = N; tree->n_nodes = nn2;
-    drop_caches4(tree);
     uint32_t* h = ctx->h_pinned + 224;
-    BVH_CUDA_TRY(cudaMemcpyAsync(h, ng + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (*h) {                                                   // exact-SAH subtrees of the groups with >= 2 shapes
-        Scratch scratch3(ctx);
-        BuildArgs4 A{};
-        Task4<T>* small = nullptr;
-        Levels4<T> L;
-        BVH_TRY(scratch3.get(&A.bkt, N));
-        BVH_TRY(scratch3.get(&A.ctl, 8));
-        BVH_TRY(scratch3.get(&small, N));
-        BVH_TRY(levels4_alloc(scratch3, N, &L));
-        A.idx[0] = idx; A.idx[1] = idx + N; A.small = small;
-        BVH_CUDA_TRY(cudaMemsetAsync(A.ctl, 0, 8 * sizeof(uint32_t), st));
-        root_seed4_kernel<T><<<std::min<uint32_t>((k + 255) / 256, (uint32_t)wave), 256, 0, st>>>(tree->d_nodes, tree->d_node_start, roots, ng + 1,
-                                                                                                 keys, L.tasks, A);
-        LAUNCHED(ctx, 1);
-        BVH_CUDA_TRY(cudaMemcpyAsync(h, A.ctl, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaStreamSynchronize(st));
-        BVH_TRY(run_levels4(tree, A, L, h[CTL_NEXT], h[CTL_SMALL], "add_shapes"));
-    }
-    // boxes of the affected paths (+ the growth test)
-    BVH_CUDA_TRY(cudaMemsetAsync(arrive, 0, sizeof(uint32_t) * nn2, st));
-    if (rebuild) {
-        BVH_TRY(dalloc_t(ctx, &tree->d_bad, nn2));
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_bad, 0, nn2, st));
-    }
-    climb_affected_kernel<4, T><<<(nn2 + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn2, aff, tree->d_aabb, arrive, sa_new, (T)max_growth,
-                                                                 rebuild ? tree->d_bad : nullptr, ng + 5, dirty, ng + 2);
-    LAUNCHED(ctx, 1);
-    if (sa_new) { graft_rebase_kernel<4, T><<<wave, 256, 0, st>>>(tree->d_nodes, gbase, G.cnt, ng, sa_new); LAUNCHED(ctx, 1); }
-    if (rebuild) {
-        BVH_CUDA_TRY(cudaMemcpyAsync(h, ng + 5, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-        BVH_CUDA_TRY(cudaStreamSynchronize(st));
-        if (*h) BVH_TRY(rebuild_degraded4(tree, dirty, ng + 2, rebuilt, "add_shapes"));   // a node failed the growth test
-    }
-    drop_caches4(tree);                                         // (the growth flags: all clear again, dropped with the counters)
-    return BVHGPU_OK;
-}
-
-// d_rm: [n + 1] removed flag of every shape (0 / 1, the last word 0), 1 <= k <= n.  A failure with tree->d_nodes unchanged left the
-// tree untouched.
-template <class T> int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint32_t k) {
-    using Node = typename D4<T>::Node;
-    using Aabb = typename D4<T>::Aabb;
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = tree->n, nn = tree->n_nodes, m = n - k, nn2 = m ? 2 * m - 1 : 0;
-    if (m == 0) {                                               // everything goes: the tree of an n == 0 build
-        dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
-        tree->d_nodes = nullptr; tree->d_node_start = nullptr; tree->d_node_index = nullptr; tree->d_aabb = nullptr; tree->d_sa_base = nullptr;
-        tree->n = 0; tree->n_nodes = 0;
-        drop_caches4(tree);
-        return BVHGPU_OK;
-    }
-    Scratch scratch(ctx);
-    uint32_t *flag = nullptr, *newidx = nullptr, *arrive = nullptr;
-    uint8_t* aff = nullptr;
-    Ranks rk;
-    BVH_TRY(remove_ranks(ctx, scratch, d_rm, n, k, tree->d_node_index, tree->d_node_start, &rk));
-    BVH_TRY(scratch.get(&flag, (size_t)nn + 1));
-    BVH_TRY(scratch.get(&newidx, (size_t)nn + 1));
-    BVH_TRY(scratch.get(&aff, nn2));
-    BVH_TRY(scratch.get(&arrive, nn2));
-    BVH_CUDA_TRY(cudaMemsetAsync(arrive, 0, sizeof(uint32_t) * nn2, st));
-    survive_kernel<<<(nn + 256) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, nn, rk.R, flag);
-    LAUNCHED(ctx, 1);
-    BVH_TRY(exclusive_sum_u32(scratch, flag, newidx, (size_t)nn + 1, st));
-    Node* nw = nullptr;
-    uint32_t *nstart = nullptr, *nidx = nullptr;
-    Aabb* a_new = nullptr;
-    T* sa_new = nullptr;
-    int rc = dalloc_t(ctx, &nw, nn2);
-    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nstart, nn2);
-    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &nidx, m);
-    if (rc == BVHGPU_OK) rc = dalloc_t(ctx, &a_new, m);
-    if (rc == BVHGPU_OK && tree->d_sa_base) rc = dalloc_t(ctx, &sa_new, nn2);
-    if (rc != BVHGPU_OK) { dfree(ctx, nw); dfree(ctx, nstart); dfree(ctx, nidx); dfree(ctx, a_new); dfree(ctx, sa_new); return rc; }
-    contract_kernel<T><<<(nn + 255) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, nn, rk.R, newidx, m, rk.Rm, rk.holes,
-                                                          tree->d_sa_base, nw, nstart, nidx, aff, sa_new);
-    permute_shapes_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_rm, n, m, rk.Rm, rk.holes, tree->d_aabb, a_new, nullptr, nullptr, 0u);
-    LAUNCHED(ctx, 2);
-    dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
-    tree->d_nodes = nw; tree->d_node_start = nstart; tree->d_node_index = nidx; tree->d_aabb = a_new; tree->d_sa_base = sa_new;
-    tree->n = m; tree->n_nodes = nn2;
-    drop_caches4(tree);
-    if (nn2 > 1) {
-        climb_affected_kernel<4, T><<<(nn2 + 255) / 256, 256, 0, st>>>(tree->d_nodes, nn2, aff, tree->d_aabb, arrive, nullptr, T(0), nullptr, nullptr,
-                                                                     nullptr, nullptr);
-        LAUNCHED(ctx, 1);
-    }
-    return BVHGPU_OK;
+    return run_levels4(tree, A, L, h[CTL_NEXT], h[CTL_SMALL], who);
 }
 
 #define INSTANTIATE4(T)                                                                                                              \
@@ -1264,13 +1012,10 @@ template <class T> int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint
     template int nearest4_device<T>(Tree4<T>*, int, const T*, size_t, uint32_t*, T*);                                               \
     template int ordered4_device<T>(Tree4<T>*, const void*, size_t, int, uint32_t*, uint32_t*, T*, size_t, size_t*);               \
     template int knn4_device<T>(Tree4<T>*, const T*, size_t, uint32_t, const T*, uint32_t*, T*);                                    \
-    template int check4<T>(Tree4<T>*, const uint32_t*, const D4<T>::Aabb*, uint32_t, Scratch&, const char*);                        \
-    template int put4<T>(Tree4<T>*, const uint32_t*, const D4<T>::Aabb*, uint32_t);                                                 \
-    template int refit4<T>(Tree4<T>*);                                                                                              \
-    template int update4<T>(Tree4<T>*, const uint32_t*, uint32_t, double, size_t*);                                                 \
-    template int add_shapes4<T>(Tree4<T>*, D4<T>::Aabb*, uint32_t, double, size_t*);                                                \
-    template int remove_shapes4<T>(Tree4<T>*, const uint32_t*, uint32_t);                                                           \
-    template void drop_caches4<T>(Tree4<T>*);
+    template int refresh_caches<T>(Tree4<T>*);                                                                                      \
+    template int finish_relayout<T>(Tree4<T>*);                                                                                     \
+    template int rebuild_degraded<T>(Tree4<T>*, const uint32_t*, uint32_t*, size_t*, const char*);                                  \
+    template int build_subtrees<T>(Tree4<T>*, const uint32_t*, const uint32_t*, uint32_t, const Traits<T>::Key*, uint32_t*, const char*);
 INSTANTIATE4(float)
 INSTANTIATE4(double)
 #undef INSTANTIATE4

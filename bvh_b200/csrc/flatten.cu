@@ -1,5 +1,6 @@
 // bvh_b200/csrc/flatten.cu -- Bvh::flatten (src/flat_bvh.rs:60-143, 240-251, 312-319) as a closed-form
-// map over the preorder node array, the device-only traversal records, whole-tree SAH cost and refit.
+// map over the preorder node array, the device-only traversal records, whole-tree SAH cost, optimize and the 3-D growth rebuild of
+// update_shapes / add_shapes (the drivers of refit and the dynamic operations are in dynamic.cu).
 //
 // Closed form (DESIGN.md "flatten"): the reference's recursive flatten pushes, for every non-root
 // Bvh node i, a navigator FlatNode and, for leaves, a leaf FlatNode right behind it.  Because
@@ -271,64 +272,6 @@ template <class T> int sah_cost(Tree<T>* tree, double* out2) {
     return BVHGPU_OK;
 }
 
-// ---- refit: bottom-up recomputation of the child AABBs from the (new) shape AABBs ---------------------
-// (the data-parallel part of Bvh::update_shapes: fix_aabbs_ascending, src/bvh/optimization.rs:317-351).
-// One thread per shape climbs from its leaf; the second thread to reach a node carries on.
-// WITH_CB (bvhgpu_optimize): the climb also carries the bounds of the shape CENTRES below every node into cb[node][6]
-// (min xyz, max xyz) -- what the builder needs, next to the AABB, to restart from an inner node.
-template <class T, bool WITH_CB>
-__global__ void __launch_bounds__(256) refit_kernel(typename Traits<T>::Node* nodes, const uint32_t* __restrict__ node_index,
-                                                    const typename Traits<T>::DAabb* __restrict__ aabb, uint32_t n, uint32_t* arrivals, T* cb) {
-    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    T mn[3], mx[3], cmn[3], cmx[3];
-    load_aabb(aabb + s, mn, mx);
-    for (int k = 0; k < 3; ++k) cmn[k] = cmx[k] = center1(mn[k], mx[k]);
-    uint32_t node = node_index[s];
-    while (node != 0) {
-        const uint32_t p = __ldcg(&nodes[node].parent);
-        typename Traits<T>::Node* pn = nodes + p;
-        const uint32_t pl = __ldcg(&pn->child_l);
-        const bool is_left = pl == node;
-        auto* dst = is_left ? &pn->l_aabb : &pn->r_aabb;
-        for (int k = 0; k < 3; ++k) { __stcg(&dst->min[k], mn[k]); __stcg(&dst->max[k], mx[k]); }
-        if (WITH_CB) for (int k = 0; k < 3; ++k) { __stcg(cb + 6 * (size_t)node + k, cmn[k]); __stcg(cb + 6 * (size_t)node + 3 + k, cmx[k]); }
-        __threadfence();
-        if (atomicAdd(arrivals + p, 1u) == 0u) return;      // sibling subtree not finished yet
-        __threadfence();
-        const auto* sib = is_left ? &pn->r_aabb : &pn->l_aabb;
-        for (int k = 0; k < 3; ++k) {
-            const T smn = __ldcg(&sib->min[k]), smx = __ldcg(&sib->max[k]);
-            mn[k] = min_t(smn, mn[k]);
-            mx[k] = max_t(smx, mx[k]);
-        }
-        if (WITH_CB) {
-            const uint32_t sn = is_left ? __ldcg(&pn->child_r) : pl;
-            for (int k = 0; k < 3; ++k) {
-                cmn[k] = min_t(__ldcg(cb + 6 * (size_t)sn + k), cmn[k]);
-                cmx[k] = max_t(__ldcg(cb + 6 * (size_t)sn + 3 + k), cmx[k]);
-            }
-        }
-        node = p;
-    }
-    if (WITH_CB) for (int k = 0; k < 3; ++k) { __stcg(cb + k, cmn[k]); __stcg(cb + 3 + k, cmx[k]); }     // the root's
-}
-
-template <class T> int refit(Tree<T>* tree) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    if (tree->n < 2) return tree->n == 1 ? build_traversal_records(tree) : (int)BVHGPU_OK;
-    uint32_t* arrivals = nullptr;
-    Scratch scratch(ctx);
-    BVH_TRY(scratch.get(&arrivals, tree->n_nodes));
-    BVH_CUDA_TRY(cudaMemsetAsync(arrivals, 0, sizeof(uint32_t) * tree->n_nodes, ctx->stream));
-    refit_kernel<T, false><<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, tree->n, arrivals, nullptr);
-    ctx->launches++;
-    BVH_CUDA_TRY(cudaGetLastError());
-    BVH_TRY(build_traversal_records(tree));
-    if (tree->have_flat) BVH_TRY(build_flat(tree));
-    return BVHGPU_OK;
-}
-
 
 // ---- optimize: refit + exact rebuild of the subtrees the motion degraded (replaces Bvh::update_shapes) --------------------
 // The reference re-inserts every changed shape sequentially (optimization.rs:290-302).  The data-parallel counterpart:
@@ -381,13 +324,8 @@ template <class T> int optimize(Tree<T>* tree, double max_growth) {
     T* cb = nullptr;
     uint8_t* bad = nullptr;
     uint32_t *roots = nullptr, *n_roots = nullptr, *idx0 = nullptr, *arrivals = nullptr;
-    const unsigned gn0 = (nn + 255) / 256;
-    if (!tree->d_sa_base) {                                             // first optimize on this tree: the baseline is the tree as built
-        BVH_TRY(dalloc(ctx, &tree->d_sa_base, sizeof(T) * nn));
-        node_sa_kernel<3, T, typename Traits<T>::Node><<<gn0, 256, 0, st>>>(tree->d_nodes, nn, reinterpret_cast<T*>(tree->d_sa_base));
-        ctx->launches++;
-    }
-    T* sa_old = reinterpret_cast<T*>(tree->d_sa_base);
+    BVH_TRY(ensure_sa_base(tree));                                      // first optimize on this tree: the baseline is the tree as built
+    T* sa_old = tree->d_sa_base;
     Scratch scratch(ctx);                                               // released on every return path
     BVH_TRY(scratch.get(&cb, (size_t)nn * 6));
     BVH_TRY(scratch.get(&bad, nn));
@@ -398,7 +336,7 @@ template <class T> int optimize(Tree<T>* tree, double max_growth) {
     BVH_CUDA_TRY(cudaMemsetAsync(arrivals, 0, sizeof(uint32_t) * nn, st));
     BVH_CUDA_TRY(cudaMemsetAsync(n_roots, 0, sizeof(uint32_t), st));
     const unsigned gn = (nn + 255) / 256, gs = (n + 255) / 256;
-    refit_kernel<T, true><<<gs, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, n, arrivals, cb);
+    refit_kernel<3, T, true><<<gs, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, n, arrivals, cb);
     mark_bad_kernel<T><<<gn, 256, 0, st>>>(tree->d_nodes, nn, sa_old, (T)max_growth, bad);
     select_roots_kernel<T><<<gn, 256, 0, st>>>(tree->d_nodes, nn, bad, roots, n_roots);
     leaf_order_kernel<<<gs, 256, 0, st>>>(tree->d_node_index, tree->d_node_start, n, idx0);
@@ -407,37 +345,9 @@ template <class T> int optimize(Tree<T>* tree, double max_growth) {
     BVH_TRY(rebuild_subtrees(ctx, tree, roots, n_roots, cb, idx0, false));
     rebase_kernel<3, T, typename Traits<T>::Node><<<std::max(1, std::min(ctx->sm_count * 4, (int)n)), 256, 0, st>>>(tree->d_nodes, roots, n_roots, sa_old);
     ctx->launches++;
-    BVH_TRY(build_traversal_records(tree));
-    if (tree->have_flat) BVH_TRY(build_flat(tree));
-    return BVHGPU_OK;
+    return refresh_caches(tree);
 }
 
-// ---- update: Bvh::update_shapes(changed_shape_indices, shapes) (src/bvh/optimization.rs:304-315) --------------------------------
-// Only the changed shapes cross the boundary: m indices + their m new AABBs.  check: NaN / index range, BEFORE anything is written.
-template <class T>
-__global__ void __launch_bounds__(256) update_check_kernel(const uint32_t* __restrict__ changed, const typename Traits<T>::Aabb* __restrict__ fresh,
-                                                           uint32_t m, uint32_t n, uint32_t* __restrict__ flags /* [0] NaN, [1] index out of range */) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    if (changed[i] >= n) atomicExch(flags + 1, 1u);
-    const T* p = reinterpret_cast<const T*>(fresh + i);
-    bool nan = false;
-#pragma unroll
-    for (int c = 0; c < 6; ++c) nan |= p[c] != p[c];
-    if (nan) atomicExch(flags, 1u);
-}
-template <class T>
-__global__ void __launch_bounds__(256) update_scatter_kernel(const uint32_t* __restrict__ changed, const typename Traits<T>::Aabb* __restrict__ fresh,
-                                                             uint32_t m, typename Traits<T>::DAabb* __restrict__ aabb) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const T* p = reinterpret_cast<const T*>(fresh + i);
-    typename Traits<T>::DAabb d;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) { d.min[c] = p[c]; d.max[c] = p[3 + c]; }
-    if constexpr (sizeof(T) == 4) { d.pad0 = 0; d.pad1 = 0; }
-    aabb[changed[i]] = d;                                               // an index listed twice: one of its AABBs wins (the reference would use shapes[i] for both)
-}
 // one warp per rebuild root: the shapes of its subtree in leaf order (index buffer of the rebuild) and the bounds of their centres
 template <class T>
 __global__ void __launch_bounds__(256) root_prep_kernel(const typename Traits<T>::Node* __restrict__ nodes, const uint32_t* __restrict__ node_start,
@@ -462,54 +372,10 @@ __global__ void __launch_bounds__(256) root_prep_kernel(const typename Traits<T>
         }
     }
 }
-// The shapes `d_changed[0..m)` already carry their new AABBs in tree->d_aabb.  max_growth <= 0: boxes only.
-template <class T>
-int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    const uint32_t n = tree->n, nn = tree->n_nodes;
-    const bool rebuild = max_growth > 0.0;
-    if (n < 3) return rebuild ? optimize(tree, max_growth) : refit(tree);
-    const unsigned gm = (m + 255) / 256;
-    if (!tree->d_arrive) {
-        BVH_TRY(dalloc_t(ctx, &tree->d_arrive, nn));
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_arrive, 0, sizeof(uint32_t) * nn, st));
-    }
-    if (rebuild && !tree->d_bad) {
-        BVH_TRY(dalloc_t(ctx, &tree->d_bad, nn));
-        BVH_CUDA_TRY(cudaMemsetAsync(tree->d_bad, 0, nn, st));
-    }
-    if (rebuild) BVH_TRY(ensure_sa_base(tree));                         // first update on this tree: the baseline is the tree before the motion
-    Scratch scratch(ctx);
-    uint32_t *dirty = nullptr, *cnts = nullptr;
-    BVH_TRY(scratch.get(&dirty, nn));
-    BVH_TRY(scratch.get(&cnts, 2));                                     // [0] dirty nodes, [1] rebuild roots
-    BVH_CUDA_TRY(cudaMemsetAsync(cnts, 0, 2 * sizeof(uint32_t), st));
-    mark_paths_kernel<typename Traits<T>::Node><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, d_changed, m, tree->d_arrive);
-    climb_paths_kernel<3, T, typename Traits<T>::Node, typename Traits<T>::DAabb><<<gm, 256, 0, st>>>(tree->d_nodes, tree->d_node_index, tree->d_aabb, d_changed, m, tree->d_arrive,
-                                              reinterpret_cast<const T*>(tree->d_sa_base), (T)max_growth, rebuild ? tree->d_bad : nullptr, dirty, cnts);
-    ctx->launches += 2;
-    if (rebuild) BVH_TRY(rebuild_degraded(tree, dirty, cnts));
-    BVH_CUDA_TRY(cudaGetLastError());
-    BVH_TRY(build_traversal_records(tree));
-    if (tree->have_flat) BVH_TRY(build_flat(tree));
-    return BVHGPU_OK;
-}
-
-// The surface-area baseline of the growth test: the tree as it is now, unless one exists already.
-template <class T> int ensure_sa_base(Tree<T>* tree) {
-    if (tree->d_sa_base || tree->n_nodes == 0) return BVHGPU_OK;
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_TRY(dalloc(ctx, &tree->d_sa_base, sizeof(T) * tree->n_nodes));
-    node_sa_kernel<3, T, typename Traits<T>::Node><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, reinterpret_cast<T*>(tree->d_sa_base));
-    ctx->launches++;
-    BVH_CUDA_TRY(cudaGetLastError());
-    return BVHGPU_OK;
-}
-
 // dirty[0 .. cnts[0]) = the nodes whose box changed, tree->d_bad = their growth flags.  Rebuilds in place the outermost degraded
-// subtrees (cnts[1], zero on entry, counts them), gives them fresh baselines and clears the flags.
-template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* dirty, uint32_t* cnts) {
+// subtrees (cnts[1], zero on entry, counts them), gives them fresh baselines and clears the flags.  The builder counts the shapes it
+// rebuilt in tree->d_status and reports its errors there.
+template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* dirty, uint32_t* cnts, size_t*, const char*) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
     const uint32_t n = tree->n, gn = (tree->n_nodes + 255) / 256;
@@ -524,42 +390,19 @@ template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* dirty, ui
     ctx->launches += 2;
     BVH_CUDA_TRY(cudaGetLastError());
     BVH_TRY(rebuild_subtrees(ctx, tree, roots, cnts + 1, cb_roots, idx0, true));
-    rebase_kernel<3, T, typename Traits<T>::Node><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, reinterpret_cast<T*>(tree->d_sa_base));
+    rebase_kernel<3, T, typename Traits<T>::Node><<<std::max(1, ctx->sm_count * 8), 256, 0, st>>>(tree->d_nodes, roots, cnts + 1, tree->d_sa_base);
     clear_bad_kernel<<<gn, 256, 0, st>>>(dirty, cnts, tree->d_bad);
     ctx->launches += 2;
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
 }
 
-template <class T>
-int update_changed(Tree<T>* tree, const uint32_t* d_changed, const typename Traits<T>::Aabb* d_fresh, uint32_t m, uint32_t* d_flags) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    const unsigned g = (m + 255) / 256;
-    update_check_kernel<T><<<g, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->n, d_flags);
-    ctx->launches++;
-    BVH_CUDA_TRY(cudaGetLastError());
-    return BVHGPU_OK;
-}
-template <class T>
-int update_scatter(Tree<T>* tree, const uint32_t* d_changed, const typename Traits<T>::Aabb* d_fresh, uint32_t m) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    update_scatter_kernel<T><<<(m + 255) / 256, 256, 0, ctx->stream>>>(d_changed, d_fresh, m, tree->d_aabb);
-    ctx->launches++;
-    BVH_CUDA_TRY(cudaGetLastError());
-    return BVHGPU_OK;
-}
-
 #define INST(T)                                           \
-    template int update_incremental<T>(Tree<T>*, const uint32_t*, uint32_t, double); \
-    template int ensure_sa_base<T>(Tree<T>*);             \
-    template int rebuild_degraded<T>(Tree<T>*, const uint32_t*, uint32_t*); \
-    template int update_changed<T>(Tree<T>*, const uint32_t*, const typename Traits<T>::Aabb*, uint32_t, uint32_t*); \
-    template int update_scatter<T>(Tree<T>*, const uint32_t*, const typename Traits<T>::Aabb*, uint32_t); \
+    template int rebuild_degraded<T>(Tree<T>*, const uint32_t*, uint32_t*, size_t*, const char*); \
     template int optimize<T>(Tree<T>*, double);           \
     template int build_traversal_records<T>(Tree<T>*);    \
     template int build_flat<T>(Tree<T>*);                 \
-    template int sah_cost<T>(Tree<T>*, double*);          \
-    template int refit<T>(Tree<T>*);
+    template int sah_cost<T>(Tree<T>*, double*);
 INST(float)
 INST(double)
 

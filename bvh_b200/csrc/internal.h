@@ -52,8 +52,8 @@ struct bvhgpu_ctx {
     int64_t build_small = -1;      // exact builder: defer ranges <= 16 shapes to the thread-per-range kernel (-1 auto by size, 0 never, 1 always)
     // small pinned read-back area (256 words): 0-25 the ray traversal's scan tail, 64-79 the streamed path's per-chunk values,
     // 128-129 the stream probe, 200-217 the entry points' checks (200 staged boxes, 204 synchronize, 208-209 changed boxes, 212 added
-    // boxes, 216-217 removal lists), 220 / 224 the group counts of the 3-D / 4-D add, 232-235 the 4-D build, CSR_TOTAL_WORD (236-237) the total of the
-    // two-pass CSR walks (csr.cuh), 244-248 the 4-D rebuild seeds
+    // boxes, 216-217 removal lists), 220 the group count of an add, 224-225 the 4-D group seeds, 232-235 the 4-D build, CSR_TOTAL_WORD
+    // (236-237) the total of the two-pass CSR walks (csr.cuh), 244-248 the 4-D rebuild seeds
     uint32_t* h_pinned = nullptr;
     int64_t profile = 0;           // bracket dominant kernels with events
     cudaEvent_t ev_walk[2] = {nullptr, nullptr};
@@ -84,6 +84,9 @@ namespace bvhb200 {
 
 template <class T> struct Tree {
     using Tr = Traits<T>;
+    // what the dynamic drivers of dynamic.cu see: a 2-D tree runs the D = 3 kernels in the plane z = 0
+    static constexpr int D = 3;
+    using Scalar = T; using Node = typename Tr::Node; using Aabb = typename Tr::Aabb; using Box = typename Tr::DAabb;
     bvhgpu_ctx* ctx = nullptr;
     uint32_t n = 0;          // shapes
     uint32_t n_nodes = 0;    // 2n-1
@@ -100,7 +103,7 @@ template <class T> struct Tree {
     bool top_valid = false;
     uint32_t* d_arrive = nullptr;             // [2n-1] arrival counters of the incremental update (all zero between calls)
     uint8_t* d_bad = nullptr;                 // [2n-1] growth flags of the incremental update (all zero between calls)
-    void* d_sa_base = nullptr;                // [2n-1] surface area of every inner node when it was last (re)built: baseline of bvhgpu_optimize / update
+    T* d_sa_base = nullptr;                   // [2n-1] surface area of every inner node when it was last (re)built: baseline of bvhgpu_optimize / update
     void* d_tris = nullptr;                   // [n] triangle vertices (padded), optional: bvhgpu_tree_set_triangles_*
     typename Tr::Flat* d_flat = nullptr;      // [n_flat] reference-layout FlatBvh (built on demand)
     size_t n_flat = 0;
@@ -205,21 +208,35 @@ template <class T> int build_traversal_records(Tree<T>* tree);   // d_tnodes
 template <class T> int build_flat(Tree<T>* tree);                // d_flat (reference FlatNode layout)
 int build_top_records(Tree<float>* tree, uint32_t budget);        // d_top
 template <class T> int sah_cost(Tree<T>* tree, double* out2);
-template <class T> int refit(Tree<T>* tree);                     // recompute child AABBs bottom-up from d_aabb
 template <class T> int optimize(Tree<T>* tree, double max_growth);   // refit + exact rebuild of the degraded subtrees
-// update_shapes form: validate (flags[0] NaN, flags[1] bad index) / scatter m changed AABBs (device pointers) into tree->d_aabb
-template <class T> int update_changed(Tree<T>* tree, const uint32_t* d_changed, const typename Traits<T>::Aabb* d_fresh, uint32_t m, uint32_t* d_flags);
-template <class T> int update_incremental(Tree<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth);
-template <class T> int update_scatter(Tree<T>* tree, const uint32_t* d_changed, const typename Traits<T>::Aabb* d_fresh, uint32_t m);
-// growth test helpers shared by update_incremental and add_shapes
-template <class T> int ensure_sa_base(Tree<T>* tree);
-template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* d_dirty, uint32_t* d_cnts /* [0] dirty nodes, [1] roots (zeroed) */);
+// Caches after the boxes changed in place (node count unchanged, dynamic.cu): the FLAT leaf boxes of a 2-D tree first (the records
+// read them), then the traversal records, then the flat array if it was built.
+template <class T> int refresh_caches(Tree<T>* tree);
+// After a relocation (new node count or shape numbering, dynamic.cu): update buffers dropped, records and flat array rebuilt at the
+// new size.
+template <class T> int finish_relayout(Tree<T>* tree);
+// dirty[0 .. cnts[0]) = the nodes whose box changed, tree->d_bad = their growth flags.  Rebuilds in place the outermost degraded subtrees
+// (cnts[1], zero on entry, counts them), gives them fresh baselines and clears the flags.  The shapes rebuilt are counted in
+// tree->d_status (`rebuilt` and `who` serve the 4-D overload).
+template <class T> int rebuild_degraded(Tree<T>* tree, const uint32_t* d_dirty, uint32_t* d_cnts, size_t* rebuilt, const char* who);
 
-// ---- dynamic.cu: Bvh::add_shape / remove_shape, batched ----
-// aabb_all: [n + k] device AABBs (the tree's n followed by the k new ones, checked for NaN); becomes tree->d_aabb.
-template <class T> int add_shapes(Tree<T>* tree, typename Traits<T>::DAabb* aabb_all, uint32_t k, double max_growth);
-// d_rm: [n + 1] removed flag of every shape (0 / 1, the last word 0), k = number of removed shapes, 1 <= k <= n.
-template <class T> int remove_shapes(Tree<T>* tree, const uint32_t* d_rm, uint32_t k);
+// ---- dynamic.cu: refit, update_shapes, add_shape / remove_shape (batched) of Tree<T> and Tree4<T> ----
+// The shapes of the tree type's ABI box, checked on the device (flags read back, synchronises): a NaN coordinate, an index >= n when
+// d_changed is given (otherwise box i belongs to shape i).  A failure leaves the tree untouched.
+template <class TreeT> int check_boxes(TreeT* tree, const uint32_t* d_changed, const typename TreeT::Aabb* d_fresh, uint32_t m, Scratch& scratch,
+                                       const char* who);
+template <class TreeT> int scatter_boxes(TreeT* tree, const uint32_t* d_changed, const typename TreeT::Aabb* d_fresh, uint32_t m);   // into d_aabb
+template <class TreeT> int ensure_sa_base(TreeT* tree);   // the growth baseline: the tree as it is now, unless one exists already
+template <class TreeT> int refit(TreeT* tree);            // child boxes bottom-up from d_aabb, then the caches
+// The shapes d_changed[0 .. m) already carry their new boxes in d_aabb.  max_growth <= 0: boxes only.  *rebuilt: shapes in the rebuilt
+// subtrees (4-D; a 3-D tree counts them in its status).
+template <class TreeT> int update_incremental(TreeT* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt);
+// aabb_all: [n + k] device boxes (the tree's n followed by the k new ones, checked for NaN); becomes tree->d_aabb.  A failure with
+// tree->d_aabb != aabb_all left the tree untouched; after that point the caller marks it failed.  *rebuilt as update_incremental.
+template <class TreeT> int add_shapes(TreeT* tree, typename TreeT::Box* aabb_all, uint32_t k, double max_growth, size_t* rebuilt);
+// d_rm: [n + 1] removed flag of every shape (0 / 1, the last word 0), k = number of removed shapes, 1 <= k <= n.  A failure with
+// tree->d_nodes unchanged left the tree untouched.
+template <class TreeT> int remove_shapes(TreeT* tree, const uint32_t* d_rm, uint32_t k);
 // validation of a removal list: d_rm[n + 1] zeroed by the caller; d_flags[0] = index >= n, d_flags[1] = duplicate index
 int remove_check(bvhgpu_ctx* ctx, const uint32_t* d_idx, uint32_t k, uint32_t n, uint32_t* d_rm, uint32_t* d_flags);
 
@@ -310,6 +327,8 @@ template <> struct D4<double> { using Aabb = bvh_aabb4d; using Ray = bvh_ray4d; 
 // Bvh<T,4>: its own node types and pipeline (a fourth axis cannot hide in the 3-D kernels the way D = 2 hides in z = 0).
 template <class T> struct Tree4 {
     using Aabb = typename D4<T>::Aabb; using Node = typename D4<T>::Node; using Flat = typename D4<T>::Flat; using Rec = typename D4<T>::Rec;
+    static constexpr int D = 4;
+    using Scalar = T; using Box = Aabb;   // the shape boxes keep the ABI layout on the device
     bvhgpu_ctx* ctx = nullptr;
     uint32_t n = 0, n_nodes = 0;
     Aabb* d_aabb = nullptr;            // [n]      shape AABBs (ABI layout: already whole sectors)
@@ -356,16 +375,17 @@ template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_
                                        T* d_dists, size_t cap, size_t* total);
 // k nearest shapes: checks n, k and the tree's status, as knn_device does.
 template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
-// m new boxes (and their shape indices, when d_changed is given) checked for NaN / range; the verdict is read back (synchronises).
-template <class T> int check4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m, Scratch& scratch, const char* who);
-template <class T> int put4(Tree4<T>* tree, const uint32_t* d_changed, const typename D4<T>::Aabb* d_fresh, uint32_t m);   // scatter into d_aabb
-template <class T> int refit4(Tree4<T>* tree);                      // bottom-up refit of every node from d_aabb
-template <class T> int update4(Tree4<T>* tree, const uint32_t* d_changed, uint32_t m, double max_growth, size_t* rebuilt);
-// aabb_all: [n + k] boxes (checked), becomes d_aabb; a failure with tree->d_aabb != aabb_all left the tree untouched.
-template <class T> int add_shapes4(Tree4<T>* tree, typename D4<T>::Aabb* aabb_all, uint32_t k, double max_growth, size_t* rebuilt);
-// d_rm: [n + 1] removed flags, 1 <= k <= n; a failure with tree->d_nodes unchanged left the tree untouched.
-template <class T> int remove_shapes4(Tree4<T>* tree, const uint32_t* d_rm, uint32_t k);
-template <class T> void drop_caches4(Tree4<T>* tree);              // after a relocation: records, flat array, update buffers
+// The 4-D overloads of the steps the dynamic drivers of dynamic.cu leave to the tree type (the 3-D ones are declared above):
+// records and flat array, if built, rewritten in place from the new boxes
+template <class T> int refresh_caches(Tree4<T>* tree);
+// after a relocation: records and flat array dropped (rebuilt at the new size on first use), update buffers dropped
+template <class T> int finish_relayout(Tree4<T>* tree);
+// the growth rebuild of the level loop and small4_kernel of the build; *rebuilt = shapes in the rebuilt subtrees
+template <class T> int rebuild_degraded(Tree4<T>* tree, const uint32_t* d_dirty, uint32_t* d_cnts, size_t* rebuilt, const char* who);
+// Exact-SAH subtrees built in place under the roots d_roots[0 .. *d_n_roots) (at most max_roots): their shapes in leaf order in
+// idx[0 .. n) (idx holds the builder's two index buffers, 2 n), their centre bounds as keys in cb[8 slot ..].  Synchronous.
+template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* d_roots, const uint32_t* d_n_roots, uint32_t max_roots,
+                                      const typename Traits<T>::Key* cb, uint32_t* idx, const char* who);
 
 }  // namespace bvhb200
 

@@ -1,5 +1,5 @@
-// bvh_b200/csrc/update.cuh -- the kernels of the incremental update (Bvh::update_shapes, src/bvh/optimization.rs:304-351) that
-// D = 3 (flatten.cu, and D = 2 through the z = 0 embedding of dim2.cu) and D = 4 (dim4.cu) share.
+// bvh_b200/csrc/update.cuh -- the kernels of refit and the incremental update (Bvh::update_shapes, src/bvh/optimization.rs:304-351)
+// that D = 3 (and D = 2 through the z = 0 embedding of dim2.cu) and D = 4 share; the host drivers are in dynamic.cu.
 //
 // Every node POD starts with the same 16 bytes {parent, child_l, child_r, shape}, so the kernels that only follow links are
 // templated on the node type.  The kernels that touch boxes are templated on D as well: they load a shape box with load_box of
@@ -24,6 +24,86 @@ template <int D, class T> __device__ __forceinline__ T surface_area_d(const T mn
     static_assert(D == 3 || D == 4, "surface_area_d: D = 3 or 4");
     if constexpr (D == 3) return surface_area(mn, mx);
     else return surface_area4(mn, mx);
+}
+
+// ---- refit: bottom-up recomputation of the child boxes from the (new) shape boxes ----
+// (the data-parallel part of Bvh::update_shapes: fix_aabbs_ascending, src/bvh/optimization.rs:317-351).  One thread per shape climbs
+// from its leaf and writes its box into the parent's child slot; the second thread to reach a node joins the two slots and carries on.
+// Topology, node_index and node_start are kept; leaves keep their Aabb::empty() child boxes.
+// WITH_CB (bvhgpu_optimize, D = 3 only): the climb also carries the bounds of the shape CENTRES below every node into cb[node][6]
+// (min xyz, max xyz) -- what the builder needs, next to the box, to restart from an inner node.
+template <int D, class T, bool WITH_CB, class Node, class Box>
+__global__ void __launch_bounds__(256) refit_kernel(Node* nodes, const uint32_t* __restrict__ node_index,
+                                                    const Box* __restrict__ aabb, uint32_t n, uint32_t* arrivals, T* cb) {
+    static_assert(D == 3 || !WITH_CB, "refit_kernel: centre bounds for D = 3 only");
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    T mn[D], mx[D], cmn[D], cmx[D];
+    load_box(aabb + s, mn, mx);
+    for (int k = 0; k < D; ++k) cmn[k] = cmx[k] = center1(mn[k], mx[k]);
+    uint32_t node = node_index[s];
+    while (node != 0) {
+        const uint32_t p = __ldcg(&nodes[node].parent);
+        Node* pn = nodes + p;
+        const uint32_t pl = __ldcg(&pn->child_l);
+        const bool is_left = pl == node;
+        auto* dst = is_left ? &pn->l_aabb : &pn->r_aabb;
+        for (int k = 0; k < D; ++k) { __stcg(&dst->min[k], mn[k]); __stcg(&dst->max[k], mx[k]); }
+        if (WITH_CB) for (int k = 0; k < D; ++k) { __stcg(cb + 2 * D * (size_t)node + k, cmn[k]); __stcg(cb + 2 * D * (size_t)node + D + k, cmx[k]); }
+        __threadfence();
+        if (atomicAdd(arrivals + p, 1u) == 0u) return;      // sibling subtree not finished yet
+        __threadfence();
+        const auto* sib = is_left ? &pn->r_aabb : &pn->l_aabb;
+        for (int k = 0; k < D; ++k) {
+            const T smn = __ldcg(&sib->min[k]), smx = __ldcg(&sib->max[k]);
+            mn[k] = min_t(smn, mn[k]);
+            mx[k] = max_t(smx, mx[k]);
+        }
+        if (WITH_CB) {
+            const uint32_t sn = is_left ? __ldcg(&pn->child_r) : pl;
+            for (int k = 0; k < D; ++k) {
+                cmn[k] = min_t(__ldcg(cb + 2 * D * (size_t)sn + k), cmn[k]);
+                cmx[k] = max_t(__ldcg(cb + 2 * D * (size_t)sn + D + k), cmx[k]);
+            }
+        }
+        node = p;
+    }
+    if (WITH_CB) for (int k = 0; k < D; ++k) { __stcg(cb + k, cmn[k]); __stcg(cb + D + k, cmx[k]); }     // the root's
+}
+
+// ---- new shape boxes of refit / update_shapes / add_shapes, checked before anything is written ----
+// flags[0]: a NaN coordinate, flags[1]: an index >= n.  Box = the ABI box of D (2 D scalars); changed == nullptr: box i belongs to
+// shape i (no index to check).
+template <int D, class T, class Box>
+__global__ void __launch_bounds__(256) check_boxes_kernel(const uint32_t* __restrict__ changed, const Box* __restrict__ fresh,
+                                                          uint32_t m, uint32_t n, uint32_t* __restrict__ flags) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    if (changed && changed[i] >= n) atomicExch(flags + 1, 1u);
+    const T* p = reinterpret_cast<const T*>(fresh + i);
+    bool nan = false;
+#pragma unroll
+    for (int c = 0; c < 2 * D; ++c) nan |= p[c] != p[c];
+    if (nan) atomicExch(flags, 1u);
+}
+// a checked ABI box into the tree's array: converted to the padded 3-D device layout, or copied (the 4-D ABI box is the device layout)
+template <class T> __device__ __forceinline__ void store_padded(typename Traits<T>::DAabb* dst, const T* p) {
+    typename Traits<T>::DAabb d;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { d.min[c] = p[c]; d.max[c] = p[3 + c]; }
+    if constexpr (sizeof(T) == 4) { d.pad0 = 0; d.pad1 = 0; }
+    *dst = d;
+}
+__device__ __forceinline__ void store_box(DAabbF* dst, const bvh_aabb3f* src) { store_padded<float>(dst, reinterpret_cast<const float*>(src)); }
+__device__ __forceinline__ void store_box(DAabbD* dst, const bvh_aabb3d* src) { store_padded<double>(dst, reinterpret_cast<const double*>(src)); }
+__device__ __forceinline__ void store_box(bvh_aabb4f* dst, const bvh_aabb4f* src) { *dst = *src; }
+__device__ __forceinline__ void store_box(bvh_aabb4d* dst, const bvh_aabb4d* src) { *dst = *src; }
+template <class Box, class DBox>
+__global__ void __launch_bounds__(256) scatter_boxes_kernel(const uint32_t* __restrict__ changed, const Box* __restrict__ fresh, uint32_t m,
+                                                            DBox* __restrict__ aabb) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    store_box(aabb + changed[i], fresh + i);            // an index listed twice: one of its boxes wins (the reference would use shapes[i] for both)
 }
 
 // ---- rebuild roots ----
