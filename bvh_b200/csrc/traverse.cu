@@ -480,7 +480,7 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
             if (__popc(idle_mask) >= leave) break;
             if (STREAM) {                                            // look for arrivals every 16 visits, at once if nobody walks
                 const uint32_t pend = __ballot_sync(FULL, r != NONE && !loaded);
-                if (pend && (((rounds += VPC) & 15u) == 0u || (pend | idle_mask) == FULL)) break;
+                if (pend && ((rounds += VPC) >= 16u || (pend | idle_mask) == FULL)) break;
             }
         }
     }
@@ -948,6 +948,7 @@ constexpr unsigned long long STREAM_TIMEOUT_NS = 4ull * 1000ull * 1000ull * 1000
 // The shared-memory top-tree walk: f32 trees only; false = not applicable (the caller launches the plain persistent kernel).
 constexpr uint32_t TOP_BUDGET = 7000;                               // entries: 224 000 B of the 227 KB a CTA may own
 constexpr size_t TOP_UNROLL_MAX_BYTES = (size_t)32 << 20;           // traversal records that count as L2-resident (H100: 50 MB of L2)
+constexpr int TOP_VPC_L2 = 5;                                       // visits per vote on those trees (see launch_top)
 template <class T> static bool launch_top(Tree<T>*, bool, RaySrc<T>, uint32_t, uint32_t*, uint32_t*, uint32_t, unsigned long long*, uint32_t*, bool) { return false; }
 template <> bool launch_top<float>(Tree<float>* tree, bool flat, RaySrc<float> rays, uint32_t R, uint32_t* counts, uint32_t* slots, uint32_t K,
                                    unsigned long long* tail, uint32_t* gate, bool stream_mode) {
@@ -960,8 +961,8 @@ template <> bool launch_top<float>(Tree<float>* tree, bool flat, RaySrc<float> r
         auto raise = [&](const void* f) { return cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess; };
         if (!raise((const void*)walk_top_kernel<false, false, 1>) || !raise((const void*)walk_top_kernel<true, false, 1>) ||
             !raise((const void*)walk_top_kernel<false, true, 1>) || !raise((const void*)walk_top_kernel<true, true, 1>) ||
-            !raise((const void*)walk_top_kernel<false, false, 4>) || !raise((const void*)walk_top_kernel<true, false, 4>) ||
-            !raise((const void*)walk_top_kernel<false, true, 4>) || !raise((const void*)walk_top_kernel<true, true, 4>)) { cudaGetLastError(); return false; }
+            !raise((const void*)walk_top_kernel<false, false, TOP_VPC_L2>) || !raise((const void*)walk_top_kernel<true, false, TOP_VPC_L2>) ||
+            !raise((const void*)walk_top_kernel<false, true, TOP_VPC_L2>) || !raise((const void*)walk_top_kernel<true, true, TOP_VPC_L2>)) { cudaGetLastError(); return false; }
         ctx->top_attr_set = true;
     }
     const size_t smem = (size_t)budget * 32;                            // n_top <= budget lives on the device: reserve for the budget
@@ -970,14 +971,15 @@ template <> bool launch_top<float>(Tree<float>* tree, bool flat, RaySrc<float> r
     uint32_t* err = reinterpret_cast<uint32_t*>(tail + S_ERR);
     const float4* top = reinterpret_cast<const float4*>(tree->d_top);
     static const int top_refill = getenv("BVHGPU_TOP_REFILL") ? std::max(1, std::min(32, atoi(getenv("BVHGPU_TOP_REFILL")))) : 8;   // dev knob: idle lanes per refill
-    // Visits per vote: 4 where the records stay L2-resident (config 2, 7.7 MB: the step is about 4 % faster than with a vote after every
-    // visit, measured on H100), 1 for trees beyond L2 (hbm_bound, 640 MB: 4 is 2 % slower there, its visits wait on DRAM).
+    // Visits per vote: TOP_VPC_L2 = 5 where the records stay L2-resident, 1 for trees beyond L2 (hbm_bound, 640 MB: 4 was 2 % slower
+    // there, its visits wait on DRAM).  On config 2 (7.7 MB, H100) the walk kernel took 0.316 ms at 5 visits per vote, 0.327 at 3,
+    // 0.317-0.322 at 7, but 0.361 at 2, 0.352 at 4 (the previous choice), 0.350 at 6 and 0.351 at 8 (DESIGN §4.3).
     const bool l2_tree = (size_t)tree->n_trec * sizeof(TNodeF) <= TOP_UNROLL_MAX_BYTES;
 #define BVH_TOP_LAUNCH(F, S, V, TMO) walk_top_kernel<F, S, V><<<grid, 1024, smem, ctx->stream>>>(tree->d_tnodes, walk_aabbs(tree), tree->n_trec, top, rays, R, ticket, \
                                                                     ctx->d_ready, counts, slots, K, tail + S_VISITS, gate, 0u, err, TMO, top_refill)
 #define BVH_TOP_FORMS(V) do { if (stream_mode) { if (flat) BVH_TOP_LAUNCH(true, true, V, STREAM_TIMEOUT_NS); else BVH_TOP_LAUNCH(false, true, V, STREAM_TIMEOUT_NS); } \
                               else             { if (flat) BVH_TOP_LAUNCH(true, false, V, 0ull); else BVH_TOP_LAUNCH(false, false, V, 0ull); } } while (0)
-    if (l2_tree) BVH_TOP_FORMS(4); else BVH_TOP_FORMS(1);
+    if (l2_tree) BVH_TOP_FORMS(TOP_VPC_L2); else BVH_TOP_FORMS(1);
 #undef BVH_TOP_FORMS
 #undef BVH_TOP_LAUNCH
     ctx->launches++;

@@ -1,5 +1,6 @@
 // tools/sim_top.cpp -- DEV TOOL (not product): CPU model of walk_top_kernel's shared-memory wavefronts.
 //   g++ -O3 -march=x86-64-v3 -ffp-contract=off -std=c++17 -I oracle tools/sim_top.cpp -o /tmp/sim_top && /tmp/sim_top
+//   /tmp/sim_top 60000 5000 4 2000     (rays, tier-1 budget B1, cluster size S, tier-2 entries per CTA B2: the two-tier model)
 // Model: warps of 32 lanes with the kernel's refill rule (>= 8 idle lanes -> new tickets); per warp step, an LDS.128 costs, per
 // quarter-warp, the largest number of DISTINCT 16-byte chunks that fall into one of the 8 bank groups.  Variants: plain SoA
 // (lo[j], hi[j]); the first H entries replicated 8 x (lane & 7 picks the copy: conflict-free).
@@ -45,6 +46,52 @@ int main(int argc, char** argv) {
     std::vector<Ray3<float>> rays(R); uint64_t seed = 0;
     for (uint32_t i = 0; i < R; ++i) rays[i] = create_ray(seed, bounds);
     auto hit = [&](const Ray3<float>& ray, const Rec& r) { Aabb3<float> b; for (int k = 0; k < 3; ++k) { b.min[k] = r.mn[k]; b.max[k] = r.mx[k]; } return ray_intersects_aabb(ray, b); };
+    if (argc > 4) {
+        // Two tiers (walk_top_kernel under a cluster of S CTAs): tier 1 = T(C1) for budget B1 (argument 2), replicated; tier 2 =
+        // T(C2) \ T(C1) for C2 fitting |T(C1)| + S * B2, entry t on CTA rank t % S.  Plain preorder walk (the kernel's visit order)
+        // under the kernel's refill rule, one visit per lane per step, warp w on CTA rank w % S.  Reports visits per ray by tier,
+        // remote (other-rank) tier-2 reads, and the share of warp steps with a lane below the tiers / a lane reading a peer, for
+        // one visit per step and for the kernel's four (a group of 4 steps with one such lane in any of them).
+        const uint32_t S = atoi(argv[3]), B2 = atoi(argv[4]);
+        auto size_for = [&](uint32_t c) { uint32_t t = 0; for (uint32_t i = 1; i < nn; ++i) t += cnt[nodes[i].parent] >= c; return t; };
+        const uint32_t n1 = nT, C1 = C;
+        uint32_t C2 = C1; while (C2 > 2 && size_for(C2 - 1) <= n1 + S * B2) --C2;
+        std::vector<uint32_t> tier(nn, 2), t2(nn, 0);                  // 0 tier 1, 1 tier 2, 2 below
+        uint32_t n2 = 0;
+        for (uint32_t i = 1; i < nn; ++i) { const uint32_t c = cnt[nodes[i].parent]; tier[i] = c >= C1 ? 0 : c >= C2 ? 1 : 2; if (tier[i] == 1) t2[i] = n2++; }
+        const int W = 512;
+        std::vector<uint32_t> ray(W * 32, U32_MAX), at(W * 32, 0);
+        uint32_t ticket = 0; uint64_t steps = 0, v[3] = {0, 0, 0}, remote = 0, st_below = 0, st_remote = 0, grp = 0, grp_below = 0, grp_remote = 0;
+        for (bool any = true; any;) {
+            any = false;
+            for (int w = 0; w < W; ++w) {
+                uint32_t* wr = &ray[32 * w]; uint32_t* wa = &at[32 * w];
+                int idle = 0; for (int l = 0; l < 32; ++l) idle += wr[l] == U32_MAX;
+                if (idle >= 8 && ticket < R) for (int l = 0; l < 32 && ticket < R; ++l) if (wr[l] == U32_MAX) { wr[l] = ticket++; wa[l] = 0; }
+                bool gb = false, gr = false, act = false;
+                for (int u = 0; u < 4; ++u) {
+                    bool sb = false, sr = false, sa = false;
+                    for (int l = 0; l < 32; ++l) if (wr[l] != U32_MAX) {
+                        const uint32_t i = wa[l] + 1;                     // record wa = node wa + 1
+                        sa = true; ++v[tier[i]];
+                        if (tier[i] == 2) sb = true;
+                        if (tier[i] == 1 && t2[i] % S != (uint32_t)w % S) { sr = true; ++remote; }
+                        wa[l] = hit(rays[wr[l]], rec[wa[l]]) ? wa[l] + 1 : rec[wa[l]].w3;
+                        if (wa[l] >= nn - 1) wr[l] = U32_MAX;
+                    }
+                    if (!sa) break;
+                    ++steps; st_below += sb; st_remote += sr; gb |= sb; gr |= sr; act = true;
+                }
+                if (act) { any = true; ++grp; grp_below += gb; grp_remote += gr; }
+            }
+        }
+        printf("S %u  B1 %u  B2 %u: C1 %u (%u entries)  C2 %u (tier 2: %u entries, %u per CTA)\n", S, atoi(argv[2]), B2, C1, n1, C2, n2, (n2 + S - 1) / S);
+        printf("  visits/ray: tier 1 %.2f  tier 2 %.2f (remote %.2f)  below %.2f  total %.3f\n", (double)v[0] / R, (double)v[1] / R, (double)remote / R,
+               (double)v[2] / R, (double)(v[0] + v[1] + v[2]) / R);
+        printf("  P(step has a lane below) %.3f  P(step has a remote lane) %.3f  | per 4-visit step: below %.3f  remote %.3f\n",
+               (double)st_below / steps, (double)st_remote / steps, (double)grp_below / grp, (double)grp_remote / grp);
+        return 0;
+    }
     for (uint32_t H : {0u, 64u, 128u, 256u, 512u, 1024u}) {
         const int W = 512;
         struct Warp { uint32_t ray[32], j[32], g[32], gend[32]; };

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Instruction mix of one visit of the shared-memory top walk (walk_top_kernel), read from the SASS; no GPU needed.
 
-usage: tools/visit_sass.py [--source bvh_b200/csrc/traverse.cu] [--kernel '<false, false, 4>'] [--all]
+usage: tools/visit_sass.py [--source bvh_b200/csrc/traverse.cu] [--kernel '<false, false, 5>'] [--all]
 
 Compiles traverse.cu to a cubin with the library's nvcc flags (bvh_b200/build.py), prints each walk_top_kernel instance's
 registers, stack, spills and shared memory from ptxas, and splits the warp-step loop (VPC visits, then the vote on idle
@@ -174,7 +174,7 @@ def report(name: str, pretty: str, code, vpc: int, ptx: str, verbose: bool):
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--source", default=os.path.join(ROOT, "bvh_b200", "csrc", "traverse.cu"))
-    ap.add_argument("--kernel", default="<false, false, 4>", help="template arguments of the instance to list (substring)")
+    ap.add_argument("--kernel", default="<false, false, 5>", help="template arguments of the instance to list (substring)")
     ap.add_argument("--all", action="store_true", help="every walk_top_kernel instance")
     ap.add_argument("-v", "--verbose", action="store_true", help="print the visit's instructions")
     a = ap.parse_args()
