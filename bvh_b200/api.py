@@ -386,6 +386,31 @@ class Bvh:
             capi.check(st)
         return offsets, hits[: total.value]
 
+    def overlap_pairs(self, cap: int | None = None):
+        """Every pair of shapes whose own current AABBs intersect (touching faces included), each once: CSR (offsets[n + 1], hits)
+        indexed by shape, row s = the shapes t with node_index[t] > node_index[s] whose box meets s's, in DFS order.  A short
+        capacity (default max(4 n, 1024)) is completed from the retained list (bvhgpu_traverse_fetch_*)."""
+        n = self.num_shapes
+        offsets = np.zeros(n + 1, dtype=np.uint32)
+        cap = max(4 * n, 1024) if cap is None else int(cap)
+        hits = np.zeros(cap, dtype=np.uint32)
+        total = C.c_size_t(0)
+        st = getattr(capi.lib(), f"bvhgpu_overlap_pairs_{self._d['suffix']}")(self._h, _ptr(offsets), _ptr(hits), cap, C.byref(total))
+        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
+            hits = np.zeros(total.value, dtype=np.uint32)
+            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), total.value))
+        else:
+            capi.check(st)
+        return offsets, hits[: total.value]
+
+    def overlap_pairs_dev(self, offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
+        """overlap_pairs into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets are
+        always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        total = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_overlap_pairs_dev_{self._d['suffix']}")(self._h, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr or None),
+                                                                                       cap, C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
     def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
         """Bvh::nearest_to / FlatBvh::nearest_to (bvh_impl.rs:221-238, flat_bvh.rs:513-562) for shapes whose PointDistance is their AABB
         distance (the reference's UnitBox): (shape index per point, U32_MAX for an empty tree; distance per point)."""
@@ -623,6 +648,12 @@ class Bvh2:
         fn = getattr(capi.lib(), f"bvhgpu_query_{self._d['suffix']}")
         return self._csr_call(fn, len(q), max(16 * len(q), 1024), self._h, mode, kind, _ptr(q), len(q))
 
+    def overlap_pairs(self, cap: int | None = None):
+        """Every pair of shapes whose own current AABBs intersect, each once, with the contract of Bvh.overlap_pairs: CSR (offsets[n + 1],
+        hits) indexed by shape.  A short capacity (default max(4 n, 1024)) is retried once at the exact total."""
+        fn = getattr(capi.lib(), f"bvhgpu_overlap_pairs_{self._d['suffix']}")
+        return self._csr_call(fn, self.n, max(4 * self.n, 1024) if cap is None else int(cap), self._h)
+
     def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
         """Bvh::nearest_to / FlatBvh::nearest_to for shapes whose distance is their AABB's: (shape index per point, U32_MAX for an
         empty tree; distance per point).  points: (n, D)."""
@@ -779,6 +810,14 @@ class Bvh4(Bvh2):
         fn = getattr(capi.lib(), f"bvhgpu_query_dev_{self._d['suffix']}")
         capi.check(fn(self._h, mode, kind, C.c_void_p(queries_ptr), n, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
                       C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
+    def overlap_pairs_dev(self, offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
+        """overlap_pairs into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets are
+        always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        total = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_overlap_pairs_dev_{self._d['suffix']}")(self._h, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr or None),
+                                                                                       cap, C.byref(total) if want_total else None))
         return total.value if want_total else None
 
     def closest_hit_dev(self, rays_ptr: int, nrays: int, shape_ptr: int, dist_ptr: int):

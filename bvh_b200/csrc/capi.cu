@@ -418,6 +418,53 @@ static int query_dev_impl(TreeOf<D, T>* tree, int mode, int kind, const void* d_
     return rc;
 }
 
+// Self-overlap pairs, host pointers.  D = 2, 3: overlap_device into the retained buffers (bvhgpu_traverse_fetch_* reads them in 3-D).
+// D = 4: overlap4_host.  n < 2: all-zero offsets, no device work.
+template <int D, class T>
+static int overlap_host_impl(TreeOf<D, T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+    if (!tree || !offsets) { set_error("overlap_pairs: null argument"); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    const size_t n = tree->n;
+    if (n < 2) {
+        std::fill(offsets, offsets + n + 1, 0u);
+        if (total) *total = 0;
+        if constexpr (D != 4) tree->last_total = 0;
+        return BVHGPU_OK;
+    }
+    if constexpr (D == 4) {
+        return overlap4_host<T>(tree, offsets, hits, cap, total);
+    } else {
+        return retained_to_host<D>(tree, "overlap_pairs", n, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+            const int rc = overlap_device<T>(tree, d_off, d_hits, hcap, t);
+            if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) tree->last_total = *t;
+            return rc;
+        });
+    }
+}
+// Self-overlap pairs, device pointers (D = 3, 4), on the context's stream.  With `total` the call returns once the total is known
+// and the CSR is complete.
+template <int D, class T>
+static int overlap_dev_impl(TreeOf<D, T>* tree, void* d_offsets, void* d_hits, size_t cap, size_t* total) {
+    if (!tree || !d_offsets) { set_error("overlap_pairs_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    int rc;
+    if constexpr (D == 4) {
+        BVH_TRY(resolve_status(tree));
+        if (tree->n < 2) {
+            BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (tree->n + 1), tree->ctx->stream));
+            if (total) *total = 0;
+            return BVHGPU_OK;
+        }
+        rc = overlap4_device<T>(tree, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
+    } else {
+        rc = overlap_device<T>(tree, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
+    }
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
+    return rc;
+}
+
 // nearest_to, host pointers: D T per point.  The mode of a 3-D call is checked by nearest_device.
 template <int D, class T>
 static int nearest_host_impl(TreeOf<D, T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist, int use_triangles = 0) {
@@ -1354,6 +1401,12 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
                                           void* dev_hits, size_t cap, size_t* total) {                                    \
         return query_dev_impl<3, T>(tree, mode, kind, dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
     }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_overlap_pairs_##SUF(TREE* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) { \
+        return overlap_host_impl<3, T>(tree, offsets, hits, cap, total);                                                  \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_overlap_pairs_dev_##SUF(TREE* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
+        return overlap_dev_impl<3, T>(tree, dev_offsets, dev_hits, cap, total);                                           \
+    }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<3, T>(tree, mode, points, n, out_shape, out_dist);                                         \
     }                                                                                                                     \
@@ -1484,6 +1537,9 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
                                       size_t cap, size_t* total) {                                                        \
         return query_host_impl<2, T>(tree, mode, kind, queries, n, offsets, hits, cap, total);                             \
     }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_overlap_pairs_##SUF(TREE* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {  \
+        return overlap_host_impl<2, T>(tree, offsets, hits, cap, total);                                                   \
+    }                                                                                                                      \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<2, T>(tree, mode, points, n, out_shape, out_dist);                                        \
     }                                                                                                                      \
@@ -1550,6 +1606,12 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_query_dev_##SUF(TREE* tree, int mode, int kind, const void* dev_queries, size_t n,              \
                                           void* dev_offsets, void* dev_hits, size_t cap, size_t* total) {                 \
         return query_dev_impl<4, T>(tree, mode, kind, dev_queries, n, (uint32_t*)dev_offsets, (uint32_t*)dev_hits, cap, total); \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_overlap_pairs_##SUF(TREE* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {  \
+        return overlap_host_impl<4, T>(tree, offsets, hits, cap, total);                                                   \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_overlap_pairs_dev_##SUF(TREE* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
+        return overlap_dev_impl<4, T>(tree, dev_offsets, dev_hits, cap, total);                                            \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<4, T>(tree, mode, points, n, out_shape, out_dist);                                        \

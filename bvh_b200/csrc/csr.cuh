@@ -1,6 +1,6 @@
 // bvh_b200/csrc/csr.cuh -- the two-pass CSR walk that every batched walk except the 3-D ray traversal produces its hit lists with:
 // the traversal records of D = 3 and D = 4 and their fetch, the record walk generic in D, the count / fill kernel, the ordered
-// traversal's kernel, and the host driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries, nearest_candidates and the
+// traversal's kernel, the self-overlap kernel, and the host driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries, nearest_candidates and the
 // ordered traversal, D = 2 through the z = 0 lift) and dim4.cu (D = 4 rays, queries, nearest_candidates and the ordered traversal).
 // The 3-D ray kernels of traverse.cu use the same fetch.
 //
@@ -187,6 +187,71 @@ __global__ void __launch_bounds__(256) ordered_kernel(const typename CsrRecords<
     }
 }
 
+// ---- self-overlap (bvhgpu_overlap_pairs_*): row s lists every shape t with leaf(t) > leaf(s) whose own box intersects s's own box
+// (Aabb::intersects_aabb: for every axis !(a.max < b.min || b.max < a.min)), in DFS order.  Record r is node r + 1, so the walk of s
+// starts at record leaf(s), the node right after s's leaf in preorder: every node it can reach lies after the leaf, and each pair is
+// found once, by whichever leaf comes first.  A record is entered when its box intersects s's box or has min > max on some axis (the
+// Aabb::empty() child box of a "no split wins" node); every other record box contains the boxes of the shapes below it, so a miss
+// prunes no pair.  Thread k walks the shape of leaf rank k (order[k], neighbouring threads walk neighbouring leaves); its row is
+// written at the shape's scanned offset.  Count pass (FILL = false) and fill pass as csr_walk_kernel.
+template <int D, class T>
+__device__ __forceinline__ bool overlap_enter(const T smn[D], const T smx[D], const T mn[D], const T mx[D]) {
+    bool hit = true, empty = false;
+#pragma unroll
+    for (int k = 0; k < D; ++k) {
+        hit = hit && !(smx[k] < mn[k] || mx[k] < smn[k]);
+        empty = empty || mn[k] > mx[k];
+    }
+    return hit || empty;
+}
+template <int D, class T>
+__device__ __forceinline__ bool overlap_boxes(const T smn[D], const T smx[D], const T mn[D], const T mx[D]) {
+    bool hit = true;
+#pragma unroll
+    for (int k = 0; k < D; ++k) hit = hit && !(smx[k] < mn[k] || mx[k] < smn[k]);
+    return hit;
+}
+template <int D, class T, bool FILL>
+__global__ void __launch_bounds__(256) overlap_kernel(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                                      const typename CsrRecords<D, T>::Box* __restrict__ aabb, const uint32_t* __restrict__ node_index,
+                                                      const uint32_t* __restrict__ order, uint32_t n, uint32_t* __restrict__ counts,
+                                                      const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
+                                                      const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets,
+                                                      uint32_t* __restrict__ hits, unsigned long long cap) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (FILL && k == 0) { const unsigned long long t = *total; offsets[n] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
+    if (k >= n) return;
+    const uint32_t s = __ldg(order + k);
+    T smn[D], smx[D];
+    load_box(aabb + s, smn, smx);
+    unsigned long long w = 0;
+    if (FILL) {
+        w = blocksum[s / CSR_SCAN_TILE] + local[s];
+        offsets[s] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
+        if (!hits) return;                                        // offsets only
+    }
+    uint32_t cnt = 0, i = __ldg(node_index + s);
+    while (i < n_rec) {
+        T mn[D], mx[D];
+        uint32_t skip, shape;
+        fetch(trec + i, mn, mx, skip, shape);
+        if (overlap_enter<D, T>(smn, smx, mn, mx)) {
+            if (shape != BVH_INVALID) {
+                T tmn[D], tmx[D];
+                load_box(aabb + shape, tmn, tmx);
+                if (overlap_boxes<D, T>(smn, smx, tmn, tmx)) {
+                    if (FILL) { if (w < cap) hits[w] = shape; ++w; }
+                    else ++cnt;
+                }
+            }
+            ++i;
+        } else {
+            i = skip;
+        }
+    }
+    if (!FILL) counts[s] = cnt;
+}
+
 // ---- host: count -> scan -> fill ----
 // A walk is what the driver launches: walk.count(stream, n, counts) enqueues the count pass, walk.fill(stream, n, local, sums, total,
 // offsets, hits, cap) the fill pass.  CsrWalk is the one of csr_walk_kernel, OrderedWalk the one of ordered_kernel.
@@ -218,6 +283,21 @@ template <int D, class T> struct OrderedWalk {
     void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
               uint32_t* offsets, uint32_t* hits, size_t cap) const {
         ordered_kernel<D, T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, rays, n, ascending, nullptr, local, sums, total, offsets, hits, dists, (unsigned long long)cap);
+    }
+};
+// The walk of overlap_kernel over the tree's n shapes (n >= 2).  order: the shapes in leaf order (leaf_order_kernel).
+template <int D, class T> struct OverlapWalk {
+    const typename CsrRecords<D, T>::Rec* trec;
+    uint32_t n_rec;
+    const typename CsrRecords<D, T>::Box* aabb;       // the shapes' own boxes (D = 2: z = [0, 0])
+    const uint32_t* node_index;
+    const uint32_t* order;
+    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const {
+        overlap_kernel<D, T, false><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb, node_index, order, n, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    }
+    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
+              uint32_t* offsets, uint32_t* hits, size_t cap) const {
+        overlap_kernel<D, T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb, node_index, order, n, nullptr, local, sums, total, offsets, hits, (unsigned long long)cap);
     }
 };
 

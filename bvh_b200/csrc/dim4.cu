@@ -797,20 +797,13 @@ template <class P, class T> static int csr4_dev(Tree4<T>* tree, bool flat, const
     return csr_two_pass(ctx, walk, (uint32_t)n, what, d_offsets, d_hits, cap, total);
 }
 
-// Host CSR out of a batch already on the device (d_src, n > 0, tree->n > 0): count, read the total, size the retained hit buffer
-// exactly, fill, copy back.  Hits that do not fit `cap` are not copied; offsets and *total are, and the call returns
-// BVHGPU_ERR_CAPACITY -- the caller's second call with cap = *total is the only extra walk.
-template <class P, class T> static int csr4_host_p(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
-                                                   size_t cap, size_t* total, const char* what) {
+// Host CSR out of n > 0 items of a walk over the records: count, read the total, size the retained hit buffer exactly, fill, copy
+// back.  Hits that do not fit `cap` are not copied; offsets and *total are, and the call returns BVHGPU_ERR_CAPACITY -- the caller's
+// second call with cap = *total is the only extra walk.
+template <class Walk, class T> static int csr4_host_walk(Tree4<T>* tree, const Walk& walk, size_t n, uint32_t* offsets, uint32_t* hits,
+                                                         size_t cap, size_t* total, const char* what) {
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
-    if (n == 0 || tree->n == 0) {                                  // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
-        std::fill(offsets, offsets + n + 1, 0u);
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    BVH_TRY(ensure_trec4(tree));
-    const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
     CsrPasses passes(ctx, (uint32_t)n);
     BVH_TRY(passes.count_and_scan(walk, true));
     size_t tot = 0;
@@ -825,6 +818,43 @@ template <class P, class T> static int csr4_host_p(Tree4<T>* tree, bool flat, co
     BVH_CUDA_TRY(cudaStreamSynchronize(st));
     if (tot > cap) { set_error("%s: %zu hits do not fit the caller's capacity %zu (call again with cap = *total)", what, tot, cap); return BVHGPU_ERR_CAPACITY; }
     return BVHGPU_OK;
+}
+// The CSR of a batch already on the device (d_src): n = 0 or an empty tree give all-zero offsets with no device work.
+template <class P, class T> static int csr4_host_p(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
+                                                   size_t cap, size_t* total, const char* what) {
+    if (n == 0 || tree->n == 0) {                                  // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
+        std::fill(offsets, offsets + n + 1, 0u);
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    BVH_TRY(ensure_trec4(tree));
+    const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
+    return csr4_host_walk(tree, walk, n, offsets, hits, cap, total, what);
+}
+
+// ---- self-overlap: overlap_kernel<4, T> of csr.cuh over the records and the ABI boxes (n >= 2; the caller handles n < 2).  The
+// shapes in leaf order live as long as the call (released stream-ordered after the fill). ----
+template <class T> static int overlap4_order(Tree4<T>* tree, Scratch& scratch, uint32_t** order) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_TRY(ensure_trec4(tree));
+    BVH_TRY(scratch.get(order, tree->n));
+    leaf_order_kernel<<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_node_index, tree->d_node_start, tree->n, *order);
+    LAUNCHED(ctx, 1);
+    return BVHGPU_OK;
+}
+template <class T> int overlap4_device(Tree4<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
+    Scratch scratch(tree->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(overlap4_order(tree, scratch, &order));
+    const OverlapWalk<4, T> walk{tree->d_trec, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
+    return csr_two_pass(tree->ctx, walk, tree->n, "overlap_pairs_dev", d_offsets, d_hits, cap, total);
+}
+template <class T> int overlap4_host(Tree4<T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+    Scratch scratch(tree->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(overlap4_order(tree, scratch, &order));
+    const OverlapWalk<4, T> walk{tree->d_trec, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
+    return csr4_host_walk(tree, walk, tree->n, offsets, hits, cap, total, "overlap_pairs");
 }
 
 // The probe of a CSR walk: rays, or one of the public query kinds.
@@ -1012,7 +1042,9 @@ template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* roots, con
     template int nearest4_device<T>(Tree4<T>*, int, const T*, size_t, uint32_t*, T*);                                               \
     template int ordered4_device<T>(Tree4<T>*, const void*, size_t, int, uint32_t*, uint32_t*, T*, size_t, size_t*);               \
     template int knn4_device<T>(Tree4<T>*, const T*, size_t, uint32_t, const T*, uint32_t*, T*);                                    \
-    template int refresh_caches<T>(Tree4<T>*);                                                                                      \
+    template int overlap4_device<T>(Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                                              \
+    template int overlap4_host<T>(Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                                                \
+    template int refresh_caches<T>(Tree4<T>*);                                                                                    \
     template int finish_relayout<T>(Tree4<T>*);                                                                                     \
     template int rebuild_degraded<T>(Tree4<T>*, const uint32_t*, uint32_t*, size_t*, const char*);                                  \
     template int build_subtrees<T>(Tree4<T>*, const uint32_t*, const uint32_t*, uint32_t, const Traits<T>::Key*, uint32_t*, const char*);

@@ -209,6 +209,9 @@ template <class T> int build_flat(Tree<T>* tree);                // d_flat (refe
 int build_top_records(Tree<float>* tree, uint32_t budget);        // d_top
 template <class T> int sah_cost(Tree<T>* tree, double* out2);
 template <class T> int optimize(Tree<T>* tree, double max_growth);   // refit + exact rebuild of the degraded subtrees
+// idx[node_start[node_index[s]]] = s for s < n: the shapes in leaf (DFS) order, of a 3-D or a 4-D tree
+__global__ void __launch_bounds__(256) leaf_order_kernel(const uint32_t* __restrict__ node_index, const uint32_t* __restrict__ node_start,
+                                                         uint32_t n, uint32_t* __restrict__ idx);
 // Caches after the boxes changed in place (node count unchanged, dynamic.cu): the FLAT leaf boxes of a 2-D tree first (the records
 // read them), then the traversal records, then the flat array if it was built.
 template <class T> int refresh_caches(Tree<T>* tree);
@@ -252,6 +255,9 @@ template <class T> int traverse_host_pipelined(Tree<T>* tree, int mode, const vo
 // hits sorted by entry (ascending) / exit (descending) distance, with the distances; device pointers
 template <class T> int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays, size_t nrays, int ascending,
                                                uint32_t* d_offsets, uint32_t* d_hits, T* d_dists, size_t cap, size_t* total);
+// Every pair of shapes whose own boxes intersect, once, in the row of the earlier leaf (bvhgpu_overlap_pairs_*); device pointers, on
+// the context's stream, synchronises only to return *total.  Checks the tree's status; n < 2 gives all-zero offsets.
+template <class T> int overlap_device(Tree<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
 // Aabb / Point / Ball queries (device pointers); two-pass count / fill.
 template <class T> int query_device(Tree<T>* tree, int mode, int kind, const T* d_queries, size_t nq, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
 // nearest_to for a batch of points (device pointers): exact reference walk for AABB-distance shapes; candidate lists for any shape
@@ -373,6 +379,10 @@ template <class T> int nearest4_device(Tree4<T>* tree, int mode, const T* d_poin
 // distance-ordered traversal (rays of 12 T); n = 0 or an empty tree give all-zero offsets.
 template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_t nrays, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
                                        T* d_dists, size_t cap, size_t* total);
+// self-overlap pairs (overlap_device's contract) of a tree with n >= 2 shapes, status checked by the caller: overlap4_device to device
+// pointers (synchronises only to return *total), overlap4_host to host pointers through the retained buffers, as csr4_host.
+template <class T> int overlap4_device(Tree4<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
+template <class T> int overlap4_host(Tree4<T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
 // k nearest shapes: checks n, k and the tree's status, as knn_device does.
 template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
 // The 4-D overloads of the steps the dynamic drivers of dynamic.cu leave to the tree type (the 3-D ones are declared above):

@@ -1645,6 +1645,32 @@ int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays
 template int traverse_ordered_device<float>(Tree<float>*, const bvh_ray3f*, size_t, int, uint32_t*, uint32_t*, float*, size_t, size_t*);
 template int traverse_ordered_device<double>(Tree<double>*, const bvh_ray3d*, size_t, int, uint32_t*, uint32_t*, double*, size_t, size_t*);
 
+// ---- self-overlap: overlap_kernel<3, T> of csr.cuh over the 3-D records and the shapes' own boxes.  A 2-D tree tests d_aabb
+// (z = [0, 0]) and walks the records of its embedding, whose z = [-1, +1] contains that slab. ----
+template <class T>
+int overlap_device(Tree<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_TRY(resolve_status(tree));
+    const uint32_t n = tree->n;
+    if (n < 2) {
+        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (n + 1), st));
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
+    Scratch scratch(ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(scratch.get(&order, n));
+    leaf_order_kernel<<<(n + 255) / 256, 256, 0, st>>>(tree->d_node_index, tree->d_node_start, n, order);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    const OverlapWalk<3, T> walk{tree->d_tnodes, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
+    return csr_two_pass(ctx, walk, n, "overlap_pairs", d_offsets, d_hits, cap, total);
+}
+template int overlap_device<float>(Tree<float>*, uint32_t*, uint32_t*, size_t, size_t*);
+template int overlap_device<double>(Tree<double>*, uint32_t*, uint32_t*, size_t, size_t*);
+
 // ---- Ray::new for a batch (src/ray/ray_impl.rs:70-80) -------------------------------------------------
 template <class T> __device__ __forceinline__ T sqrt_rn(T x);
 template <> __device__ __forceinline__ float sqrt_rn(float x) { return __fsqrt_rn(x); }

@@ -637,6 +637,39 @@ int bvhgpu_multi_hit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_rays, size_t
 int bvhgpu_multi_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t nrays, uint32_t k, const void* dev_tmax, void* dev_shape,
                                void* dev_dist);
 
+/* ---- self-overlap pairs: every pair of shapes of the tree whose AABBs intersect, each once (the broad phase of physics, mesh
+ * self-intersection, duplicate and contact detection in point and particle sets).  leaf(s) = the preorder node index of shape s's leaf
+ * (out_node_index of bvhgpu_tree_nodes_*).  Output: a CSR indexed by shape, offsets[n + 1]; row s lists every shape t with
+ * leaf(t) > leaf(s) and intersects(box_s, box_t), in ascending leaf(t) order (DFS order).
+ *   intersects = Aabb::intersects_aabb (src/aabb/aabb_impl.rs:240-248): for every axis !(a.max < b.min || b.max < a.min).  Touching
+ *   faces overlap; an empty box (min > max) overlaps no finite box; an inverted finite box follows the formula literally.  The boxes are
+ *   the shapes' own current boxes: from the build or the latest refit, update_shapes or add_shapes, in the numbering after
+ *   remove_shapes.  Each unordered pair {s, t}, s != t, appears exactly once, in the row of whichever leaf comes first; no shape is
+ *   paired with itself.
+ *   EXACT (equal to the brute force over all pairs) for every tree the library builds or maintains, every build mode, after refit /
+ *   update_shapes / add_shapes / remove_shapes, on overflow-scale, infinite, coincident and subnormal boxes: a record is entered when
+ *   its box intersects box_s or has min > max on some axis (the Aabb::empty() child box of a "no split wins" node); every other stored
+ *   child box contains the boxes of the shapes below it, and containment makes the test monotone.  For a tree from
+ *   bvhgpu_tree_from_nodes_* the result is exact only when the caller's node boxes contain their shapes (or are empty); otherwise it
+ *   is a subset of the true pairs, still each pair at most once.
+ *   Capacity as bvhgpu_query_*: the offsets are always complete; the hits are copied when they fit `cap`, else BVHGPU_ERR_CAPACITY
+ *   with *total (in 3-D bvhgpu_traverse_fetch_* then fetches the retained list; in 2-D and 4-D call again with cap = *total).  The
+ *   _dev forms (D = 3, 4) take device pointers and enqueue on the context's stream; `total` may be NULL (nothing synchronises), and
+ *   dev_hits receives a prefix of length cap.  Offsets saturate at 0xFFFFFFFF; a total above 2^32-1 returns BVHGPU_ERR_CAPACITY
+ *   (with the saturated offsets in the _dev forms, with *total only in the host forms).
+ *   n = 0 and n = 1: all-zero offsets.  A null tree or offsets pointer: BVHGPU_ERR_INVALID, nothing written.  A failed build is
+ *   reported sticky first. */
+int bvhgpu_overlap_pairs_f32x2(bvhgpu_tree2f* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_f64x2(bvhgpu_tree2d* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_f32x3(bvhgpu_tree3f* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_f64x3(bvhgpu_tree3d* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_f32x4(bvhgpu_tree4f* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_f64x4(bvhgpu_tree4d* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_dev_f32x3(bvhgpu_tree3f* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_dev_f64x3(bvhgpu_tree3d* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_dev_f32x4(bvhgpu_tree4f* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_overlap_pairs_dev_f64x4(bvhgpu_tree4d* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
  * leaves (user code), so there are two forms.  `points`: 3 T per query point, host pointers.

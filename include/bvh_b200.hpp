@@ -17,6 +17,7 @@
 // implement `aabb()` for their shapes (they are not a CPU fallback for the path).
 #pragma once
 #include <cmath>
+#include <algorithm>
 #include <cstdint>
 #include <limits>
 #include <memory>
@@ -103,6 +104,7 @@ template <> struct Abi<float> {
     static int multi(tree* t, const ray* r, size_t n, uint32_t k, const float* tm, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_multi_hit_f32x3(t, r, n, k, tm, tri, s, d, uv); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f32x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
+    static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f32x3(t, off, h, cap, tot); }
 };
 template <> struct Abi<double> {
     using aabb = bvh_aabb3d; using ray = bvh_ray3d; using node = bvh_node3d; using flat = bvh_flat3d; using tree = bvhgpu_tree3d;
@@ -122,6 +124,7 @@ template <> struct Abi<double> {
     static int multi(tree* t, const ray* r, size_t n, uint32_t k, const double* tm, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_multi_hit_f64x3(t, r, n, k, tm, tri, s, d, uv); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f64x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
+    static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f64x3(t, off, h, cap, tot); }
 };
 struct Ctx {
     bvhgpu_ctx* h = nullptr;
@@ -265,6 +268,16 @@ template <class T> class Bvh {
     // Bvh::traverse_iterator (src/bvh/bvh_impl.rs:128-134): same sequence; the "iterator" is the returned vector's range.
     template <class Shape> std::vector<const Shape*> traverse_iterator(const Ray<T>& ray, const std::vector<Shape>& shapes) const { return traverse(ray, shapes); }
 
+    // every pair of shapes whose current AABBs intersect, each once: CSR indexed by shape, row s = the shapes whose leaf comes after
+    // s's leaf in DFS order and whose box meets s's box (bvhgpu_overlap_pairs_*).  offsets gets n + 1 entries.
+    void overlap_pairs(std::vector<uint32_t>& offsets, std::vector<uint32_t>& hits) const {
+        offsets.assign(n_ + 1, 0);
+        hits.resize(std::max<size_t>(4 * n_, 1024));
+        size_t total = 0;
+        const int st = A::overlap(tree_, offsets.data(), hits.data(), hits.size(), &total);
+        if (st == BVHGPU_ERR_CAPACITY && total <= UINT32_MAX) { hits.resize(total); check(A::fetch(tree_, hits.data(), total)); }
+        else { check(st); hits.resize(total); }
+    }
     // the data-parallel part of Bvh::update_shapes (src/bvh/optimization.rs:304-351): refit after shapes moved
     template <class Shape> void refit(const std::vector<Shape>& shapes) {
         std::vector<typename A::aabb> boxes(shapes.size());

@@ -99,6 +99,25 @@ for prec in ("f32", "f64"):
     b4.any_hit_dev(dr.data_ptr(), 300, dd.data_ptr(), ds.data_ptr()); b4.any_hit_dev(dr.data_ptr(), 300, 0, ds.data_ptr()); ctx.synchronize()
     b4.multi_hit(r4, 3); b4.multi_hit(r4, 40, np.full(300, 50.0)); b4.multi_hit_dev(dr.data_ptr(), 300, 1, 0, ds.data_ptr(), dd.data_ptr()); ctx.synchronize()
     b4.free()
+# self-overlap pairs: host and device forms in D = 2, 3, 4, a short capacity (fetch / retry), an overflow-scale scene
+for prec in ("f32", "f64"):
+    import torch
+    for D, cls in ((2, api.Bvh2), (3, api.Bvh), (4, api.Bvh4)):
+        lo = rng.uniform(-50, 50, (800, D))
+        bo = np.zeros(len(lo), dtype=(cls._TABLE[prec] if D != 3 else api.BY_PREC[prec])["aabb"])
+        bo["min"], bo["max"] = lo, lo + rng.uniform(0, 6, (len(lo), D))
+        bt = cls.build(bo, prec=prec)
+        po, ph = bt.overlap_pairs()
+        bt.overlap_pairs(cap=len(ph) // 2)
+        if D != 2:
+            d_o = torch.zeros(len(lo) + 1, dtype=torch.int32, device="cuda:0"); d_h = torch.zeros(len(ph), dtype=torch.int32, device="cuda:0")
+            bt.overlap_pairs_dev(d_o.data_ptr(), d_h.data_ptr(), len(ph) // 3); bt.overlap_pairs_dev(d_o.data_ptr(), d_h.data_ptr(), len(ph), True)
+        bo["min"], bo["max"] = lo * 1e30, lo * 1e30 + 1e29
+        bt.free()
+        bt = cls.build(bo, prec=prec)
+        bt.overlap_pairs()
+        print("  overlap", prec, D, len(ph))
+        bt.free()
 # host path on a batch large enough to be chunked (under the sanitizer the library takes the copy-then-walk form; forced streaming too)
 a = scenes.create_n_cubes_aabbs(300)
 b = api.Bvh.build(a)
