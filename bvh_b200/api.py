@@ -30,6 +30,14 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def _same_kind(a, b):
+    """The two trees of an overlap_pairs_with call: the same class (so the same dimension) and the same precision."""
+    if type(a) is not type(b):
+        raise TypeError(f"overlap_pairs_with: {type(a).__name__} against {type(b).__name__}")
+    if a.prec != b.prec:
+        raise ValueError(f"overlap_pairs_with: {a.prec} tree against a {b.prec} tree")
+
+
 class Context:
     """One per device (stream + scratch pool)."""
 
@@ -411,6 +419,35 @@ class Bvh:
                                                                                        cap, C.byref(total) if want_total else None))
         return total.value if want_total else None
 
+    def overlap_pairs_with(self, other: "Bvh", cap: int | None = None):
+        """Every pair (a, b) of a shape of this tree and a shape of `other` whose own current AABBs intersect (touching faces included):
+        CSR (offsets[n + 1], hits) indexed by this tree's shapes, row a = other's shapes whose box meets a's, in other's DFS order.
+        Both trees must share a context; other may be self.  A short capacity (default max(4 n, 1024)) is completed from this
+        tree's retained list (bvhgpu_traverse_fetch_*)."""
+        _same_kind(self, other)
+        n = self.num_shapes
+        offsets = np.zeros(n + 1, dtype=np.uint32)
+        cap = max(4 * n, 1024) if cap is None else int(cap)
+        hits = np.zeros(cap, dtype=np.uint32)
+        total = C.c_size_t(0)
+        st = getattr(capi.lib(), f"bvhgpu_overlap_trees_{self._d['suffix']}")(self._h, other._h, _ptr(offsets), _ptr(hits), cap, C.byref(total))
+        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
+            hits = np.zeros(total.value, dtype=np.uint32)
+            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), total.value))
+        else:
+            capi.check(st)
+        return offsets, hits[: total.value]
+
+    def overlap_pairs_with_dev(self, other: "Bvh", offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
+        """overlap_pairs_with into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets
+        are always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        _same_kind(self, other)
+        total = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_overlap_trees_dev_{self._d['suffix']}")(self._h, other._h, C.c_void_p(offsets_ptr),
+                                                                                       C.c_void_p(hits_ptr or None), cap,
+                                                                                       C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
     def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
         """Bvh::nearest_to / FlatBvh::nearest_to (bvh_impl.rs:221-238, flat_bvh.rs:513-562) for shapes whose PointDistance is their AABB
         distance (the reference's UnitBox): (shape index per point, U32_MAX for an empty tree; distance per point)."""
@@ -654,6 +691,14 @@ class Bvh2:
         fn = getattr(capi.lib(), f"bvhgpu_overlap_pairs_{self._d['suffix']}")
         return self._csr_call(fn, self.n, max(4 * self.n, 1024) if cap is None else int(cap), self._h)
 
+    def overlap_pairs_with(self, other, cap: int | None = None):
+        """Every pair (a, b) of a shape of this tree and a shape of `other` whose own current AABBs intersect, with the contract of
+        Bvh.overlap_pairs_with: CSR (offsets[n + 1], hits) indexed by this tree's shapes.  A short capacity (default max(4 n, 1024))
+        is retried once at the exact total."""
+        _same_kind(self, other)
+        fn = getattr(capi.lib(), f"bvhgpu_overlap_trees_{self._d['suffix']}")
+        return self._csr_call(fn, self.n, max(4 * self.n, 1024) if cap is None else int(cap), self._h, other._h)
+
     def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
         """Bvh::nearest_to / FlatBvh::nearest_to for shapes whose distance is their AABB's: (shape index per point, U32_MAX for an
         empty tree; distance per point).  points: (n, D)."""
@@ -818,6 +863,16 @@ class Bvh4(Bvh2):
         total = C.c_size_t(0)
         capi.check(getattr(capi.lib(), f"bvhgpu_overlap_pairs_dev_{self._d['suffix']}")(self._h, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr or None),
                                                                                        cap, C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
+    def overlap_pairs_with_dev(self, other: "Bvh4", offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
+        """overlap_pairs_with into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets
+        are always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        _same_kind(self, other)
+        total = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_overlap_trees_dev_{self._d['suffix']}")(self._h, other._h, C.c_void_p(offsets_ptr),
+                                                                                       C.c_void_p(hits_ptr or None), cap,
+                                                                                       C.byref(total) if want_total else None))
         return total.value if want_total else None
 
     def closest_hit_dev(self, rays_ptr: int, nrays: int, shape_ptr: int, dist_ptr: int):

@@ -182,8 +182,10 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
     for s in ("f32x2", "f64x2", "f32x3", "f64x3", "f32x4", "f64x4"):
         getattr(L, f"bvhgpu_overlap_pairs_{s}").argtypes = [vp, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_overlap_trees_{s}").argtypes = [vp, vp, vp, vp, sz, szp]
     for s in ("f32x3", "f64x3", "f32x4", "f64x4"):
         getattr(L, f"bvhgpu_overlap_pairs_dev_{s}").argtypes = [vp, vp, vp, sz, szp]
+        getattr(L, f"bvhgpu_overlap_trees_dev_{s}").argtypes = [vp, vp, vp, vp, sz, szp]
     missing =[n for n in declared_symbols() if not hasattr(L, n)]
     if missing:
         raise ImportError(f"{SO_PATH} does not export {missing}")

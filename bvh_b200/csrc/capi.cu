@@ -465,6 +465,61 @@ static int overlap_dev_impl(TreeOf<D, T>* tree, void* d_offsets, void* d_hits, s
     return rc;
 }
 
+// Overlap between two trees: the arguments of both forms.  The trees must share a context, whose one stream then orders the walk
+// after every call pending on either tree.
+template <class Tr> static int overlap_trees_args(const char* what, const Tr* a, const Tr* b, const void* offsets) {
+    if (!a || !b || !offsets) { set_error("%s: null argument", what); return BVHGPU_ERR_INVALID; }
+    if (a->ctx != b->ctx) { set_error("%s: the two trees belong to different contexts", what); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+// Overlap between two trees, host pointers.  D = 2, 3: overlap_trees_device into A's retained buffers (bvhgpu_traverse_fetch_* on A
+// reads them in 3-D).  D = 4: overlap_trees4_host.  n_a = 0 or n_b = 0: all-zero offsets, no device work.
+template <int D, class T>
+static int overlap_trees_host_impl(TreeOf<D, T>* a, TreeOf<D, T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+    BVH_TRY(overlap_trees_args("overlap_trees", a, b, offsets));
+    BVH_CUDA_TRY(cudaSetDevice(a->ctx->device));
+    BVH_TRY(resolve_status(a));
+    BVH_TRY(resolve_status(b));
+    const size_t n = a->n;
+    if (n == 0 || b->n == 0) {
+        std::fill(offsets, offsets + n + 1, 0u);
+        if (total) *total = 0;
+        if constexpr (D != 4) a->last_total = 0;
+        return BVHGPU_OK;
+    }
+    if constexpr (D == 4) {
+        return overlap_trees4_host<T>(a, b, offsets, hits, cap, total);
+    } else {
+        return retained_to_host<D>(a, "overlap_trees", n, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+            const int rc = overlap_trees_device<T>(a, b, d_off, d_hits, hcap, t);
+            if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) a->last_total = *t;
+            return rc;
+        });
+    }
+}
+// Overlap between two trees, device pointers (D = 3, 4), on the context's stream.  With `total` the call returns once the total is
+// known and the CSR is complete.
+template <int D, class T>
+static int overlap_trees_dev_impl(TreeOf<D, T>* a, TreeOf<D, T>* b, void* d_offsets, void* d_hits, size_t cap, size_t* total) {
+    BVH_TRY(overlap_trees_args("overlap_trees_dev", a, b, d_offsets));
+    BVH_CUDA_TRY(cudaSetDevice(a->ctx->device));
+    int rc;
+    if constexpr (D == 4) {
+        BVH_TRY(resolve_status(a));
+        BVH_TRY(resolve_status(b));
+        if (a->n == 0 || b->n == 0) {
+            BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (a->n + 1), a->ctx->stream));
+            if (total) *total = 0;
+            return BVHGPU_OK;
+        }
+        rc = overlap_trees4_device<T>(a, b, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
+    } else {
+        rc = overlap_trees_device<T>(a, b, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
+    }
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
+    return rc;
+}
+
 // nearest_to, host pointers: D T per point.  The mode of a 3-D call is checked by nearest_device.
 template <int D, class T>
 static int nearest_host_impl(TreeOf<D, T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist, int use_triangles = 0) {
@@ -1407,6 +1462,12 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_overlap_pairs_dev_##SUF(TREE* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
         return overlap_dev_impl<3, T>(tree, dev_offsets, dev_hits, cap, total);                                           \
     }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_overlap_trees_##SUF(TREE* a, TREE* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) { \
+        return overlap_trees_host_impl<3, T>(a, b, offsets, hits, cap, total);                                            \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_overlap_trees_dev_##SUF(TREE* a, TREE* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
+        return overlap_trees_dev_impl<3, T>(a, b, dev_offsets, dev_hits, cap, total);                                     \
+    }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<3, T>(tree, mode, points, n, out_shape, out_dist);                                         \
     }                                                                                                                     \
@@ -1540,6 +1601,9 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     BVH_EXPORT int bvhgpu_overlap_pairs_##SUF(TREE* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {  \
         return overlap_host_impl<2, T>(tree, offsets, hits, cap, total);                                                   \
     }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_overlap_trees_##SUF(TREE* a, TREE* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) { \
+        return overlap_trees_host_impl<2, T>(a, b, offsets, hits, cap, total);                                             \
+    }                                                                                                                      \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<2, T>(tree, mode, points, n, out_shape, out_dist);                                        \
     }                                                                                                                      \
@@ -1612,6 +1676,12 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_overlap_pairs_dev_##SUF(TREE* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
         return overlap_dev_impl<4, T>(tree, dev_offsets, dev_hits, cap, total);                                            \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_overlap_trees_##SUF(TREE* a, TREE* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) { \
+        return overlap_trees_host_impl<4, T>(a, b, offsets, hits, cap, total);                                             \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_overlap_trees_dev_##SUF(TREE* a, TREE* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
+        return overlap_trees_dev_impl<4, T>(a, b, dev_offsets, dev_hits, cap, total);                                      \
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<4, T>(tree, mode, points, n, out_shape, out_dist);                                        \

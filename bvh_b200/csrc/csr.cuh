@@ -1,6 +1,6 @@
 // bvh_b200/csrc/csr.cuh -- the two-pass CSR walk that every batched walk except the 3-D ray traversal produces its hit lists with:
 // the traversal records of D = 3 and D = 4 and their fetch, the record walk generic in D, the count / fill kernel, the ordered
-// traversal's kernel, the self-overlap kernel, and the host driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries, nearest_candidates and the
+// traversal's kernel, the self-overlap and two-tree overlap kernels, and the host driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries, nearest_candidates and the
 // ordered traversal, D = 2 through the z = 0 lift) and dim4.cu (D = 4 rays, queries, nearest_candidates and the ordered traversal).
 // The 3-D ray kernels of traverse.cu use the same fetch.
 //
@@ -211,26 +211,30 @@ __device__ __forceinline__ bool overlap_boxes(const T smn[D], const T smx[D], co
     for (int k = 0; k < D; ++k) hit = hit && !(smx[k] < mn[k] || mx[k] < smn[k]);
     return hit;
 }
-template <int D, class T, bool FILL>
-__global__ void __launch_bounds__(256) overlap_kernel(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
-                                                      const typename CsrRecords<D, T>::Box* __restrict__ aabb, const uint32_t* __restrict__ node_index,
-                                                      const uint32_t* __restrict__ order, uint32_t n, uint32_t* __restrict__ counts,
-                                                      const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
-                                                      const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets,
-                                                      uint32_t* __restrict__ hits, unsigned long long cap) {
+// The body of both overlap kernels.  Self (CROSS = false): rows and records of one tree, own = other = its boxes, the walk of s
+// starts at record node_index[s].  Cross (CROSS = true, bvhgpu_overlap_trees_*): thread k takes shape order[k] of tree A (A's leaf
+// order), loads its box from `own` (A's boxes), and walks all of B's records from record 0, testing each reached leaf's shape
+// against `other` (B's boxes); node_index is unused.  The exactness argument is the same: it only needs B's records.
+template <int D, class T, bool FILL, bool CROSS>
+__device__ __forceinline__ void overlap_walk(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                             const typename CsrRecords<D, T>::Box* __restrict__ own, const typename CsrRecords<D, T>::Box* __restrict__ other,
+                                             const uint32_t* __restrict__ node_index, const uint32_t* __restrict__ order, uint32_t n,
+                                             uint32_t* __restrict__ counts, const uint32_t* __restrict__ local,
+                                             const unsigned long long* __restrict__ blocksum, const unsigned long long* __restrict__ total,
+                                             uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits, unsigned long long cap) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (FILL && k == 0) { const unsigned long long t = *total; offsets[n] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
     if (k >= n) return;
     const uint32_t s = __ldg(order + k);
     T smn[D], smx[D];
-    load_box(aabb + s, smn, smx);
+    load_box(own + s, smn, smx);
     unsigned long long w = 0;
     if (FILL) {
         w = blocksum[s / CSR_SCAN_TILE] + local[s];
         offsets[s] = w > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)w;
         if (!hits) return;                                        // offsets only
     }
-    uint32_t cnt = 0, i = __ldg(node_index + s);
+    uint32_t cnt = 0, i = CROSS ? 0u : __ldg(node_index + s);
     while (i < n_rec) {
         T mn[D], mx[D];
         uint32_t skip, shape;
@@ -238,7 +242,7 @@ __global__ void __launch_bounds__(256) overlap_kernel(const typename CsrRecords<
         if (overlap_enter<D, T>(smn, smx, mn, mx)) {
             if (shape != BVH_INVALID) {
                 T tmn[D], tmx[D];
-                load_box(aabb + shape, tmn, tmx);
+                load_box(other + shape, tmn, tmx);
                 if (overlap_boxes<D, T>(smn, smx, tmn, tmx)) {
                     if (FILL) { if (w < cap) hits[w] = shape; ++w; }
                     else ++cnt;
@@ -250,6 +254,28 @@ __global__ void __launch_bounds__(256) overlap_kernel(const typename CsrRecords<
         }
     }
     if (!FILL) counts[s] = cnt;
+}
+template <int D, class T, bool FILL>
+__global__ void __launch_bounds__(256) overlap_kernel(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                                      const typename CsrRecords<D, T>::Box* __restrict__ aabb, const uint32_t* __restrict__ node_index,
+                                                      const uint32_t* __restrict__ order, uint32_t n, uint32_t* __restrict__ counts,
+                                                      const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
+                                                      const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets,
+                                                      uint32_t* __restrict__ hits, unsigned long long cap) {
+    overlap_walk<D, T, FILL, false>(trec, n_rec, aabb, aabb, node_index, order, n, counts, local, blocksum, total, offsets, hits, cap);
+}
+// ---- overlap between two trees (bvhgpu_overlap_trees_*): row a of tree A lists every shape b of tree B whose own box intersects a's
+// own box, in B's DFS order.  trec / n_rec: B's records; aabb_b: B's boxes; aabb_a, order_a, n_a: A's boxes and shapes in A's leaf
+// order, so that neighbouring threads test neighbouring boxes.  Count pass and fill pass as overlap_kernel.
+template <int D, class T, bool FILL>
+__global__ void __launch_bounds__(256) overlap_trees_kernel(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                                            const typename CsrRecords<D, T>::Box* __restrict__ aabb_b,
+                                                            const typename CsrRecords<D, T>::Box* __restrict__ aabb_a,
+                                                            const uint32_t* __restrict__ order_a, uint32_t n_a, uint32_t* __restrict__ counts,
+                                                            const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
+                                                            const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets,
+                                                            uint32_t* __restrict__ hits, unsigned long long cap) {
+    overlap_walk<D, T, FILL, true>(trec, n_rec, aabb_a, aabb_b, nullptr, order_a, n_a, counts, local, blocksum, total, offsets, hits, cap);
 }
 
 // ---- host: count -> scan -> fill ----
@@ -298,6 +324,22 @@ template <int D, class T> struct OverlapWalk {
     void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
               uint32_t* offsets, uint32_t* hits, size_t cap) const {
         overlap_kernel<D, T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb, node_index, order, n, nullptr, local, sums, total, offsets, hits, (unsigned long long)cap);
+    }
+};
+// The walk of overlap_trees_kernel over tree A's n_a shapes (n_a >= 1) against tree B's records (n_b >= 1).  order_a: A's shapes in
+// A's leaf order (leaf_order_kernel).
+template <int D, class T> struct OverlapTreesWalk {
+    const typename CsrRecords<D, T>::Rec* trec;       // B's records
+    uint32_t n_rec;
+    const typename CsrRecords<D, T>::Box* aabb_b;     // B's own boxes (D = 2: z = [0, 0])
+    const typename CsrRecords<D, T>::Box* aabb_a;     // A's own boxes (D = 2: z = [0, 0])
+    const uint32_t* order_a;
+    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const {
+        overlap_trees_kernel<D, T, false><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb_b, aabb_a, order_a, n, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    }
+    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
+              uint32_t* offsets, uint32_t* hits, size_t cap) const {
+        overlap_trees_kernel<D, T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb_b, aabb_a, order_a, n, nullptr, local, sums, total, offsets, hits, (unsigned long long)cap);
     }
 };
 

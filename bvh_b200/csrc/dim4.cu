@@ -834,13 +834,16 @@ template <class P, class T> static int csr4_host_p(Tree4<T>* tree, bool flat, co
 
 // ---- self-overlap: overlap_kernel<4, T> of csr.cuh over the records and the ABI boxes (n >= 2; the caller handles n < 2).  The
 // shapes in leaf order live as long as the call (released stream-ordered after the fill). ----
-template <class T> static int overlap4_order(Tree4<T>* tree, Scratch& scratch, uint32_t** order) {
+template <class T> static int leaf_order4(Tree4<T>* tree, Scratch& scratch, uint32_t** order) {
     bvhgpu_ctx* ctx = tree->ctx;
-    BVH_TRY(ensure_trec4(tree));
     BVH_TRY(scratch.get(order, tree->n));
     leaf_order_kernel<<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_node_index, tree->d_node_start, tree->n, *order);
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
+}
+template <class T> static int overlap4_order(Tree4<T>* tree, Scratch& scratch, uint32_t** order) {
+    BVH_TRY(ensure_trec4(tree));
+    return leaf_order4(tree, scratch, order);
 }
 template <class T> int overlap4_device(Tree4<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
     Scratch scratch(tree->ctx);
@@ -855,6 +858,25 @@ template <class T> int overlap4_host(Tree4<T>* tree, uint32_t* offsets, uint32_t
     BVH_TRY(overlap4_order(tree, scratch, &order));
     const OverlapWalk<4, T> walk{tree->d_trec, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
     return csr4_host_walk(tree, walk, tree->n, offsets, hits, cap, total, "overlap_pairs");
+}
+
+// ---- overlap between two trees: overlap_trees_kernel<4, T>, A's shapes in A's leaf order against B's records and ABI boxes
+// (n_a >= 1, n_b >= 1; the caller handles the rest).  The host form uses A's retained buffers. ----
+template <class T> int overlap_trees4_device(Tree4<T>* a, Tree4<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
+    Scratch scratch(a->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(ensure_trec4(b));
+    BVH_TRY(leaf_order4(a, scratch, &order));
+    const OverlapTreesWalk<4, T> walk{b->d_trec, b->n_trec, b->d_aabb, a->d_aabb, order};
+    return csr_two_pass(a->ctx, walk, a->n, "overlap_trees_dev", d_offsets, d_hits, cap, total);
+}
+template <class T> int overlap_trees4_host(Tree4<T>* a, Tree4<T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+    Scratch scratch(a->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(ensure_trec4(b));
+    BVH_TRY(leaf_order4(a, scratch, &order));
+    const OverlapTreesWalk<4, T> walk{b->d_trec, b->n_trec, b->d_aabb, a->d_aabb, order};
+    return csr4_host_walk(a, walk, a->n, offsets, hits, cap, total, "overlap_trees");
 }
 
 // The probe of a CSR walk: rays, or one of the public query kinds.
@@ -1044,6 +1066,8 @@ template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* roots, con
     template int knn4_device<T>(Tree4<T>*, const T*, size_t, uint32_t, const T*, uint32_t*, T*);                                    \
     template int overlap4_device<T>(Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                                              \
     template int overlap4_host<T>(Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                                                \
+    template int overlap_trees4_device<T>(Tree4<T>*, Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                             \
+    template int overlap_trees4_host<T>(Tree4<T>*, Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                               \
     template int refresh_caches<T>(Tree4<T>*);                                                                                    \
     template int finish_relayout<T>(Tree4<T>*);                                                                                     \
     template int rebuild_degraded<T>(Tree4<T>*, const uint32_t*, uint32_t*, size_t*, const char*);                                  \

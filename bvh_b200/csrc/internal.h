@@ -258,6 +258,10 @@ template <class T> int traverse_ordered_device(Tree<T>* tree, const typename Tra
 // Every pair of shapes whose own boxes intersect, once, in the row of the earlier leaf (bvhgpu_overlap_pairs_*); device pointers, on
 // the context's stream, synchronises only to return *total.  Checks the tree's status; n < 2 gives all-zero offsets.
 template <class T> int overlap_device(Tree<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
+// Every pair (a, b) of a shape of tree A and a shape of tree B whose own boxes intersect, in A's row, B's DFS order
+// (bvhgpu_overlap_trees_*); device pointers, on the context's stream (A and B share it), synchronises only to return *total.  Checks
+// A's status, then B's; n_a = 0 or n_b = 0 give all-zero offsets.
+template <class T> int overlap_trees_device(Tree<T>* a, Tree<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
 // Aabb / Point / Ball queries (device pointers); two-pass count / fill.
 template <class T> int query_device(Tree<T>* tree, int mode, int kind, const T* d_queries, size_t nq, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
 // nearest_to for a batch of points (device pointers): exact reference walk for AABB-distance shapes; candidate lists for any shape
@@ -383,6 +387,10 @@ template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_
 // pointers (synchronises only to return *total), overlap4_host to host pointers through the retained buffers, as csr4_host.
 template <class T> int overlap4_device(Tree4<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
 template <class T> int overlap4_host(Tree4<T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+// overlap between two trees (overlap_trees_device's contract) with n_a >= 1 and n_b >= 1, statuses checked by the caller; the host
+// form runs through A's retained buffers, as overlap4_host.
+template <class T> int overlap_trees4_device(Tree4<T>* a, Tree4<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
+template <class T> int overlap_trees4_host(Tree4<T>* a, Tree4<T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
 // k nearest shapes: checks n, k and the tree's status, as knn_device does.
 template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
 // The 4-D overloads of the steps the dynamic drivers of dynamic.cu leave to the tree type (the 3-D ones are declared above):

@@ -1671,6 +1671,33 @@ int overlap_device(Tree<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t 
 template int overlap_device<float>(Tree<float>*, uint32_t*, uint32_t*, size_t, size_t*);
 template int overlap_device<double>(Tree<double>*, uint32_t*, uint32_t*, size_t, size_t*);
 
+// ---- overlap between two trees: overlap_trees_kernel<3, T> of csr.cuh, A's shapes in A's leaf order against B's records and B's own
+// boxes.  2-D trees as above: both d_aabb have z = [0, 0], B's records z = [-1, +1]. ----
+template <class T>
+int overlap_trees_device(Tree<T>* a, Tree<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
+    bvhgpu_ctx* ctx = a->ctx;
+    cudaStream_t st = ctx->stream;
+    BVH_TRY(resolve_status(a));
+    BVH_TRY(resolve_status(b));
+    const uint32_t n = a->n;
+    if (n == 0 || b->n == 0) {
+        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (n + 1), st));
+        if (total) *total = 0;
+        return BVHGPU_OK;
+    }
+    if (!b->d_tnodes) BVH_TRY(build_traversal_records(b));
+    Scratch scratch(ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(scratch.get(&order, n));
+    leaf_order_kernel<<<(n + 255) / 256, 256, 0, st>>>(a->d_node_index, a->d_node_start, n, order);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    const OverlapTreesWalk<3, T> walk{b->d_tnodes, b->n_trec, b->d_aabb, a->d_aabb, order};
+    return csr_two_pass(ctx, walk, n, "overlap_trees", d_offsets, d_hits, cap, total);
+}
+template int overlap_trees_device<float>(Tree<float>*, Tree<float>*, uint32_t*, uint32_t*, size_t, size_t*);
+template int overlap_trees_device<double>(Tree<double>*, Tree<double>*, uint32_t*, uint32_t*, size_t, size_t*);
+
 // ---- Ray::new for a batch (src/ray/ray_impl.rs:70-80) -------------------------------------------------
 template <class T> __device__ __forceinline__ T sqrt_rn(T x);
 template <> __device__ __forceinline__ float sqrt_rn(float x) { return __fsqrt_rn(x); }

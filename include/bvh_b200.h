@@ -670,6 +670,36 @@ int bvhgpu_overlap_pairs_dev_f64x3(bvhgpu_tree3d* tree, void* dev_offsets, void*
 int bvhgpu_overlap_pairs_dev_f32x4(bvhgpu_tree4f* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 int bvhgpu_overlap_pairs_dev_f64x4(bvhgpu_tree4d* tree, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 
+/* ---- overlap pairs between two trees: every pair of a shape of tree A and a shape of tree B whose AABBs intersect (a moving body
+ * against static scenery, one mesh against another, particles against obstacles).  leaf_B(b) = the preorder node index of shape b's
+ * leaf in B.  Output: a CSR indexed by A's shapes, offsets[n_a + 1]; row a lists every shape b of B with intersects(box_a, box_b), in
+ * ascending leaf_B(b) order (B's DFS order, the order of bvhgpu_query_* hits).
+ *   intersects = Aabb::intersects_aabb taken literally, as for bvhgpu_overlap_pairs_*; touching faces overlap.  The boxes are each
+ *   tree's own current shape boxes: from the build or the latest refit, update_shapes or add_shapes, in the numbering after
+ *   remove_shapes.
+ *   EXACT (equal to the brute force over all n_a x n_b pairs) for every tree the library builds or maintains, every build mode, after
+ *   every dynamic call, on overflow-scale, infinite, coincident and subnormal boxes: a record of B is entered when its box intersects
+ *   box_a or has min > max on some axis (the Aabb::empty() child box of a "no split wins" node), the argument of the self-overlap
+ *   pairs applied to B.  For a B from bvhgpu_tree_from_nodes_* the result is exact only when the caller's node boxes contain their
+ *   shapes (or are empty); otherwise it is a subset of the true pairs.
+ *   A and B must belong to the same context (its one stream orders the walk after every call pending on either tree); otherwise
+ *   BVHGPU_ERR_INVALID, nothing written.  a == b is allowed and gives the full symmetric relation, (s, s) included for every box that
+ *   intersects itself.
+ *   Capacity, saturation and the _dev forms as bvhgpu_overlap_pairs_*: the host forms of D = 2 and 3 keep the retained list on tree A
+ *   (in 3-D bvhgpu_traverse_fetch_*(a, ...) fetches it after BVHGPU_ERR_CAPACITY; in 2-D and 4-D call again with cap = *total).
+ *   n_a = 0: offsets[0] = 0.  n_b = 0: all-zero offsets, no device work.  A null a, b or offsets pointer: BVHGPU_ERR_INVALID, nothing
+ *   written.  A failed build is reported sticky, A's before B's.  The _dev forms exist for D = 3 and 4. */
+int bvhgpu_overlap_trees_f32x2(bvhgpu_tree2f* a, bvhgpu_tree2f* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_f64x2(bvhgpu_tree2d* a, bvhgpu_tree2d* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_f32x3(bvhgpu_tree3f* a, bvhgpu_tree3f* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_f64x3(bvhgpu_tree3d* a, bvhgpu_tree3d* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_f32x4(bvhgpu_tree4f* a, bvhgpu_tree4f* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_f64x4(bvhgpu_tree4d* a, bvhgpu_tree4d* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_dev_f32x3(bvhgpu_tree3f* a, bvhgpu_tree3f* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_dev_f64x3(bvhgpu_tree3d* a, bvhgpu_tree3d* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_dev_f32x4(bvhgpu_tree4f* a, bvhgpu_tree4f* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_overlap_trees_dev_f64x4(bvhgpu_tree4d* a, bvhgpu_tree4d* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
  * leaves (user code), so there are two forms.  `points`: 3 T per query point, host pointers.

@@ -105,6 +105,7 @@ template <> struct Abi<float> {
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f32x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
     static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f32x3(t, off, h, cap, tot); }
+    static int overlap_trees(tree* a, tree* b, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_trees_f32x3(a, b, off, h, cap, tot); }
 };
 template <> struct Abi<double> {
     using aabb = bvh_aabb3d; using ray = bvh_ray3d; using node = bvh_node3d; using flat = bvh_flat3d; using tree = bvhgpu_tree3d;
@@ -125,6 +126,7 @@ template <> struct Abi<double> {
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f64x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
     static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f64x3(t, off, h, cap, tot); }
+    static int overlap_trees(tree* a, tree* b, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_trees_f64x3(a, b, off, h, cap, tot); }
 };
 struct Ctx {
     bvhgpu_ctx* h = nullptr;
@@ -275,6 +277,17 @@ template <class T> class Bvh {
         hits.resize(std::max<size_t>(4 * n_, 1024));
         size_t total = 0;
         const int st = A::overlap(tree_, offsets.data(), hits.data(), hits.size(), &total);
+        if (st == BVHGPU_ERR_CAPACITY && total <= UINT32_MAX) { hits.resize(total); check(A::fetch(tree_, hits.data(), total)); }
+        else { check(st); hits.resize(total); }
+    }
+    // every pair (a, b) of a shape of this tree and a shape of `other` whose current AABBs intersect: CSR indexed by this tree's
+    // shapes, row a = other's shapes whose box meets a's, in other's DFS order (bvhgpu_overlap_trees_*).  Both trees must share a
+    // context (the default one does); other may be *this.  offsets gets n + 1 entries.
+    void overlap_pairs_with(const Bvh<T>& other, std::vector<uint32_t>& offsets, std::vector<uint32_t>& hits) const {
+        offsets.assign(n_ + 1, 0);
+        hits.resize(std::max<size_t>(4 * n_, 1024));
+        size_t total = 0;
+        const int st = A::overlap_trees(tree_, other.tree_, offsets.data(), hits.data(), hits.size(), &total);
         if (st == BVHGPU_ERR_CAPACITY && total <= UINT32_MAX) { hits.resize(total); check(A::fetch(tree_, hits.data(), total)); }
         else { check(st); hits.resize(total); }
     }

@@ -118,6 +118,31 @@ for prec in ("f32", "f64"):
         bt.overlap_pairs()
         print("  overlap", prec, D, len(ph))
         bt.free()
+# overlap pairs between two trees: host and device forms in D = 2, 3, 4, a short capacity (fetch / retry), a == b, an overflow-scale B
+for prec in ("f32", "f64"):
+    import torch
+    for D, cls in ((2, api.Bvh2), (3, api.Bvh), (4, api.Bvh4)):
+        dt = (cls._TABLE[prec] if D != 3 else api.BY_PREC[prec])["aabb"]
+        boxes = []
+        for n in (700, 500):
+            lo = rng.uniform(-50, 50, (n, D))
+            bo = np.zeros(n, dtype=dt)
+            bo["min"], bo["max"] = lo, lo + rng.uniform(0, 6, (n, D))
+            boxes.append(bo)
+        ta, tb = cls.build(boxes[0], prec=prec), cls.build(boxes[1], prec=prec)
+        po, ph = ta.overlap_pairs_with(tb)
+        ta.overlap_pairs_with(tb, cap=len(ph) // 2)
+        ta.overlap_pairs_with(ta)
+        if D != 2:
+            d_o = torch.zeros(len(boxes[0]) + 1, dtype=torch.int32, device="cuda:0"); d_h = torch.zeros(len(ph), dtype=torch.int32, device="cuda:0")
+            ta.overlap_pairs_with_dev(tb, d_o.data_ptr(), d_h.data_ptr(), len(ph) // 3); ta.overlap_pairs_with_dev(tb, d_o.data_ptr(), d_h.data_ptr(), len(ph), True)
+        tb.free()
+        boxes[1]["min"], boxes[1]["max"] = boxes[1]["min"] * 1e30, boxes[1]["min"] * 1e30 + 1e29
+        tb = cls.build(boxes[1], prec=prec)
+        ta.overlap_pairs_with(tb)
+        print("  overlap_trees", prec, D, len(ph))
+        ta.free()
+        tb.free()
 # host path on a batch large enough to be chunked (under the sanitizer the library takes the copy-then-walk form; forced streaming too)
 a = scenes.create_n_cubes_aabbs(300)
 b = api.Bvh.build(a)
