@@ -56,7 +56,12 @@ class Context:
         return cls._default[device]
 
     def set_stream(self, cuda_stream_handle: int | None):
-        """Enqueue on the given cudaStream_t handle (0 = CUDA's legacy default stream); None = the context's own stream."""
+        """Enqueue on the given cudaStream_t handle (0 = CUDA's legacy default stream); None = the context's own stream.
+
+        A change of stream keeps the context's calls in order without blocking the host: the new stream waits for
+        everything already enqueued on the old one (builds, refits, updates, tree frees), and `synchronize` afterwards
+        covers all of it.  The caller still orders the tensors it passes in (and reads back) against the stream it
+        installs, e.g. by installing `torch.cuda.current_stream().cuda_stream`."""
         if cuda_stream_handle is None:
             capi.check(capi.lib().bvhgpu_reset_stream(self._h))
         else:

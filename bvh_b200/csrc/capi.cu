@@ -1204,6 +1204,7 @@ BVH_EXPORT int bvhgpu_create(int device, bvhgpu_ctx** out) {
     for (int i = 0; i < 5; ++i) BVH_CUDA_TRY(cudaEventCreate(&ctx->ev_e2e[i]));
     BVH_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_order, cudaEventDisableTiming));
     BVH_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_total, cudaEventDisableTiming));
+    BVH_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_switch, cudaEventDisableTiming));
     for (unsigned i = 0; i < BVH_MAX_CHUNKS; ++i) BVH_CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_chunk[i], cudaEventDisableTiming));
     BVH_CUDA_TRY(cudaMalloc((void**)&ctx->d_async_err, 256));
     BVH_CUDA_TRY(cudaMemset(ctx->d_async_err, 0, 256));
@@ -1234,6 +1235,7 @@ BVH_EXPORT void bvhgpu_destroy(bvhgpu_ctx* ctx) {
     for (unsigned i = 0; i < BVH_MAX_CHUNKS; ++i) if (ctx->ev_emit[i]) cudaEventDestroy(ctx->ev_emit[i]);
     if (ctx->ev_order) cudaEventDestroy(ctx->ev_order);
     if (ctx->ev_total) cudaEventDestroy(ctx->ev_total);
+    if (ctx->ev_switch) cudaEventDestroy(ctx->ev_switch);
     for (unsigned i = 0; i < BVH_MAX_CHUNKS; ++i) if (ctx->ev_chunk[i]) cudaEventDestroy(ctx->ev_chunk[i]);
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     if (ctx->d_async_err) cudaFree(ctx->d_async_err);
@@ -1241,15 +1243,23 @@ BVH_EXPORT void bvhgpu_destroy(bvhgpu_ctx* ctx) {
     for (int i = 0; i < 2; ++i) { if (ctx->ev_walk[i]) cudaEventDestroy(ctx->ev_walk[i]); if (ctx->ev_build[i]) cudaEventDestroy(ctx->ev_build[i]); }
     delete ctx;
 }
+// Move the context to another stream without breaking the order of its calls: the incoming stream waits for everything
+// enqueued on the outgoing one (kernels, copies and the pool frees / allocations inside them). No host synchronisation.
+static int switch_stream(bvhgpu_ctx* ctx, cudaStream_t incoming) {
+    if (incoming == ctx->stream) return BVHGPU_OK;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_CUDA_TRY(cudaEventRecord(ctx->ev_switch, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamWaitEvent(incoming, ctx->ev_switch, 0));
+    ctx->stream = incoming;
+    return BVHGPU_OK;
+}
 BVH_EXPORT int bvhgpu_set_stream(bvhgpu_ctx* ctx, void* cuda_stream) {
     if (!ctx) { set_error("set_stream: null ctx"); return BVHGPU_ERR_INVALID; }
-    ctx->stream = (cudaStream_t)cuda_stream;
-    return BVHGPU_OK;
+    return switch_stream(ctx, (cudaStream_t)cuda_stream);
 }
 BVH_EXPORT int bvhgpu_reset_stream(bvhgpu_ctx* ctx) {
     if (!ctx) { set_error("reset_stream: null ctx"); return BVHGPU_ERR_INVALID; }
-    ctx->stream = ctx->own_stream;
-    return BVHGPU_OK;
+    return switch_stream(ctx, ctx->own_stream);
 }
 BVH_EXPORT int bvhgpu_synchronize(bvhgpu_ctx* ctx) {
     if (!ctx) { set_error("synchronize: null ctx"); return BVHGPU_ERR_INVALID; }

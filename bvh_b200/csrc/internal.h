@@ -41,6 +41,7 @@ struct bvhgpu_ctx {
     int sm_count = 0;
     cudaStream_t own_stream = nullptr;
     cudaStream_t stream = nullptr;
+    cudaEvent_t ev_switch = nullptr; // set_stream / reset_stream: recorded on the outgoing stream, waited on by the incoming one
     uint64_t launches = 0;
     int64_t traverse_slots = -1;   // per-ray hit slots of the single-pass traversal (0 = two-pass, -1 = auto by batch size)
     int64_t traverse_persistent = 2;   // 0: one ray per thread, 1: persistent refill kernel, 2: coherence probe decides on the device

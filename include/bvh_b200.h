@@ -120,11 +120,21 @@ void bvhgpu_destroy(bvhgpu_ctx* ctx);
 const char* bvhgpu_last_error(void);
 const char* bvhgpu_version(void);
 /* Enqueue on an externally owned cudaStream_t (e.g. torch's current stream; 0 is CUDA's legacy default
- * stream and is honoured as such).  bvhgpu_reset_stream returns to the context's own stream. */
+ * stream and is honoured as such, on either side of a switch).  bvhgpu_reset_stream returns to the context's own stream.
+ * Ordering: when the stream changes, the context records an event on the outgoing stream and makes the incoming stream
+ * wait for it (no host synchronisation).  So every call on a context is ordered after every earlier call on that context,
+ * on whatever stream each one ran -- builds, refits, updates, tree frees and the stream-ordered pool allocations and frees
+ * inside them included.  Setting the stream the context already uses is a no-op.  If a CUDA call fails the function
+ * returns BVHGPU_ERR_CUDA and the context stays on its previous stream.
+ * What stays the caller's job: ordering the production of its input buffers (device rays, boxes, triangles, ...) before
+ * the call, and the consumption of its output buffers after it, against the stream it installs.
+ * Out of scope: switching streams while a CUDA graph is being captured, and calls on one context from several host
+ * threads at once. */
 int bvhgpu_set_stream(bvhgpu_ctx* ctx, void* cuda_stream);
 int bvhgpu_reset_stream(bvhgpu_ctx* ctx);
-/* Waits for the context's stream.  Also the point where errors of asynchronous multi-GPU steps surface: a peer that never
- * answered (BVHGPU_ERR_TIMEOUT) is reported here, once, and the step's result must not be used. */
+/* Waits for the context's stream, and so (see bvhgpu_set_stream) for every earlier call on the context, including work
+ * enqueued on streams it used before.  Also the point where errors of asynchronous multi-GPU steps surface: a peer that
+ * never answered (BVHGPU_ERR_TIMEOUT) is reported here, once, and the step's result must not be used. */
 int bvhgpu_synchronize(bvhgpu_ctx* ctx);
 /* Pinned host memory for ray / result staging, placed on the NUMA node the device hangs off (sysfs numa_node of the
  * PCI function) -- on a two-socket host a buffer pinned on the far socket moves at a fraction of the PCIe rate. */
