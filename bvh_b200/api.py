@@ -381,6 +381,60 @@ class Bvh:
             self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None), C.c_void_p(shape_ptr), C.c_void_p(dist_ptr),
             C.c_void_p(closest_ptr or None)))
 
+    def count_hits(self, rays: np.ndarray, tmax=None):
+        """Crossing counts per ray over the triangles of set_triangles: (front (n,) u32, back (n,) u32).  front counts the triangles whose
+        Ray::intersects_triangle distance is finite (and < tmax), back the same with the winding reversed (b and c exchanged).  tmax:
+        one limit per ray, a scalar for all, or None for none.  Without a limit exactly the loop over Bvh::traverse with both windings
+        (DESIGN.md 4.21)."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        n = len(rays)
+        front = np.zeros(n, dtype=np.uint32)
+        back = np.zeros(n, dtype=np.uint32)
+        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_count_hits_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), _ptr(front), _ptr(back)))
+        return front, back
+
+    def count_hits_dev(self, rays_ptr: int, nrays: int, tmax_ptr: int, front_ptr: int, back_ptr: int, layout: int = capi.RAYS_FULL):
+        """count_hits from device pointers: nrays rays (RAYS_FULL or RAYS_OD) and nrays limits (tmax_ptr = 0: none) in, nrays u32 front
+        and back counts out, enqueued on the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_count_hits_dev_{self._d['suffix']}")(
+            self._h, C.c_void_p(rays_ptr), layout, nrays, C.c_void_p(tmax_ptr or None), C.c_void_p(front_ptr), C.c_void_p(back_ptr)))
+
+    _RULES = {"even_odd": capi.FILL_EVEN_ODD, "nonzero": capi.FILL_NONZERO}
+
+    def contains(self, points, rule: str = "even_odd") -> np.ndarray:
+        """Point-in-mesh over the closed triangle mesh of set_triangles: bool (n,).  Three fixed rays per point vote; rule "even_odd"
+        (front + back odd, orientation ignored) or "nonzero" (back != front, outward-oriented shells).  Points on the surface are
+        undefined; a NaN point is outside (DESIGN.md 4.21)."""
+        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        out = np.zeros(len(p), dtype=np.uint8)
+        capi.check(getattr(capi.lib(), f"bvhgpu_contains_points_{self._d['suffix']}")(self._h, _ptr(p), len(p), self._RULES[rule], _ptr(out)))
+        return out.astype(bool)
+
+    def contains_dev(self, points_ptr: int, n: int, inside_ptr: int, rule: str = "even_odd"):
+        """contains from device pointers: n points (3 scalars each) in, n bytes (0 / 1) out, on the context's stream without host
+        synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_contains_points_dev_{self._d['suffix']}")(
+            self._h, C.c_void_p(points_ptr), n, self._RULES[rule], C.c_void_p(inside_ptr)))
+
+    def signed_distance(self, points, rule: str = "even_odd", closest: bool = False):
+        """Signed distance to the closed triangle mesh of set_triangles: (shape (n,) u32, dist (n,)), plus closest (n, 3) with
+        closest=True.  shape, |dist| and closest are knn_triangles(points, 1); dist is negated where contains(points, rule) is true."""
+        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        n = len(p)
+        shape = np.zeros(n, dtype=np.uint32)
+        dist = np.zeros(n, dtype=self._d["scalar"])
+        q = np.zeros((n, 3), dtype=self._d["scalar"]) if closest else None
+        capi.check(getattr(capi.lib(), f"bvhgpu_signed_distance_{self._d['suffix']}")(self._h, _ptr(p), n, self._RULES[rule], _ptr(shape),
+                                                                                     _ptr(dist), _ptr(q)))
+        return (shape, dist, q) if closest else (shape, dist)
+
+    def signed_distance_dev(self, points_ptr: int, n: int, shape_ptr: int, dist_ptr: int, closest_ptr: int = 0, rule: str = "even_odd"):
+        """signed_distance from device pointers: n points in, n u32 shapes, distances and (closest_ptr != 0) 3 n coordinates out, on
+        the context's stream without host synchronisation."""
+        capi.check(getattr(capi.lib(), f"bvhgpu_signed_distance_dev_{self._d['suffix']}")(
+            self._h, C.c_void_p(points_ptr), n, self._RULES[rule], C.c_void_p(shape_ptr), C.c_void_p(dist_ptr), C.c_void_p(closest_ptr or None)))
+
     def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
         """Bvh::traverse with Aabb / Point / Ball queries (IntersectsAabb implementors other than Ray).
         queries: (n, 6) {min,max} for capi.QUERY_AABB, (n, 3) for QUERY_POINT, (n, 4) {center, radius} for QUERY_BALL."""

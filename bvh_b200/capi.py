@@ -17,6 +17,7 @@ QUERY_AABB, QUERY_POINT, QUERY_BALL = 1, 2, 3
 
 
 RAYS_FULL, RAYS_OD = 0, 1
+FILL_EVEN_ODD, FILL_NONZERO = 0, 1
 MAX_PEERS, MAILBOX_BYTES, IPC_HANDLE_BYTES = 8, 65536, 64
 MB_TRACE_WORD, MB_TRACE_LEN = 128, 1024          # mailbox trace ring (u64 words), see traverse.cu
 
@@ -153,6 +154,12 @@ def lib() -> C.CDLL:
         getattr(L, f"bvhgpu_knn_triangles_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
         getattr(L, f"bvhgpu_multi_hit_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, i32, vp, vp, vp]
         getattr(L, f"bvhgpu_multi_hit_dev_{s}").argtypes = [vp, vp, i32, sz, C.c_uint32, vp, i32, vp, vp, vp]
+        getattr(L, f"bvhgpu_count_hits_{s}").argtypes = [vp, vp, sz, vp, vp, vp]
+        getattr(L, f"bvhgpu_count_hits_dev_{s}").argtypes = [vp, vp, i32, sz, vp, vp, vp]
+        getattr(L, f"bvhgpu_contains_points_{s}").argtypes = [vp, vp, sz, i32, vp]
+        getattr(L, f"bvhgpu_contains_points_dev_{s}").argtypes = [vp, vp, sz, i32, vp]
+        getattr(L, f"bvhgpu_signed_distance_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp]
+        getattr(L, f"bvhgpu_signed_distance_dev_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp]
     for s in ("f32x2", "f64x2", "f32x4", "f64x4"):
         getattr(L, f"bvhgpu_multi_hit_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
     for s in ("f32x4", "f64x4"):

@@ -809,6 +809,99 @@ static int multi_hit_dev_impl(TreeOf<D, T>* tree, const void* d_rays, uint32_t f
     return multi_hit_driver<D, T>(tree, d_rays, fmt, nrays, k, (const T*)d_tmax, use_triangles, (uint32_t*)d_shape, (T*)d_dist, (T*)d_uv);
 }
 
+// Crossing counts, point-in-mesh and signed distance (D = 3).  Host forms: the null checks, n, the rule, the tree's status and n = 0 are
+// settled before anything is staged; the device drivers (closest.cu) check the layout, the status and the triangles before they launch,
+// and the caller's buffers are written only after they returned OK.
+template <class T>
+static int count_hits_host_impl(Tree<T>* tree, const void* rays, size_t nrays, const T* tmax, uint32_t* out_front, uint32_t* out_back) {
+    if (!tree || (nrays && (!rays || !out_front || !out_back))) { set_error("count_hits: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("count_hits", nrays));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (nrays == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    T *d_rays = nullptr, *d_tmax = nullptr;
+    uint32_t *d_f = nullptr, *d_b = nullptr;
+    BVH_TRY(scratch.get(&d_rays, 9 * nrays));
+    BVH_TRY(scratch.get(&d_f, nrays));
+    BVH_TRY(scratch.get(&d_b, nrays));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_rays, rays, sizeof(T) * 9 * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    if (tmax) {
+        BVH_TRY(scratch.get(&d_tmax, nrays));
+        BVH_CUDA_TRY(cudaMemcpyAsync(d_tmax, tmax, sizeof(T) * nrays, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    BVH_TRY(count_hits_device<T>(tree, d_rays, BVHGPU_RAYS_FULL, nrays, d_tmax, d_f, d_b));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_front, d_f, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_back, d_b, sizeof(uint32_t) * nrays, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T>
+static int count_hits_dev_impl(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const void* d_tmax, void* d_front, void* d_back) {
+    if (!tree || (nrays && (!d_rays || !d_front || !d_back))) { set_error("count_hits_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return count_hits_device<T>(tree, d_rays, fmt, nrays, (const T*)d_tmax, (uint32_t*)d_front, (uint32_t*)d_back);
+}
+static int check_fill_rule(const char* what, int rule) {
+    if (rule != BVHGPU_FILL_EVEN_ODD && rule != BVHGPU_FILL_NONZERO) { set_error("%s: unknown fill rule %d", what, rule); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+template <class T>
+static int contains_host_impl(Tree<T>* tree, const T* points, size_t n, int rule, uint8_t* out_inside) {
+    if (!tree || (n && (!points || !out_inside))) { set_error("contains_points: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("contains_points", n));
+    BVH_TRY(check_fill_rule("contains_points", rule));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    T* d_p = nullptr;
+    uint8_t* d_in = nullptr;
+    BVH_TRY(upload_records<3>(ctx, scratch, points, n, 1, 0, &d_p));
+    BVH_TRY(scratch.get(&d_in, n));
+    BVH_TRY(contains_points_device<T>(tree, d_p, n, rule, d_in));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_inside, d_in, n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T>
+static int contains_dev_impl(Tree<T>* tree, const void* d_points, size_t n, int rule, void* d_inside) {
+    if (!tree || (n && (!d_points || !d_inside))) { set_error("contains_points_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return contains_points_device<T>(tree, (const T*)d_points, n, rule, (uint8_t*)d_inside);
+}
+template <class T>
+static int signed_distance_host_impl(Tree<T>* tree, const T* points, size_t n, int rule, uint32_t* out_shape, T* out_dist, T* out_closest) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("signed_distance: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_TRY(check_n("signed_distance", n));
+    BVH_TRY(check_fill_rule("signed_distance", rule));
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(resolve_status(tree));
+    if (n == 0) return BVHGPU_OK;
+    Scratch scratch(ctx);
+    T *d_p = nullptr, *d_d = nullptr, *d_q = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(upload_records<3>(ctx, scratch, points, n, 1, 0, &d_p));
+    BVH_TRY(scratch.get(&d_s, n));
+    BVH_TRY(scratch.get(&d_d, n));
+    if (out_closest) BVH_TRY(scratch.get(&d_q, 3 * n));
+    BVH_TRY(signed_distance_device<T>(tree, d_p, n, rule, d_s, d_d, d_q));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_closest) BVH_CUDA_TRY(cudaMemcpyAsync(out_closest, d_q, sizeof(T) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T>
+static int signed_distance_dev_impl(Tree<T>* tree, const void* d_points, size_t n, int rule, void* d_shape, void* d_dist, void* d_closest) {
+    if (!tree || (n && (!d_points || !d_shape || !d_dist))) { set_error("signed_distance_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return signed_distance_device<T>(tree, (const T*)d_points, n, rule, (uint32_t*)d_shape, (T*)d_dist, (T*)d_closest);
+}
+
 template <class T> static int fetch_impl(Tree<T>* tree, uint32_t* hits, size_t cap) {
     if (!tree || !hits) { set_error("traverse_fetch: null argument"); return BVHGPU_ERR_INVALID; }
     if (cap < tree->last_total) { set_error("traverse_fetch: capacity %zu < %zu hits", cap, tree->last_total); return BVHGPU_ERR_CAPACITY; }
@@ -1541,6 +1634,28 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
                                               void* dev_uv) {                                                             \
         return multi_hit_dev_impl<3, T>(tree, dev_rays, (uint32_t)ray_layout, nrays, k, dev_tmax, use_triangles, dev_shape, \
                                         dev_dist, dev_uv);                                                                \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_count_hits_##SUF(TREE* tree, const RAY* rays, size_t nrays, const T* tmax, uint32_t* out_front, \
+                                           uint32_t* out_back) {                                                          \
+        return count_hits_host_impl<T>(tree, rays, nrays, tmax, out_front, out_back);                                     \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_count_hits_dev_##SUF(TREE* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax, \
+                                               void* dev_front, void* dev_back) {                                         \
+        return count_hits_dev_impl<T>(tree, dev_rays, (uint32_t)ray_layout, nrays, dev_tmax, dev_front, dev_back);        \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_contains_points_##SUF(TREE* tree, const T* points, size_t n, int rule, uint8_t* out_inside) {  \
+        return contains_host_impl<T>(tree, points, n, rule, out_inside);                                                  \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_contains_points_dev_##SUF(TREE* tree, const void* dev_points, size_t n, int rule, void* dev_inside) { \
+        return contains_dev_impl<T>(tree, dev_points, n, rule, dev_inside);                                               \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_signed_distance_##SUF(TREE* tree, const T* points, size_t n, int rule, uint32_t* out_shape,    \
+                                                T* out_dist, T* out_closest) {                                            \
+        return signed_distance_host_impl<T>(tree, points, n, rule, out_shape, out_dist, out_closest);                     \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_signed_distance_dev_##SUF(TREE* tree, const void* dev_points, size_t n, int rule, void* dev_shape, \
+                                                    void* dev_dist, void* dev_closest) {                                  \
+        return signed_distance_dev_impl<T>(tree, dev_points, n, rule, dev_shape, dev_dist, dev_closest);                  \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_stats_##SUF(TREE* tree, uint64_t* out2) {                                              \
         if (!tree || !out2) { set_error("traverse_stats: null argument"); return BVHGPU_ERR_INVALID; }                    \

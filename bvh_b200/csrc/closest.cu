@@ -65,6 +65,16 @@ __device__ __forceinline__ T moeller_trumbore(const T o[3], const T dir[3], cons
     return dist > EPS ? dist : INF;
 }
 
+// Both windings of one triangle for the crossing counts: moeller_trumbore as it is, then the same function with b and c exchanged
+// (the back-face test).  Each counts when its distance is < tmax (+inf without a limit: finite).
+template <class T>
+__device__ __forceinline__ void count_windings(const T o[3], const T dir[3], const T a[3], const T b[3], const T c[3], T tmax,
+                                               uint32_t& front, uint32_t& back) {
+    T u, v;
+    front += moeller_trumbore(o, dir, a, b, c, u, v) < tmax ? 1u : 0u;
+    back += moeller_trumbore(o, dir, a, c, b, u, v) < tmax ? 1u : 0u;
+}
+
 template <class T> struct DTri { T a[3], pa, b[3], pb, c[3], pc; };       // 48 B / 96 B: three vector loads per triangle
 
 template <class T>
@@ -496,6 +506,209 @@ int multi_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::N
     if (nrays == 0) return BVHGPU_OK;
     return multi_hit_launch<D, T, false>(ctx, nodes, n_shapes, aabb, nullptr, d_rays, 3 * D, nrays, k, d_tmax, d_shape, d_dist, nullptr);
 }
+
+// ---- crossing counts (bvhgpu_count_hits_*), point-in-mesh (bvhgpu_contains_points_*) and the sign of bvhgpu_signed_distance_* ----
+// Per ray: front = #shapes of Bvh::traverse's set whose moeller_trumbore(o, d, a, b, c) is < tmax, back = the same with b and c
+// exchanged (count_windings).  The walk is closest_kernel's stackless parent-link walk, ray loading and slab test, without a near / far
+// order: the left child is judged first, the right one when the walk comes back from the left, and a child is entered when its slab
+// test passes and its entry <= fl(tmax * (1 + 2^-16)), the any-hit walk's triangle margin (+inf without a limit: every child whose slab
+// test passes, i.e. exactly Bvh::traverse's set).  Only the judged child's box is loaded.  A root leaf (n = 1) tests the shape's own box.
+template <class T> __device__ __forceinline__ T crossings_sqrt(T x);
+template <> __device__ __forceinline__ float crossings_sqrt(float x) { return __fsqrt_rn(x); }
+template <> __device__ __forceinline__ double crossings_sqrt(double x) { return __dsqrt_rn(x); }
+
+template <class T>
+__device__ __forceinline__ void crossings_walk(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_shapes,
+                                               const typename Traits<T>::DAabb* __restrict__ aabb, const DTri<T>* __restrict__ tris,
+                                               const T o[3], const T dir[3], const T inv[3], T tmax, uint32_t& front, uint32_t& back) {
+    const T bound = mul_rn(tmax, add_rn(T(1), T(1.0 / 65536.0)));      // inf stays inf, NaN stays NaN (nothing is entered)
+    auto leaf = [&](uint32_t shape) {
+        const DTri<T>& t = tris[shape];
+        T a[3], b[3], c[3];
+#pragma unroll
+        for (int q = 0; q < 3; ++q) { a[q] = __ldg(&t.a[q]); b[q] = __ldg(&t.b[q]); c[q] = __ldg(&t.c[q]); }
+        count_windings(o, dir, a, b, c, tmax, front, back);
+    };
+    auto enter = [&](const typename Traits<T>::Aabb& box) {
+        T mn[3], mx[3], e, x;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) { mn[q] = __ldg(&box.min[q]); mx[q] = __ldg(&box.max[q]); }
+        return slab_slice<3, T>(o, inv, mn, mx, e, x) && e <= bound;
+    };
+    if (n_shapes == 1) {                                       // root leaf (bvh_node.rs:314 tests the shape's own AABB)
+        T mn[3], mx[3], e, x;
+        load_box(aabb + nodes[0].shape, mn, mx);
+        if (slab_slice<3, T>(o, inv, mn, mx, e, x)) leaf(nodes[0].shape);
+        return;
+    }
+    uint32_t node = 0, from = BVH_INVALID;                      // from: the child we are coming back from (BVH_INVALID: from the parent)
+    for (;;) {
+        const uint4 meta = __ldg(reinterpret_cast<const uint4*>(nodes + node));      // parent, child_l, child_r, shape / count
+        if (meta.y == BVH_INVALID) {
+            leaf(meta.w);
+            from = node; node = meta.x;
+            continue;
+        }
+        const typename Traits<T>::Node& nd = nodes[node];
+        uint32_t next = BVH_INVALID;
+        if (from == BVH_INVALID) {
+            if (enter(nd.l_aabb)) next = meta.y;
+            else from = meta.y;                                 // skipped: as if we had just come back from it
+        }
+        if (next == BVH_INVALID && from == meta.y) {
+            if (enter(nd.r_aabb)) next = meta.z;
+            else from = meta.z;
+        }
+        if (next != BVH_INVALID) { node = next; from = BVH_INVALID; continue; }
+        if (node == 0) break;                                   // back from the right child of the root
+        from = node; node = meta.x;
+    }
+}
+
+// FROM_POINTS = false: one ray per thread, FULL (9 T) or OD (6 T) rays, ray_tmax nrays limits or nullptr; writes out_front / out_back.
+// FROM_POINTS = true: one POINT per thread (3 T each); the three rays Ray::new(p, BVHGPU_CONTAINS_DIRECTIONS[j]) are built in registers
+// with rays_new_kernel's arithmetic and walked one after the other without a limit, so neighbouring threads walk neighbouring points in
+// the same direction at the same time and the vote needs no scratch.  out_inside[i] = 1 when at least two of the three rays vote inside
+// (rule EVEN_ODD: front + back odd; NONZERO: back != front).
+template <class T, bool FROM_POINTS>
+__global__ void __launch_bounds__(128) crossings_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_shapes,
+                                                        const typename Traits<T>::DAabb* __restrict__ aabb, const DTri<T>* __restrict__ tris,
+                                                        const T* __restrict__ in, uint32_t ray_stride, uint32_t n, const T* __restrict__ ray_tmax,
+                                                        uint32_t* __restrict__ out_front, uint32_t* __restrict__ out_back, int rule,
+                                                        uint8_t* __restrict__ out_inside) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if constexpr (!FROM_POINTS) {
+        T o[3], dir[3], inv[3];
+        const T* p = in + (size_t)ray_stride * i;
+        const bool full = ray_stride == 9;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { o[k] = __ldg(p + k); dir[k] = __ldg(p + 3 + k); inv[k] = full ? __ldg(p + 6 + k) : div_rn(T(1), dir[k]); }
+        uint32_t front = 0, back = 0;
+        crossings_walk<T>(nodes, n_shapes, aabb, tris, o, dir, inv, ray_tmax ? __ldg(ray_tmax + i) : Traits<T>::inf(), front, back);
+        out_front[i] = front;
+        out_back[i] = back;
+    } else {
+        constexpr double DIRS[3][3] = BVHGPU_CONTAINS_DIRECTIONS;
+        T o[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) o[k] = __ldg(in + 3 * (size_t)i + k);
+        uint32_t votes = 0;
+#pragma unroll 1
+        for (int j = 0; j < 3; ++j) {
+            const T dx = T(j == 0 ? DIRS[0][0] : j == 1 ? DIRS[1][0] : DIRS[2][0]);
+            const T dy = T(j == 0 ? DIRS[0][1] : j == 1 ? DIRS[1][1] : DIRS[2][1]);
+            const T dz = T(j == 0 ? DIRS[0][2] : j == 1 ? DIRS[1][2] : DIRS[2][2]);
+            const T nrm = crossings_sqrt(add_rn(add_rn(mul_rn(dx, dx), mul_rn(dy, dy)), mul_rn(dz, dz)));     // rays_new_kernel
+            const T dir[3] = {div_rn(dx, nrm), div_rn(dy, nrm), div_rn(dz, nrm)};
+            const T inv[3] = {div_rn(T(1), dir[0]), div_rn(T(1), dir[1]), div_rn(T(1), dir[2])};
+            uint32_t front = 0, back = 0;
+            crossings_walk<T>(nodes, n_shapes, aabb, tris, o, dir, inv, Traits<T>::inf(), front, back);
+            votes += (rule == BVHGPU_FILL_EVEN_ODD ? ((front + back) & 1u) != 0u : back != front) ? 1u : 0u;
+        }
+        out_inside[i] = votes >= 2 ? 1 : 0;
+    }
+}
+
+// Signed distance: the knn_triangles row (k = 1) negated where the point is inside; a point without a triangle keeps +inf.
+template <class T>
+__global__ void __launch_bounds__(256) apply_sign_kernel(uint32_t n, const uint8_t* __restrict__ inside, const uint32_t* __restrict__ shape,
+                                                         T* __restrict__ dist) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (inside[i] && shape[i] != BVH_INVALID) dist[i] = -dist[i];       // inside at distance 0 gives -0
+}
+
+// The checks shared by the three calls, in multi hit's order after the caller's null and layout / rule checks: n, the tree's status,
+// then the triangles.  *nothing: n = 0, nothing to launch.
+template <class T>
+static int crossings_checks(Tree<T>* tree, size_t n, const char* who, bool* nothing) {
+    *nothing = false;
+    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", who, n); return BVHGPU_ERR_INVALID; }
+    if (n == 0) { *nothing = true; return BVHGPU_OK; }
+    BVH_TRY(resolve_status(tree));
+    if (tree->n && !tree->d_tris) { set_error("%s: needs bvhgpu_tree_set_triangles_* first", who); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+
+template <class T>
+int count_hits_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const T* d_tmax, uint32_t* d_front, uint32_t* d_back) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    cudaStream_t st = ctx->stream;
+    if (nrays > 0x7FFFFFFFull) { set_error("count_hits: too many rays"); return BVHGPU_ERR_INVALID; }
+    if (fmt != BVHGPU_RAYS_FULL && fmt != BVHGPU_RAYS_OD) { set_error("count_hits: bad ray layout %u", fmt); return BVHGPU_ERR_INVALID; }
+    bool nothing;
+    BVH_TRY(crossings_checks(tree, nrays, "count_hits", &nothing));
+    if (nothing) return BVHGPU_OK;
+    if (tree->n == 0) {
+        BVH_CUDA_TRY(cudaMemsetAsync(d_front, 0, sizeof(uint32_t) * nrays, st));
+        BVH_CUDA_TRY(cudaMemsetAsync(d_back, 0, sizeof(uint32_t) * nrays, st));
+        return BVHGPU_OK;
+    }
+    crossings_kernel<T, false><<<(unsigned)((nrays + 127) / 128), 128, 0, st>>>(
+        tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), reinterpret_cast<const T*>(d_rays),
+        fmt == BVHGPU_RAYS_FULL ? 9u : 6u, (uint32_t)nrays, d_tmax, d_front, d_back, 0, nullptr);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+static int check_rule(const char* who, int rule) {
+    if (rule != BVHGPU_FILL_EVEN_ODD && rule != BVHGPU_FILL_NONZERO) { set_error("%s: unknown fill rule %d", who, rule); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+
+// The containment walk after the checks: out_inside[n] (device), all zero for an empty tree.
+template <class T>
+static int contains_launch(Tree<T>* tree, const T* d_points, size_t n, int rule, uint8_t* d_inside) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    if (tree->n == 0) {
+        BVH_CUDA_TRY(cudaMemsetAsync(d_inside, 0, n, ctx->stream));
+        return BVHGPU_OK;
+    }
+    crossings_kernel<T, true><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(
+        tree->d_nodes, tree->n, tree->d_aabb, reinterpret_cast<const DTri<T>*>(tree->d_tris), d_points, 3u, (uint32_t)n, nullptr, nullptr,
+        nullptr, rule, d_inside);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+template <class T>
+int contains_points_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint8_t* d_inside) {
+    BVH_TRY(check_rule("contains_points", rule));
+    bool nothing;
+    BVH_TRY(crossings_checks(tree, n, "contains_points", &nothing));
+    if (nothing) return BVHGPU_OK;
+    return contains_launch(tree, d_points, n, rule, d_inside);
+}
+
+// knn_tri_device with k = 1 and no limit, the containment walk into scratch from the context's pool, apply_sign_kernel: three launches
+// on the context's stream, nothing synchronises.
+template <class T>
+int signed_distance_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint32_t* d_shape, T* d_dist, T* d_closest) {
+    BVH_TRY(check_rule("signed_distance", rule));
+    bool nothing;
+    BVH_TRY(crossings_checks(tree, n, "signed_distance", &nothing));
+    if (nothing) return BVHGPU_OK;
+    bvhgpu_ctx* ctx = tree->ctx;
+    Scratch scratch(ctx);
+    uint8_t* inside = nullptr;
+    BVH_TRY(scratch.get(&inside, n));
+    BVH_TRY(knn_tri_device<T>(tree, d_points, n, 1, nullptr, d_shape, d_dist, d_closest));
+    BVH_TRY(contains_launch(tree, d_points, n, rule, inside));
+    apply_sign_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>((uint32_t)n, inside, d_shape, d_dist);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+
+template int count_hits_device<float>(Tree<float>*, const void*, uint32_t, size_t, const float*, uint32_t*, uint32_t*);
+template int count_hits_device<double>(Tree<double>*, const void*, uint32_t, size_t, const double*, uint32_t*, uint32_t*);
+template int contains_points_device<float>(Tree<float>*, const float*, size_t, int, uint8_t*);
+template int contains_points_device<double>(Tree<double>*, const double*, size_t, int, uint8_t*);
+template int signed_distance_device<float>(Tree<float>*, const float*, size_t, int, uint32_t*, float*, float*);
+template int signed_distance_device<double>(Tree<double>*, const double*, size_t, int, uint32_t*, double*, double*);
 
 template int set_triangles<float>(Tree<float>*, const float*, size_t, bool);
 template int set_triangles<double>(Tree<double>*, const double*, size_t, bool);

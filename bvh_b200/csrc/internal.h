@@ -319,6 +319,14 @@ template <class T> int multi_hit_device(Tree<T>* tree, const void* d_rays, uint3
 template <int D, class T> int multi_hit_aabb_device(bvhgpu_ctx* ctx, const typename ClosestLayout<D, T>::Node* nodes, uint32_t n_shapes,
                                                     const typename ClosestLayout<D, T>::Box* aabb, const T* d_rays, size_t nrays, uint32_t k,
                                                     const T* d_tmax, uint32_t* d_shape, T* d_dist);
+// Crossing counts, point-in-mesh and signed distance (closest.cu, crossings_kernel): device pointers, on the context's stream, nothing
+// synchronises.  Each checks n (<= 2^31-1), its layout / rule, then (n > 0) the tree's status and the triangles; the pointers are
+// checked by the caller.  An empty tree gives zeros (counts, inside); signed_distance_device is knn_tri_device (k = 1, no limit), the
+// containment walk into scratch and the sign.
+template <class T> int count_hits_device(Tree<T>* tree, const void* d_rays, uint32_t fmt, size_t nrays, const T* d_tmax, uint32_t* d_front,
+                                         uint32_t* d_back);
+template <class T> int contains_points_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint8_t* d_inside);
+template <class T> int signed_distance_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint32_t* d_shape, T* d_dist, T* d_closest);
 template <class T> int rays_new_device(bvhgpu_ctx* ctx, const T* d_origins, const T* d_dirs, size_t n,
                                        typename Traits<T>::Ray* d_rays);
 

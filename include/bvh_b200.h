@@ -647,6 +647,77 @@ int bvhgpu_multi_hit_dev_f32x4(bvhgpu_tree4f* tree, const void* dev_rays, size_t
 int bvhgpu_multi_hit_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_rays, size_t nrays, uint32_t k, const void* dev_tmax, void* dev_shape,
                                void* dev_dist);
 
+/* ---- crossing counts per ray (D = 3): how many triangles a ray crosses, front and back faces apart.  The triangles are those of
+ * bvhgpu_tree_set_triangles_* (shape s carries triangle (a, b, c)).  mt(o, d, a, b, c) = Ray::intersects_triangle (Moeller-Trumbore
+ * with back-face culling, the reference's operation order, no FMA; the function of closest_hit), evaluated twice per triangle:
+ *   out_front[r] = #{ s : mt(o, d, a, b, c) is finite and < tmax[r] }
+ *   out_back[r]  = #{ s : mt(o, d, a, c, b) is finite and < tmax[r] }   (b and c exchanged: the back-face test, the same function)
+ * A triangle whose two evaluations are both finite counts in both columns.  `tmax` NULL: no limit and no comparison; tmax[r] <= 0 (-0
+ * included) or NaN gives 0 / 0 (the comparison is strict).
+ *   Candidates: Bvh::traverse's set (BVH semantics: leaves reached through the child boxes their ancestors store, a NaN slab value
+ *   rejects; n = 1: the shape's own box).  No distance pruning.  With a limit, a child is entered when its slab test passes and its
+ *   entry <= fl(tmax[r] * (1 + 2^-16)), the margin of any_hit.
+ *   tmax NULL: the counts are EXACTLY the loop over Bvh::traverse(ray) with both windings, for every input.
+ *   With a limit: the same wherever every counted triangle is bounded: the box its parent stores for it passes the slab test with
+ *   entry <= fl(d_s * (1 + 2^-16)), d_s the distance it is counted with.  A triangle that is not bounded (a grazing hit whose rounded
+ *   distance lies more than 2^-16 in front of its box's entry, or a stale triangle outside its box) may be missed; then its exact
+ *   intersection lies beyond tmax.  Every count is at most the unpruned one.
+ *   A null argument, nrays > 2^31-1, an unknown ray_layout, or a non-empty tree without triangles (never set, or dropped by
+ *   bvhgpu_add_shapes_*): BVHGPU_ERR_INVALID, nothing written.  nrays = 0: no-op.  An empty tree gives zeros.  A failed build is
+ *   reported sticky, before missing triangles.  After bvhgpu_remove_shapes_* the triangles follow their shapes.  The _dev forms take
+ *   device pointers (FULL or OD rays, dev_tmax may be NULL) and enqueue on the context's stream without synchronising. */
+int bvhgpu_count_hits_f32x3(bvhgpu_tree3f* tree, const bvh_ray3f* rays, size_t nrays, const float* tmax, uint32_t* out_front,
+                            uint32_t* out_back);
+int bvhgpu_count_hits_f64x3(bvhgpu_tree3d* tree, const bvh_ray3d* rays, size_t nrays, const double* tmax, uint32_t* out_front,
+                            uint32_t* out_back);
+int bvhgpu_count_hits_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax,
+                                void* dev_front, void* dev_back);   /* FULL or OD rays, as closest_hit_dev */
+int bvhgpu_count_hits_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_rays, int ray_layout, size_t nrays, const void* dev_tmax,
+                                void* dev_front, void* dev_back);
+
+/* ---- point-in-mesh (D = 3): is each point inside the closed triangle mesh of bvhgpu_tree_set_triangles_*?  (voxelisation, occupancy
+ * grids, particle-in-body tests.)  From every point p three rays r_j = Ray::new(p, D_j) are cast, j = 0, 1, 2, with the fixed directions
+ * BVHGPU_CONTAINS_DIRECTIONS (normalised as bvhgpu_rays_new_dev_* normalises, bit for bit; in f32 each literal is first rounded to
+ * float).  They are not axis-aligned, not parallel to a face diagonal of an axis-aligned cube, and not parallel to each other.  Each
+ * ray counts (front_j, back_j) as bvhgpu_count_hits_* with no limit and votes inside:
+ *   BVHGPU_FILL_EVEN_ODD   front_j + back_j odd.  Ignores orientation (flipped triangles do not matter); overlapping closed parts cancel.
+ *   BVHGPU_FILL_NONZERO    back_j != front_j.  Needs consistently oriented (outward) shells; gives the union of overlapping parts.
+ * out_inside[i] = 1 when at least two of the three rays vote inside, else 0.  The vote is there because Moeller-Trumbore is not
+ * watertight: a ray through a shared edge or vertex can count twice or not at all; three directions make one such ray harmless.
+ * Limits:
+ *   - the result is meaningful for closed meshes only (an open mesh, such as a scene without its floor, gives whatever the rays count);
+ *   - a point on the surface is undefined;
+ *   - a triangle with |det| < eps (f32::EPSILON / f64::EPSILON, the reference's test) is invisible to every ray.  det scales with the
+ *     square of the edge lengths (the directions are normalised), so in f32 triangles with edges below about 3e-4 never count: a mesh
+ *     whose triangles are all that small (a tiny mesh in absolute units) contains no point; scale it up first.
+ * A point with a NaN coordinate gives 0.  An unknown `rule`: BVHGPU_ERR_INVALID; the other refusals, the sticky failure and the empty
+ * tree (all 0) as bvhgpu_count_hits_*.  The _dev form takes device pointers and enqueues on the context's stream without synchronising. */
+typedef enum { BVHGPU_FILL_EVEN_ODD = 0, BVHGPU_FILL_NONZERO = 1 } bvhgpu_fill_rule;
+#define BVHGPU_CONTAINS_DIRECTIONS \
+    { { 0.7548776662466927, 0.5698402909980532, 0.3247179572447460 },  \
+      { -0.5698402909980532, 0.3247179572447460, 0.7548776662466927 }, \
+      { 0.3247179572447460, -0.7548776662466927, 0.5698402909980532 } }
+int bvhgpu_contains_points_f32x3(bvhgpu_tree3f* tree, const float* points, size_t n, int rule, uint8_t* out_inside);
+int bvhgpu_contains_points_f64x3(bvhgpu_tree3d* tree, const double* points, size_t n, int rule, uint8_t* out_inside);
+int bvhgpu_contains_points_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_points, size_t n, int rule, void* dev_inside);
+int bvhgpu_contains_points_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_points, size_t n, int rule, void* dev_inside);
+
+/* ---- signed distance to a closed triangle mesh (D = 3): SDF generation, penetration depth, contact.  out_shape, |out_dist| and
+ * out_closest (may be NULL) are bit for bit bvhgpu_knn_triangles_* with k = 1 and no radius, with its guarantee (the brute-force
+ * nearest triangle wherever the qualifying triangles are bounded).  out_dist is negated exactly where bvhgpu_contains_points_* with the
+ * same rule says inside (inside at distance 0 gives -0).  A point without a qualifying triangle keeps +inf, BVHGPU_INVALID_INDEX and a
+ * NaN closest point, whatever its vote.  The limits of bvhgpu_contains_points_* apply to the sign.  Refusals as
+ * bvhgpu_contains_points_*, nothing written.  The _dev form enqueues the k = 1 query, the containment walk and the sign on the
+ * context's stream without synchronising. */
+int bvhgpu_signed_distance_f32x3(bvhgpu_tree3f* tree, const float* points, size_t n, int rule, uint32_t* out_shape, float* out_dist,
+                                 float* out_closest);
+int bvhgpu_signed_distance_f64x3(bvhgpu_tree3d* tree, const double* points, size_t n, int rule, uint32_t* out_shape, double* out_dist,
+                                 double* out_closest);
+int bvhgpu_signed_distance_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_points, size_t n, int rule, void* dev_shape, void* dev_dist,
+                                     void* dev_closest);
+int bvhgpu_signed_distance_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_points, size_t n, int rule, void* dev_shape, void* dev_dist,
+                                     void* dev_closest);
+
 /* ---- self-overlap pairs: every pair of shapes of the tree whose AABBs intersect, each once (the broad phase of physics, mesh
  * self-intersection, duplicate and contact detection in point and particle sets).  leaf(s) = the preorder node index of shape s's leaf
  * (out_node_index of bvhgpu_tree_nodes_*).  Output: a CSR indexed by shape, offsets[n + 1]; row s lists every shape t with

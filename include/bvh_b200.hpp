@@ -102,6 +102,9 @@ template <> struct Abi<float> {
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_closest_hit_f32x3(t, r, n, tri, s, d, uv); }
     static int any(tree* t, const ray* r, size_t n, const float* tm, int tri, uint32_t* s) { return bvhgpu_any_hit_f32x3(t, r, n, tm, tri, s); }
     static int multi(tree* t, const ray* r, size_t n, uint32_t k, const float* tm, int tri, uint32_t* s, float* d, float* uv) { return bvhgpu_multi_hit_f32x3(t, r, n, k, tm, tri, s, d, uv); }
+    static int count_hits(tree* t, const ray* r, size_t n, const float* tm, uint32_t* f, uint32_t* b) { return bvhgpu_count_hits_f32x3(t, r, n, tm, f, b); }
+    static int contains(tree* t, const float* p, size_t n, int rule, uint8_t* in) { return bvhgpu_contains_points_f32x3(t, p, n, rule, in); }
+    static int signed_distance(tree* t, const float* p, size_t n, int rule, uint32_t* s, float* d, float* q) { return bvhgpu_signed_distance_f32x3(t, p, n, rule, s, d, q); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f32x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
     static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f32x3(t, off, h, cap, tot); }
@@ -123,6 +126,9 @@ template <> struct Abi<double> {
     static int closest(tree* t, const ray* r, size_t n, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_closest_hit_f64x3(t, r, n, tri, s, d, uv); }
     static int any(tree* t, const ray* r, size_t n, const double* tm, int tri, uint32_t* s) { return bvhgpu_any_hit_f64x3(t, r, n, tm, tri, s); }
     static int multi(tree* t, const ray* r, size_t n, uint32_t k, const double* tm, int tri, uint32_t* s, double* d, double* uv) { return bvhgpu_multi_hit_f64x3(t, r, n, k, tm, tri, s, d, uv); }
+    static int count_hits(tree* t, const ray* r, size_t n, const double* tm, uint32_t* f, uint32_t* b) { return bvhgpu_count_hits_f64x3(t, r, n, tm, f, b); }
+    static int contains(tree* t, const double* p, size_t n, int rule, uint8_t* in) { return bvhgpu_contains_points_f64x3(t, p, n, rule, in); }
+    static int signed_distance(tree* t, const double* p, size_t n, int rule, uint32_t* s, double* d, double* q) { return bvhgpu_signed_distance_f64x3(t, p, n, rule, s, d, q); }
     static int add(tree* t, const aabb* a, size_t k, double g, size_t* r) { return bvhgpu_add_shapes_f64x3(t, a, k, g, r); }
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
     static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f64x3(t, off, h, cap, tot); }
@@ -381,6 +387,29 @@ template <class T> class Bvh {
         if (uv) uv->assign(2 * rays.size() * k, T(0));
         check(A::multi(tree_, reinterpret_cast<const typename A::ray*>(rays.data()), rays.size(), k, tmax.empty() ? nullptr : tmax.data(),
                        triangles ? 1 : 0, shape.data(), distance.data(), uv ? uv->data() : nullptr));
+    }
+    // Crossing counts per ray over the triangles of set_triangles: front[i] / back[i] = the triangles ray i crosses at a distance < tmax[i]
+    // (tmax empty: no limit) through their front / back face (Ray::intersects_triangle with the winding as given / reversed).
+    void count_hits(const std::vector<Ray<T>>& rays, const std::vector<T>& tmax, std::vector<uint32_t>& front, std::vector<uint32_t>& back) const {
+        if (!tmax.empty() && tmax.size() != rays.size()) throw Error(BVHGPU_ERR_INVALID, "count_hits: one limit per ray, or none");
+        front.assign(rays.size(), 0); back.assign(rays.size(), 0);
+        check(A::count_hits(tree_, reinterpret_cast<const typename A::ray*>(rays.data()), rays.size(), tmax.empty() ? nullptr : tmax.data(),
+                            front.data(), back.data()));
+    }
+    // Point-in-mesh over the closed mesh of set_triangles (3 T per point): inside[i] = 1 when two of three fixed rays from point i vote
+    // inside under `rule` (BVHGPU_FILL_EVEN_ODD or BVHGPU_FILL_NONZERO).  Points on the surface are undefined.
+    void contains(const std::vector<T>& points, int rule, std::vector<uint8_t>& inside) const {
+        inside.assign(points.size() / 3, 0);
+        check(A::contains(tree_, points.data(), points.size() / 3, rule, inside.data()));
+    }
+    // Signed distance to the closed mesh: knn_triangles with k = 1 (shape, distance, and closest point when given), the distance negated
+    // where contains(rule) says inside.
+    void signed_distance(const std::vector<T>& points, int rule, std::vector<uint32_t>& shape, std::vector<T>& distance,
+                         std::vector<T>* closest = nullptr) const {
+        const size_t n = points.size() / 3;
+        shape.assign(n, 0); distance.assign(n, T(0));
+        if (closest) closest->assign(3 * n, T(0));
+        check(A::signed_distance(tree_, points.data(), n, rule, shape.data(), distance.data(), closest ? closest->data() : nullptr));
     }
     size_t num_shapes() const { return n_; }
 

@@ -65,6 +65,14 @@ for prec, ncubes in (("f32", 60), ("f32", 700), ("f64", 300)):
     d_ms = torch.empty(len(rays) * 7, dtype=torch.int32, device="cuda:0"); d_md = torch.empty(len(rays) * 7, dtype=tdt, device="cuda:0")
     b.multi_hit_dev(d_r.data_ptr(), len(rays), 7, d_tm.data_ptr(), d_ms.data_ptr(), d_md.data_ptr(), triangles=True, layout=capi.RAYS_OD)
     ctx.synchronize()
+    # crossing counts (with and without limits, OD rays on the device), point-in-mesh under both rules, signed distance with closest points
+    b.count_hits(rays); b.count_hits(rays, cd)
+    b.count_hits_dev(d_r.data_ptr(), len(rays), d_tm.data_ptr(), d_ms.data_ptr(), d_ms.data_ptr() + 4 * len(rays), layout=capi.RAYS_OD)
+    cpts = np.concatenate([pts[:200], scenes.create_n_cubes_tris(ncubes, prec).reshape(-1, 12, 9)[:, :, :3].mean(axis=1)[:200]])
+    b.contains(cpts, "even_odd"); b.contains(cpts, "nonzero"); b.signed_distance(cpts, closest=True)
+    d_cp = torch.from_numpy(np.ascontiguousarray(cpts, dtype=a["min"].dtype)).to("cuda:0")
+    b.signed_distance_dev(d_cp.data_ptr(), len(cpts), d_ms.data_ptr(), d_md.data_ptr(), 0, rule="nonzero")
+    ctx.synchronize()
     b.free()
 # D = 2
 from bvh_b200.dtypes import BY_PREC_2D
