@@ -3,8 +3,8 @@ bvhgpu_signed_distance_* and their _dev forms), f32 and f64, against the restate
 - count_hits without a limit equals the loop over traverse_batch's CSR with both windings, on the configs[1] 120 k-triangle cube scene
   (10^5 rays aimed at its cubes) and on Sponza (an open mesh), host form and _dev with FULL and OD rays; the difference to the brute
   force over every triangle is reported, and the device never counts more;
-- with per-ray and scalar limits (0, -0, NaN, +inf, random) the counts equal the loop on every bounded row, never exceed it elsewhere,
-  and the number of unbounded rows is reported;
+- with per-ray and scalar limits (0, -0, NaN, +inf, random) the counts equal the limited-walk model of tests/crosswalk.py on every
+  row and the loop on every bounded row, never exceed the loop elsewhere, and the number of unbounded rows is reported;
 - contains equals the vote on the device's own counts and on restated counts, and the truth on the cube scene, an icosphere, a torus
   and (EVEN_ODD) an icosphere with flipped triangles; signed_distance is knn_triangles(k = 1) with the sign of contains;
 - the contract: empty tree, n = 1, n = 0, NaN points and rays, refusals that write nothing, the sticky build before missing triangles,
@@ -15,6 +15,7 @@ import pytest
 
 from oracle import oracle as O
 from tests import crossings as X
+from tests import crosswalk as W
 from tests.test_crossings_cpu import cube_points, flip_some, sphere_points, torus_points
 from tests.test_knn_triangles_cpu import sponza_tris
 
@@ -129,10 +130,13 @@ def test_count_hits_with_limits_on_bounded_rows(scene):
     sub = slice(0, 20_000)
     r = rays[sub]
     o2, h2 = bvh.traverse_batch(r)
+    cand = W.candidates(bvh.nodes, shapes, r)
     for lname, tm in _limit_families(r, bvh, F, np.random.default_rng(4)).items():
         want = X.counts_csr(r, tris, o2, h2, tm)
         ok = X.bounded_rows(r, tris, bvh.nodes, shapes, o2, h2, tm)
+        model = W.model(bvh.nodes, shapes, tris, r, tm, cand)
         for i, got in enumerate(_forms(bvh, r, tm, prec)):
+            assert np.array_equal(got[0], model[0]) and np.array_equal(got[1], model[1]), (name, lname, i)
             assert np.array_equal(got[0][ok], want[0][ok]) and np.array_equal(got[1][ok], want[1][ok]), (name, lname, i)
             assert np.all(got[0] <= want[0]) and np.all(got[1] <= want[1]), (name, lname, i)
         if lname in ("zero", "-zero", "nan"):
