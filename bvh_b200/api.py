@@ -149,14 +149,155 @@ class FlatBvh:
         return self._bvh.traverse_batch(rays, mode=capi.TRAVERSE_FLAT)
 
 
-class Bvh:
-    """Device-resident Bvh<T,3>."""
+class _Tree:
+    """What the trees of every dimension share: the handle of one device tree and the calls whose arguments do not depend on D.
+    A subclass sets _TABLE (dtypes.BY_PREC*) and _DIM, and defines _num_shapes()."""
+
+    _TABLE: dict
+    _DIM: int
 
     def __init__(self, handle, prec: str, ctx: Context):
-        self._h = handle
-        self.prec = prec
-        self.ctx = ctx
-        self._d = BY_PREC[prec]
+        self._h, self.prec, self.ctx, self._d = handle, prec, ctx, self._TABLE[prec]
+
+    def free(self):
+        if self._h:
+            getattr(capi.lib(), f"bvhgpu_tree_free_{self._d['suffix']}")(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+    def _points(self, points) -> np.ndarray:
+        return np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, self._DIM)
+
+    def _limits(self, x, n: int):
+        """A per-item limit (tmax, max_dist) as n contiguous scalars of the tree's precision: x is a scalar for all items or one value
+        per item.  None stays None, the null pointer that means no limit."""
+        return None if x is None else np.ascontiguousarray(np.broadcast_to(np.asarray(x, dtype=self._d["scalar"]), (n,)))
+
+    def _csr(self, fn, n: int, cap: int, *args, dists: bool = False):
+        """CSR (offsets u32[n + 1], hits u32[total]) from fn(*args, offsets, hits, cap, &total); with dists=True fn also takes the
+        distances after the hits, and they are returned third.  A short capacity (ERR_CAPACITY with a total the u32 offsets can hold)
+        is completed as the ABI fixes it: a 3-D tree copies the list its walk retained (bvhgpu_traverse_fetch_*); 2-D and 4-D trees
+        retain nothing, and nothing retains distances, so those call again with cap = total."""
+        offsets = np.zeros(n + 1, dtype=np.uint32)
+        while True:
+            out = [np.zeros(cap, dtype=np.uint32)]
+            if dists:
+                out.append(np.zeros(cap, dtype=self._d["scalar"]))
+            total = C.c_size_t(0)
+            st = fn(*args, _ptr(offsets), *map(_ptr, out), cap, C.byref(total))
+            t = total.value
+            if st == capi.ERR_CAPACITY and t <= U32_MAX:
+                if self._DIM == 3 and not dists:
+                    hits = np.zeros(t, dtype=np.uint32)
+                    capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), t))
+                    return offsets, hits
+                if t > cap:
+                    cap = t
+                    continue
+            capi.check(st)
+            return (offsets, *(a[:t] for a in out))
+
+    def flatten(self) -> np.ndarray:
+        n = self._num_shapes()
+        cap = 0 if n == 0 else (1 if n == 1 else 3 * n - 2)
+        out = np.zeros(cap, dtype=self._d["flat"])
+        ln = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_flatten_{self._d['suffix']}")(self._h, _ptr(out), cap, C.byref(ln)))
+        return out[: ln.value]
+
+    def traverse_ordered(self, rays, ascending: bool = True):
+        """Batched nearest_traverse_iterator (ascending: by entry distance) / farthest_traverse_iterator (by exit distance,
+        descending): (offsets, hits, dists), the set of traverse_batch(..., TRAVERSE_BVH) perfectly sorted per ray, ties in DFS order,
+        with the slice distance of the child box the tree stores for each leaf.  A short capacity (default max(8 n, 1024)) is retried
+        at the exact total, hits and distances together."""
+        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
+        fn = getattr(capi.lib(), f"bvhgpu_traverse_ordered_{self._d['suffix']}")
+        return self._csr(fn, len(rays), max(8 * len(rays), 1024), self._h, _ptr(rays), len(rays), 1 if ascending else 0, dists=True)
+
+    def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
+        """Bvh::traverse with Aabb / Point / Ball queries (IntersectsAabb implementors other than Ray): (n, 2D) {min, max} for
+        capi.QUERY_AABB, (n, D) points for QUERY_POINT, (n, D+1) {center, radius} for QUERY_BALL.  CSR (offsets, hits), hits of a
+        query in the reference's DFS order."""
+        D = self._DIM
+        stride = {capi.QUERY_AABB: 2 * D, capi.QUERY_POINT: D, capi.QUERY_BALL: D + 1}[kind]
+        q = np.ascontiguousarray(queries, dtype=self._d["scalar"]).reshape(-1, stride)
+        fn = getattr(capi.lib(), f"bvhgpu_query_{self._d['suffix']}")
+        return self._csr(fn, len(q), max(16 * len(q), 1024), self._h, mode, kind, _ptr(q), len(q))
+
+    def overlap_pairs(self, cap: int | None = None):
+        """Every pair of shapes whose own current AABBs intersect (touching faces included), each once: CSR (offsets[n + 1], hits)
+        indexed by shape, row s = the shapes t with node_index[t] > node_index[s] whose box meets s's, in DFS order.  A short
+        capacity (default max(4 n, 1024)) is completed from the retained list in 3-D (bvhgpu_traverse_fetch_*) and retried once at the
+        exact total in 2-D and 4-D."""
+        n = self._num_shapes()
+        fn = getattr(capi.lib(), f"bvhgpu_overlap_pairs_{self._d['suffix']}")
+        return self._csr(fn, n, max(4 * n, 1024) if cap is None else int(cap), self._h)
+
+    def overlap_pairs_with(self, other, cap: int | None = None):
+        """Every pair (a, b) of a shape of this tree and a shape of `other` whose own current AABBs intersect (touching faces included):
+        CSR (offsets[n + 1], hits) indexed by this tree's shapes, row a = other's shapes whose box meets a's, in other's DFS order.
+        Both trees must share a context; other may be self.  A short capacity (default max(4 n, 1024)) is completed from this tree's
+        retained list in 3-D (bvhgpu_traverse_fetch_*) and retried once at the exact total in 2-D and 4-D."""
+        _same_kind(self, other)
+        n = self._num_shapes()
+        fn = getattr(capi.lib(), f"bvhgpu_overlap_trees_{self._d['suffix']}")
+        return self._csr(fn, n, max(4 * n, 1024) if cap is None else int(cap), self._h, other._h)
+
+    def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
+        """Bvh::nearest_to / FlatBvh::nearest_to (bvh_impl.rs:221-238, flat_bvh.rs:513-562) for shapes whose PointDistance is their AABB
+        distance (the reference's UnitBox): (shape index per point, U32_MAX for an empty tree; distance per point).  points: (n, D)."""
+        p = self._points(points)
+        shape = np.zeros(len(p), dtype=np.uint32)
+        dist = np.zeros(len(p), dtype=self._d["scalar"])
+        capi.check(getattr(capi.lib(), f"bvhgpu_nearest_{self._d['suffix']}")(self._h, mode, _ptr(p), len(p), _ptr(shape), _ptr(dist)))
+        return shape, dist
+
+    def nearest_candidates(self, points):
+        """For shapes with their own PointDistance: CSR (offsets, shape indices) of candidate lists that contain the nearest shape of
+        every point; evaluate distance_squared on each list and keep the minimum (see `nearest_to`).  points: (n, D)."""
+        p = self._points(points)
+        fn = getattr(capi.lib(), f"bvhgpu_nearest_candidates_{self._d['suffix']}")
+        return self._csr(fn, len(p), max(64 * len(p), 1024), self._h, _ptr(p), len(p))
+
+    def nearest_to(self, point, shapes, distance_squared):
+        """BoundingHierarchy::nearest_to for one point and an arbitrary shape distance: `distance_squared(shape, point)` is the shape's
+        PointDistance::distance_squared.  Returns (shape, distance) or None for an empty tree."""
+        off, cand = self.nearest_candidates([point])
+        best = None
+        for s in cand[off[0]:off[1]]:
+            d = distance_squared(shapes[int(s)], point)
+            if best is None or d < best[1]:
+                best = (shapes[int(s)], d)
+        return None if best is None else (best[0], float(np.sqrt(best[1])))
+
+    def knn(self, points, k: int, max_dist=None):
+        """The k nearest shapes of every point (points (n, D)): (shape (n, k) u32, dist (n, k)).  Row i lists the shapes in ascending
+        (Aabb::min_distance_squared of the shape's own box, index) order with their distances; with `max_dist` (a scalar for all points,
+        one limit per point, or None for no limit) only shapes at squared distance <= fl(r * r) qualify (r < 0 or NaN: none).  Slots
+        past the qualifying shapes hold U32_MAX and +inf.  Exact: the head of a stable brute-force sort.  1 <= k <= 64."""
+        p = self._points(points)
+        n = len(p)
+        kk = max(int(k), 0)
+        shape = np.zeros((n, kk), dtype=np.uint32)
+        dist = np.zeros((n, kk), dtype=self._d["scalar"])
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_{self._d['suffix']}")(self._h, _ptr(p), n, int(k) & 0xFFFFFFFF, _ptr(self._limits(max_dist, n)),
+                                                                         _ptr(shape), _ptr(dist)))
+        return shape, dist
+
+
+class Bvh(_Tree):
+    """Device-resident Bvh<T,3>."""
+
+    _TABLE = BY_PREC
+    _DIM = 3
+
+    def __init__(self, handle, prec: str, ctx: Context):
+        super().__init__(handle, prec, ctx)
         self._nodes = None
         self._node_index = None
 
@@ -195,21 +336,13 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_tree_from_nodes_{d['suffix']}")(ctx._h, _ptr(nodes), len(nodes), _ptr(aabbs), len(aabbs), C.byref(h)))
         return cls(h, prec, ctx)
 
-    def free(self):
-        if self._h:
-            getattr(capi.lib(), f"bvhgpu_tree_free_{self._d['suffix']}")(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
-
     # ---- Bvh.nodes / node indices ------------------------------------------------------------------
     @property
     def num_shapes(self) -> int:
         return int(getattr(capi.lib(), f"bvhgpu_tree_num_shapes_{self._d['suffix']}")(self._h))
+
+    def _num_shapes(self) -> int:
+        return self.num_shapes
 
     def _materialise(self):
         if self._nodes is None:
@@ -231,12 +364,7 @@ class Bvh:
 
     # ---- flatten -----------------------------------------------------------------------------------
     def flatten(self) -> FlatBvh:
-        n = self.num_shapes
-        cap = 0 if n == 0 else (1 if n == 1 else 3 * n - 2)
-        out = np.zeros(cap, dtype=self._d["flat"])
-        ln = C.c_size_t(0)
-        capi.check(getattr(capi.lib(), f"bvhgpu_flatten_{self._d['suffix']}")(self._h, _ptr(out), cap, C.byref(ln)))
-        return FlatBvh(self, out[: ln.value])
+        return FlatBvh(self, super().flatten())
 
     def flatten_custom(self, constructor):
         """Bvh::flatten_custom (src/flat_bvh.rs:240-251): `constructor(aabb, entry, exit, shape)` applied to every FlatNode in the
@@ -257,40 +385,12 @@ class Bvh:
         the division Ray::new uses, so the result is bit-identical."""
         rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
         nrays = len(rays)
-        offsets = np.zeros(nrays + 1, dtype=np.uint32)
-        cap = max(4 * nrays, 1024) if cap is None else cap
-        hits = np.zeros(cap, dtype=np.uint32)
-        total = C.c_size_t(0)
         fn = getattr(capi.lib(), f"bvhgpu_traverse_{self._d['suffix']}")
         if compact:
             od = np.empty((nrays, 6), dtype=self._d["scalar"])
             od[:, :3], od[:, 3:] = rays["origin"], rays["direction"]
             rays, fn = od, getattr(capi.lib(), f"bvhgpu_traverse_od_{self._d['suffix']}")
-        st = fn(self._h, mode, _ptr(rays), nrays, _ptr(offsets), _ptr(hits), cap, C.byref(total))
-        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
-            hits = np.zeros(total.value, dtype=np.uint32)
-            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), total.value))
-        else:
-            capi.check(st)
-        return offsets, hits[: total.value]
-
-    def traverse_ordered(self, rays: np.ndarray, ascending: bool = True):
-        """Batched nearest_traverse_iterator / farthest_traverse_iterator: CSR + distances, perfectly sorted per ray."""
-        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
-        n = len(rays)
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(8 * n, 1024)
-        fn = getattr(capi.lib(), f"bvhgpu_traverse_ordered_{self._d['suffix']}")
-        while True:
-            hits = np.zeros(cap, dtype=np.uint32)
-            dists = np.zeros(cap, dtype=self._d["scalar"])
-            total = C.c_size_t(0)
-            st = fn(self._h, _ptr(rays), n, 1 if ascending else 0, _ptr(offsets), _ptr(hits), _ptr(dists), cap, C.byref(total))
-            if st == capi.ERR_CAPACITY and total.value <= U32_MAX and total.value > cap:
-                cap = total.value
-                continue
-            capi.check(st)
-            return offsets, hits[: total.value], dists[: total.value]
+        return self._csr(fn, nrays, max(4 * nrays, 1024) if cap is None else cap, self._h, mode, _ptr(rays), nrays)
 
     def set_triangles(self, triangles):
         """Triangle vertices of the shapes (n, 3, 3) or (n, 9): enables closest_hit(..., triangles=True).  Triangle i must lie inside shape i's AABB."""
@@ -315,8 +415,8 @@ class Bvh:
         rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
         n = len(rays)
         shape = np.zeros(n, dtype=np.uint32)
-        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
-        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), 1 if triangles else 0, _ptr(shape)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(self._limits(tmax, n)),
+                                                                             1 if triangles else 0, _ptr(shape)))
         return shape
 
     def multi_hit(self, rays: np.ndarray, k: int, tmax=None, triangles: bool = False, uv: bool = False):
@@ -331,9 +431,9 @@ class Bvh:
         shape = np.zeros((n, kk), dtype=np.uint32)
         dist = np.zeros((n, kk), dtype=self._d["scalar"])
         u = np.zeros((n, kk, 2), dtype=self._d["scalar"]) if uv else None
-        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
-        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, int(k) & 0xFFFFFFFF, _ptr(tm),
-                                                                                1 if triangles else 0, _ptr(shape), _ptr(dist), _ptr(u)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, int(k) & 0xFFFFFFFF,
+                                                                                _ptr(self._limits(tmax, n)), 1 if triangles else 0, _ptr(shape),
+                                                                                _ptr(dist), _ptr(u)))
         return shape, dist, u
 
     def multi_hit_dev(self, rays_ptr: int, nrays: int, k: int, tmax_ptr: int, shape_ptr: int, dist_ptr: int, uv_ptr: int = 0,
@@ -345,15 +445,8 @@ class Bvh:
             self._h, C.c_void_p(rays_ptr), layout, nrays, k, C.c_void_p(tmax_ptr or None), 1 if triangles else 0, C.c_void_p(shape_ptr),
             C.c_void_p(dist_ptr), C.c_void_p(uv_ptr or None)))
 
-    def knn(self, points, k: int, max_dist=None):
-        """The k nearest shapes of every point: (shape (n, k) u32, dist (n, k)).  Row i lists the shapes in ascending
-        (Aabb::min_distance_squared of the shape's own box, index) order with their distances; with `max_dist` (a scalar for all points,
-        one limit per point, or None for no limit) only shapes at squared distance <= fl(r * r) qualify (r < 0 or NaN: none).  Slots
-        past the qualifying shapes hold U32_MAX and +inf.  Exact: the head of a stable brute-force sort.  1 <= k <= 64."""
-        return _knn_call(self, points, 3, k, max_dist)
-
     def knn_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int):
-        """knn from device pointers: n points (3 scalars each) and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes and
+        """knn from device pointers: n points (D scalars each) and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes and
         distances out, enqueued on the context's stream without host synchronisation."""
         capi.check(getattr(capi.lib(), f"bvhgpu_knn_dev_{self._d['suffix']}")(self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None),
                                                                              C.c_void_p(shape_ptr), C.c_void_p(dist_ptr)))
@@ -363,15 +456,15 @@ class Bvh:
         closest=True.  Keys are Triangle::distance_squared (testbase.rs:353-443), the distance of nearest_triangles_batch; NaN keys never
         qualify; `max_dist` as in knn.  Slots past the qualifying triangles hold U32_MAX, +inf and NaN closest points.  Equal to a
         stable brute-force sort wherever every qualifying triangle's key is at least its own box's pruning bound (DESIGN.md 4.17)."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        p = self._points(points)
         n = len(p)
-        r = None if max_dist is None else np.ascontiguousarray(np.broadcast_to(np.asarray(max_dist, dtype=self._d["scalar"]), (n,)))
         kk = max(int(k), 0)
         shape = np.zeros((n, kk), dtype=np.uint32)
         dist = np.zeros((n, kk), dtype=self._d["scalar"])
         q = np.zeros((n, kk, 3), dtype=self._d["scalar"]) if closest else None
-        capi.check(getattr(capi.lib(), f"bvhgpu_knn_triangles_{self._d['suffix']}")(self._h, _ptr(p), n, int(k) & 0xFFFFFFFF, _ptr(r), _ptr(shape),
-                                                                                   _ptr(dist), _ptr(q)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_triangles_{self._d['suffix']}")(self._h, _ptr(p), n, int(k) & 0xFFFFFFFF,
+                                                                                   _ptr(self._limits(max_dist, n)), _ptr(shape), _ptr(dist),
+                                                                                   _ptr(q)))
         return (shape, dist, q) if closest else (shape, dist)
 
     def knn_triangles_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int, closest_ptr: int = 0):
@@ -390,8 +483,8 @@ class Bvh:
         n = len(rays)
         front = np.zeros(n, dtype=np.uint32)
         back = np.zeros(n, dtype=np.uint32)
-        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
-        capi.check(getattr(capi.lib(), f"bvhgpu_count_hits_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), _ptr(front), _ptr(back)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_count_hits_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(self._limits(tmax, n)), _ptr(front),
+                                                                                _ptr(back)))
         return front, back
 
     def count_hits_dev(self, rays_ptr: int, nrays: int, tmax_ptr: int, front_ptr: int, back_ptr: int, layout: int = capi.RAYS_FULL):
@@ -406,7 +499,7 @@ class Bvh:
         """Point-in-mesh over the closed triangle mesh of set_triangles: bool (n,).  Three fixed rays per point vote; rule "even_odd"
         (front + back odd, orientation ignored) or "nonzero" (back != front, outward-oriented shells).  Points on the surface are
         undefined; a NaN point is outside (DESIGN.md 4.21)."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        p = self._points(points)
         out = np.zeros(len(p), dtype=np.uint8)
         capi.check(getattr(capi.lib(), f"bvhgpu_contains_points_{self._d['suffix']}")(self._h, _ptr(p), len(p), self._RULES[rule], _ptr(out)))
         return out.astype(bool)
@@ -420,7 +513,7 @@ class Bvh:
     def signed_distance(self, points, rule: str = "even_odd", closest: bool = False):
         """Signed distance to the closed triangle mesh of set_triangles: (shape (n,) u32, dist (n,)), plus closest (n, 3) with
         closest=True.  shape, |dist| and closest are knn_triangles(points, 1); dist is negated where contains(points, rule) is true."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        p = self._points(points)
         n = len(p)
         shape = np.zeros(n, dtype=np.uint32)
         dist = np.zeros(n, dtype=self._d["scalar"])
@@ -435,41 +528,6 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_signed_distance_dev_{self._d['suffix']}")(
             self._h, C.c_void_p(points_ptr), n, self._RULES[rule], C.c_void_p(shape_ptr), C.c_void_p(dist_ptr), C.c_void_p(closest_ptr or None)))
 
-    def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
-        """Bvh::traverse with Aabb / Point / Ball queries (IntersectsAabb implementors other than Ray).
-        queries: (n, 6) {min,max} for capi.QUERY_AABB, (n, 3) for QUERY_POINT, (n, 4) {center, radius} for QUERY_BALL."""
-        stride = {capi.QUERY_AABB: 6, capi.QUERY_POINT: 3, capi.QUERY_BALL: 4}[kind]
-        q = np.ascontiguousarray(queries, dtype=self._d["scalar"]).reshape(-1, stride)
-        n = len(q)
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(16 * n, 1024)
-        hits = np.zeros(cap, dtype=np.uint32)
-        total = C.c_size_t(0)
-        st = getattr(capi.lib(), f"bvhgpu_query_{self._d['suffix']}")(self._h, mode, kind, _ptr(q), n, _ptr(offsets), _ptr(hits), cap, C.byref(total))
-        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
-            hits = np.zeros(total.value, dtype=np.uint32)
-            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), total.value))
-        else:
-            capi.check(st)
-        return offsets, hits[: total.value]
-
-    def overlap_pairs(self, cap: int | None = None):
-        """Every pair of shapes whose own current AABBs intersect (touching faces included), each once: CSR (offsets[n + 1], hits)
-        indexed by shape, row s = the shapes t with node_index[t] > node_index[s] whose box meets s's, in DFS order.  A short
-        capacity (default max(4 n, 1024)) is completed from the retained list (bvhgpu_traverse_fetch_*)."""
-        n = self.num_shapes
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(4 * n, 1024) if cap is None else int(cap)
-        hits = np.zeros(cap, dtype=np.uint32)
-        total = C.c_size_t(0)
-        st = getattr(capi.lib(), f"bvhgpu_overlap_pairs_{self._d['suffix']}")(self._h, _ptr(offsets), _ptr(hits), cap, C.byref(total))
-        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
-            hits = np.zeros(total.value, dtype=np.uint32)
-            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), total.value))
-        else:
-            capi.check(st)
-        return offsets, hits[: total.value]
-
     def overlap_pairs_dev(self, offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
         """overlap_pairs into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets are
         always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
@@ -477,25 +535,6 @@ class Bvh:
         capi.check(getattr(capi.lib(), f"bvhgpu_overlap_pairs_dev_{self._d['suffix']}")(self._h, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr or None),
                                                                                        cap, C.byref(total) if want_total else None))
         return total.value if want_total else None
-
-    def overlap_pairs_with(self, other: "Bvh", cap: int | None = None):
-        """Every pair (a, b) of a shape of this tree and a shape of `other` whose own current AABBs intersect (touching faces included):
-        CSR (offsets[n + 1], hits) indexed by this tree's shapes, row a = other's shapes whose box meets a's, in other's DFS order.
-        Both trees must share a context; other may be self.  A short capacity (default max(4 n, 1024)) is completed from this
-        tree's retained list (bvhgpu_traverse_fetch_*)."""
-        _same_kind(self, other)
-        n = self.num_shapes
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(4 * n, 1024) if cap is None else int(cap)
-        hits = np.zeros(cap, dtype=np.uint32)
-        total = C.c_size_t(0)
-        st = getattr(capi.lib(), f"bvhgpu_overlap_trees_{self._d['suffix']}")(self._h, other._h, _ptr(offsets), _ptr(hits), cap, C.byref(total))
-        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
-            hits = np.zeros(total.value, dtype=np.uint32)
-            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(hits), total.value))
-        else:
-            capi.check(st)
-        return offsets, hits[: total.value]
 
     def overlap_pairs_with_dev(self, other: "Bvh", offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
         """overlap_pairs_with into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets
@@ -507,54 +546,19 @@ class Bvh:
                                                                                        C.byref(total) if want_total else None))
         return total.value if want_total else None
 
-    def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
-        """Bvh::nearest_to / FlatBvh::nearest_to (bvh_impl.rs:221-238, flat_bvh.rs:513-562) for shapes whose PointDistance is their AABB
-        distance (the reference's UnitBox): (shape index per point, U32_MAX for an empty tree; distance per point)."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
-        shape = np.zeros(len(p), dtype=np.uint32)
-        dist = np.zeros(len(p), dtype=self._d["scalar"])
-        capi.check(getattr(capi.lib(), f"bvhgpu_nearest_{self._d['suffix']}")(self._h, mode, _ptr(p), len(p), _ptr(shape), _ptr(dist)))
-        return shape, dist
-
     def nearest_triangles_batch(self, points, mode: int = capi.TRAVERSE_BVH):
         """Bvh::nearest_to / FlatBvh::nearest_to for triangle shapes (set_triangles first): the reference's walk with
         Triangle::distance_squared (testbase.rs:353-443) at the leaves, on the device: (shape index, distance) per point."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
+        p = self._points(points)
         shape = np.zeros(len(p), dtype=np.uint32)
         dist = np.zeros(len(p), dtype=self._d["scalar"])
         capi.check(getattr(capi.lib(), f"bvhgpu_nearest_triangles_{self._d['suffix']}")(self._h, mode, _ptr(p), len(p), _ptr(shape), _ptr(dist)))
         return shape, dist
 
-    def nearest_candidates(self, points):
-        """For shapes with their own PointDistance: CSR (offsets, shape indices) of candidate lists that contain the nearest shape of
-        every point; evaluate distance_squared on each list and keep the minimum (see `nearest_to`)."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, 3)
-        n = len(p)
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(64 * n, 1024)
-        cand = np.zeros(cap, dtype=np.uint32)
-        total = C.c_size_t(0)
-        st = getattr(capi.lib(), f"bvhgpu_nearest_candidates_{self._d['suffix']}")(self._h, _ptr(p), n, _ptr(offsets), _ptr(cand), cap, C.byref(total))
-        if st == capi.ERR_CAPACITY and total.value <= U32_MAX:
-            cand = np.zeros(total.value, dtype=np.uint32)
-            capi.check(getattr(capi.lib(), f"bvhgpu_traverse_fetch_{self._d['suffix']}")(self._h, _ptr(cand), total.value))
-        else:
-            capi.check(st)
-        return offsets, cand[: total.value]
-
-    def nearest_to(self, point, shapes, distance_squared):
-        """BoundingHierarchy::nearest_to for one point and an arbitrary shape distance: `distance_squared(shape, point)` is the shape's
-        PointDistance::distance_squared.  Returns (shape, distance) or None for an empty tree."""
-        off, cand = self.nearest_candidates([point])
-        best = None
-        for s in cand[off[0]:off[1]]:
-            d = distance_squared(shapes[int(s)], point)
-            if best is None or d < best[1]:
-                best = (shapes[int(s)], d)
-        return None if best is None else (best[0], float(np.sqrt(best[1])))
-
     def traverse_dev(self, rays_ptr: int, nrays: int, offsets_ptr: int, hits_ptr: int, cap: int, mode: int = capi.TRAVERSE_BVH,
                      want_total: bool = False):
+        """Device pointers (e.g. torch tensors' data_ptr()), enqueued on the context's stream.  want_total = False: no host
+        synchronisation, hits beyond `cap` are dropped."""
         total = C.c_size_t(0)
         fn = getattr(capi.lib(), f"bvhgpu_traverse_dev_{self._d['suffix']}")
         capi.check(fn(self._h, mode, C.c_void_p(rays_ptr), nrays, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
@@ -637,18 +641,6 @@ class Bvh:
         return swap_moves(n, idx)
 
 
-def _knn_call(bvh, points, D: int, k: int, max_dist):
-    """bvhgpu_knn_<suffix> on host arrays: points (n, D), max_dist None, a scalar or (n,)."""
-    p = np.ascontiguousarray(points, dtype=bvh._d["scalar"]).reshape(-1, D)
-    n = len(p)
-    r = None if max_dist is None else np.ascontiguousarray(np.broadcast_to(np.asarray(max_dist, dtype=bvh._d["scalar"]), (n,)))
-    kk = max(int(k), 0)
-    shape = np.zeros((n, kk), dtype=np.uint32)
-    dist = np.zeros((n, kk), dtype=bvh._d["scalar"])
-    capi.check(getattr(capi.lib(), f"bvhgpu_knn_{bvh._d['suffix']}")(bvh._h, _ptr(p), n, int(k) & 0xFFFFFFFF, _ptr(r), _ptr(shape), _ptr(dist)))
-    return shape, dist
-
-
 def swap_moves(n: int, indices) -> np.ndarray:
     """The renumbering of Bvh.remove_shapes: (m, 2) rows (new index, old index) of the survivors that move.  Survivors with index
     >= n-k take the vacated indices < n-k, smallest hole first (for k = 1: remove_shape(i, true) followed by pop())."""
@@ -660,7 +652,7 @@ def swap_moves(n: int, indices) -> np.ndarray:
     return np.stack([holes, tail], axis=1).astype(np.uint32).reshape(-1, 2)
 
 
-class Bvh2:
+class Bvh2(_Tree):
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays
     (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries, nearest_to, the distance-ordered traversal, the AABB closest hit and any hit.  Rays: structured array with 2-component origin, direction
     (normalised), inv_direction."""
@@ -669,7 +661,8 @@ class Bvh2:
     _DIM = 2
 
     def __init__(self, handle, prec: str, ctx: Context, n: int):
-        self._h, self.prec, self.ctx, self._d, self.n = handle, prec, ctx, self._TABLE[prec], n
+        super().__init__(handle, prec, ctx)
+        self.n = n
 
     @classmethod
     def build(cls, aabbs, prec: str = "f32", ctx: Context | None = None, mode: int = capi.BUILD_EXACT_SAH) -> "Bvh2":
@@ -680,16 +673,8 @@ class Bvh2:
         capi.check(getattr(capi.lib(), f"bvhgpu_build_{d['suffix']}")(ctx._h, _ptr(a), len(a), mode, C.byref(h)))
         return cls(h, prec, ctx, len(a))
 
-    def free(self):
-        if self._h:
-            getattr(capi.lib(), f"bvhgpu_tree_free_{self._d['suffix']}")(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
+    def _num_shapes(self) -> int:
+        return self.n
 
     def nodes_and_index(self):
         nodes = np.zeros(max(2 * self.n - 1, 0), dtype=self._d["node"])
@@ -697,118 +682,10 @@ class Bvh2:
         capi.check(getattr(capi.lib(), f"bvhgpu_tree_nodes_{self._d['suffix']}")(self._h, _ptr(nodes), _ptr(idx)))
         return nodes, idx
 
-    def flatten(self) -> np.ndarray:
-        cap = 0 if self.n == 0 else (1 if self.n == 1 else 3 * self.n - 2)
-        out = np.zeros(cap, dtype=self._d["flat"])
-        ln = C.c_size_t(0)
-        capi.check(getattr(capi.lib(), f"bvhgpu_flatten_{self._d['suffix']}")(self._h, _ptr(out), cap, C.byref(ln)))
-        return out[: ln.value]
-
     def traverse_batch(self, rays, mode: int = capi.TRAVERSE_BVH):
         rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
-        n = len(rays)
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(16 * n, 1024)
         fn = getattr(capi.lib(), f"bvhgpu_traverse_{self._d['suffix']}")
-        while True:
-            hits = np.zeros(cap, dtype=np.uint32)
-            total = C.c_size_t(0)
-            st = fn(self._h, mode, _ptr(rays), n, _ptr(offsets), _ptr(hits), cap, C.byref(total))
-            if st == capi.ERR_CAPACITY and total.value > cap and total.value <= U32_MAX:
-                cap = total.value
-                continue
-            capi.check(st)
-            return offsets, hits[: total.value]
-
-    def _query_stride(self, kind: int) -> int:
-        D = self._DIM
-        return {capi.QUERY_AABB: 2 * D, capi.QUERY_POINT: D, capi.QUERY_BALL: D + 1}[kind]
-
-    def _csr_call(self, fn, n: int, cap: int, *args):
-        """Calls fn(*args, offsets, out, cap, &total) again with cap = total when the first capacity is short (there is no fetch call)."""
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        while True:
-            out = np.zeros(cap, dtype=np.uint32)
-            total = C.c_size_t(0)
-            st = fn(*args, _ptr(offsets), _ptr(out), cap, C.byref(total))
-            if st == capi.ERR_CAPACITY and total.value > cap and total.value <= U32_MAX:
-                cap = total.value
-                continue
-            capi.check(st)
-            return offsets, out[: total.value]
-
-    def query_batch(self, kind: int, queries, mode: int = capi.TRAVERSE_BVH):
-        """Bvh::traverse with Aabb / Point / Ball queries: (n, 2D) {min, max} for capi.QUERY_AABB, (n, D) points for QUERY_POINT,
-        (n, D+1) {center, radius} for QUERY_BALL.  CSR (offsets, hits), hits of a query in the reference's DFS order."""
-        q = np.ascontiguousarray(queries, dtype=self._d["scalar"]).reshape(-1, self._query_stride(kind))
-        fn = getattr(capi.lib(), f"bvhgpu_query_{self._d['suffix']}")
-        return self._csr_call(fn, len(q), max(16 * len(q), 1024), self._h, mode, kind, _ptr(q), len(q))
-
-    def overlap_pairs(self, cap: int | None = None):
-        """Every pair of shapes whose own current AABBs intersect, each once, with the contract of Bvh.overlap_pairs: CSR (offsets[n + 1],
-        hits) indexed by shape.  A short capacity (default max(4 n, 1024)) is retried once at the exact total."""
-        fn = getattr(capi.lib(), f"bvhgpu_overlap_pairs_{self._d['suffix']}")
-        return self._csr_call(fn, self.n, max(4 * self.n, 1024) if cap is None else int(cap), self._h)
-
-    def overlap_pairs_with(self, other, cap: int | None = None):
-        """Every pair (a, b) of a shape of this tree and a shape of `other` whose own current AABBs intersect, with the contract of
-        Bvh.overlap_pairs_with: CSR (offsets[n + 1], hits) indexed by this tree's shapes.  A short capacity (default max(4 n, 1024))
-        is retried once at the exact total."""
-        _same_kind(self, other)
-        fn = getattr(capi.lib(), f"bvhgpu_overlap_trees_{self._d['suffix']}")
-        return self._csr_call(fn, self.n, max(4 * self.n, 1024) if cap is None else int(cap), self._h, other._h)
-
-    def nearest_to_batch(self, points, mode: int = capi.TRAVERSE_BVH):
-        """Bvh::nearest_to / FlatBvh::nearest_to for shapes whose distance is their AABB's: (shape index per point, U32_MAX for an
-        empty tree; distance per point).  points: (n, D)."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, self._DIM)
-        shape = np.zeros(len(p), dtype=np.uint32)
-        dist = np.zeros(len(p), dtype=self._d["scalar"])
-        capi.check(getattr(capi.lib(), f"bvhgpu_nearest_{self._d['suffix']}")(self._h, mode, _ptr(p), len(p), _ptr(shape), _ptr(dist)))
-        return shape, dist
-
-    def nearest_candidates(self, points):
-        """CSR (offsets, shape indices) of candidate lists that contain the nearest shape of every point, for shapes with their own
-        distance (see `nearest_to`).  points: (n, D)."""
-        p = np.ascontiguousarray(points, dtype=self._d["scalar"]).reshape(-1, self._DIM)
-        fn = getattr(capi.lib(), f"bvhgpu_nearest_candidates_{self._d['suffix']}")
-        return self._csr_call(fn, len(p), max(64 * len(p), 1024), self._h, _ptr(p), len(p))
-
-    def nearest_to(self, point, shapes, distance_squared):
-        """BoundingHierarchy::nearest_to for one point and an arbitrary shape distance: `distance_squared(shape, point)` is the shape's
-        PointDistance::distance_squared.  Returns (shape, distance) or None for an empty tree."""
-        off, cand = self.nearest_candidates([point])
-        best = None
-        for s in cand[off[0]:off[1]]:
-            d = distance_squared(shapes[int(s)], point)
-            if best is None or d < best[1]:
-                best = (shapes[int(s)], d)
-        return None if best is None else (best[0], float(np.sqrt(best[1])))
-
-    def knn(self, points, k: int, max_dist=None):
-        """The k nearest shapes of every point (points (n, D)), with the contract of Bvh.knn: (shape (n, k) u32, dist (n, k))."""
-        return _knn_call(self, points, self._DIM, k, max_dist)
-
-    def traverse_ordered(self, rays, ascending: bool = True):
-        """Batched nearest_traverse_iterator (ascending: by entry distance) / farthest_traverse_iterator (by exit distance,
-        descending): (offsets, hits, dists), the set of traverse_batch(..., TRAVERSE_BVH) perfectly sorted per ray, ties in DFS order,
-        with the slice distance of the child box the tree stores for each leaf.  A short capacity is retried once at the exact total,
-        hits and distances together."""
-        rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
-        n = len(rays)
-        offsets = np.zeros(n + 1, dtype=np.uint32)
-        cap = max(8 * n, 1024)
-        fn = getattr(capi.lib(), f"bvhgpu_traverse_ordered_{self._d['suffix']}")
-        while True:
-            hits = np.zeros(cap, dtype=np.uint32)
-            dists = np.zeros(cap, dtype=self._d["scalar"])
-            total = C.c_size_t(0)
-            st = fn(self._h, _ptr(rays), n, 1 if ascending else 0, _ptr(offsets), _ptr(hits), _ptr(dists), cap, C.byref(total))
-            if st == capi.ERR_CAPACITY and total.value > cap and total.value <= U32_MAX:
-                cap = total.value
-                continue
-            capi.check(st)
-            return offsets, hits[: total.value], dists[: total.value]
+        return self._csr(fn, len(rays), max(16 * len(rays), 1024), self._h, mode, _ptr(rays), len(rays))
 
     def closest_hit(self, rays):
         """Per ray: (shape whose own AABB the ray enters first, key (entry distance, DFS order), or U32_MAX; that entry distance or
@@ -826,8 +703,7 @@ class Bvh2:
         rays = np.ascontiguousarray(rays, dtype=self._d["ray"])
         n = len(rays)
         shape = np.zeros(n, dtype=np.uint32)
-        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
-        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(tm), _ptr(shape)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_any_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, _ptr(self._limits(tmax, n)), _ptr(shape)))
         return shape
 
     def multi_hit(self, rays, k: int, tmax=None):
@@ -838,9 +714,8 @@ class Bvh2:
         kk = max(int(k), 0)
         shape = np.zeros((n, kk), dtype=np.uint32)
         dist = np.zeros((n, kk), dtype=self._d["scalar"])
-        tm = None if tmax is None else np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=self._d["scalar"]), (n,)))
-        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, int(k) & 0xFFFFFFFF, _ptr(tm),
-                                                                                _ptr(shape), _ptr(dist)))
+        capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_{self._d['suffix']}")(self._h, _ptr(rays), n, int(k) & 0xFFFFFFFF,
+                                                                                _ptr(self._limits(tmax, n)), _ptr(shape), _ptr(dist)))
         return shape, dist, None
 
     def refit(self, aabbs):
@@ -896,15 +771,9 @@ class Bvh4(Bvh2):
     _TABLE = BY_PREC_4D
     _DIM = 4
 
-    def traverse_dev(self, rays_ptr: int, nrays: int, offsets_ptr: int, hits_ptr: int, cap: int, mode: int = capi.TRAVERSE_BVH,
-                     want_total: bool = False):
-        """Device pointers (e.g. torch tensors' data_ptr()), enqueued on the context's stream.  want_total = False: no host
-        synchronisation, hits beyond `cap` are dropped."""
-        total = C.c_size_t(0)
-        fn = getattr(capi.lib(), f"bvhgpu_traverse_dev_{self._d['suffix']}")
-        capi.check(fn(self._h, mode, C.c_void_p(rays_ptr), nrays, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
-                      C.byref(total) if want_total else None))
-        return total.value if want_total else None
+    # The device-pointer forms the 3-D tree has too (Bvh2 has no C entry point for them).
+    traverse_dev, overlap_pairs_dev, overlap_pairs_with_dev, knn_dev = (Bvh.traverse_dev, Bvh.overlap_pairs_dev, Bvh.overlap_pairs_with_dev,
+                                                                        Bvh.knn_dev)
 
     def query_dev(self, kind: int, queries_ptr: int, n: int, offsets_ptr: int, hits_ptr: int, cap: int, mode: int = capi.TRAVERSE_BVH,
                   want_total: bool = False):
@@ -914,24 +783,6 @@ class Bvh4(Bvh2):
         fn = getattr(capi.lib(), f"bvhgpu_query_dev_{self._d['suffix']}")
         capi.check(fn(self._h, mode, kind, C.c_void_p(queries_ptr), n, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr), cap,
                       C.byref(total) if want_total else None))
-        return total.value if want_total else None
-
-    def overlap_pairs_dev(self, offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
-        """overlap_pairs into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets are
-        always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
-        total = C.c_size_t(0)
-        capi.check(getattr(capi.lib(), f"bvhgpu_overlap_pairs_dev_{self._d['suffix']}")(self._h, C.c_void_p(offsets_ptr), C.c_void_p(hits_ptr or None),
-                                                                                       cap, C.byref(total) if want_total else None))
-        return total.value if want_total else None
-
-    def overlap_pairs_with_dev(self, other: "Bvh4", offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
-        """overlap_pairs_with into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets
-        are always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
-        _same_kind(self, other)
-        total = C.c_size_t(0)
-        capi.check(getattr(capi.lib(), f"bvhgpu_overlap_trees_dev_{self._d['suffix']}")(self._h, other._h, C.c_void_p(offsets_ptr),
-                                                                                       C.c_void_p(hits_ptr or None), cap,
-                                                                                       C.byref(total) if want_total else None))
         return total.value if want_total else None
 
     def closest_hit_dev(self, rays_ptr: int, nrays: int, shape_ptr: int, dist_ptr: int):
@@ -952,12 +803,6 @@ class Bvh4(Bvh2):
         capi.check(getattr(capi.lib(), f"bvhgpu_multi_hit_dev_{self._d['suffix']}")(self._h, C.c_void_p(rays_ptr), nrays, k,
                                                                                     C.c_void_p(tmax_ptr or None), C.c_void_p(shape_ptr),
                                                                                     C.c_void_p(dist_ptr)))
-
-    def knn_dev(self, points_ptr: int, n: int, k: int, max_dist_ptr: int, shape_ptr: int, dist_ptr: int):
-        """knn from device pointers: n points (4 scalars each) and n limits (max_dist_ptr = 0: no limit) in, n * k u32 shapes and
-        distances out, enqueued on the context's stream without host synchronisation."""
-        capi.check(getattr(capi.lib(), f"bvhgpu_knn_dev_{self._d['suffix']}")(self._h, C.c_void_p(points_ptr), n, k, C.c_void_p(max_dist_ptr or None),
-                                                                             C.c_void_p(shape_ptr), C.c_void_p(dist_ptr)))
 
     def refit_dev(self, aabbs_ptr: int, n: int):
         """refit from the new boxes of all n shapes on the device (C-ABI layout), enqueued on the context's stream."""

@@ -41,11 +41,42 @@ class BvhGpuError(RuntimeError):
         self.status = status
 
 
+# C types of the header's parameters and return values.  Every other pointer parameter is c_void_p, and `T**` (an out-handle) is
+# POINTER(c_void_p).  A type outside these tables raises instead of falling back to ctypes' int, which truncates pointers and sizes.
+_ARG_TYPES = {"int": C.c_int, "size_t": C.c_size_t, "uint32_t": C.c_uint32, "int64_t": C.c_int64, "double": C.c_double,
+              "size_t*": C.POINTER(C.c_size_t), "uint64_t*": C.POINTER(C.c_uint64), "const bvhgpu_shard*": C.POINTER(Shard),
+              "const char*": C.c_char_p}
+_RET_TYPES = {"int": C.c_int, "size_t": C.c_size_t, "uint64_t": C.c_uint64, "void": None, "const char*": C.c_char_p}
+
+
+def _ctype(fn: str, ctype: str, table: dict, header: str):
+    t = re.sub(r"\s*\*", "*", " ".join(ctype.split()))
+    if t in table:
+        return table[t]
+    if table is _ARG_TYPES and t.endswith("*"):
+        return C.POINTER(C.c_void_p) if t.endswith("**") else C.c_void_p
+    raise ImportError(f"{header}: {fn} uses the C type {t!r}, which has no ctypes mapping in bvh_b200/capi.py")
+
+
+def signatures(header: str = HEADER) -> dict:
+    """{name: (restype, argtypes)} of every prototype `RET bvhgpu_name(PARAMS);` the header declares."""
+    text = re.sub(r"/\*.*?\*/", "", open(header).read(), flags=re.S)
+    out = {}
+    for ret, name, params in re.findall(r"((?:const\s+)?\w+\s*\**)\s*\b(bvhgpu_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", text):
+        args = []
+        for p in ([] if params.strip() in ("", "void") else params.split(",")):
+            m = re.fullmatch(r"(.+?)\s*\b\w+", p.strip(), flags=re.S)                 # drop the parameter's name
+            args.append(_ctype(name, m[1] if m else p, _ARG_TYPES, header))
+        out[name] = (_ctype(name, ret, _RET_TYPES, header), args)
+    unread = set(re.findall(r"\b(bvhgpu_[a-z0-9_]+)\s*\(", text)) - set(out)
+    if unread:
+        raise ImportError(f"{header}: cannot read the prototypes of {sorted(unread)}")
+    return out
+
+
 def declared_symbols() -> list[str]:
     """Every function include/bvh_b200.h declares."""
-    text = open(HEADER).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(bvhgpu_[a-z0-9_]+)\s*\(", text)))
+    return sorted(signatures())
 
 
 _lib = None
@@ -61,141 +92,13 @@ def lib() -> C.CDLL:
             "bvh_b200 has no CPU fallback."
         )
     L = C.CDLL(SO_PATH)
-    vp, sz, i32, u64p = C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_uint64)
-    szp = C.POINTER(C.c_size_t)
-    L.bvhgpu_last_error.restype = C.c_char_p
-    L.bvhgpu_version.restype = C.c_char_p
-    L.bvhgpu_create.argtypes = [i32, C.POINTER(vp)]
-    L.bvhgpu_destroy.argtypes = [vp]
-    L.bvhgpu_destroy.restype = None
-    L.bvhgpu_set_stream.argtypes = [vp, vp]
-    L.bvhgpu_reset_stream.argtypes = [vp]
-    L.bvhgpu_synchronize.argtypes = [vp]
-    L.bvhgpu_launch_count.argtypes = [vp]
-    L.bvhgpu_launch_count.restype = C.c_uint64
-    L.bvhgpu_set_option.argtypes = [vp, C.c_char_p, C.c_int64]
-    L.bvhgpu_get_metric.argtypes = [vp, C.c_char_p, C.POINTER(C.c_double)]
-    L.bvhgpu_peer_alloc.argtypes = [vp, sz, C.POINTER(vp), vp]
-    L.bvhgpu_peer_open.argtypes = [vp, vp, C.POINTER(vp)]
-    L.bvhgpu_peer_close.argtypes = [vp, vp]
-    L.bvhgpu_peer_free.argtypes = [vp, vp]
-    L.bvhgpu_memcpy_d2h.argtypes = [vp, vp, vp, sz]
-    L.bvhgpu_memcpy_h2d_async.argtypes = [vp, vp, vp, sz]
-    L.bvhgpu_host_alloc.argtypes = [vp, sz, C.POINTER(vp)]
-    L.bvhgpu_host_free.argtypes = [vp, vp]
-    for s in ("f32x3", "f64x3"):
-        getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
-        getattr(L, f"bvhgpu_build_dev_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
-        getattr(L, f"bvhgpu_tree_from_nodes_{s}").argtypes = [vp, vp, sz, vp, sz, C.POINTER(vp)]
-        getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]
-        getattr(L, f"bvhgpu_tree_free_{s}").restype = None
-        for f in ("num_shapes", "num_nodes"):
-            getattr(L, f"bvhgpu_tree_{f}_{s}").argtypes = [vp]
-            getattr(L, f"bvhgpu_tree_{f}_{s}").restype = sz
-        getattr(L, f"bvhgpu_tree_nodes_{s}").argtypes = [vp, vp, vp]
-        getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_fetch_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_tree_set_triangles_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_tree_set_triangles_dev_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_closest_hit_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp]
-        getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, i32, sz, i32, vp, vp, vp]
-        getattr(L, f"bvhgpu_any_hit_{s}").argtypes = [vp, vp, sz, vp, i32, vp]
-        getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, i32, sz, vp, i32, vp]
-        getattr(L, f"bvhgpu_traverse_od_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_od_dev_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_refit_dev_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
-        getattr(L, f"bvhgpu_update_dev_{s}").argtypes = [vp, vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
-        getattr(L, f"bvhgpu_optimize_dev_{s}").argtypes = [vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
-        getattr(L, f"bvhgpu_traverse_dev_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_stats_{s}").argtypes = [vp, u64p]
-        getattr(L, f"bvhgpu_traverse_ordered_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_query_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_query_dev_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_sharded_dev_{s}").argtypes = [vp, i32, vp, sz, C.POINTER(Shard)]
-        getattr(L, f"bvhgpu_rays_new_dev_{s}").argtypes = [vp, vp, vp, sz, vp]
-        getattr(L, f"bvhgpu_sah_cost_{s}").argtypes = [vp, C.POINTER(C.c_double)]
-        getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_nearest_{s}").argtypes = [vp, C.c_int, vp, sz, vp, vp]
-        getattr(L, f"bvhgpu_nearest_triangles_{s}").argtypes = [vp, C.c_int, vp, sz, vp, vp]
-        getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, C.POINTER(C.c_size_t)]
-        getattr(L, f"bvhgpu_optimize_{s}").argtypes = [vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
-        for f in ("add_shapes", "add_shapes_dev"):
-            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz, C.c_double, C.POINTER(C.c_size_t)]
-        for f in ("remove_shapes", "remove_shapes_dev"):
-            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz]
-    for s in ("f32x2", "f64x2"):
-        getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
-        getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]
-        getattr(L, f"bvhgpu_tree_free_{s}").restype = None
-        getattr(L, f"bvhgpu_tree_num_shapes_{s}").argtypes = [vp]
-        getattr(L, f"bvhgpu_tree_num_shapes_{s}").restype = sz
-        getattr(L, f"bvhgpu_tree_nodes_{s}").argtypes = [vp, vp, vp]
-        getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_query_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_nearest_{s}").argtypes = [vp, i32, vp, sz, vp, vp]
-        getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
-        getattr(L, f"bvhgpu_add_shapes_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
-        getattr(L, f"bvhgpu_remove_shapes_{s}").argtypes = [vp, vp, sz]
-    for s in ("f32x2", "f64x2", "f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_traverse_ordered_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_closest_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
-        getattr(L, f"bvhgpu_any_hit_{s}").argtypes = [vp, vp, sz, vp, vp]
-    for s in ("f32x2", "f64x2", "f32x3", "f64x3", "f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_knn_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
-    for s in ("f32x3", "f64x3", "f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_knn_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
-    for s in ("f32x3", "f64x3"):
-        getattr(L, f"bvhgpu_knn_triangles_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
-        getattr(L, f"bvhgpu_knn_triangles_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp, vp]
-        getattr(L, f"bvhgpu_multi_hit_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, i32, vp, vp, vp]
-        getattr(L, f"bvhgpu_multi_hit_dev_{s}").argtypes = [vp, vp, i32, sz, C.c_uint32, vp, i32, vp, vp, vp]
-        getattr(L, f"bvhgpu_count_hits_{s}").argtypes = [vp, vp, sz, vp, vp, vp]
-        getattr(L, f"bvhgpu_count_hits_dev_{s}").argtypes = [vp, vp, i32, sz, vp, vp, vp]
-        getattr(L, f"bvhgpu_contains_points_{s}").argtypes = [vp, vp, sz, i32, vp]
-        getattr(L, f"bvhgpu_contains_points_dev_{s}").argtypes = [vp, vp, sz, i32, vp]
-        getattr(L, f"bvhgpu_signed_distance_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp]
-        getattr(L, f"bvhgpu_signed_distance_dev_{s}").argtypes = [vp, vp, sz, i32, vp, vp, vp]
-    for s in ("f32x2", "f64x2", "f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_multi_hit_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
-    for s in ("f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_multi_hit_dev_{s}").argtypes = [vp, vp, sz, C.c_uint32, vp, vp, vp]
-        getattr(L, f"bvhgpu_closest_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
-        getattr(L, f"bvhgpu_any_hit_dev_{s}").argtypes = [vp, vp, sz, vp, vp]
-        for f in ("add_shapes", "add_shapes_dev"):
-            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz, C.c_double, szp]
-        for f in ("remove_shapes", "remove_shapes_dev"):
-            getattr(L, f"bvhgpu_{f}_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_refit_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_refit_dev_{s}").argtypes = [vp, vp, sz]
-        getattr(L, f"bvhgpu_update_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
-        getattr(L, f"bvhgpu_update_dev_{s}").argtypes = [vp, vp, vp, sz, C.c_double, szp]
-        getattr(L, f"bvhgpu_build_{s}").argtypes = [vp, vp, sz, i32, C.POINTER(vp)]
-        getattr(L, f"bvhgpu_tree_free_{s}").argtypes = [vp]
-        getattr(L, f"bvhgpu_tree_free_{s}").restype = None
-        getattr(L, f"bvhgpu_tree_num_shapes_{s}").argtypes = [vp]
-        getattr(L, f"bvhgpu_tree_num_shapes_{s}").restype = sz
-        getattr(L, f"bvhgpu_tree_nodes_{s}").argtypes = [vp, vp, vp]
-        getattr(L, f"bvhgpu_flatten_{s}").argtypes = [vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_traverse_dev_{s}").argtypes = [vp, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_query_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_query_dev_{s}").argtypes = [vp, i32, i32, vp, sz, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_nearest_{s}").argtypes = [vp, i32, vp, sz, vp, vp]
-        getattr(L, f"bvhgpu_nearest_candidates_{s}").argtypes = [vp, vp, sz, vp, vp, sz, szp]
-    for s in ("f32x2", "f64x2", "f32x3", "f64x3", "f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_overlap_pairs_{s}").argtypes = [vp, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_overlap_trees_{s}").argtypes = [vp, vp, vp, vp, sz, szp]
-    for s in ("f32x3", "f64x3", "f32x4", "f64x4"):
-        getattr(L, f"bvhgpu_overlap_pairs_dev_{s}").argtypes = [vp, vp, vp, sz, szp]
-        getattr(L, f"bvhgpu_overlap_trees_dev_{s}").argtypes = [vp, vp, vp, vp, sz, szp]
-    missing =[n for n in declared_symbols() if not hasattr(L, n)]
+    sigs = signatures()
+    missing = [n for n in sorted(sigs) if not hasattr(L, n)]
     if missing:
         raise ImportError(f"{SO_PATH} does not export {missing}")
+    for name, (restype, argtypes) in sigs.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 

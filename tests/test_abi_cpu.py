@@ -30,8 +30,8 @@ UNCALLED_ENTRY_POINTS: dict[str, str] = {}
 def test_every_declared_entry_point_is_called_somewhere():
     """Every function of include/bvh_b200.h is called from the suite, tools/check_sharded.py, the Python wrappers or the C++
     mirror.  A symbol counts as called when its literal name appears there, or when an f-string stem `bvhgpu_<stem>_{` does
-    (a stem stands for every precision / dimension suffix).  bvh_b200/capi.py is not scanned: its argtypes table names
-    every symbol.  This file is not scanned either, so that an entry in the exemption list above does not cover itself."""
+    (a stem stands for every precision / dimension suffix).  bvh_b200/capi.py is not scanned: it types every symbol the
+    header declares and calls none.  This file is not scanned either, so that an entry in the exemption list above does not cover itself."""
     import glob
     import re
 
