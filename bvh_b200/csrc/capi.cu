@@ -1416,6 +1416,7 @@ BVH_EXPORT int bvhgpu_peer_alloc(bvhgpu_ctx* ctx, size_t bytes, void** dev_ptr, 
     if (!ctx || !dev_ptr || !handle64) { set_error("peer_alloc: null argument"); return BVHGPU_ERR_INVALID; }
     static_assert(sizeof(cudaIpcMemHandle_t) == BVHGPU_IPC_HANDLE_BYTES, "ipc handle size");
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    BVH_TRY(preload_shard_kernels());                            // every rank allocates before its first step
     BVH_CUDA_TRY(cudaMalloc(dev_ptr, bytes ? bytes : 16));
     BVH_CUDA_TRY(cudaMemset(*dev_ptr, 0, bytes ? bytes : 16));
     BVH_CUDA_TRY(cudaIpcGetMemHandle((cudaIpcMemHandle_t*)handle64, *dev_ptr));
@@ -1544,11 +1545,9 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_traverse_sharded_dev_##SUF(TREE* tree, int mode, const void* dev_rays, size_t nrays, const bvhgpu_shard* shard) { \
         if (!tree || !shard || (nrays && !dev_rays)) { set_error("traverse_sharded: null argument"); return BVHGPU_ERR_INVALID; } \
-        if (shard->world < 1 || shard->world > BVHGPU_MAX_PEERS || shard->rank < 0 || shard->rank >= shard->world) {       \
-            set_error("traverse_sharded: bad rank/world %d/%d", shard->rank, shard->world); return BVHGPU_ERR_INVALID; }     \
         if (nrays == 0 || tree->n == 0) { set_error("traverse_sharded: every rank needs a non-empty shard and tree"); return BVHGPU_ERR_UNSUPPORTED; } \
+        BVH_TRY(check_shard(shard, nrays));                                                                               \
         BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                   \
-        if (!shard->offsets) { set_error("traverse_sharded: shard->offsets is null"); return BVHGPU_ERR_INVALID; }     \
         return traverse_device<T>(tree, mode, dev_rays, (uint32_t)shard->ray_layout, nrays, nullptr, nullptr, shard->cap, nullptr, shard); \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_query_##SUF(TREE* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, \

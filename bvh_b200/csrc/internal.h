@@ -250,6 +250,11 @@ int remove_check(bvhgpu_ctx* ctx, const uint32_t* d_idx, uint32_t k, uint32_t n,
 template <class T> int traverse_device(Tree<T>* tree, int mode, const void* d_rays, uint32_t fmt,
                                        size_t nrays, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total,
                                        const bvhgpu_shard* shard = nullptr);
+// Every argument check of a sharded step (rank / world, seq >= 1, ray layout, non-null peer buffers, shard sizes): BVHGPU_OK or the
+// status the entry point returns before it enqueues anything.
+int check_shard(const bvhgpu_shard* shard, size_t nrays);
+// Loads the sharded step's kernels (scan_post_kernel<true>, emit_goffsets_kernel) on the current device before any step runs.
+int preload_shard_kernels();
 // Host rays in, host CSR out; H2D / walk+scan+emit / D2H overlapped.  Needs tree->d_offsets / d_hits sized by the caller.
 template <class T> int traverse_host_pipelined(Tree<T>* tree, int mode, const void* h_rays, uint32_t fmt, size_t nrays,
                                                uint32_t* h_offsets, uint32_t* h_hits, size_t h_cap, size_t* total);
@@ -276,8 +281,8 @@ template <class T> int knn_device(Tree<T>* tree, const T* d_points, size_t nq, u
 template <class T> int knn_tri_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist,
                                       T* d_closest);
 // CSR scan of per-item counts (traverse.cu), launched by the count -> scan -> fill driver of csr.cuh (CsrPasses) for every two-pass
-// walk: scan_local_kernel runs CSR_SCAN_THREADS threads per block over CSR_SCAN_TILE counts and leaves local exclusive offsets and
-// block totals; scan_blocks_kernel (one block of 1024 threads) turns the block totals into exclusive 64-bit block offsets and adds the
+// walk: scan_local_kernel runs CSR_SCAN_THREADS threads per block over CSR_SCAN_TILE counts and leaves local exclusive offsets
+// (saturated at 0xFFFFFFFF) and 64-bit block totals; scan_blocks_kernel (one block of 1024 threads) turns the block totals into exclusive 64-bit block offsets and adds the
 // grand total to *total (zeroed by the caller).
 constexpr int CSR_SCAN_THREADS = 256;
 constexpr int CSR_SCAN_TILE = 2048;

@@ -488,27 +488,33 @@ __global__ void __launch_bounds__(1024, 1) walk_top_kernel(const TNodeF* __restr
     if (lane == 0 && visits) atomicAdd(visit_total, (unsigned long long)visits);
 }
 
+// A tile of SCAN_TILE counts can sum past 2^32 (2048 rays through 2^21 + 1 boxes), so the scans below add in 64 bits.  The in-tile
+// offsets they leave in `local` (u32) are saturated at 0xFFFFFFFF: every reader adds the tile's 64-bit offset and clamps the sum to
+// 0xFFFFFFFF, and a clamped offset means a total past 2^32, which the call reports as BVHGPU_ERR_CAPACITY.
+__device__ __forceinline__ uint32_t sat_u32(unsigned long long x) { return x > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)x; }
+
 // Exclusive scan of counts, phase A: per-block local exclusive offsets + block totals (+ the largest count, if asked for).
 __global__ void __launch_bounds__(SCAN_THREADS) scan_local_kernel(const uint32_t* __restrict__ counts, uint32_t n,
                                                                   uint32_t* __restrict__ local, unsigned long long* __restrict__ blocksum,
                                                                   uint32_t* __restrict__ maxcount) {
-    __shared__ uint32_t wsum[SCAN_THREADS / 32];
+    __shared__ unsigned long long wsum[SCAN_THREADS / 32];
     const uint32_t base = blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-    uint32_t v[SCAN_ITEMS], s = 0, m = 0;
+    uint32_t v[SCAN_ITEMS], m = 0;
+    unsigned long long s = 0;
 #pragma unroll
     for (int k = 0; k < SCAN_ITEMS; ++k) { v[k] = (base + k < n) ? counts[base + k] : 0u; s += v[k]; m = v[k] > m ? v[k] : m; }
-    uint32_t incl = s;
+    unsigned long long incl = s;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
     if (lane_id() == 31) wsum[threadIdx.x >> 5] = incl;
     if (maxcount) { m = __reduce_max_sync(0xffffffffu, m); if (lane_id() == 0 && m) atomicMax(maxcount, m); }
     __syncthreads();
-    uint32_t woff = 0;
+    unsigned long long woff = 0;
     for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) woff += wsum[w];
-    uint32_t run = woff + incl - s;
+    unsigned long long run = woff + incl - s;
 #pragma unroll
-    for (int k = 0; k < SCAN_ITEMS; ++k) { if (base + k < n) local[base + k] = run; run += v[k]; }
-    if (threadIdx.x == SCAN_THREADS - 1) blocksum[blockIdx.x] = (unsigned long long)(woff + incl);
+    for (int k = 0; k < SCAN_ITEMS; ++k) { if (base + k < n) local[base + k] = sat_u32(run); run += v[k]; }
+    if (threadIdx.x == SCAN_THREADS - 1) blocksum[blockIdx.x] = woff + incl;
 }
 // Phase B: one block turns block totals into exclusive block offsets (64-bit) and the grand total.
 __global__ void __launch_bounds__(1024) scan_blocks_kernel(unsigned long long* __restrict__ blocksum, uint32_t nblocks,
@@ -615,28 +621,30 @@ template <bool SHARDED>
 __global__ void __launch_bounds__(SCAN_THREADS) scan_post_kernel(const uint32_t* __restrict__ counts, uint32_t n, uint32_t* __restrict__ local,
                                                                  unsigned long long* __restrict__ blocksum, unsigned long long* __restrict__ total,
                                                                  uint32_t* __restrict__ arrival, PeerBoxes pb, unsigned long long* __restrict__ xinfo) {
-    __shared__ uint32_t wsum[SCAN_THREADS / 32], wmax[SCAN_THREADS / 32];
+    __shared__ uint32_t wmax[SCAN_THREADS / 32];
     __shared__ XInfo xs;
-    __shared__ unsigned long long wsum64[SCAN_THREADS / 32];
+    __shared__ unsigned long long wsum[SCAN_THREADS / 32], wsum64[SCAN_THREADS / 32];
     __shared__ unsigned long long carry_s;
     __shared__ bool last;
     const uint32_t base = blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-    uint32_t v[SCAN_ITEMS], s = 0, m = 0;
+    uint32_t v[SCAN_ITEMS], m = 0;
+    unsigned long long s = 0;                                             // 64-bit sums: see sat_u32
 #pragma unroll
     for (int k = 0; k < SCAN_ITEMS; ++k) { v[k] = (base + k < n) ? counts[base + k] : 0u; s += v[k]; m = v[k] > m ? v[k] : m; }
-    uint32_t incl = s;
+    unsigned long long incl = s;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
     m = __reduce_max_sync(0xffffffffu, m);
     if (lane_id() == 31) wsum[threadIdx.x >> 5] = incl;
     if (lane_id() == 0) wmax[threadIdx.x >> 5] = m;
     __syncthreads();
-    uint32_t woff = 0, tsum = 0, tmax = 0;
+    unsigned long long woff = 0, tsum = 0;                                // tsum < 2^43 (2048 counts < 2^32): fits below the width byte
+    uint32_t tmax = 0;
 #pragma unroll
     for (int w = 0; w < SCAN_THREADS / 32; ++w) { if (w < (int)(threadIdx.x >> 5)) woff += wsum[w]; tsum += wsum[w]; tmax = wmax[w] > tmax ? wmax[w] : tmax; }
-    uint32_t run = woff + incl - s;
+    unsigned long long run = woff + incl - s;
 #pragma unroll
-    for (int k = 0; k < SCAN_ITEMS; ++k) { if (base + k < n) local[base + k] = run; run += v[k]; }
+    for (int k = 0; k < SCAN_ITEMS; ++k) { if (base + k < n) local[base + k] = sat_u32(run); run += v[k]; }
     const unsigned long long width = tmax <= 0xFFu ? 1ull : (tmax <= 0xFFFFu ? 2ull : 4ull);
     if (SHARDED) {
         unsigned long long tb_mine = 0;
@@ -657,7 +665,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_post_kernel(const uint32_t*
             for (int d = 0; d < BVHGPU_MAX_PEERS; ++d) if (d < pb.world) { *reinterpret_cast<uint4*>(pb.stage[d] + at) = q0; *reinterpret_cast<uint4*>(pb.stage[d] + at + 16) = q1; }
         }
     }
-    if (threadIdx.x == 0) blocksum[blockIdx.x] = (unsigned long long)tsum | (width << 56);
+    if (threadIdx.x == 0) blocksum[blockIdx.x] = tsum | (width << 56);
     // the block's stores -> barrier -> ONE fence (cumulative over what the barrier ordered) -> arrival counter
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -724,7 +732,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_post_kernel(const uint32_t*
 // Global offsets: one block per tile of every source rank.
 __device__ __forceinline__ void goffsets_body(const PeerBoxes& pb, const unsigned long long* __restrict__ xinfo, uint32_t* __restrict__ offsets,
                                               uint32_t bid, uint32_t ntiles) {
-    __shared__ uint32_t wsum[SCAN_THREADS / 32];
+    __shared__ unsigned long long wsum[SCAN_THREADS / 32];
     __shared__ uint32_t failed;
     if (threadIdx.x == 0) failed = *(volatile uint32_t*)pb.err;
     __syncthreads();
@@ -741,7 +749,8 @@ __device__ __forceinline__ void goffsets_body(const PeerBoxes& pb, const unsigne
         const unsigned long long entry = __ldcg(reinterpret_cast<const unsigned long long*>(stage + pb.table_off + 8ull * g));
         const unsigned long long width = entry >> 56;
         const unsigned char* p = stage + TILE_BYTES * g + (unsigned long long)threadIdx.x * SCAN_ITEMS * width;
-        uint32_t v[SCAN_ITEMS], s = 0;
+        uint32_t v[SCAN_ITEMS];
+        unsigned long long s = 0;                                  // 64-bit sums: see sat_u32
         static_assert(SCAN_ITEMS == 8, "8 counts per thread");
         if (width == 1) {
             const uint2 q = __ldcg(reinterpret_cast<const uint2*>(p));
@@ -755,18 +764,18 @@ __device__ __forceinline__ void goffsets_body(const PeerBoxes& pb, const unsigne
         }
 #pragma unroll
         for (int k = 0; k < SCAN_ITEMS; ++k) s += v[k];
-        uint32_t incl = s;
+        unsigned long long incl = s;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
+        for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane_id() >= o) incl += t; }
         if (lane_id() == 31) wsum[threadIdx.x >> 5] = incl;
         __syncthreads();
-        uint32_t woff = 0;
+        unsigned long long woff = 0;
         for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) woff += wsum[w];
         unsigned long long run = hb + (entry & OFF_MASK) + woff + incl - s;
         const unsigned long long j0 = rb + (g - tb) * SCAN_TILE + (unsigned long long)threadIdx.x * SCAN_ITEMS;
         uint32_t ov[SCAN_ITEMS];
 #pragma unroll
-        for (int k = 0; k < SCAN_ITEMS; ++k) { ov[k] = run > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)run; run += v[k]; }
+        for (int k = 0; k < SCAN_ITEMS; ++k) { ov[k] = sat_u32(run); run += v[k]; }
         if (j0 + SCAN_ITEMS <= re && (j0 & 3ull) == 0ull) {
             uint4* o4 = reinterpret_cast<uint4*>(offsets + j0);
             o4[0] = make_uint4(ov[0], ov[1], ov[2], ov[3]);
@@ -1037,6 +1046,42 @@ static int launch_pass1(Tree<T>* tree, bool flat, RaySrc<T> rays, uint32_t R, ui
     return BVHGPU_OK;
 }
 
+// Loads the kernels of the sharded step into the current device's context.  Under lazy module loading the first launch of a kernel
+// loads it, and a load can wait for kernels already running -- such as a scan kernel spinning on a peer whose own launch is held up
+// behind the load (ranks of one process share the device's context).  bvhgpu_peer_alloc, which every rank calls before its first
+// step, loads them up front.
+int preload_shard_kernels() {
+    cudaFuncAttributes a;
+    BVH_CUDA_TRY(cudaFuncGetAttributes(&a, scan_post_kernel<true>));
+    BVH_CUDA_TRY(cudaFuncGetAttributes(&a, emit_goffsets_kernel<float, false>));
+    BVH_CUDA_TRY(cudaFuncGetAttributes(&a, emit_goffsets_kernel<float, true>));
+    BVH_CUDA_TRY(cudaFuncGetAttributes(&a, emit_goffsets_kernel<double, false>));
+    BVH_CUDA_TRY(cudaFuncGetAttributes(&a, emit_goffsets_kernel<double, true>));
+    return BVHGPU_OK;
+}
+
+// Every check of a sharded step's arguments, made before the call enqueues anything: a bad shard must not leave a walk (or a scan
+// that stores through a null peer pointer) behind on the stream.  The mailbox starts zeroed, so seq 0 would let every wait pass at once.
+int check_shard(const bvhgpu_shard* shard, size_t nrays) {
+    const int W = shard->world;
+    if (W < 1 || W > BVHGPU_MAX_PEERS || shard->rank < 0 || shard->rank >= W) { set_error("traverse_sharded: bad rank/world %d/%d", shard->rank, W); return BVHGPU_ERR_INVALID; }
+    if (shard->seq == 0) { set_error("traverse_sharded: seq must start at 1 (the zeroed mailbox already holds 0)"); return BVHGPU_ERR_INVALID; }
+    if (shard->ray_layout != BVHGPU_RAYS_FULL && shard->ray_layout != BVHGPU_RAYS_OD) { set_error("traverse_sharded: bad ray layout %d", shard->ray_layout); return BVHGPU_ERR_INVALID; }
+    if (!shard->offsets) { set_error("traverse_sharded: shard->offsets is null"); return BVHGPU_ERR_INVALID; }
+    unsigned long long NG = 0, NT = 0;
+    for (int d = 0; d < W; ++d) {
+        if (!shard->peer_counts[d] || !shard->peer_hits[d] || !shard->peer_mailbox[d]) { set_error("traverse_sharded: a peer buffer of rank %d is null", d); return BVHGPU_ERR_INVALID; }
+        if (shard->shard_rays[d] == 0) { set_error("traverse_sharded: rank %d has an empty shard (every rank needs rays)", d); return BVHGPU_ERR_INVALID; }
+        if (shard->shard_rays[d] > 0x7FFFFFFFull) { set_error("traverse_sharded: shard_rays[%d] = %zu exceeds 2^31-1", d, shard->shard_rays[d]); return BVHGPU_ERR_INVALID; }
+        NG += shard->shard_rays[d];
+        NT += (shard->shard_rays[d] + SCAN_TILE - 1) / SCAN_TILE;
+    }
+    if (shard->shard_rays[shard->rank] != nrays) { set_error("traverse_sharded: shard_rays[rank] = %zu but nrays = %zu", shard->shard_rays[shard->rank], nrays); return BVHGPU_ERR_INVALID; }
+    if (NG > 0x7FFFFFFFull) { set_error("traverse_sharded: %llu rays in total exceed 2^31-1", NG); return BVHGPU_ERR_INVALID; }
+    if (TILE_BYTES * NT + 8ull * NT > BVHGPU_SHARD_STAGE_BYTES(NG)) { set_error("internal: staging layout exceeds BVHGPU_SHARD_STAGE_BYTES"); return BVHGPU_ERR_INTERNAL; }
+    return BVHGPU_OK;
+}
+
 template <class T>
 int traverse_device(Tree<T>* tree, int mode, const void* d_rays, uint32_t fmt, size_t nrays,
                     uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total, const bvhgpu_shard* shard) {
@@ -1096,14 +1141,11 @@ int traverse_device(Tree<T>* tree, int mode, const void* d_rays, uint32_t fmt, s
         const unsigned long long NG = pb.rays_before[W], NT = pb.tiles_before[W];
         pb.table_off = TILE_BYTES * NT;
         const size_t half = BVHGPU_SHARD_STAGE_BYTES(NG);                // the staging alternates between two halves (parity of seq)
-        if (pb.table_off + 8ull * NT > half) { set_error("internal: staging layout exceeds BVHGPU_SHARD_STAGE_BYTES"); return BVHGPU_ERR_INTERNAL; }
-        for (int d = 0; d < W; ++d) {
+        for (int d = 0; d < W; ++d) {                                    // (check_shard has vetted the shard before anything ran)
             pb.box[d] = (unsigned long long*)shard->peer_mailbox[d];
             pb.stage[d] = (unsigned char*)shard->peer_counts[d] + (shard->seq & 1ull) * half;
             pb.hits[d] = (uint32_t*)shard->peer_hits[d];
         }
-        if (shard->shard_rays[shard->rank] != nrays) { set_error("traverse_sharded: shard_rays[rank] = %zu but nrays = %zu", shard->shard_rays[shard->rank], nrays); return BVHGPU_ERR_INVALID; }
-        if (NG > 0x7FFFFFFFull) { set_error("traverse_sharded: %llu rays in total exceed 2^31-1", NG); return BVHGPU_ERR_INVALID; }
         cap = shard->cap;
         dst.offsets = nullptr; dst.hits = pb.hits[pb.rank];
         scan_post_kernel<true><<<nblk, SCAN_THREADS, 0, st>>>(counts, R, local, sums, tail + S_TOTAL, arrival, pb, tail + S_XINFO);

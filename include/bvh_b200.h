@@ -412,8 +412,12 @@ int bvhgpu_traverse_od_dev_f64x3(bvhgpu_tree3d* tree, int mode, const void* dev_
  *   3. extra blocks of the same launch rebuild the global u32 offsets on every rank from the staged counts (1 byte per ray
  *      crossed NVLink instead of 4) and end the step by waiting for the peers' done flags: when the stream reaches the end of
  *      the step, this rank's copy of the global CSR is complete.  Same number of launches as a single-GPU step.
- * `seq` must increase by one per call on all ranks.  No host synchronisation; failures (a peer that never answers)
- * are reported by bvhgpu_synchronize.  Mailbox layout (trace words for diagnostics included): traverse.cu. */
+ * `seq` must increase by one per call on all ranks, starting at 1: seq 0 is refused with BVHGPU_ERR_INVALID (the mailbox
+ * starts zeroed, so a wait for 0 would pass before any peer posted).  Every argument check (rank / world, seq, ray_layout, a
+ * null peer buffer or offsets, an empty shard, shard_rays[rank] != nrays) fails before the call enqueues anything.  No host
+ * synchronisation; failures (a peer that never answers) are reported by bvhgpu_synchronize.  A global hit total past 2^32
+ * leaves every offset at or past 2^32 as 0xFFFFFFFF (the closing entry included).  Mailbox layout (trace words for diagnostics
+ * included): traverse.cu. */
 #define BVHGPU_MAX_PEERS 8
 #define BVHGPU_MAILBOX_BYTES 65536
 #define BVHGPU_IPC_HANDLE_BYTES 64
@@ -424,7 +428,7 @@ typedef struct {
     void* peer_hits[BVHGPU_MAX_PEERS];      /* u32[cap] on every rank: the global hit lists                          */
     void* peer_mailbox[BVHGPU_MAX_PEERS];   /* BVHGPU_MAILBOX_BYTES on every rank, zero-initialised                  */
     void* offsets;                          /* LOCAL device memory, u32[nrays_global + 1]: the global CSR offsets     */
-    uint64_t seq;                           /* 1, 2, 3, ... identical on all ranks for the same step                 */
+    uint64_t seq;                           /* 1, 2, 3, ... identical on all ranks for the same step (0: refused)    */
     size_t shard_rays[BVHGPU_MAX_PEERS];    /* rays of every rank's shard (shard_rays[rank] == nrays of the call)     */
     size_t cap;                             /* capacity of the global hit buffers                                    */
     int ray_layout;                         /* bvhgpu_ray_layout of dev_rays                                         */

@@ -88,6 +88,7 @@ def _check_traversal(api, bvh, D, shapes, rays, prec):
                 assert np.array_equal(d_off.cpu().numpy().view(np.uint32), off)
                 d_off.fill_(7)
             total = bvh.traverse_dev(d_rays.data_ptr(), len(rays), d_off.data_ptr(), d_hits.data_ptr(), len(hits), mode=mode, want_total=True)
+            bvh.ctx.synchronize()                            # the call returns once the total is known; the fill may still run
             assert total == len(hits) and np.array_equal(d_off.cpu().numpy().view(np.uint32), off)
             assert np.array_equal(d_hits.cpu().numpy().view(np.uint32)[:len(hits)], hits)
     return sum(map(len, want_b))
