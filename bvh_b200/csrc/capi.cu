@@ -68,7 +68,7 @@ template <class T> static void tree_release(Tree4<T>* t) {
     if (!t || !t->ctx) return;
     bvhgpu_ctx* ctx = t->ctx;
     dfree(ctx, t->d_aabb); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
-    dfree(ctx, t->d_trec); dfree(ctx, t->d_flat); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
+    dfree(ctx, t->d_tnodes); dfree(ctx, t->d_flat); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
     dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad);
 }
 
@@ -250,12 +250,6 @@ template <class T> static int flatten_impl(Tree4<T>* tree, typename D4<T>::Flat*
     return BVHGPU_OK;
 }
 
-// The size guard of the batched calls: n must fit the kernels' u32 item indices.
-static int check_n(const char* what, size_t n) {
-    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
-    return BVHGPU_OK;
-}
-
 // The tree type of dimension D: Bvh<T,2> lives embedded in the 3-D tree (dim2.cu), Bvh<T,4> has its own (dim4.cu).
 template <int D, class T> using TreeOf = typename std::conditional<D == 4, Tree4<T>, Tree<T>>::type;
 
@@ -278,11 +272,12 @@ template <int D, class T> static int upload_records(bvhgpu_ctx* ctx, Scratch& sc
     *d_out = d_lift;
     return BVHGPU_OK;
 }
-// The host-pointer CSR calls of a 3-D (or lifted 2-D) tree run into the tree's retained buffers, which bvhgpu_traverse_fetch_*
-// reads later.  The hit buffer starts at max(hits_cap, per_item * n, 1024).  When run(d_offsets, d_hits, cap, &tot) reports
-// BVHGPU_ERR_CAPACITY with a total the u32 offsets can hold, the buffer grows to that total and the call runs once more.
-template <class T, class Run> static int run_retained(Tree<T>* tree, size_t n, size_t per_item, size_t* tot, Run run) {
-    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, per_item * n), 1024);
+// The host-pointer ray traversal of a 2-D or 3-D tree runs into the tree's retained buffers, which bvhgpu_traverse_fetch_* reads
+// later.  The hit buffer starts at max(hits_cap, 4 n, 1024).  traverse_device has a scan of its own and cannot fill again from it:
+// when run(d_offsets, d_hits, cap, &tot) reports BVHGPU_ERR_CAPACITY with a total the u32 offsets can hold, the buffer grows to that
+// total and the call runs once more.  (The other CSR walks grow their buffer between the passes, csr_run of csr.cuh.)
+template <class T, class Run> static int run_retained(Tree<T>* tree, size_t n, size_t* tot, Run run) {
+    size_t want = std::max<size_t>(std::max<size_t>(tree->hits_cap, 4 * n), 1024);
     int rc = BVHGPU_OK;
     for (int attempt = 0; attempt < 2; ++attempt) {
         rc = ensure_result_buffers(tree, n, want);
@@ -293,32 +288,17 @@ template <class T, class Run> static int run_retained(Tree<T>* tree, size_t n, s
     }
     return rc;
 }
-static const char* capacity_hint(int D) { return D == 3 ? "use bvhgpu_traverse_fetch_*" : "call again with cap = *total"; }
-// run_retained, then the CSR copied from the retained buffers: the offsets always, the hits when they fit `cap`.
-template <int D, class T, class Run>
-static int retained_to_host(Tree<T>* tree, const char* what, size_t n, size_t per_item, uint32_t* offsets, uint32_t* hits, size_t cap,
-                            size_t* total, Run run) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    size_t tot = 0;
-    const int rc = run_retained(tree, n, per_item, &tot, run);
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK) return rc;
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
-    int ret = BVHGPU_OK;
-    if (hits && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, ctx->stream)); }
-    else if (tot > cap) { set_error("%s: %zu hits do not fit the caller's capacity %zu (%s)", what, tot, cap, capacity_hint(D)); ret = BVHGPU_ERR_CAPACITY; }
-    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return ret;
-}
+
+static bool bad_mode(int mode) { return mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT; }
 
 // Ray traversal, host pointers.  D = 3: the streamed host traversal.  D = 2: rays of 6 T lifted on the device (dim2_expand_rays)
-// and walked by traverse_device.  D = 4: rays of 12 T through csr4_host.
+// and walked by traverse_device.  D = 4: rays of 12 T through traverse_csr.
 template <int D, class T>
 static int traverse_host_impl(TreeOf<D, T>* tree, int mode, const void* rays, uint32_t fmt, size_t nrays,
                               uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || (nrays && !rays) || !offsets) { set_error("traverse: null argument"); return BVHGPU_ERR_INVALID; }
     if (D != 2) BVH_TRY(check_n("traverse", nrays));
-    if (D == 4 && mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+    if (D == 4 && bad_mode(mode)) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
@@ -327,12 +307,16 @@ static int traverse_host_impl(TreeOf<D, T>* tree, int mode, const void* rays, ui
     T* d_rays = nullptr;
     if constexpr (D == 4) {
         if (nrays && tree->n) BVH_TRY(upload_records<D>(ctx, scratch, rays, nrays, RAY_RECORD, 0, &d_rays));
-        return csr4_host<T>(tree, PROBE_RAYS4, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, offsets, hits, cap, total, "traverse");
+        return traverse_csr<T>(tree, mode, d_rays, nrays, CsrOut::to_host(offsets, hits, cap, total, 4), "traverse");
     } else if constexpr (D == 2) {
         if (nrays) BVH_TRY(upload_records<D>(ctx, scratch, rays, nrays, RAY_RECORD, 0, &d_rays));
-        return retained_to_host<D>(tree, "traverse", nrays, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
+        size_t tot = 0;
+        const int rc = run_retained(tree, nrays, &tot, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
             return traverse_device<T>(tree, mode, d_rays, BVHGPU_RAYS_FULL, nrays, d_off, d_hits, hcap, t);
         });
+        if (total) *total = tot;
+        if (rc != BVHGPU_OK) return rc;
+        return copy_retained(tree, "traverse", nrays, tot, offsets, hits, cap);
     } else {
         if (nrays == 0 || tree->n == 0) {                            // nothing to pipeline
             size_t tot0 = 0;
@@ -344,7 +328,7 @@ static int traverse_host_impl(TreeOf<D, T>* tree, int mode, const void* rays, ui
             return BVHGPU_OK;
         }
         size_t tot = 0;
-        const int rc = run_retained(tree, nrays, 4, &tot, [&](uint32_t*, uint32_t*, size_t, size_t* t) {   // copies back for itself
+        const int rc = run_retained(tree, nrays, &tot, [&](uint32_t*, uint32_t*, size_t, size_t* t) {   // copies back for itself
             return traverse_host_pipelined<T>(tree, mode, rays, fmt, nrays, offsets, hits, cap, t);
         });
         if (total) *total = tot;
@@ -361,27 +345,19 @@ template <int D, class T>
 static int traverse_dev_impl(TreeOf<D, T>* tree, int mode, const void* d_rays, uint32_t fmt, size_t nrays, uint32_t* d_offsets, uint32_t* d_hits,
                              size_t cap, size_t* total, const char* what) {
     if (!tree || !d_offsets || (nrays && !d_rays)) { set_error("%s: null argument", what); return BVHGPU_ERR_INVALID; }
-    if constexpr (D == 4) {
-        BVH_TRY(check_n("traverse", nrays));
-        if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("traverse: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
-        BVH_TRY(resolve_status(tree));
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-        return csr4_device<T>(tree, PROBE_RAYS4, mode == BVHGPU_TRAVERSE_FLAT, d_rays, nrays, d_offsets, d_hits, cap, total, "traverse");
-    } else {
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-        return traverse_device<T>(tree, mode, d_rays, fmt, nrays, d_offsets, d_hits, cap, total);
-    }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    if constexpr (D == 4) return traverse_csr<T>(tree, mode, d_rays, nrays, CsrOut::device(d_offsets, d_hits, cap, total), "traverse");
+    else return traverse_device<T>(tree, mode, d_rays, fmt, nrays, d_offsets, d_hits, cap, total);
 }
 
-static bool bad_mode(int mode) { return mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT; }
-
-// Aabb / Point / Ball queries, host pointers: records of 2D / D / D + 1 T.  The mode of a 3-D call is checked by query_device.
+// Aabb / Point / Ball queries, host pointers: records of 2D / D / D + 1 T.  query_csr also serves the library's internal kinds
+// (nearest_candidates): only the public ones get through here.
 template <int D, class T>
 static int query_host_impl(TreeOf<D, T>* tree, int mode, int kind, const T* queries, size_t n, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || (n && !queries) || !offsets) { set_error("query: null argument"); return BVHGPU_ERR_INVALID; }
     if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
     BVH_TRY(check_n("query", n));
-    if (D != 3 && bad_mode(mode)) { set_error("query: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
+    if (bad_mode(mode)) { set_error("query: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
     bvhgpu_ctx* ctx = tree->ctx;
     BVH_CUDA_TRY(cudaSetDevice(ctx->device));
     BVH_TRY(resolve_status(tree));
@@ -389,59 +365,26 @@ static int query_host_impl(TreeOf<D, T>* tree, int mode, int kind, const T* quer
     T* d_q = nullptr;
     Scratch scratch(ctx);                                           // released on every return path
     if (n) BVH_TRY(upload_records<D>(ctx, scratch, queries, n, nvec, nscal, &d_q));
-    if constexpr (D == 4) {
-        return csr4_host<T>(tree, kind, mode == BVHGPU_TRAVERSE_FLAT, d_q, n, offsets, hits, cap, total, "query");
-    } else {
-        return retained_to_host<D>(tree, "query", n, 16, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-            return query_device<T>(tree, mode, kind, d_q, n, d_off, d_hits, hcap, t);
-        });
-    }
+    return query_csr(tree, mode, kind, d_q, n, CsrOut::to_host(offsets, hits, cap, total, 16), "query");
 }
-// Queries, device pointers (D = 3, 4).  query_device also serves the library's internal kinds (nearest_candidates): only the public
-// ones get through here.  With `total` given the call synchronises, and the CSR is complete when it returns.
+// Queries, device pointers (D = 3, 4).  With `total` given the call synchronises, and the CSR is complete when it returns.
 template <int D, class T>
 static int query_dev_impl(TreeOf<D, T>* tree, int mode, int kind, const void* d_queries, size_t n, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
     if (!tree || !d_offsets || (n && !d_queries)) { set_error("query_dev: null argument"); return BVHGPU_ERR_INVALID; }
     if (kind < BVHGPU_QUERY_AABB || kind > BVHGPU_QUERY_BALL) { set_error("query_dev: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
-    int rc;
-    if constexpr (D == 4) {
-        BVH_TRY(check_n("query_dev", n));
-        if (bad_mode(mode)) { set_error("query_dev: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
-        BVH_TRY(resolve_status(tree));
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-        rc = csr4_device<T>(tree, kind, mode == BVHGPU_TRAVERSE_FLAT, d_queries, n, d_offsets, d_hits, cap, total, "query_dev");
-    } else {
-        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-        rc = query_device<T>(tree, mode, kind, (const T*)d_queries, n, d_offsets, d_hits, cap, total);
-    }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    const int rc = query_csr(tree, mode, kind, d_queries, n, CsrOut::device(d_offsets, d_hits, cap, total), "query_dev");
     if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
     return rc;
 }
 
-// Self-overlap pairs, host pointers.  D = 2, 3: overlap_device into the retained buffers (bvhgpu_traverse_fetch_* reads them in 3-D).
-// D = 4: overlap4_host.  n < 2: all-zero offsets, no device work.
+// Self-overlap pairs, host pointers: through the retained buffers (bvhgpu_traverse_fetch_* reads them in 3-D).  n < 2: all-zero
+// offsets, no device work.
 template <int D, class T>
 static int overlap_host_impl(TreeOf<D, T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     if (!tree || !offsets) { set_error("overlap_pairs: null argument"); return BVHGPU_ERR_INVALID; }
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
-    BVH_TRY(resolve_status(tree));
-    const size_t n = tree->n;
-    if (n < 2) {
-        std::fill(offsets, offsets + n + 1, 0u);
-        if (total) *total = 0;
-        if constexpr (D != 4) tree->last_total = 0;
-        return BVHGPU_OK;
-    }
-    if constexpr (D == 4) {
-        return overlap4_host<T>(tree, offsets, hits, cap, total);
-    } else {
-        return retained_to_host<D>(tree, "overlap_pairs", n, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-            const int rc = overlap_device<T>(tree, d_off, d_hits, hcap, t);
-            if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) tree->last_total = *t;
-            return rc;
-        });
-    }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return overlap_csr(tree, CsrOut::to_host(offsets, hits, cap, total, 4), "overlap_pairs");
 }
 // Self-overlap pairs, device pointers (D = 3, 4), on the context's stream.  With `total` the call returns once the total is known
 // and the CSR is complete.
@@ -449,18 +392,7 @@ template <int D, class T>
 static int overlap_dev_impl(TreeOf<D, T>* tree, void* d_offsets, void* d_hits, size_t cap, size_t* total) {
     if (!tree || !d_offsets) { set_error("overlap_pairs_dev: null argument"); return BVHGPU_ERR_INVALID; }
     BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
-    int rc;
-    if constexpr (D == 4) {
-        BVH_TRY(resolve_status(tree));
-        if (tree->n < 2) {
-            BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (tree->n + 1), tree->ctx->stream));
-            if (total) *total = 0;
-            return BVHGPU_OK;
-        }
-        rc = overlap4_device<T>(tree, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
-    } else {
-        rc = overlap_device<T>(tree, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
-    }
+    const int rc = overlap_csr(tree, CsrOut::device((uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total), "overlap_pairs_dev");
     if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
     return rc;
 }
@@ -472,30 +404,13 @@ template <class Tr> static int overlap_trees_args(const char* what, const Tr* a,
     if (a->ctx != b->ctx) { set_error("%s: the two trees belong to different contexts", what); return BVHGPU_ERR_INVALID; }
     return BVHGPU_OK;
 }
-// Overlap between two trees, host pointers.  D = 2, 3: overlap_trees_device into A's retained buffers (bvhgpu_traverse_fetch_* on A
-// reads them in 3-D).  D = 4: overlap_trees4_host.  n_a = 0 or n_b = 0: all-zero offsets, no device work.
+// Overlap between two trees, host pointers: through A's retained buffers (bvhgpu_traverse_fetch_* on A reads them in 3-D).
+// n_a = 0 or n_b = 0: all-zero offsets, no device work.
 template <int D, class T>
 static int overlap_trees_host_impl(TreeOf<D, T>* a, TreeOf<D, T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
     BVH_TRY(overlap_trees_args("overlap_trees", a, b, offsets));
     BVH_CUDA_TRY(cudaSetDevice(a->ctx->device));
-    BVH_TRY(resolve_status(a));
-    BVH_TRY(resolve_status(b));
-    const size_t n = a->n;
-    if (n == 0 || b->n == 0) {
-        std::fill(offsets, offsets + n + 1, 0u);
-        if (total) *total = 0;
-        if constexpr (D != 4) a->last_total = 0;
-        return BVHGPU_OK;
-    }
-    if constexpr (D == 4) {
-        return overlap_trees4_host<T>(a, b, offsets, hits, cap, total);
-    } else {
-        return retained_to_host<D>(a, "overlap_trees", n, 4, offsets, hits, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-            const int rc = overlap_trees_device<T>(a, b, d_off, d_hits, hcap, t);
-            if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) a->last_total = *t;
-            return rc;
-        });
-    }
+    return overlap_trees_csr(a, b, CsrOut::to_host(offsets, hits, cap, total, 4), "overlap_trees");
 }
 // Overlap between two trees, device pointers (D = 3, 4), on the context's stream.  With `total` the call returns once the total is
 // known and the CSR is complete.
@@ -503,19 +418,7 @@ template <int D, class T>
 static int overlap_trees_dev_impl(TreeOf<D, T>* a, TreeOf<D, T>* b, void* d_offsets, void* d_hits, size_t cap, size_t* total) {
     BVH_TRY(overlap_trees_args("overlap_trees_dev", a, b, d_offsets));
     BVH_CUDA_TRY(cudaSetDevice(a->ctx->device));
-    int rc;
-    if constexpr (D == 4) {
-        BVH_TRY(resolve_status(a));
-        BVH_TRY(resolve_status(b));
-        if (a->n == 0 || b->n == 0) {
-            BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (a->n + 1), a->ctx->stream));
-            if (total) *total = 0;
-            return BVHGPU_OK;
-        }
-        rc = overlap_trees4_device<T>(a, b, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
-    } else {
-        rc = overlap_trees_device<T>(a, b, (uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total);
-    }
+    const int rc = overlap_trees_csr(a, b, CsrOut::device((uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total), "overlap_trees_dev");
     if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
     return rc;
 }
@@ -629,13 +532,7 @@ static int nearest_candidates_host_impl(TreeOf<D, T>* tree, const T* points, siz
     T* d_p = nullptr;
     Scratch scratch(ctx);
     if (n) BVH_TRY(upload_records<D>(ctx, scratch, points, n, 1, 0, &d_p));
-    if constexpr (D == 4) {
-        return nearest_candidates4<T>(tree, d_p, n, offsets, cand, cap, total);
-    } else {
-        return retained_to_host<D>(tree, "nearest_candidates", n, 16, offsets, cand, cap, total, [&](uint32_t* d_off, uint32_t* d_hits, size_t hcap, size_t* t) {
-            return nearest_candidates_device<T>(tree, d_p, n, d_off, d_hits, hcap, t);
-        });
-    }
+    return nearest_candidates_csr(tree, d_p, n, CsrOut::to_host(offsets, cand, cap, total, 16));
 }
 
 // Distance-ordered traversal, host pointers.  D = 3, 4: the C-ABI rays as they are.  D = 2: rays of 6 T lifted on the device
@@ -658,9 +555,7 @@ static int ordered_host_impl(TreeOf<D, T>* tree, const void* rays, size_t nrays,
     BVH_TRY(scratch.get(&d_hits, cap));
     BVH_TRY(scratch.get(&d_dists, cap));
     size_t tot = 0;
-    int rc;
-    if constexpr (D == 4) rc = ordered4_device<T>(tree, d_rays, nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
-    else rc = traverse_ordered_device<T>(tree, reinterpret_cast<const typename Traits<T>::Ray*>(d_rays), nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
+    int rc = ordered_csr(tree, d_rays, nrays, ascending, d_off, d_hits, d_dists, cap, &tot);
     if (total) *total = tot;
     if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) {
         cudaMemcpyAsync(offsets, d_off, sizeof(uint32_t) * (nrays + 1), cudaMemcpyDeviceToHost, ctx->stream);

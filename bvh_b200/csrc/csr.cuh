@@ -1,13 +1,16 @@
 // bvh_b200/csrc/csr.cuh -- the two-pass CSR walk that every batched walk except the 3-D ray traversal produces its hit lists with:
 // the traversal records of D = 3 and D = 4 and their fetch, the record walk generic in D, the count / fill kernel, the ordered
-// traversal's kernel, the self-overlap and two-tree overlap kernels, and the host driver of count -> scan -> fill.  Used by traverse.cu (D = 3 queries, nearest_candidates and the
-// ordered traversal, D = 2 through the z = 0 lift) and dim4.cu (D = 4 rays, queries, nearest_candidates and the ordered traversal).
+// traversal's kernel, the self-overlap and two-tree overlap kernels, the host driver of count -> scan -> fill, and the device
+// drivers of the CSR families (queries, 4-D rays, nearest_candidates, ordered traversal, overlap, overlap between two trees), written
+// once over the tree type and instantiated in traverse.cu (Tree<T>: D = 3, and D = 2 through the z = 0 lift) and dim4.cu (Tree4<T>).
 // The 3-D ray kernels of traverse.cu use the same fetch.
 //
 // CSR: offsets[n + 1] (u32, saturated to 0xFFFFFFFF) and the hit list hits[total]; the fill pass stores hits[0 .. cap) only, so a
 // short `cap` leaves a prefix of the full list.
 #pragma once
 #include "internal.h"
+#include "queries.cuh"
+#include <algorithm>
 
 namespace bvhb200 {
 
@@ -402,6 +405,142 @@ template <class Walk> int csr_two_pass(bvhgpu_ctx* ctx, const Walk& walk, uint32
     BVH_TRY(passes.fill(walk, offsets, hits, cap));
     return total ? passes.total(what, hits, cap, total) : BVHGPU_OK;
 }
+
+// ---- the device drivers of the CSR families (declared in internal.h) ----
+// Where a tree type differs they call an overload of internal.h: ensure_records, walk_aabbs, nearest_bound, keep_total.
+
+// The status step: a call with nothing to walk does not wait for a build that may still run on the device.
+template <class TreeT> int csr_status(TreeT* tree, size_t n) {
+    return n || tree->failed_status != BVHGPU_OK ? resolve_status(tree) : BVHGPU_OK;
+}
+// The CSR of a call with nothing to walk: all-zero offsets; the host form does no device work.
+template <class TreeT> int csr_zero(TreeT* tree, size_t n, const CsrOut& out) {
+    if (out.host) {
+        std::fill(out.offsets, out.offsets + n + 1, 0u);
+        keep_total(tree, 0);
+    } else {
+        BVH_CUDA_TRY(cudaMemsetAsync(out.offsets, 0, sizeof(uint32_t) * (n + 1), tree->ctx->stream));
+    }
+    if (out.total) *out.total = 0;
+    return BVHGPU_OK;
+}
+// The CSR of a walk over n > 0 items.  Device form: csr_two_pass.  Host form: count and scan once, fill into the tree's retained
+// buffers, read the total; when it did not fit and fits the u32 offsets, grow the hit buffer to it and fill again from the same
+// scan, if the list is wanted: the caller's cap holds it, or a 3-D tree keeps it for bvhgpu_traverse_fetch_*.  (2-D and 4-D have no
+// fetch: a short cap needs the offsets only, which the first fill completed.)  Then copy_retained.
+template <class TreeT, class Walk> int csr_run(TreeT* tree, const Walk& walk, size_t n, const CsrOut& out, const char* what) {
+    if (!out.host) return csr_two_pass(tree->ctx, walk, (uint32_t)n, what, out.offsets, out.hits, out.cap, out.total);
+    BVH_TRY(ensure_result_buffers(tree, n, std::max<size_t>(std::max<size_t>(tree->hits_cap, out.per_item * n), 1024)));
+    CsrPasses passes(tree->ctx, (uint32_t)n);
+    BVH_TRY(passes.count_and_scan(walk, true));
+    BVH_TRY(passes.fill(walk, tree->d_offsets, tree->d_hits, tree->hits_cap));
+    size_t tot = 0;
+    const int rc = passes.total(what, nullptr, 0, &tot);
+    if (out.total) *out.total = tot;
+    if (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY) keep_total(tree, tot);
+    if (rc != BVHGPU_OK) return rc;
+    if (tot > tree->hits_cap && (tree->dims == 3 || (out.hits && tot <= out.cap))) {
+        BVH_TRY(ensure_result_buffers(tree, n, tot));
+        BVH_TRY(passes.fill(walk, tree->d_offsets, tree->d_hits, tree->hits_cap));
+    }
+    return copy_retained(tree, what, n, tot, out.offsets, out.hits, out.cap);
+}
+
+// One probe over the records: status, empty input, then the walk (FLAT: leaves re-test the shape's own box).
+template <class Probe, class TreeT> int probe_csr(TreeT* tree, bool flat, const void* src, size_t n, const CsrOut& out, const char* what) {
+    BVH_TRY(csr_status(tree, n));
+    if (n == 0 || tree->n == 0) return csr_zero(tree, n, out);     // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
+    BVH_TRY(ensure_records(tree));
+    const CsrWalk<TreeT::D, typename TreeT::Scalar, Probe> walk{flat, tree->d_tnodes, tree->n_trec, walk_aabbs(tree), src};
+    return csr_run(tree, walk, n, out, what);
+}
+inline int check_walk(const char* what, size_t n, int mode) {
+    BVH_TRY(check_n(what, n));
+    if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("%s: bad mode %d", what, mode); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+template <class TreeT> int query_csr(TreeT* tree, int mode, int kind, const void* src, size_t n, const CsrOut& out, const char* what) {
+    using T = typename TreeT::Scalar;
+    constexpr int D = TreeT::D;
+    BVH_TRY(check_walk(what, n, mode));
+    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
+    switch (kind) {
+    case BVHGPU_QUERY_AABB: return probe_csr<Query<T, BVHGPU_QUERY_AABB, D>>(tree, flat, src, n, out, what);
+    case BVHGPU_QUERY_POINT: return probe_csr<Query<T, BVHGPU_QUERY_POINT, D>>(tree, flat, src, n, out, what);
+    case BVHGPU_QUERY_BALL: return probe_csr<Query<T, BVHGPU_QUERY_BALL, D>>(tree, flat, src, n, out, what);
+    case QUERY_WITHIN: return probe_csr<Query<T, QUERY_WITHIN, D>>(tree, flat, src, n, out, what);
+    default: set_error("%s: bad kind %d", what, kind); return BVHGPU_ERR_INVALID;
+    }
+}
+
+template <class TreeT> int nearest_candidates_csr(TreeT* tree, const typename TreeT::Scalar* points, size_t n, const CsrOut& out) {
+    using T = typename TreeT::Scalar;
+    const char* what = "nearest_candidates";
+    BVH_TRY(check_n(what, n));
+    BVH_TRY(csr_status(tree, n));
+    if (n == 0 || tree->n == 0) return csr_zero(tree, n, out);
+    Scratch scratch(tree->ctx);
+    T* rec = nullptr;
+    BVH_TRY(scratch.get(&rec, (TreeT::D + 1) * n));
+    BVH_TRY(nearest_bound(tree, points, (uint32_t)n, rec));
+    return probe_csr<Query<T, QUERY_WITHIN, TreeT::D>>(tree, true, rec, n, out, what);
+}
+
+// Ordered traversal: ordered_kernel over the records (a 2-D tree walks the lifted rays of dim2_expand_rays in its embedding).
+template <class TreeT> int ordered_csr(TreeT* tree, const void* rays, size_t n, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
+                                       typename TreeT::Scalar* d_dists, size_t cap, size_t* total) {
+    using T = typename TreeT::Scalar;
+    const char* what = "traverse_ordered";
+    BVH_TRY(check_n(what, n));
+    BVH_TRY(csr_status(tree, n));
+    if (n == 0 || tree->n == 0) return csr_zero(tree, n, CsrOut::device(d_offsets, d_hits, cap, total));
+    BVH_TRY(ensure_records(tree));
+    const OrderedWalk<TreeT::D, T> walk{tree->d_tnodes, tree->n_trec, reinterpret_cast<const typename CsrRecords<TreeT::D, T>::Ray*>(rays), ascending, d_dists};
+    return csr_two_pass(tree->ctx, walk, (uint32_t)n, what, d_offsets, d_hits, cap, total);
+}
+
+// The shapes of a tree in leaf (DFS) order, as long as `scratch` lives (released stream-ordered after the fill).
+template <class TreeT> int leaf_order(TreeT* tree, Scratch& scratch, uint32_t** order) {
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_TRY(scratch.get(order, tree->n));
+    leaf_order_kernel<<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_node_index, tree->d_node_start, tree->n, *order);
+    ctx->launches++;
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
+}
+// Self-overlap: overlap_kernel over the records and the shapes' own boxes.  A 2-D tree tests d_aabb (z = [0, 0]) and walks the records
+// of its embedding, whose z = [-1, +1] contains that slab.
+template <class TreeT> int overlap_csr(TreeT* tree, const CsrOut& out, const char* what) {
+    BVH_TRY(resolve_status(tree));
+    if (tree->n < 2) return csr_zero(tree, tree->n, out);
+    BVH_TRY(ensure_records(tree));
+    Scratch scratch(tree->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(leaf_order(tree, scratch, &order));
+    const OverlapWalk<TreeT::D, typename TreeT::Scalar> walk{tree->d_tnodes, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
+    return csr_run(tree, walk, tree->n, out, what);
+}
+// Overlap between two trees: overlap_trees_kernel, A's shapes in A's leaf order against B's records and B's own boxes (2-D trees as
+// above: both d_aabb have z = [0, 0], B's records z = [-1, +1]).
+template <class TreeT> int overlap_trees_csr(TreeT* a, TreeT* b, const CsrOut& out, const char* what) {
+    BVH_TRY(resolve_status(a));
+    BVH_TRY(resolve_status(b));
+    if (a->n == 0 || b->n == 0) return csr_zero(a, a->n, out);
+    BVH_TRY(ensure_records(b));
+    Scratch scratch(a->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(leaf_order(a, scratch, &order));
+    const OverlapTreesWalk<TreeT::D, typename TreeT::Scalar> walk{b->d_tnodes, b->n_trec, b->d_aabb, a->d_aabb, order};
+    return csr_run(a, walk, a->n, out, what);
+}
+
+// Explicit instantiations of the drivers of one tree type (traverse.cu: Tree<T>, dim4.cu: Tree4<T>).
+#define BVH_INSTANTIATE_CSR(TR, T)                                                                                                  \
+    template int query_csr<TR>(TR*, int, int, const void*, size_t, const CsrOut&, const char*);                                    \
+    template int nearest_candidates_csr<TR>(TR*, const T*, size_t, const CsrOut&);                                                  \
+    template int ordered_csr<TR>(TR*, const void*, size_t, int, uint32_t*, uint32_t*, T*, size_t, size_t*);                         \
+    template int overlap_csr<TR>(TR*, const CsrOut&, const char*);                                                                  \
+    template int overlap_trees_csr<TR>(TR*, TR*, const CsrOut&, const char*);
 #endif  // __CUDACC__
 
 }  // namespace bvhb200

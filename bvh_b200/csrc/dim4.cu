@@ -4,8 +4,9 @@
 // 4-wide slab tests for Ray<f32,4> / Ray<f64,4> (src/ray/intersect_simd.rs).  A fourth axis cannot hide in the 3-D kernels the way
 // D = 2 hides in z = 0 (dim2.cu): surface areas, largest_axis and the slab test all see it.  So D = 4 has its own pipeline here, with
 // its own node types and its own Tree4<T>; it shares the exact-arithmetic helpers and keys of common.cuh, Scratch, the records,
-// walk and count -> scan -> fill driver of csr.cuh, and the predicates of queries.cuh.  DESIGN.md section 4.11 describes the design.
-// This file holds the kernels and the device-side drivers declared in internal.h; the bvhgpu_*_f32x4 / _f64x4 entry points are the
+// walk, count -> scan -> fill driver and CSR drivers of csr.cuh, and the predicates of queries.cuh.  DESIGN.md section 4.11
+// describes the design.  This file holds the kernels, the Tree4<T> instances of the CSR drivers with the 4-D steps they call
+// (ensure_records, nearest_bound, the ray probe), and the other device-side drivers declared in internal.h; the bvhgpu_*_f32x4 / _f64x4 entry points are the
 // D = 4 instances of the host layer in capi.cu, which checks the arguments and the tree's status and stages the batch.  Refit,
 // update_shapes, add_shapes and remove_shapes run the drivers of dynamic.cu; the 4-D steps they call (the builder seeded from
 // subtree roots, the growth rebuild, the caches) are at the end of this file.
@@ -513,7 +514,7 @@ __device__ __forceinline__ bool slab4(const T o[4], const T inv[4], const T mn[4
 }
 
 // The probe of a ray batch for csr_walk_kernel (csr.cuh): load(src, r) reads ray r, hit(mn, mx) is the 4-wide slab test.  Queries
-// use Query<T, KIND, 4> of queries.cuh directly.
+// use Query<T, KIND, 4> of queries.cuh (query_csr).
 template <class T> struct RayProbe4 {
     T o[4], inv[4];
     __device__ __forceinline__ void load(const void* src, uint32_t r) { load_ray_full(reinterpret_cast<const typename D4<T>::Ray*>(src) + r, o, inv); }
@@ -771,130 +772,27 @@ template <class T> int build_flat4(Tree4<T>* tree) {
     return BVHGPU_OK;
 }
 
-// The traversal records of the two-pass walks, built on first use.
-template <class T> static int ensure_trec4(Tree4<T>* tree) {
+// The traversal records of the CSR walks, built on first use.
+template <class T> int ensure_records(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
-    if (tree->d_trec) return BVHGPU_OK;
+    if (tree->d_tnodes) return BVHGPU_OK;
     tree->n_trec = tree->n == 1 ? 1u : tree->n_nodes - 1;
-    BVH_TRY(dalloc_t(ctx, &tree->d_trec, tree->n_trec));
-    trec4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec);
+    BVH_TRY(dalloc_t(ctx, &tree->d_tnodes, tree->n_trec));
+    trec4_kernel<T><<<(tree->n_nodes + 255) / 256, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_tnodes);
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
 }
 
-// Device pointers, enqueued on the context's stream; synchronises only to return *total.  Arguments checked by the caller.
-template <class P, class T> static int csr4_dev(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* d_offsets, uint32_t* d_hits,
-                                                size_t cap, size_t* total, const char* what) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    if (n == 0 || tree->n == 0) {                                  // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (n + 1), st));
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    BVH_TRY(ensure_trec4(tree));
-    const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
-    return csr_two_pass(ctx, walk, (uint32_t)n, what, d_offsets, d_hits, cap, total);
+// ---- the CSR walks of csr.cuh: the 4-D ray traversal is the query walk with RayProbe4 ----
+template <class T> int traverse_csr(Tree4<T>* tree, int mode, const void* rays, size_t n, const CsrOut& out, const char* what) {
+    BVH_TRY(check_walk(what, n, mode));
+    return probe_csr<RayProbe4<T>>(tree, mode == BVHGPU_TRAVERSE_FLAT, rays, n, out, what);
 }
-
-// Host CSR out of n > 0 items of a walk over the records: count, read the total, size the retained hit buffer exactly, fill, copy
-// back.  Hits that do not fit `cap` are not copied; offsets and *total are, and the call returns BVHGPU_ERR_CAPACITY -- the caller's
-// second call with cap = *total is the only extra walk.
-template <class Walk, class T> static int csr4_host_walk(Tree4<T>* tree, const Walk& walk, size_t n, uint32_t* offsets, uint32_t* hits,
-                                                         size_t cap, size_t* total, const char* what) {
+template <class T> int nearest_bound(Tree4<T>* tree, const T* d_points, uint32_t n, T* d_records) {
     bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    CsrPasses passes(ctx, (uint32_t)n);
-    BVH_TRY(passes.count_and_scan(walk, true));
-    size_t tot = 0;
-    const int rc = passes.total(what, nullptr, 0, &tot);
-    if (total) *total = tot;
-    if (rc != BVHGPU_OK) return rc;
-    const bool fits = hits && tot <= cap;
-    BVH_TRY(ensure_result_buffers(tree, n, fits ? tot : 0));
-    BVH_TRY(passes.fill(walk, tree->d_offsets, fits ? tree->d_hits : nullptr, fits ? tot : 0));
-    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
-    if (fits && tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, st));
-    BVH_CUDA_TRY(cudaStreamSynchronize(st));
-    if (tot > cap) { set_error("%s: %zu hits do not fit the caller's capacity %zu (call again with cap = *total)", what, tot, cap); return BVHGPU_ERR_CAPACITY; }
-    return BVHGPU_OK;
-}
-// The CSR of a batch already on the device (d_src): n = 0 or an empty tree give all-zero offsets with no device work.
-template <class P, class T> static int csr4_host_p(Tree4<T>* tree, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
-                                                   size_t cap, size_t* total, const char* what) {
-    if (n == 0 || tree->n == 0) {                                  // nothing to walk / empty Bvh: no hits (bvh_impl.rs:109-112)
-        std::fill(offsets, offsets + n + 1, 0u);
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    BVH_TRY(ensure_trec4(tree));
-    const CsrWalk<4, T, P> walk{flat, tree->d_trec, tree->n_trec, tree->d_aabb, d_src};
-    return csr4_host_walk(tree, walk, n, offsets, hits, cap, total, what);
-}
-
-// ---- self-overlap: overlap_kernel<4, T> of csr.cuh over the records and the ABI boxes (n >= 2; the caller handles n < 2).  The
-// shapes in leaf order live as long as the call (released stream-ordered after the fill). ----
-template <class T> static int leaf_order4(Tree4<T>* tree, Scratch& scratch, uint32_t** order) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    BVH_TRY(scratch.get(order, tree->n));
-    leaf_order_kernel<<<(tree->n + 255) / 256, 256, 0, ctx->stream>>>(tree->d_node_index, tree->d_node_start, tree->n, *order);
+    nearest_bound4_kernel<T><<<(n + 127) / 128, 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, d_points, n, d_records);
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
-}
-template <class T> static int overlap4_order(Tree4<T>* tree, Scratch& scratch, uint32_t** order) {
-    BVH_TRY(ensure_trec4(tree));
-    return leaf_order4(tree, scratch, order);
-}
-template <class T> int overlap4_device(Tree4<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
-    Scratch scratch(tree->ctx);
-    uint32_t* order = nullptr;
-    BVH_TRY(overlap4_order(tree, scratch, &order));
-    const OverlapWalk<4, T> walk{tree->d_trec, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
-    return csr_two_pass(tree->ctx, walk, tree->n, "overlap_pairs_dev", d_offsets, d_hits, cap, total);
-}
-template <class T> int overlap4_host(Tree4<T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
-    Scratch scratch(tree->ctx);
-    uint32_t* order = nullptr;
-    BVH_TRY(overlap4_order(tree, scratch, &order));
-    const OverlapWalk<4, T> walk{tree->d_trec, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
-    return csr4_host_walk(tree, walk, tree->n, offsets, hits, cap, total, "overlap_pairs");
-}
-
-// ---- overlap between two trees: overlap_trees_kernel<4, T>, A's shapes in A's leaf order against B's records and ABI boxes
-// (n_a >= 1, n_b >= 1; the caller handles the rest).  The host form uses A's retained buffers. ----
-template <class T> int overlap_trees4_device(Tree4<T>* a, Tree4<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
-    Scratch scratch(a->ctx);
-    uint32_t* order = nullptr;
-    BVH_TRY(ensure_trec4(b));
-    BVH_TRY(leaf_order4(a, scratch, &order));
-    const OverlapTreesWalk<4, T> walk{b->d_trec, b->n_trec, b->d_aabb, a->d_aabb, order};
-    return csr_two_pass(a->ctx, walk, a->n, "overlap_trees_dev", d_offsets, d_hits, cap, total);
-}
-template <class T> int overlap_trees4_host(Tree4<T>* a, Tree4<T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
-    Scratch scratch(a->ctx);
-    uint32_t* order = nullptr;
-    BVH_TRY(ensure_trec4(b));
-    BVH_TRY(leaf_order4(a, scratch, &order));
-    const OverlapTreesWalk<4, T> walk{b->d_trec, b->n_trec, b->d_aabb, a->d_aabb, order};
-    return csr4_host_walk(a, walk, a->n, offsets, hits, cap, total, "overlap_trees");
-}
-
-// The probe of a CSR walk: rays, or one of the public query kinds.
-template <class T, class F> static int with_probe4(int probe, F f) {
-    switch (probe) {
-    case PROBE_RAYS4: return f(RayProbe4<T>{});
-    case BVHGPU_QUERY_AABB: return f(Query<T, BVHGPU_QUERY_AABB, 4>{});
-    case BVHGPU_QUERY_POINT: return f(Query<T, BVHGPU_QUERY_POINT, 4>{});
-    default: return f(Query<T, BVHGPU_QUERY_BALL, 4>{});
-    }
-}
-template <class T> int csr4_device(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* d_offsets, uint32_t* d_hits,
-                                   size_t cap, size_t* total, const char* what) {
-    return with_probe4<T>(probe, [&](auto p) { return csr4_dev<decltype(p)>(tree, flat, d_src, n, d_offsets, d_hits, cap, total, what); });
-}
-template <class T> int csr4_host(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
-                                 size_t cap, size_t* total, const char* what) {
-    return with_probe4<T>(probe, [&](auto p) { return csr4_host_p<decltype(p)>(tree, flat, d_src, n, offsets, hits, cap, total, what); });
 }
 
 // ---- nearest_to: 4 T per point ----
@@ -917,33 +815,6 @@ template <class T> int nearest4_device(Tree4<T>* tree, int mode, const T* d_poin
     LAUNCHED(ctx, 1);
     return BVHGPU_OK;
 }
-// Candidate lists that contain the nearest shape of every point, for shapes with their own distance (bvh_b200.h): the bound walk,
-// then a QUERY_WITHIN pass over the records in FLAT semantics (leaves re-test the shape's own AABB).
-template <class T> int nearest_candidates4(Tree4<T>* tree, const T* d_points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    if (n == 0 || tree->n == 0) return csr4_host_p<Query<T, QUERY_WITHIN, 4>>(tree, true, nullptr, n, offsets, cand, cap, total, "nearest_candidates");
-    Scratch scratch(ctx);
-    T* rec = nullptr;
-    BVH_TRY(scratch.get(&rec, 5 * n));
-    nearest_bound4_kernel<T><<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, d_points, (uint32_t)n, rec);
-    LAUNCHED(ctx, 1);
-    return csr4_host_p<Query<T, QUERY_WITHIN, 4>>(tree, true, rec, n, offsets, cand, cap, total, "nearest_candidates");
-}
-
-// ---- distance-ordered traversal (the contract of the 3-D calls; DESIGN.md section 4.14): ordered_kernel<4, T> of csr.cuh ----
-template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_t nrays, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
-                                       T* d_dists, size_t cap, size_t* total) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    if (nrays == 0 || tree->n == 0) {
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (nrays + 1), ctx->stream));
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    BVH_TRY(ensure_trec4(tree));
-    const OrderedWalk<4, T> walk{tree->d_trec, tree->n_trec, reinterpret_cast<const typename D4<T>::Ray*>(d_rays), ascending, d_dists};
-    return csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_offsets, d_hits, cap, total);
-}
-
 // ---- k nearest shapes: 4 T per point, n limits (nullptr: none), n * k results ----
 template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist) {
     if (n > 0x7FFFFFFFull) { set_error("knn: n = %zu exceeds 2^31-1", n); return BVHGPU_ERR_INVALID; }
@@ -965,7 +836,7 @@ template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, 
 template <class T> int refresh_caches(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
     const unsigned g = (tree->n_nodes + 255) / 256;
-    if (tree->d_trec) { trec4_kernel<T><<<g, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_trec); LAUNCHED(ctx, 1); }
+    if (tree->d_tnodes) { trec4_kernel<T><<<g, 256, 0, ctx->stream>>>(tree->d_nodes, tree->n_nodes, tree->d_aabb, tree->d_tnodes); LAUNCHED(ctx, 1); }
     if (tree->d_flat) { flat4_kernel<T><<<g, 256, 0, ctx->stream>>>(tree->d_nodes, tree->d_node_start, tree->n_nodes, tree->d_flat); LAUNCHED(ctx, 1); }
     return BVHGPU_OK;
 }
@@ -975,7 +846,7 @@ template <class T> int refresh_caches(Tree4<T>* tree) {
 // update's arrival counters and growth flags are reallocated by the next update.
 template <class T> int finish_relayout(Tree4<T>* tree) {
     bvhgpu_ctx* ctx = tree->ctx;
-    dfree(ctx, tree->d_trec); tree->d_trec = nullptr;
+    dfree(ctx, tree->d_tnodes); tree->d_tnodes = nullptr;
     dfree(ctx, tree->d_flat); tree->d_flat = nullptr;
     dfree(ctx, tree->d_arrive); tree->d_arrive = nullptr;
     dfree(ctx, tree->d_bad); tree->d_bad = nullptr;
@@ -1058,16 +929,9 @@ template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* roots, con
 #define INSTANTIATE4(T)                                                                                                              \
     template int build4<T>(Tree4<T>*, const D4<T>::Aabb*, cudaMemcpyKind);                                                          \
     template int build_flat4<T>(Tree4<T>*);                                                                                         \
-    template int csr4_device<T>(Tree4<T>*, int, bool, const void*, size_t, uint32_t*, uint32_t*, size_t, size_t*, const char*);     \
-    template int csr4_host<T>(Tree4<T>*, int, bool, const void*, size_t, uint32_t*, uint32_t*, size_t, size_t*, const char*);       \
-    template int nearest_candidates4<T>(Tree4<T>*, const T*, size_t, uint32_t*, uint32_t*, size_t, size_t*);                        \
+    template int traverse_csr<T>(Tree4<T>*, int, const void*, size_t, const CsrOut&, const char*);                                  \
     template int nearest4_device<T>(Tree4<T>*, int, const T*, size_t, uint32_t*, T*);                                               \
-    template int ordered4_device<T>(Tree4<T>*, const void*, size_t, int, uint32_t*, uint32_t*, T*, size_t, size_t*);               \
     template int knn4_device<T>(Tree4<T>*, const T*, size_t, uint32_t, const T*, uint32_t*, T*);                                    \
-    template int overlap4_device<T>(Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                                              \
-    template int overlap4_host<T>(Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                                                \
-    template int overlap_trees4_device<T>(Tree4<T>*, Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                             \
-    template int overlap_trees4_host<T>(Tree4<T>*, Tree4<T>*, uint32_t*, uint32_t*, size_t, size_t*);                               \
     template int refresh_caches<T>(Tree4<T>*);                                                                                    \
     template int finish_relayout<T>(Tree4<T>*);                                                                                     \
     template int rebuild_degraded<T>(Tree4<T>*, const uint32_t*, uint32_t*, size_t*, const char*);                                  \
@@ -1075,5 +939,7 @@ template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* roots, con
 INSTANTIATE4(float)
 INSTANTIATE4(double)
 #undef INSTANTIATE4
+BVH_INSTANTIATE_CSR(Tree4<float>, float)
+BVH_INSTANTIATE_CSR(Tree4<double>, double)
 
 }  // namespace bvhb200

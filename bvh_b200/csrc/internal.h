@@ -162,6 +162,27 @@ template <class TreeT> int ensure_result_buffers(TreeT* tree, size_t n, size_t h
     }
     return BVHGPU_OK;
 }
+// The CSR a host-pointer call left in the tree's retained buffers, copied back: the offsets always, the hits when they fit `cap`;
+// otherwise BVHGPU_ERR_CAPACITY, with a hint that depends on whether the tree type has bvhgpu_traverse_fetch_* (D = 3 only).
+// Synchronises.
+template <class TreeT> int copy_retained(TreeT* tree, const char* what, size_t n, size_t tot, uint32_t* offsets, uint32_t* hits, size_t cap) {
+    cudaStream_t st = tree->ctx->stream;
+    BVH_CUDA_TRY(cudaMemcpyAsync(offsets, tree->d_offsets, sizeof(uint32_t) * (n + 1), cudaMemcpyDeviceToHost, st));
+    int ret = BVHGPU_OK;
+    if (hits && tot <= cap) { if (tot) BVH_CUDA_TRY(cudaMemcpyAsync(hits, tree->d_hits, sizeof(uint32_t) * tot, cudaMemcpyDeviceToHost, st)); }
+    else if (tot > cap) {
+        set_error("%s: %zu hits do not fit the caller's capacity %zu (%s)", what, tot, cap,
+                  tree->dims == 3 ? "use bvhgpu_traverse_fetch_*" : "call again with cap = *total");
+        ret = BVHGPU_ERR_CAPACITY;
+    }
+    BVH_CUDA_TRY(cudaStreamSynchronize(st));
+    return ret;
+}
+// The size guard of the batched calls: n must fit the kernels' u32 item indices.
+inline int check_n(const char* what, size_t n) {
+    if (n > 0x7FFFFFFFull) { set_error("%s: n = %zu exceeds 2^31-1", what, n); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
 // Scratch that is released (stream-ordered) when the scope ends, on every return path.
 struct Scratch {
     bvhgpu_ctx* ctx;
@@ -258,21 +279,8 @@ int preload_shard_kernels();
 // Host rays in, host CSR out; H2D / walk+scan+emit / D2H overlapped.  Needs tree->d_offsets / d_hits sized by the caller.
 template <class T> int traverse_host_pipelined(Tree<T>* tree, int mode, const void* h_rays, uint32_t fmt, size_t nrays,
                                                uint32_t* h_offsets, uint32_t* h_hits, size_t h_cap, size_t* total);
-// hits sorted by entry (ascending) / exit (descending) distance, with the distances; device pointers
-template <class T> int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays, size_t nrays, int ascending,
-                                               uint32_t* d_offsets, uint32_t* d_hits, T* d_dists, size_t cap, size_t* total);
-// Every pair of shapes whose own boxes intersect, once, in the row of the earlier leaf (bvhgpu_overlap_pairs_*); device pointers, on
-// the context's stream, synchronises only to return *total.  Checks the tree's status; n < 2 gives all-zero offsets.
-template <class T> int overlap_device(Tree<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
-// Every pair (a, b) of a shape of tree A and a shape of tree B whose own boxes intersect, in A's row, B's DFS order
-// (bvhgpu_overlap_trees_*); device pointers, on the context's stream (A and B share it), synchronises only to return *total.  Checks
-// A's status, then B's; n_a = 0 or n_b = 0 give all-zero offsets.
-template <class T> int overlap_trees_device(Tree<T>* a, Tree<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
-// Aabb / Point / Ball queries (device pointers); two-pass count / fill.
-template <class T> int query_device(Tree<T>* tree, int mode, int kind, const T* d_queries, size_t nq, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
 // nearest_to for a batch of points (device pointers): exact reference walk for AABB-distance shapes; candidate lists for any shape
 template <class T> int nearest_device(Tree<T>* tree, int mode, const T* d_points, size_t nq, uint32_t* d_shape, T* d_dist, int use_triangles = 0);
-template <class T> int nearest_candidates_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t* d_offsets, uint32_t* d_cand, size_t cap, size_t* total);
 // k nearest shapes of every point (device pointers: 3 T per point, nq limits or nullptr, nq * k outputs), on the context's stream.
 // Checks nq, k and the tree's status; the pointers are checked by the caller.
 template <class T> int knn_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
@@ -351,7 +359,7 @@ template <> struct D4<double> { using Aabb = bvh_aabb4d; using Ray = bvh_ray4d; 
 // Bvh<T,4>: its own node types and pipeline (a fourth axis cannot hide in the 3-D kernels the way D = 2 hides in z = 0).
 template <class T> struct Tree4 {
     using Aabb = typename D4<T>::Aabb; using Node = typename D4<T>::Node; using Flat = typename D4<T>::Flat; using Rec = typename D4<T>::Rec;
-    static constexpr int D = 4;
+    static constexpr int D = 4, dims = 4;
     using Scalar = T; using Box = Aabb;   // the shape boxes keep the ABI layout on the device
     bvhgpu_ctx* ctx = nullptr;
     uint32_t n = 0, n_nodes = 0;
@@ -359,7 +367,7 @@ template <class T> struct Tree4 {
     Node* d_nodes = nullptr;           // [2n-1]   Bvh.nodes, reference preorder layout
     uint32_t* d_node_index = nullptr;  // [n]      leaf node of every shape
     uint32_t* d_node_start = nullptr;  // [2n-1]   first position of the node's shape range (== leaves before it)
-    Rec* d_trec = nullptr;             // [n_trec] traversal records (built on first use)
+    Rec* d_tnodes = nullptr;           // [n_trec] traversal records (built on first use)
     uint32_t n_trec = 0;
     Flat* d_flat = nullptr;            // [n_flat] FlatBvh (built on demand)
     size_t n_flat = 0;
@@ -376,35 +384,13 @@ template <class T> inline int resolve_status(const Tree4<T>* t) {
     if (t->failed_status != BVHGPU_OK) set_error("%s", t->failed_message.c_str());
     return t->failed_status;
 }
-// The device-side drivers of dim4.cu.  Arguments and the tree's status are checked by the caller unless said otherwise; everything
-// runs on the context's stream.
+// The device-side drivers of dim4.cu (the CSR walks are the shared drivers declared below).  Arguments and the tree's status are
+// checked by the caller unless said otherwise; everything runs on the context's stream.
 // Exact SAH build of tree->n shapes (tree->n, n_nodes set, n >= 1) from `aabbs` (kind: the direction of that copy).  Synchronous.
 template <class T> int build4(Tree4<T>* tree, const typename D4<T>::Aabb* aabbs, cudaMemcpyKind kind);
 template <class T> int build_flat4(Tree4<T>* tree);                 // tree->n_flat; d_flat built once
-// The CSR walks over the traversal records: probe 0 (PROBE_RAYS4) walks rays, BVHGPU_QUERY_AABB / POINT / BALL the queries.
-// csr4_device: device pointers, synchronises only to return *total; n = 0 or an empty tree give all-zero offsets.  csr4_host: a batch
-// already on the device, host CSR out through the tree's retained buffers (count, read the total, fill, copy back; hits that do not
-// fit `cap` are not copied and the call returns BVHGPU_ERR_CAPACITY); n = 0 or an empty tree give all-zero offsets with no device work.
-constexpr int PROBE_RAYS4 = 0;
-template <class T> int csr4_device(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* d_offsets, uint32_t* d_hits,
-                                   size_t cap, size_t* total, const char* what);
-template <class T> int csr4_host(Tree4<T>* tree, int probe, bool flat, const void* d_src, size_t n, uint32_t* offsets, uint32_t* hits,
-                                 size_t cap, size_t* total, const char* what);
-// nearest_candidates: the bound walk, then the QUERY_WITHIN CSR of csr4_host.
-template <class T> int nearest_candidates4(Tree4<T>* tree, const T* d_points, size_t n, uint32_t* offsets, uint32_t* cand, size_t cap, size_t* total);
 // nearest_to (4 T per point); an empty tree gives BVH_INVALID and 0 for every point.
 template <class T> int nearest4_device(Tree4<T>* tree, int mode, const T* d_points, size_t n, uint32_t* d_shape, T* d_dist);
-// distance-ordered traversal (rays of 12 T); n = 0 or an empty tree give all-zero offsets.
-template <class T> int ordered4_device(Tree4<T>* tree, const void* d_rays, size_t nrays, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
-                                       T* d_dists, size_t cap, size_t* total);
-// self-overlap pairs (overlap_device's contract) of a tree with n >= 2 shapes, status checked by the caller: overlap4_device to device
-// pointers (synchronises only to return *total), overlap4_host to host pointers through the retained buffers, as csr4_host.
-template <class T> int overlap4_device(Tree4<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
-template <class T> int overlap4_host(Tree4<T>* tree, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
-// overlap between two trees (overlap_trees_device's contract) with n_a >= 1 and n_b >= 1, statuses checked by the caller; the host
-// form runs through A's retained buffers, as overlap4_host.
-template <class T> int overlap_trees4_device(Tree4<T>* a, Tree4<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total);
-template <class T> int overlap_trees4_host(Tree4<T>* a, Tree4<T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
 // k nearest shapes: checks n, k and the tree's status, as knn_device does.
 template <class T> int knn4_device(Tree4<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist);
 // The 4-D overloads of the steps the dynamic drivers of dynamic.cu leave to the tree type (the 3-D ones are declared above):
@@ -418,6 +404,55 @@ template <class T> int rebuild_degraded(Tree4<T>* tree, const uint32_t* d_dirty,
 // idx[0 .. n) (idx holds the builder's two index buffers, 2 n), their centre bounds as keys in cb[8 slot ..].  Synchronous.
 template <class T> int build_subtrees(Tree4<T>* tree, const uint32_t* d_roots, const uint32_t* d_n_roots, uint32_t max_roots,
                                       const typename Traits<T>::Key* cb, uint32_t* idx, const char* who);
+
+// ---- the CSR walks of every D (csr.cuh): one device driver per family over the tree type, instantiated for Tree<T> in traverse.cu
+// and for Tree4<T> in dim4.cu.  Each checks, in this order, the size of the batch, the mode, the query kind, the tree's status and
+// the empty input; the pointers are checked by the caller.  A call with nothing to walk (n = 0) does not wait for a build still
+// running on the device: it reports only a failure that is already known.
+// Where a driver leaves its CSR: device pointers (CsrOut::device), enqueued on the context's stream and synchronising only to return
+// *total; or host pointers (CsrOut::to_host) through the tree's retained buffers (csr_run): the offsets always, the hits when they fit
+// `cap`, otherwise BVHGPU_ERR_CAPACITY.  per_item sizes the first retained hit buffer: max(hits_cap, per_item * n, 1024).
+struct CsrOut {
+    uint32_t* offsets;
+    uint32_t* hits;
+    size_t cap;
+    size_t* total;
+    bool host;
+    size_t per_item;
+    static CsrOut device(uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) { return {d_offsets, d_hits, cap, total, false, 0}; }
+    static CsrOut to_host(uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total, size_t per_item) {
+        return {offsets, hits, cap, total, true, per_item};
+    }
+};
+// Aabb / Point / Ball queries and the internal QUERY_WITHIN (queries.cuh) over `src`: records of 2D / D / D + 1 / D + 1 T.
+template <class TreeT> int query_csr(TreeT* tree, int mode, int kind, const void* src, size_t n, const CsrOut& out, const char* what);
+// Ray traversal of a 4-D tree (rays of 12 T): the query walk with the 4-wide slab test.  D = 2, 3 have traverse_device.
+template <class T> int traverse_csr(Tree4<T>* tree, int mode, const void* rays, size_t n, const CsrOut& out, const char* what);
+// Candidate lists that contain the nearest shape of every point (D T per point): the candidate bound, then QUERY_WITHIN, FLAT.
+template <class TreeT> int nearest_candidates_csr(TreeT* tree, const typename TreeT::Scalar* points, size_t n, const CsrOut& out);
+// Hits sorted by entry (ascending) / exit (descending) distance, with the distances (device pointers, cap entries each).
+template <class TreeT> int ordered_csr(TreeT* tree, const void* rays, size_t n, int ascending, uint32_t* d_offsets, uint32_t* d_hits,
+                                       typename TreeT::Scalar* d_dists, size_t cap, size_t* total);
+// Every pair of shapes whose own boxes intersect, once, in the row of the earlier leaf; n < 2 gives all-zero offsets.
+template <class TreeT> int overlap_csr(TreeT* tree, const CsrOut& out, const char* what);
+// Every pair (a, b) of a shape of tree A and a shape of tree B whose own boxes intersect, in A's row, B's DFS order (A and B share a
+// context).  A's status is checked before B's; n_a = 0 or n_b = 0 give all-zero offsets.  A host CSR uses A's retained buffers.
+template <class TreeT> int overlap_trees_csr(TreeT* a, TreeT* b, const CsrOut& out, const char* what);
+
+// The steps in which the CSR drivers tell the tree types apart.
+// The traversal records (d_tnodes, n_trec), built on first use.
+template <class T> inline int ensure_records(Tree<T>* t) { return t->d_tnodes ? BVHGPU_OK : build_traversal_records(t); }
+template <class T> int ensure_records(Tree4<T>* t);
+// The shape boxes of the FLAT leaf re-test: a 2-D tree re-tests the boxes with z = [-1, +1] (dim2.cu).
+template <class T> inline const typename Traits<T>::DAabb* walk_aabbs(const Tree<T>* t) { return t->dims == 2 && t->d_aabb_trav ? t->d_aabb_trav : t->d_aabb; }
+template <class T> inline const typename D4<T>::Aabb* walk_aabbs(const Tree4<T>* t) { return t->d_aabb; }
+// nearest_candidates' first pass: records {p, U} of D + 1 T per point, U the farthest-corner bound (nearest_bound_kernel of
+// traverse.cu, nearest_bound4_kernel of dim4.cu).
+template <class T> int nearest_bound(Tree<T>* t, const T* d_points, uint32_t n, T* d_records);
+template <class T> int nearest_bound(Tree4<T>* t, const T* d_points, uint32_t n, T* d_records);
+// The total of the last host CSR call, which bvhgpu_traverse_fetch_* and bvhgpu_traverse_stats_* of a 3-D tree read.
+template <class T> inline void keep_total(Tree<T>* t, size_t total) { t->last_total = total; }
+template <class T> inline void keep_total(Tree4<T>*, size_t) {}
 
 }  // namespace bvhb200
 

@@ -41,9 +41,6 @@ static inline uint32_t pick_slots(bvhgpu_ctx* ctx, uint32_t nrays) {
     return p;
 }
 
-// shape AABBs the FLAT leaf re-test reads: a 2-D tree keeps a copy whose z slab never constrains (dim2.cu)
-template <class T> static inline const typename Traits<T>::DAabb* walk_aabbs(const Tree<T>* tree) { return tree->dims == 2 && tree->d_aabb_trav ? tree->d_aabb_trav : tree->d_aabb; }
-
 constexpr int SCAN_ITEMS = 8;
 constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_TILE = SCAN_ITEMS * SCAN_THREADS;     // 2048 counts per block
@@ -1399,42 +1396,6 @@ int traverse_host_pipelined(Tree<T>* tree, int mode, const void* h_rays, uint32_
 template int traverse_host_pipelined<float>(Tree<float>*, int, const void*, uint32_t, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 template int traverse_host_pipelined<double>(Tree<double>*, int, const void*, uint32_t, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 
-// ---- the other IntersectsAabb implementors: Aabb, Point, Ball (src/aabb/intersection.rs:35-45, src/ball.rs:85-106) ----
-// The two-pass walk of csr.cuh with the predicates of queries.cuh; query batches are small.
-template <class T, int KIND>
-static int query_passes(Tree<T>* tree, bool flat, const T* d_queries, uint32_t nq, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
-    const CsrWalk<3, T, Query<T, KIND, 3>> walk{flat, tree->d_tnodes, tree->n_trec, walk_aabbs(tree), d_queries};
-    return csr_two_pass(tree->ctx, walk, nq, "query", d_offsets, d_hits, cap, total);
-}
-
-template <class T>
-int query_device(Tree<T>* tree, int mode, int kind, const T* d_queries, size_t nq, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    if (nq > 0x7FFFFFFFull) { set_error("query: too many queries"); return BVHGPU_ERR_INVALID; }
-    if (mode != BVHGPU_TRAVERSE_BVH && mode != BVHGPU_TRAVERSE_FLAT) { set_error("query: bad mode %d", mode); return BVHGPU_ERR_INVALID; }
-    if (kind != BVHGPU_QUERY_AABB && kind != BVHGPU_QUERY_POINT && kind != BVHGPU_QUERY_BALL && kind != QUERY_WITHIN) { set_error("query: bad kind %d", kind); return BVHGPU_ERR_INVALID; }
-    if (nq == 0 || tree->n == 0) {
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (nq + 1), st));
-        if (total) *total = 0;
-        tree->last_total = 0;
-        return BVHGPU_OK;
-    }
-    BVH_TRY(resolve_status(tree));
-    if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
-    const uint32_t R = (uint32_t)nq;
-    const bool flat = mode == BVHGPU_TRAVERSE_FLAT;
-    const int rc = kind == BVHGPU_QUERY_AABB  ? query_passes<T, BVHGPU_QUERY_AABB>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total)
-                 : kind == BVHGPU_QUERY_POINT ? query_passes<T, BVHGPU_QUERY_POINT>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total)
-                 : kind == BVHGPU_QUERY_BALL  ? query_passes<T, BVHGPU_QUERY_BALL>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total)
-                                              : query_passes<T, QUERY_WITHIN>(tree, flat, d_queries, R, d_offsets, d_hits, cap, total);
-    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) tree->last_total = *total;
-    return rc;
-}
-template int query_device<float>(Tree<float>*, int, int, const float*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
-template int query_device<double>(Tree<double>*, int, int, const double*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
-
-
 // ---- nearest_to (SURVEY 8f N4): Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
 // FlatBvh::nearest_to (src/flat_bvh.rs:513-562) for a batch of points ---------------------------------------------------
 // The reference calls the shape's own PointDistance::distance_squared at the leaves -- user code.  Two device forms:
@@ -1565,19 +1526,12 @@ int nearest_device(Tree<T>* tree, int mode, const T* d_points, size_t nq, uint32
     BVH_CUDA_TRY(cudaGetLastError());
     return BVHGPU_OK;
 }
-template <class T>
-int nearest_candidates_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t* d_offsets, uint32_t* d_cand, size_t cap, size_t* total) {
+template <class T> int nearest_bound(Tree<T>* tree, const T* d_points, uint32_t n, T* d_records) {
     bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    if (nq > 0x7FFFFFFFull) { set_error("nearest_candidates: too many points"); return BVHGPU_ERR_INVALID; }
-    BVH_TRY(resolve_status(tree));
-    if (nq == 0 || tree->n == 0) return query_device<T>(tree, BVHGPU_TRAVERSE_FLAT, QUERY_WITHIN, nullptr, nq, d_offsets, d_cand, cap, total);
-    T* rec = nullptr;
-    Scratch scratch(ctx);
-    BVH_TRY(scratch.get(&rec, nq * 4));
-    nearest_bound_kernel<T><<<(unsigned)((nq + 127) / 128), 128, 0, st>>>(tree->d_nodes, tree->d_aabb, d_points, (uint32_t)nq, rec);
+    nearest_bound_kernel<T><<<(n + 127) / 128, 128, 0, ctx->stream>>>(tree->d_nodes, tree->d_aabb, d_points, n, d_records);
     ctx->launches++;
-    return query_device<T>(tree, BVHGPU_TRAVERSE_FLAT, QUERY_WITHIN, rec, nq, d_offsets, d_cand, cap, total);
+    BVH_CUDA_TRY(cudaGetLastError());
+    return BVHGPU_OK;
 }
 template int nearest_device<float>(Tree<float>*, int, const float*, size_t, uint32_t*, float*, int);
 template int nearest_device<double>(Tree<double>*, int, const double*, size_t, uint32_t*, double*, int);
@@ -1664,81 +1618,10 @@ int knn_tri_device(Tree<T>* tree, const T* d_points, size_t nq, uint32_t k, cons
 }
 template int knn_tri_device<float>(Tree<float>*, const float*, size_t, uint32_t, const float*, uint32_t*, float*, float*);
 template int knn_tri_device<double>(Tree<double>*, const double*, size_t, uint32_t, const double*, uint32_t*, double*, double*);
-template int nearest_candidates_device<float>(Tree<float>*, const float*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
-template int nearest_candidates_device<double>(Tree<double>*, const double*, size_t, uint32_t*, uint32_t*, size_t, size_t*);
 
-// ---- ordered traversal: ordered_kernel<3, T> of csr.cuh over the 3-D records (2-D trees: the lifted rays of dim2_expand_rays) ----
-template <class T>
-int traverse_ordered_device(Tree<T>* tree, const typename Traits<T>::Ray* d_rays, size_t nrays, int ascending,
-                            uint32_t* d_offsets, uint32_t* d_hits, T* d_dists, size_t cap, size_t* total) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    if (nrays > 0x7FFFFFFFull) { set_error("traverse_ordered: too many rays"); return BVHGPU_ERR_INVALID; }
-    if (nrays == 0 || tree->n == 0) {
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (nrays + 1), st));
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    BVH_TRY(resolve_status(tree));
-    if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
-    const OrderedWalk<3, T> walk{tree->d_tnodes, tree->n_trec, d_rays, ascending, d_dists};
-    return csr_two_pass(ctx, walk, (uint32_t)nrays, "traverse_ordered", d_offsets, d_hits, cap, total);
-}
-template int traverse_ordered_device<float>(Tree<float>*, const bvh_ray3f*, size_t, int, uint32_t*, uint32_t*, float*, size_t, size_t*);
-template int traverse_ordered_device<double>(Tree<double>*, const bvh_ray3d*, size_t, int, uint32_t*, uint32_t*, double*, size_t, size_t*);
-
-// ---- self-overlap: overlap_kernel<3, T> of csr.cuh over the 3-D records and the shapes' own boxes.  A 2-D tree tests d_aabb
-// (z = [0, 0]) and walks the records of its embedding, whose z = [-1, +1] contains that slab. ----
-template <class T>
-int overlap_device(Tree<T>* tree, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
-    bvhgpu_ctx* ctx = tree->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_TRY(resolve_status(tree));
-    const uint32_t n = tree->n;
-    if (n < 2) {
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (n + 1), st));
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    if (!tree->d_tnodes) BVH_TRY(build_traversal_records(tree));
-    Scratch scratch(ctx);
-    uint32_t* order = nullptr;
-    BVH_TRY(scratch.get(&order, n));
-    leaf_order_kernel<<<(n + 255) / 256, 256, 0, st>>>(tree->d_node_index, tree->d_node_start, n, order);
-    ctx->launches++;
-    BVH_CUDA_TRY(cudaGetLastError());
-    const OverlapWalk<3, T> walk{tree->d_tnodes, tree->n_trec, tree->d_aabb, tree->d_node_index, order};
-    return csr_two_pass(ctx, walk, n, "overlap_pairs", d_offsets, d_hits, cap, total);
-}
-template int overlap_device<float>(Tree<float>*, uint32_t*, uint32_t*, size_t, size_t*);
-template int overlap_device<double>(Tree<double>*, uint32_t*, uint32_t*, size_t, size_t*);
-
-// ---- overlap between two trees: overlap_trees_kernel<3, T> of csr.cuh, A's shapes in A's leaf order against B's records and B's own
-// boxes.  2-D trees as above: both d_aabb have z = [0, 0], B's records z = [-1, +1]. ----
-template <class T>
-int overlap_trees_device(Tree<T>* a, Tree<T>* b, uint32_t* d_offsets, uint32_t* d_hits, size_t cap, size_t* total) {
-    bvhgpu_ctx* ctx = a->ctx;
-    cudaStream_t st = ctx->stream;
-    BVH_TRY(resolve_status(a));
-    BVH_TRY(resolve_status(b));
-    const uint32_t n = a->n;
-    if (n == 0 || b->n == 0) {
-        BVH_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(uint32_t) * (n + 1), st));
-        if (total) *total = 0;
-        return BVHGPU_OK;
-    }
-    if (!b->d_tnodes) BVH_TRY(build_traversal_records(b));
-    Scratch scratch(ctx);
-    uint32_t* order = nullptr;
-    BVH_TRY(scratch.get(&order, n));
-    leaf_order_kernel<<<(n + 255) / 256, 256, 0, st>>>(a->d_node_index, a->d_node_start, n, order);
-    ctx->launches++;
-    BVH_CUDA_TRY(cudaGetLastError());
-    const OverlapTreesWalk<3, T> walk{b->d_tnodes, b->n_trec, b->d_aabb, a->d_aabb, order};
-    return csr_two_pass(ctx, walk, n, "overlap_trees", d_offsets, d_hits, cap, total);
-}
-template int overlap_trees_device<float>(Tree<float>*, Tree<float>*, uint32_t*, uint32_t*, size_t, size_t*);
-template int overlap_trees_device<double>(Tree<double>*, Tree<double>*, uint32_t*, uint32_t*, size_t, size_t*);
+// ---- the CSR walks of csr.cuh (queries, nearest_candidates, ordered traversal, overlap, overlap between two trees) over Tree<T> ----
+BVH_INSTANTIATE_CSR(Tree<float>, float)
+BVH_INSTANTIATE_CSR(Tree<double>, double)
 
 // ---- Ray::new for a batch (src/ray/ray_impl.rs:70-80) -------------------------------------------------
 template <class T> __device__ __forceinline__ T sqrt_rn(T x);

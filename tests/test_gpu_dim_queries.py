@@ -389,3 +389,49 @@ def test_nearest_to_with_sphere_shapes(A, D):
         want = min(dist2(s, p) for s in spheres)
         assert dist2(shape, p) == want and dist == np.sqrt(want)
     bvh.free()
+
+
+@pytest.mark.parametrize("D", [2, 3, 4])
+def test_a_total_past_the_first_buffer_fits_cap(A, D):
+    """A host CSR call whose total passes the tree's first retained hit buffer (max(per_item * n, 1024) on a fresh tree) but fits the
+    caller's cap: the fill runs again into the grown buffer and returns the CSR of a call whose first buffer fits, for queries and
+    self-overlap.  In 3-D a short cap leaves the full list for bvhgpu_traverse_fetch_*."""
+    from bvh_b200 import capi
+
+    F, prec, n, m = np.float32, "f32", 300, 8
+    rng = np.random.default_rng(40 + D)
+    mn = rng.uniform(0, 4, (n, D)).astype(F)
+    mx = (mn + rng.uniform(1, 3, (n, D))).astype(F)
+    d = _table(D)[prec]
+    q = np.concatenate([np.full((m, D), -1, F), np.full((m, D), 10, F)], axis=1)   # every query meets every box: n hits each
+    query = _fn("query", d)
+    total = C.c_size_t(0)
+    for short in (False, True):
+        bvh = _cls(A, D).build(_shapes(mn, mx, prec), prec=prec)
+        off = np.zeros(m + 1, dtype=np.uint32)
+        hits = np.zeros(m * n, dtype=np.uint32)
+        cap = 10 if short else m * n                            # m n = 2400 > 1024 = the first buffer
+        st = query(bvh._h, capi.TRAVERSE_BVH, dimref.AABB, _p(q), m, _p(off), _p(hits), cap, C.byref(total))
+        assert total.value == m * n and st == (capi.ERR_CAPACITY if short else capi.OK), capi.lib().bvhgpu_last_error()
+        if short and D == 3:
+            capi.check(capi.lib().bvhgpu_traverse_fetch_f32x3(bvh._h, _p(hits), m * n))
+        elif short:                                             # no retained list: the call again with cap = *total refills
+            st = query(bvh._h, capi.TRAVERSE_BVH, dimref.AABB, _p(q), m, _p(off), _p(hits), m * n, C.byref(total))
+            assert st == capi.OK and total.value == m * n, capi.lib().bvhgpu_last_error()
+        want_off, want_hits = bvh.query_batch(dimref.AABB, q)      # the retained buffer holds the total now: no refill
+        assert np.array_equal(off, want_off) and np.array_equal(hits, want_hits)
+        assert all(sorted(hits[off[i]:off[i + 1]].tolist()) == list(range(n)) for i in range(m))
+        if not short:
+            fresh = _cls(A, D).build(_shapes(mn, mx, prec), prec=prec)
+            o1, p1 = fresh.overlap_pairs(cap=n * n)                 # about n (n - 1) / 2 pairs > max(4 n, 1024)
+            fresh.free()
+            o2, p2 = bvh.overlap_pairs(cap=n * n)
+            o3, p3 = bvh.overlap_pairs(cap=n * n)
+            assert len(p1) > max(4 * n, 1024) and np.array_equal(o1, o3) and np.array_equal(p1, p3)
+            assert np.array_equal(o2, o3) and np.array_equal(p2, p3)
+            meet = np.all((mx[:, None, :] >= mn[None, :, :]) & (mx[None, :, :] >= mn[:, None, :]), axis=2)   # brute force
+            want = sorted(zip(*np.nonzero(np.triu(meet, 1))))
+            rows = np.repeat(np.arange(n), np.diff(o1.astype(np.int64)))
+            got = sorted((min(a_, b_), max(a_, b_)) for a_, b_ in zip(rows.tolist(), p1.tolist()))
+            assert got == [(int(a_), int(b_)) for a_, b_ in want]            # every intersecting pair, each once
+        bvh.free()
