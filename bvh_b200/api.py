@@ -30,12 +30,13 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
-def _same_kind(a, b):
-    """The two trees of an overlap_pairs_with call: the same class (so the same dimension) and the same precision."""
+def _same_kind(a, b, what: str = "overlap_pairs_with"):
+    """The two trees of an overlap_pairs_with / triangle_pairs_with call: the same class (so the same dimension) and the same
+    precision."""
     if type(a) is not type(b):
-        raise TypeError(f"overlap_pairs_with: {type(a).__name__} against {type(b).__name__}")
+        raise TypeError(f"{what}: {type(a).__name__} against {type(b).__name__}")
     if a.prec != b.prec:
-        raise ValueError(f"overlap_pairs_with: {a.prec} tree against a {b.prec} tree")
+        raise ValueError(f"{what}: {a.prec} tree against a {b.prec} tree")
 
 
 class Context:
@@ -544,6 +545,44 @@ class Bvh(_Tree):
         capi.check(getattr(capi.lib(), f"bvhgpu_overlap_trees_dev_{self._d['suffix']}")(self._h, other._h, C.c_void_p(offsets_ptr),
                                                                                        C.c_void_p(hits_ptr or None), cap,
                                                                                        C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
+    def triangle_pairs(self, skip_shared: bool = True, cap: int | None = None):
+        """Every pair of triangles (set_triangles) of this tree that meet, decided exactly: CSR (offsets[n + 1], hits), row s = row s
+        of overlap_pairs keeping the shapes t whose closed triangle has a point in common with s's (touching included).  Excluded
+        triangles (a non-finite coordinate, or degenerate) meet nothing; skip_shared drops the pairs that share a vertex (the
+        non-adjacent self-intersections); f64 triangles with a nonzero coordinate outside [2^-300, 2^300] keep their box pairs
+        (include/bvh_b200.h).  A short capacity (default max(4 n, 1024)) is completed from the retained list."""
+        n = self._num_shapes()
+        fn = getattr(capi.lib(), f"bvhgpu_triangle_pairs_{self._d['suffix']}")
+        return self._csr(fn, n, max(4 * n, 1024) if cap is None else int(cap), self._h, 1 if skip_shared else 0)
+
+    def triangle_pairs_with(self, other: "Bvh", cap: int | None = None):
+        """Every pair (a, b) of a triangle of this tree and a triangle of `other` that meet, decided exactly: row a of
+        overlap_pairs_with(other) keeping the shapes b whose triangle meets a's (a shared vertex is a contact).  Both trees must share
+        a context; other may be self.  A short capacity (default max(4 n, 1024)) is completed from this tree's retained list."""
+        _same_kind(self, other, "triangle_pairs_with")
+        n = self._num_shapes()
+        fn = getattr(capi.lib(), f"bvhgpu_triangle_pairs_trees_{self._d['suffix']}")
+        return self._csr(fn, n, max(4 * n, 1024) if cap is None else int(cap), self._h, other._h)
+
+    def triangle_pairs_dev(self, offsets_ptr: int, hits_ptr: int, cap: int, skip_shared: bool = True, want_total: bool = False):
+        """triangle_pairs into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets are
+        always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        total = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_triangle_pairs_dev_{self._d['suffix']}")(self._h, 1 if skip_shared else 0, C.c_void_p(offsets_ptr),
+                                                                                         C.c_void_p(hits_ptr or None), cap,
+                                                                                         C.byref(total) if want_total else None))
+        return total.value if want_total else None
+
+    def triangle_pairs_with_dev(self, other: "Bvh", offsets_ptr: int, hits_ptr: int, cap: int, want_total: bool = False):
+        """triangle_pairs_with into device pointers (n + 1 u32 offsets, cap u32 hits), enqueued on the context's stream.  The offsets
+        are always complete and hits[0 .. cap) is a prefix of the full list; want_total = False: no host synchronisation."""
+        _same_kind(self, other, "triangle_pairs_with")
+        total = C.c_size_t(0)
+        capi.check(getattr(capi.lib(), f"bvhgpu_triangle_pairs_trees_dev_{self._d['suffix']}")(self._h, other._h, C.c_void_p(offsets_ptr),
+                                                                                               C.c_void_p(hits_ptr or None), cap,
+                                                                                               C.byref(total) if want_total else None))
         return total.value if want_total else None
 
     def nearest_triangles_batch(self, points, mode: int = capi.TRAVERSE_BVH):

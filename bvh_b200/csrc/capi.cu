@@ -423,6 +423,37 @@ static int overlap_trees_dev_impl(TreeOf<D, T>* a, TreeOf<D, T>* b, void* d_offs
     return rc;
 }
 
+// Triangle pairs (D = 3): the overlap forms above with the triangles' predicate.  Self: host pointers through the retained buffers,
+// device pointers on the context's stream.
+template <class T>
+static int triangle_pairs_host_impl(Tree<T>* tree, int skip_shared, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+    if (!tree || !offsets) { set_error("triangle_pairs: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    return triangle_pairs_csr(tree, skip_shared, CsrOut::to_host(offsets, hits, cap, total, 4), "triangle_pairs");
+}
+template <class T>
+static int triangle_pairs_dev_impl(Tree<T>* tree, int skip_shared, void* d_offsets, void* d_hits, size_t cap, size_t* total) {
+    if (!tree || !d_offsets) { set_error("triangle_pairs_dev: null argument"); return BVHGPU_ERR_INVALID; }
+    BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));
+    const int rc = triangle_pairs_csr(tree, skip_shared, CsrOut::device((uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total), "triangle_pairs_dev");
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(tree->ctx->stream));
+    return rc;
+}
+template <class T>
+static int triangle_pairs_trees_host_impl(Tree<T>* a, Tree<T>* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) {
+    BVH_TRY(overlap_trees_args("triangle_pairs_trees", a, b, offsets));
+    BVH_CUDA_TRY(cudaSetDevice(a->ctx->device));
+    return triangle_pairs_trees_csr(a, b, CsrOut::to_host(offsets, hits, cap, total, 4), "triangle_pairs_trees");
+}
+template <class T>
+static int triangle_pairs_trees_dev_impl(Tree<T>* a, Tree<T>* b, void* d_offsets, void* d_hits, size_t cap, size_t* total) {
+    BVH_TRY(overlap_trees_args("triangle_pairs_trees_dev", a, b, d_offsets));
+    BVH_CUDA_TRY(cudaSetDevice(a->ctx->device));
+    const int rc = triangle_pairs_trees_csr(a, b, CsrOut::device((uint32_t*)d_offsets, (uint32_t*)d_hits, cap, total), "triangle_pairs_trees_dev");
+    if (total && (rc == BVHGPU_OK || rc == BVHGPU_ERR_CAPACITY)) BVH_CUDA_TRY(cudaStreamSynchronize(a->ctx->stream));
+    return rc;
+}
+
 // nearest_to, host pointers: D T per point.  The mode of a 3-D call is checked by nearest_device.
 template <int D, class T>
 static int nearest_host_impl(TreeOf<D, T>* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist, int use_triangles = 0) {
@@ -1464,6 +1495,18 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_overlap_trees_dev_##SUF(TREE* a, TREE* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
         return overlap_trees_dev_impl<3, T>(a, b, dev_offsets, dev_hits, cap, total);                                     \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_triangle_pairs_##SUF(TREE* tree, int skip_shared, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) { \
+        return triangle_pairs_host_impl<T>(tree, skip_shared, offsets, hits, cap, total);                                 \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_triangle_pairs_dev_##SUF(TREE* tree, int skip_shared, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
+        return triangle_pairs_dev_impl<T>(tree, skip_shared, dev_offsets, dev_hits, cap, total);                          \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_triangle_pairs_trees_##SUF(TREE* a, TREE* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total) { \
+        return triangle_pairs_trees_host_impl<T>(a, b, offsets, hits, cap, total);                                        \
+    }                                                                                                                     \
+    BVH_EXPORT int bvhgpu_triangle_pairs_trees_dev_##SUF(TREE* a, TREE* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total) { \
+        return triangle_pairs_trees_dev_impl<T>(a, b, dev_offsets, dev_hits, cap, total);                                 \
     }                                                                                                                     \
     BVH_EXPORT int bvhgpu_nearest_##SUF(TREE* tree, int mode, const T* points, size_t n, uint32_t* out_shape, T* out_dist) { \
         return nearest_host_impl<3, T>(tree, mode, points, n, out_shape, out_dist);                                         \

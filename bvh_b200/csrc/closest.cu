@@ -75,8 +75,6 @@ __device__ __forceinline__ void count_windings(const T o[3], const T dir[3], con
     back += moeller_trumbore(o, dir, a, c, b, u, v) < tmax ? 1u : 0u;
 }
 
-template <class T> struct DTri { T a[3], pa, b[3], pb, c[3], pc; };       // 48 B / 96 B: three vector loads per triangle
-
 template <class T>
 __global__ void __launch_bounds__(256) pack_tris_kernel(const T* __restrict__ tris9, uint32_t n, DTri<T>* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

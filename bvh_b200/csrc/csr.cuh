@@ -3,6 +3,7 @@
 // traversal's kernel, the self-overlap and two-tree overlap kernels, the host driver of count -> scan -> fill, and the device
 // drivers of the CSR families (queries, 4-D rays, nearest_candidates, ordered traversal, overlap, overlap between two trees), written
 // once over the tree type and instantiated in traverse.cu (Tree<T>: D = 3, and D = 2 through the z = 0 lift) and dim4.cu (Tree4<T>).
+// The triangle pairs (3-D only) reuse the overlap walk with a leaf policy and are instantiated in tripairs.cu.
 // The 3-D ray kernels of traverse.cu use the same fetch.
 //
 // CSR: offsets[n + 1] (u32, saturated to 0xFFFFFFFF) and the hit list hits[total]; the fill pass stores hits[0 .. cap) only, so a
@@ -214,17 +215,25 @@ __device__ __forceinline__ bool overlap_boxes(const T smn[D], const T smx[D], co
     for (int k = 0; k < D; ++k) hit = hit && !(smx[k] < mn[k] || mx[k] < smn[k]);
     return hit;
 }
-// The body of both overlap kernels.  Self (CROSS = false): rows and records of one tree, own = other = its boxes, the walk of s
-// starts at record node_index[s].  Cross (CROSS = true, bvhgpu_overlap_trees_*): thread k takes shape order[k] of tree A (A's leaf
-// order), loads its box from `own` (A's boxes), and walks all of B's records from record 0, testing each reached leaf's shape
-// against `other` (B's boxes); node_index is unused.  The exactness argument is the same: it only needs B's records.
-template <int D, class T, bool FILL, bool CROSS>
+// The leaf policy of the overlap kernels: the boxes decide.  A policy has row(s), false when row s is empty whatever the boxes say,
+// and keep(t), which filters a shape whose box passed (TriPairsLeaf, tritri.cuh: the triangle pairs).
+struct BoxesDecide {
+    __device__ __forceinline__ bool row(uint32_t) const { return true; }
+    __device__ __forceinline__ bool keep(uint32_t) const { return true; }
+};
+// The body of the overlap and triangle-pair kernels.  Self (CROSS = false): rows and records of one tree, own = other = its boxes, the
+// walk of s starts at record node_index[s].  Cross (CROSS = true, bvhgpu_overlap_trees_*): thread k takes shape order[k] of tree A (A's
+// leaf order), loads its box from `own` (A's boxes), and walks all of B's records from record 0, testing each reached leaf's shape
+// against `other` (B's boxes); node_index is unused.  The exactness argument is the same: it only needs B's records.  A reached shape
+// whose box passes is reported when leaf.keep(shape) holds.
+template <int D, class T, bool FILL, bool CROSS, class Leaf = BoxesDecide>
 __device__ __forceinline__ void overlap_walk(const typename CsrRecords<D, T>::Rec* __restrict__ trec, uint32_t n_rec,
                                              const typename CsrRecords<D, T>::Box* __restrict__ own, const typename CsrRecords<D, T>::Box* __restrict__ other,
                                              const uint32_t* __restrict__ node_index, const uint32_t* __restrict__ order, uint32_t n,
                                              uint32_t* __restrict__ counts, const uint32_t* __restrict__ local,
                                              const unsigned long long* __restrict__ blocksum, const unsigned long long* __restrict__ total,
-                                             uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits, unsigned long long cap) {
+                                             uint32_t* __restrict__ offsets, uint32_t* __restrict__ hits, unsigned long long cap,
+                                             Leaf leaf = Leaf()) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (FILL && k == 0) { const unsigned long long t = *total; offsets[n] = t > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)t; }
     if (k >= n) return;
@@ -238,6 +247,7 @@ __device__ __forceinline__ void overlap_walk(const typename CsrRecords<D, T>::Re
         if (!hits) return;                                        // offsets only
     }
     uint32_t cnt = 0, i = CROSS ? 0u : __ldg(node_index + s);
+    if (!leaf.row(s)) i = n_rec;
     while (i < n_rec) {
         T mn[D], mx[D];
         uint32_t skip, shape;
@@ -246,7 +256,7 @@ __device__ __forceinline__ void overlap_walk(const typename CsrRecords<D, T>::Re
             if (shape != BVH_INVALID) {
                 T tmn[D], tmx[D];
                 load_box(other + shape, tmn, tmx);
-                if (overlap_boxes<D, T>(smn, smx, tmn, tmx)) {
+                if (overlap_boxes<D, T>(smn, smx, tmn, tmx) && leaf.keep(shape)) {
                     if (FILL) { if (w < cap) hits[w] = shape; ++w; }
                     else ++cnt;
                 }
@@ -279,6 +289,25 @@ __global__ void __launch_bounds__(256) overlap_trees_kernel(const typename CsrRe
                                                             const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets,
                                                             uint32_t* __restrict__ hits, unsigned long long cap) {
     overlap_walk<D, T, FILL, true>(trec, n_rec, aabb_a, aabb_b, nullptr, order_a, n_a, counts, local, blocksum, total, offsets, hits, cap);
+}
+// ---- triangle pairs (bvhgpu_triangle_pairs_*, D = 3): the overlap walks with the leaf policy TriPairsLeaf (tritri.cuh, included by the
+// translation unit that instantiates them), which keeps a box pair only when the two closed triangles meet.  Self (CROSS = false): the
+// rows, records, boxes and triangles of one tree.  Cross: A's boxes, triangles and leaf order against B's records, boxes and triangles.
+template <class T> struct TriPairsLeaf;
+template <class T, bool FILL, bool CROSS>
+__global__ void __launch_bounds__(256) triangle_pairs_kernel(const typename CsrRecords<3, T>::Rec* __restrict__ trec, uint32_t n_rec,
+                                                             const typename CsrRecords<3, T>::Box* __restrict__ aabb_own,
+                                                             const typename CsrRecords<3, T>::Box* __restrict__ aabb_other,
+                                                             const DTri<T>* __restrict__ tris_own, const DTri<T>* __restrict__ tris_other,
+                                                             int skip_shared, const uint32_t* __restrict__ node_index,
+                                                             const uint32_t* __restrict__ order, uint32_t n, uint32_t* __restrict__ counts,
+                                                             const uint32_t* __restrict__ local, const unsigned long long* __restrict__ blocksum,
+                                                             const unsigned long long* __restrict__ total, uint32_t* __restrict__ offsets,
+                                                             uint32_t* __restrict__ hits, unsigned long long cap) {
+    TriPairsLeaf<T> leaf;
+    leaf.own = tris_own; leaf.other = tris_other; leaf.skip_shared = skip_shared;
+    overlap_walk<3, T, FILL, CROSS, TriPairsLeaf<T>&>(trec, n_rec, aabb_own, aabb_other, node_index, order, n, counts, local, blocksum,
+                                                      total, offsets, hits, cap, leaf);
 }
 
 // ---- host: count -> scan -> fill ----
@@ -343,6 +372,29 @@ template <int D, class T> struct OverlapTreesWalk {
     void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
               uint32_t* offsets, uint32_t* hits, size_t cap) const {
         overlap_trees_kernel<D, T, true><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb_b, aabb_a, order_a, n, nullptr, local, sums, total, offsets, hits, (unsigned long long)cap);
+    }
+};
+// The walk of triangle_pairs_kernel: self over one tree's n >= 2 shapes (CROSS = false; node_index of that tree) or tree A's n_a >= 1
+// shapes against tree B (CROSS = true, n_b >= 1).  order: the row tree's shapes in its leaf order.
+template <class T, bool CROSS> struct TrianglePairsWalk {
+    const typename CsrRecords<3, T>::Rec* trec;       // the walked tree's records (B's in the cross form)
+    uint32_t n_rec;
+    const typename CsrRecords<3, T>::Box* aabb_own;   // the row tree's own boxes
+    const typename CsrRecords<3, T>::Box* aabb_other; // the walked tree's own boxes
+    const DTri<T>* tris_own;
+    const DTri<T>* tris_other;
+    int skip_shared;
+    const uint32_t* node_index;
+    const uint32_t* order;
+    void count(cudaStream_t st, uint32_t n, uint32_t* counts) const {
+        triangle_pairs_kernel<T, false, CROSS><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb_own, aabb_other, tris_own, tris_other, skip_shared,
+                                                                                 node_index, order, n, counts, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    }
+    void fill(cudaStream_t st, uint32_t n, const uint32_t* local, const unsigned long long* sums, const unsigned long long* total,
+              uint32_t* offsets, uint32_t* hits, size_t cap) const {
+        triangle_pairs_kernel<T, true, CROSS><<<(n + 255) / 256, 256, 0, st>>>(trec, n_rec, aabb_own, aabb_other, tris_own, tris_other, skip_shared,
+                                                                                node_index, order, n, nullptr, local, sums, total, offsets, hits,
+                                                                                (unsigned long long)cap);
     }
 };
 
@@ -531,6 +583,39 @@ template <class TreeT> int overlap_trees_csr(TreeT* a, TreeT* b, const CsrOut& o
     uint32_t* order = nullptr;
     BVH_TRY(leaf_order(a, scratch, &order));
     const OverlapTreesWalk<TreeT::D, typename TreeT::Scalar> walk{b->d_tnodes, b->n_trec, b->d_aabb, a->d_aabb, order};
+    return csr_run(a, walk, a->n, out, what);
+}
+// Triangle pairs (D = 3): the overlap rows filtered by the triangles' predicate.  The checks run in this order: the sticky failure
+// (A's before B's), then the triangles of every non-empty tree.
+template <class T> int triangle_pairs_check(Tree<T>* tree, const char* what) {
+    if (tree->n && !tree->d_tris) { set_error("%s: needs bvhgpu_tree_set_triangles_* first", what); return BVHGPU_ERR_INVALID; }
+    return BVHGPU_OK;
+}
+template <class T> int triangle_pairs_csr(Tree<T>* tree, int skip_shared, const CsrOut& out, const char* what) {
+    BVH_TRY(resolve_status(tree));
+    BVH_TRY(triangle_pairs_check(tree, what));
+    if (tree->n < 2) return csr_zero(tree, tree->n, out);
+    BVH_TRY(ensure_records(tree));
+    Scratch scratch(tree->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(leaf_order(tree, scratch, &order));
+    const DTri<T>* tris = reinterpret_cast<const DTri<T>*>(tree->d_tris);
+    const TrianglePairsWalk<T, false> walk{tree->d_tnodes, tree->n_trec, tree->d_aabb, tree->d_aabb, tris, tris, skip_shared != 0,
+                                           tree->d_node_index, order};
+    return csr_run(tree, walk, tree->n, out, what);
+}
+template <class T> int triangle_pairs_trees_csr(Tree<T>* a, Tree<T>* b, const CsrOut& out, const char* what) {
+    BVH_TRY(resolve_status(a));
+    BVH_TRY(resolve_status(b));
+    BVH_TRY(triangle_pairs_check(a, what));
+    BVH_TRY(triangle_pairs_check(b, what));
+    if (a->n == 0 || b->n == 0) return csr_zero(a, a->n, out);
+    BVH_TRY(ensure_records(b));
+    Scratch scratch(a->ctx);
+    uint32_t* order = nullptr;
+    BVH_TRY(leaf_order(a, scratch, &order));
+    const TrianglePairsWalk<T, true> walk{b->d_tnodes, b->n_trec, a->d_aabb, b->d_aabb, reinterpret_cast<const DTri<T>*>(a->d_tris),
+                                          reinterpret_cast<const DTri<T>*>(b->d_tris), 0, nullptr, order};
     return csr_run(a, walk, a->n, out, what);
 }
 

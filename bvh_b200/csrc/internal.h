@@ -83,6 +83,9 @@ struct bvhgpu_ctx {
 
 namespace bvhb200 {
 
+// The device layout of a triangle of bvhgpu_tree_set_triangles_* (Tree::d_tris).
+template <class T> struct DTri { T a[3], pa, b[3], pb, c[3], pc; };       // 48 B / 96 B: three vector loads per triangle
+
 template <class T> struct Tree {
     using Tr = Traits<T>;
     // what the dynamic drivers of dynamic.cu see: a 2-D tree runs the D = 3 kernels in the plane z = 0
@@ -438,6 +441,11 @@ template <class TreeT> int overlap_csr(TreeT* tree, const CsrOut& out, const cha
 // Every pair (a, b) of a shape of tree A and a shape of tree B whose own boxes intersect, in A's row, B's DFS order (A and B share a
 // context).  A's status is checked before B's; n_a = 0 or n_b = 0 give all-zero offsets.  A host CSR uses A's retained buffers.
 template <class TreeT> int overlap_trees_csr(TreeT* a, TreeT* b, const CsrOut& out, const char* what);
+// The overlap rows of overlap_csr / overlap_trees_csr (D = 3) keeping only the pairs whose triangles (bvhgpu_tree_set_triangles_*)
+// meet (tritri.cuh); skip_shared: the self form drops pairs that share a vertex.  A non-empty tree without triangles: BVHGPU_ERR_INVALID,
+// checked after the sticky failures.  Instantiated in tripairs.cu.
+template <class T> int triangle_pairs_csr(Tree<T>* tree, int skip_shared, const CsrOut& out, const char* what);
+template <class T> int triangle_pairs_trees_csr(Tree<T>* a, Tree<T>* b, const CsrOut& out, const char* what);
 
 // The steps in which the CSR drivers tell the tree types apart.
 // The traversal records (d_tnodes, n_trec), built on first use.

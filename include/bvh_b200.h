@@ -785,6 +785,49 @@ int bvhgpu_overlap_trees_dev_f64x3(bvhgpu_tree3d* a, bvhgpu_tree3d* b, void* dev
 int bvhgpu_overlap_trees_dev_f32x4(bvhgpu_tree4f* a, bvhgpu_tree4f* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 int bvhgpu_overlap_trees_dev_f64x4(bvhgpu_tree4d* a, bvhgpu_tree4d* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
 
+/* ---- triangle pairs (D = 3): which triangles of a mesh cut each other (self-intersection, mesh repair), where one mesh touches another
+ * (contact, boolean operations, clearance checks).  The narrow phase of the overlap pairs, decided exactly.  The triangles are those of
+ * bvhgpu_tree_set_triangles_* (shape s carries triangle (a, b, c)).  The CSR is a filter of the overlap CSR:
+ *   self:   row s of bvhgpu_triangle_pairs_* is row s of bvhgpu_overlap_pairs_*, in the same order (ascending leaf(t)), keeping only the
+ *           shapes t with meets(tri_s, tri_t).  Every pair appears once.
+ *   trees:  row a of bvhgpu_triangle_pairs_trees_*(a, b) is row a of bvhgpu_overlap_trees_*(a, b), filtered the same way, A's triangle
+ *           against B's.
+ * So the result equals the brute force over all pairs exactly where the overlap pairs do, provided every triangle lies inside its
+ * shape's own box (the condition bvhgpu_tree_set_triangles_* asks for).  With stale triangles (a refit or update without a new
+ * set_triangles) it is still precisely the filtered overlap row.
+ * meets(P, Q), in this order:
+ *   1. Excluded triangles meet nothing: a coordinate that is not finite, or degenerate: (b - a) x (c - a) exactly zero (collinear
+ *      points, a repeated vertex, a single point).
+ *   2. f64 only: a triangle with a nonzero coordinate of magnitude outside [2^-300, 2^300] is unchecked: it is never excluded as
+ *      degenerate, and a pair with it (the other triangle not excluded) is KEPT as its boxes decided it.  A stated superset: no contact
+ *      is dropped, and overflow-scale and subnormal scenes get a defined result.
+ *   3. Shared vertex: some vertex of P equals some vertex of Q (all three coordinates compare ==, so -0 equals +0).  With
+ *      skip_shared != 0 (self form only) the pair is NOT reported: the usual "non-adjacent self-intersections" of mesh repair tools;
+ *      the cost is that a fold-over between two triangles that share a vertex is not reported either.  Otherwise (skip_shared = 0, and
+ *      always between trees) it IS reported: the closed triangles share that point.  No predicate runs.
+ *   4. Otherwise: true exactly when the closed triangles, as sets of real points with the input coordinates as exact real numbers,
+ *      have a point in common.  Touching counts: a vertex on a face, an edge on an edge, coplanar triangles that only touch; coplanar
+ *      overlap counts too.
+ * Exactness of 4: every sign comes from orient3d / orient2d evaluated in double with a static error bound and, where that cannot
+ * decide, in exact double-precision expansion arithmetic (DESIGN.md §4.22).  f32: exact for every finite input (f32 values are
+ * multiples of 2^-149 below 2^128; nothing underflows or overflows).  f64: exact on [2^-300, 2^300] and zero, the range of step 2.
+ * Refusals: a null tree, a or b, or offsets pointer; a non-empty tree without triangles (never set, or dropped by
+ * bvhgpu_add_shapes_*); two trees of different contexts: BVHGPU_ERR_INVALID, nothing written.  A failed build is reported sticky
+ * first, A's before B's, before missing triangles.  Self with n < 2: all-zero offsets.  Trees: n_a = 0 gives offsets[0] = 0, n_b = 0
+ * all-zero offsets.  a == b is allowed and gives the full symmetric relation, (s, s) included for every non-excluded triangle.
+ * After bvhgpu_remove_shapes_* the triangles follow their shapes.
+ * Capacity, u32 saturation, BVHGPU_ERR_CAPACITY with *total, and the retained list for bvhgpu_traverse_fetch_* (kept on tree A) as
+ * bvhgpu_overlap_pairs_* / bvhgpu_overlap_trees_*.  The _dev forms take device pointers and enqueue on the context's stream; with
+ * `total` NULL they never synchronise the host, and dev_hits receives a prefix of length cap. */
+int bvhgpu_triangle_pairs_f32x3(bvhgpu_tree3f* tree, int skip_shared, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_f64x3(bvhgpu_tree3d* tree, int skip_shared, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_dev_f32x3(bvhgpu_tree3f* tree, int skip_shared, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_dev_f64x3(bvhgpu_tree3d* tree, int skip_shared, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_trees_f32x3(bvhgpu_tree3f* a, bvhgpu_tree3f* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_trees_f64x3(bvhgpu_tree3d* a, bvhgpu_tree3d* b, uint32_t* offsets, uint32_t* hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_trees_dev_f32x3(bvhgpu_tree3f* a, bvhgpu_tree3f* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+int bvhgpu_triangle_pairs_trees_dev_f64x3(bvhgpu_tree3d* a, bvhgpu_tree3d* b, void* dev_offsets, void* dev_hits, size_t cap, size_t* total);
+
 /* ---- nearest_to (SURVEY.md 8f N4): batched Bvh::nearest_to (src/bvh/bvh_impl.rs:221-238, src/bvh/bvh_node.rs:327-372) and
  * FlatBvh::nearest_to (src/flat_bvh.rs:513-562).  The reference calls the shape's own PointDistance::distance_squared at the
  * leaves (user code), so there are two forms.  `points`: 3 T per query point, host pointers.

@@ -109,6 +109,8 @@ template <> struct Abi<float> {
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f32x3(t, i, k); }
     static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f32x3(t, off, h, cap, tot); }
     static int overlap_trees(tree* a, tree* b, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_trees_f32x3(a, b, off, h, cap, tot); }
+    static int tri_pairs(tree* t, int skip, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_triangle_pairs_f32x3(t, skip, off, h, cap, tot); }
+    static int tri_pairs_trees(tree* a, tree* b, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_triangle_pairs_trees_f32x3(a, b, off, h, cap, tot); }
 };
 template <> struct Abi<double> {
     using aabb = bvh_aabb3d; using ray = bvh_ray3d; using node = bvh_node3d; using flat = bvh_flat3d; using tree = bvhgpu_tree3d;
@@ -133,6 +135,8 @@ template <> struct Abi<double> {
     static int remove(tree* t, const uint32_t* i, size_t k) { return bvhgpu_remove_shapes_f64x3(t, i, k); }
     static int overlap(tree* t, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_pairs_f64x3(t, off, h, cap, tot); }
     static int overlap_trees(tree* a, tree* b, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_overlap_trees_f64x3(a, b, off, h, cap, tot); }
+    static int tri_pairs(tree* t, int skip, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_triangle_pairs_f64x3(t, skip, off, h, cap, tot); }
+    static int tri_pairs_trees(tree* a, tree* b, uint32_t* off, uint32_t* h, size_t cap, size_t* tot) { return bvhgpu_triangle_pairs_trees_f64x3(a, b, off, h, cap, tot); }
 };
 struct Ctx {
     bvhgpu_ctx* h = nullptr;
@@ -294,6 +298,28 @@ template <class T> class Bvh {
         hits.resize(std::max<size_t>(4 * n_, 1024));
         size_t total = 0;
         const int st = A::overlap_trees(tree_, other.tree_, offsets.data(), hits.data(), hits.size(), &total);
+        if (st == BVHGPU_ERR_CAPACITY && total <= UINT32_MAX) { hits.resize(total); check(A::fetch(tree_, hits.data(), total)); }
+        else { check(st); hits.resize(total); }
+    }
+    // every pair of triangles (set_triangles) that meet, decided exactly: row s of overlap_pairs keeping the shapes whose closed
+    // triangle has a point in common with s's (bvhgpu_triangle_pairs_*).  Excluded triangles (non-finite or degenerate) meet nothing;
+    // skip_shared drops pairs that share a vertex; in f64 a triangle with a nonzero coordinate outside [2^-300, 2^300] keeps its box
+    // pairs.  offsets gets n + 1 entries.
+    void triangle_pairs(bool skip_shared, std::vector<uint32_t>& offsets, std::vector<uint32_t>& hits) const {
+        offsets.assign(n_ + 1, 0);
+        hits.resize(std::max<size_t>(4 * n_, 1024));
+        size_t total = 0;
+        const int st = A::tri_pairs(tree_, skip_shared ? 1 : 0, offsets.data(), hits.data(), hits.size(), &total);
+        if (st == BVHGPU_ERR_CAPACITY && total <= UINT32_MAX) { hits.resize(total); check(A::fetch(tree_, hits.data(), total)); }
+        else { check(st); hits.resize(total); }
+    }
+    // every pair (a, b) of a triangle of this tree and a triangle of `other` that meet (a shared vertex is a contact): row a of
+    // overlap_pairs_with filtered the same way (bvhgpu_triangle_pairs_trees_*).  Both trees must share a context; other may be *this.
+    void triangle_pairs_with(const Bvh<T>& other, std::vector<uint32_t>& offsets, std::vector<uint32_t>& hits) const {
+        offsets.assign(n_ + 1, 0);
+        hits.resize(std::max<size_t>(4 * n_, 1024));
+        size_t total = 0;
+        const int st = A::tri_pairs_trees(tree_, other.tree_, offsets.data(), hits.data(), hits.size(), &total);
         if (st == BVHGPU_ERR_CAPACITY && total <= UINT32_MAX) { hits.resize(total); check(A::fetch(tree_, hits.data(), total)); }
         else { check(st); hits.resize(total); }
     }

@@ -151,6 +151,37 @@ for prec in ("f32", "f64"):
         print("  overlap_trees", prec, D, len(ph))
         ta.free()
         tb.free()
+# triangle pairs (3-D): self (both skip_shared values) and between trees, host and device forms, a short capacity (fetch), a == b,
+# refused without triangles; a soup on a half-integer grid puts pairs on the exact coplanar path
+for prec in ("f32", "f64"):
+    import torch
+    F = api.BY_PREC[prec]["scalar"]
+    tris = []
+    for n in (600, 450):
+        c = rng.integers(0, 10, size=(n, 1, 3))
+        tris.append(((2 * c + rng.integers(0, 5, size=(n, 3, 3))) / 2).astype(F))
+    ts = []
+    for t in tris:
+        bo = np.zeros(len(t), dtype=api.BY_PREC[prec]["aabb"])
+        bo["min"], bo["max"] = t.min(axis=1), t.max(axis=1)
+        ts.append(api.Bvh.build(bo, prec=prec))
+    try:
+        ts[0].triangle_pairs()
+    except capi.BvhGpuError:
+        pass
+    for b, t in zip(ts, tris):
+        b.set_triangles(t)
+    po, ph = ts[0].triangle_pairs(skip_shared=False)
+    ts[0].triangle_pairs(skip_shared=True)
+    ts[0].triangle_pairs(skip_shared=False, cap=len(ph) // 2)
+    qo, qh = ts[0].triangle_pairs_with(ts[1])
+    ts[0].triangle_pairs_with(ts[0])
+    d_o = torch.zeros(len(tris[0]) + 1, dtype=torch.int32, device="cuda:0"); d_h = torch.zeros(max(len(ph), len(qh), 1), dtype=torch.int32, device="cuda:0")
+    ts[0].triangle_pairs_dev(d_o.data_ptr(), d_h.data_ptr(), len(ph) // 3, skip_shared=False)
+    ts[0].triangle_pairs_with_dev(ts[1], d_o.data_ptr(), d_h.data_ptr(), len(qh), True)
+    print("  triangle_pairs", prec, len(ph), len(qh))
+    for b in ts:
+        b.free()
 # host path on a batch large enough to be chunked (under the sanitizer the library takes the copy-then-walk form; forced streaming too)
 a = scenes.create_n_cubes_aabbs(300)
 b = api.Bvh.build(a)
