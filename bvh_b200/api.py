@@ -693,8 +693,9 @@ def swap_moves(n: int, indices) -> np.ndarray:
 
 class Bvh2(_Tree):
     """Device-resident Bvh<T,2> (the reference is generic in the dimension): build / nodes / flatten / traverse for 2-D AABBs and rays
-    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries, nearest_to, the distance-ordered traversal, the AABB closest hit and any hit.  Rays: structured array with 2-component origin, direction
-    (normalised), inv_direction."""
+    (bvhgpu_*_f32x2 / _f64x2), Aabb / Point / Ball queries, nearest_to, the distance-ordered traversal, the AABB closest hit and any hit,
+    and polygons over segments (set_segments: exact contains, knn_segments, signed_distance).  Rays: structured array with 2-component
+    origin, direction (normalised), inv_direction."""
 
     _TABLE = BY_PREC_2D
     _DIM = 2
@@ -800,6 +801,64 @@ class Bvh2(_Tree):
             self._sync_n()
         return swap_moves(n, idx)
 
+    # ---- polygons: the segments of set_segments (D = 2 only; include/bvh_b200.h, DESIGN.md 4.23) ----
+    _POLY_RULES = {"even_odd": capi.FILL_EVEN_ODD, "nonzero": capi.FILL_NONZERO}
+
+    def set_segments(self, segs):
+        """Segment s = (a, b) for every shape s: segs of shape (n, 2, 2) (or (n, 4): ax, ay, bx, by), n = num shapes.  Shape s's box
+        must contain segment s (not checked).  remove_shapes permutes them, add_shapes drops them, refit / update_shapes keep them."""
+        sg = np.ascontiguousarray(segs, dtype=self._d["scalar"]).reshape(-1, 4)
+        capi.check(getattr(capi.lib(), f"bvhgpu_tree_set_segments_{self._d['suffix']}")(self._h, _ptr(sg), len(sg)))
+
+    @classmethod
+    def from_segments(cls, segs, prec: str = "f32", ctx: Context | None = None, mode: int = capi.BUILD_EXACT_SAH) -> "Bvh2":
+        """A tree over the exact end-point boxes of the segments ((n, 2, 2)), with the segments set.  A NaN coordinate takes the other
+        end point's value in the box (the segment is excluded by every query anyway)."""
+        d = cls._TABLE[prec]
+        sg = np.ascontiguousarray(segs, dtype=d["scalar"]).reshape(-1, 2, 2)
+        a = np.zeros(len(sg), dtype=d["aabb"])
+        a["min"] = np.fmin(sg[:, 0], sg[:, 1])
+        a["max"] = np.fmax(sg[:, 0], sg[:, 1])
+        bvh = cls.build(a, prec, ctx, mode)
+        bvh.set_segments(sg)
+        return bvh
+
+    def contains(self, points, rule: str = "even_odd", winding: bool = False):
+        """Exact point-in-polygon over the segments: class (n,) u8 (0 outside, 1 inside, 2 boundary, 3 undecided: f64 coordinates
+        outside [2^-300, 2^300]), plus the winding number (n,) i32 with winding=True."""
+        p = self._points(points)
+        n = len(p)
+        cls_ = np.zeros(n, dtype=np.uint8)
+        w = np.zeros(n, dtype=np.int32) if winding else None
+        capi.check(getattr(capi.lib(), f"bvhgpu_contains_points_{self._d['suffix']}")(self._h, _ptr(p), n, self._POLY_RULES[rule], _ptr(cls_),
+                                                                                     _ptr(w)))
+        return (cls_, w) if winding else cls_
+
+    def knn_segments(self, points, k: int, max_dist=None, closest: bool = False):
+        """The k nearest segments of every point: (shape (n, k) u32, dist (n, k)), plus closest (n, k, 2) with closest=True; the
+        contract of Bvh.knn_triangles with the segment key (include/bvh_b200.h)."""
+        p = self._points(points)
+        n = len(p)
+        kk = max(int(k), 0)
+        shape = np.zeros((n, kk), dtype=np.uint32)
+        dist = np.zeros((n, kk), dtype=self._d["scalar"])
+        q = np.zeros((n, kk, 2), dtype=self._d["scalar"]) if closest else None
+        capi.check(getattr(capi.lib(), f"bvhgpu_knn_segments_{self._d['suffix']}")(self._h, _ptr(p), n, int(k) & 0xFFFFFFFF,
+                                                                                  _ptr(self._limits(max_dist, n)), _ptr(shape), _ptr(dist), _ptr(q)))
+        return (shape, dist, q) if closest else (shape, dist)
+
+    def signed_distance(self, points, rule: str = "even_odd", closest: bool = False):
+        """Signed distance to the segments: (shape (n,) u32, dist (n,)), plus closest (n, 2) with closest=True.  shape, |dist| and
+        closest are knn_segments(points, 1); dist is negated where contains(points, rule) gives 1 (inside)."""
+        p = self._points(points)
+        n = len(p)
+        shape = np.zeros(n, dtype=np.uint32)
+        dist = np.zeros(n, dtype=self._d["scalar"])
+        q = np.zeros((n, 2), dtype=self._d["scalar"]) if closest else None
+        capi.check(getattr(capi.lib(), f"bvhgpu_signed_distance_{self._d['suffix']}")(self._h, _ptr(p), n, self._POLY_RULES[rule], _ptr(shape),
+                                                                                     _ptr(dist), _ptr(q)))
+        return (shape, dist, q) if closest else (shape, dist)
+
 
 class Bvh4(Bvh2):
     """Device-resident Bvh<T,4> (bvhgpu_*_f32x4 / _f64x4): the exact SAH build (the only mode for D = 4), nodes, flatten, batched
@@ -809,6 +868,12 @@ class Bvh4(Bvh2):
 
     _TABLE = BY_PREC_4D
     _DIM = 4
+
+    def _segments_are_2d(self, *args, **kwargs):
+        raise TypeError("Bvh4 has no segments: polygons (set_segments, contains, knn_segments, signed_distance) are 2-D only")
+
+    set_segments = contains = knn_segments = signed_distance = _segments_are_2d
+    from_segments = classmethod(_segments_are_2d)
 
     # The device-pointer forms the 3-D tree has too (Bvh2 has no C entry point for them).
     traverse_dev, overlap_pairs_dev, overlap_pairs_with_dev, knn_dev = (Bvh.traverse_dev, Bvh.overlap_pairs_dev, Bvh.overlap_pairs_with_dev,

@@ -18,8 +18,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 SO = os.path.join(HERE, "libbvh_b200.so")
-SOURCES = ["capi.cu", "build_sah.cu", "flatten.cu", "traverse.cu", "lbvh.cu", "closest.cu", "dim2.cu", "dynamic.cu", "dim4.cu", "tripairs.cu"]
-HEADERS = ["common.cuh", "internal.h", "build_types.cuh", "csr.cuh", "queries.cuh", "update.cuh", "dynamic.cuh", "tritri.cuh", os.path.join("..", "..", "include", "bvh_b200.h")]
+SOURCES = ["capi.cu", "build_sah.cu", "flatten.cu", "traverse.cu", "lbvh.cu", "closest.cu", "dim2.cu", "dynamic.cu", "dim4.cu", "tripairs.cu", "segments.cu"]
+HEADERS = ["common.cuh", "internal.h", "build_types.cuh", "csr.cuh", "queries.cuh", "update.cuh", "dynamic.cuh", "tritri.cuh", "exact.cuh", os.path.join("..", "..", "include", "bvh_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -60,7 +60,7 @@ template <class T> static void tree_release(Tree<T>* t) {
     bvhgpu_ctx* ctx = t->ctx;
     if (ctx) {
         dfree(ctx, t->d_aabb); dfree(ctx, t->d_aabb_trav); dfree(ctx, t->d_nodes); dfree(ctx, t->d_node_index); dfree(ctx, t->d_node_start);
-        dfree(ctx, t->d_tris); dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad); dfree(ctx, t->d_tnodes); dfree(ctx, t->d_top); dfree(ctx, t->d_flat); dfree(ctx, t->d_status); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
+        dfree(ctx, t->d_tris); dfree(ctx, t->d_segs); dfree(ctx, t->d_sa_base); dfree(ctx, t->d_arrive); dfree(ctx, t->d_bad); dfree(ctx, t->d_tnodes); dfree(ctx, t->d_top); dfree(ctx, t->d_flat); dfree(ctx, t->d_status); dfree(ctx, t->d_offsets); dfree(ctx, t->d_hits);
     }
 }
 
@@ -828,6 +828,78 @@ static int signed_distance_dev_impl(Tree<T>* tree, const void* d_points, size_t 
     return signed_distance_device<T>(tree, (const T*)d_points, n, rule, (uint32_t*)d_shape, (T*)d_dist, (T*)d_closest);
 }
 
+// Polygons of a 2-D tree (segments.cu), host pointers: 2 T per point, copied back after the device driver, whose checks (n, rule / k,
+// status, segments) all run before anything is written.
+template <class T>
+static int polygon_contains_host_impl(Tree<T>* tree, const T* points, size_t n, int rule, uint8_t* out_class, int32_t* out_winding) {
+    if (!tree || (n && (!points || !out_class))) { set_error("contains_points: null argument"); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return polygon_contains_device<T>(tree, nullptr, 0, rule, nullptr, nullptr);
+    BVH_TRY(check_n("contains_points", n));
+    Scratch scratch(ctx);
+    T* d_p = nullptr;
+    uint8_t* d_c = nullptr;
+    int32_t* d_w = nullptr;
+    BVH_TRY(scratch.get(&d_p, 2 * n));
+    BVH_TRY(scratch.get(&d_c, n));
+    if (out_winding) BVH_TRY(scratch.get(&d_w, n));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_p, points, sizeof(T) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
+    BVH_TRY(polygon_contains_device<T>(tree, d_p, n, rule, d_c, d_w));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_class, d_c, n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_winding) BVH_CUDA_TRY(cudaMemcpyAsync(out_winding, d_w, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T>
+static int knn_seg_host_impl(Tree<T>* tree, const T* points, size_t n, uint32_t k, const T* max_dist, uint32_t* out_shape, T* out_dist, T* out_closest) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("knn_segments: null argument"); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return knn_seg_device<T>(tree, nullptr, 0, k, nullptr, nullptr, nullptr, nullptr);
+    BVH_TRY(check_n("knn_segments", n));
+    if (k < 1 || k > BVHGPU_KNN_MAX_K) { set_error("knn_segments: k = %u outside 1 .. %d", k, BVHGPU_KNN_MAX_K); return BVHGPU_ERR_INVALID; }
+    Scratch scratch(ctx);
+    T *d_p = nullptr, *d_r = nullptr, *d_d = nullptr, *d_q = nullptr;
+    uint32_t* d_s = nullptr;
+    const size_t nk = n * k;
+    BVH_TRY(scratch.get(&d_p, 2 * n));
+    if (max_dist) BVH_TRY(scratch.get(&d_r, n));
+    BVH_TRY(scratch.get(&d_s, nk));
+    BVH_TRY(scratch.get(&d_d, nk));
+    if (out_closest) BVH_TRY(scratch.get(&d_q, 2 * nk));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_p, points, sizeof(T) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
+    if (max_dist) BVH_CUDA_TRY(cudaMemcpyAsync(d_r, max_dist, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
+    BVH_TRY(knn_seg_device<T>(tree, d_p, n, k, d_r, d_s, d_d, d_q));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * nk, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * nk, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_closest) BVH_CUDA_TRY(cudaMemcpyAsync(out_closest, d_q, sizeof(T) * 2 * nk, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+template <class T>
+static int polygon_distance_host_impl(Tree<T>* tree, const T* points, size_t n, int rule, uint32_t* out_shape, T* out_dist, T* out_closest) {
+    if (!tree || (n && (!points || !out_shape || !out_dist))) { set_error("signed_distance: null argument"); return BVHGPU_ERR_INVALID; }
+    bvhgpu_ctx* ctx = tree->ctx;
+    BVH_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (n == 0) return polygon_distance_device<T>(tree, nullptr, 0, rule, nullptr, nullptr, nullptr);
+    BVH_TRY(check_n("signed_distance", n));
+    Scratch scratch(ctx);
+    T *d_p = nullptr, *d_d = nullptr, *d_q = nullptr;
+    uint32_t* d_s = nullptr;
+    BVH_TRY(scratch.get(&d_p, 2 * n));
+    BVH_TRY(scratch.get(&d_s, n));
+    BVH_TRY(scratch.get(&d_d, n));
+    if (out_closest) BVH_TRY(scratch.get(&d_q, 2 * n));
+    BVH_CUDA_TRY(cudaMemcpyAsync(d_p, points, sizeof(T) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
+    BVH_TRY(polygon_distance_device<T>(tree, d_p, n, rule, d_s, d_d, d_q));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_shape, d_s, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaMemcpyAsync(out_dist, d_d, sizeof(T) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_closest) BVH_CUDA_TRY(cudaMemcpyAsync(out_closest, d_q, sizeof(T) * 2 * n, cudaMemcpyDeviceToHost, ctx->stream));
+    BVH_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return BVHGPU_OK;
+}
+
 template <class T> static int fetch_impl(Tree<T>* tree, uint32_t* hits, size_t cap) {
     if (!tree || !hits) { set_error("traverse_fetch: null argument"); return BVHGPU_ERR_INVALID; }
     if (cap < tree->last_total) { set_error("traverse_fetch: capacity %zu < %zu hits", cap, tree->last_total); return BVHGPU_ERR_CAPACITY; }
@@ -1047,8 +1119,8 @@ template <class T> static int build_into_empty(Tree<T>* tree, const typename Tra
     int rc = build_exact_sah<T>(ctx, d_in, k, &fresh);
     if (rc == BVHGPU_OK) rc = resolve_status(&fresh);
     if (rc != BVHGPU_OK) { tree_release(&fresh); return rc; }
-    dfree(ctx, tree->d_status); dfree(ctx, tree->d_sa_base); dfree(ctx, tree->d_tris);
-    tree->d_sa_base = nullptr; tree->d_tris = nullptr;
+    dfree(ctx, tree->d_status); dfree(ctx, tree->d_sa_base); dfree(ctx, tree->d_tris); dfree(ctx, tree->d_segs);
+    tree->d_sa_base = nullptr; tree->d_tris = nullptr; tree->d_segs = nullptr;
     tree->n = fresh.n; tree->n_nodes = fresh.n_nodes; tree->d_status = fresh.d_status;
     tree->d_aabb = fresh.d_aabb; tree->d_nodes = fresh.d_nodes; tree->d_node_index = fresh.d_node_index; tree->d_node_start = fresh.d_node_start;
     if (tree->dims == 2) {                                              // the FLAT leaf boxes, read by the records, at the new n
@@ -1700,6 +1772,23 @@ BVH_EXPORT int bvhgpu_host_free(bvhgpu_ctx* ctx, void* p) {
     }                                                                                                                      \
     BVH_EXPORT int bvhgpu_remove_shapes_##SUF(TREE* tree, const uint32_t* indices, size_t k) {                             \
         return remove_impl<2, T>(tree, indices, k, false);                                                                 \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_tree_set_segments_##SUF(TREE* tree, const T* segments, size_t n) {                               \
+        if (!tree || (n && !segments)) { set_error("set_segments: null argument"); return BVHGPU_ERR_INVALID; }            \
+        BVH_CUDA_TRY(cudaSetDevice(tree->ctx->device));                                                                    \
+        return set_segments<T>(tree, segments, n);                                                                         \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_contains_points_##SUF(TREE* tree, const T* points, size_t n, int rule, uint8_t* out_class,       \
+                                                int32_t* out_winding) {                                                    \
+        return polygon_contains_host_impl<T>(tree, points, n, rule, out_class, out_winding);                               \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_knn_segments_##SUF(TREE* tree, const T* points, size_t n, uint32_t k, const T* max_dist,         \
+                                             uint32_t* out_shape, T* out_dist, T* out_closest) {                           \
+        return knn_seg_host_impl<T>(tree, points, n, k, max_dist, out_shape, out_dist, out_closest);                       \
+    }                                                                                                                      \
+    BVH_EXPORT int bvhgpu_signed_distance_##SUF(TREE* tree, const T* points, size_t n, int rule, uint32_t* out_shape,      \
+                                                T* out_dist, T* out_closest) {                                             \
+        return polygon_distance_host_impl<T>(tree, points, n, rule, out_shape, out_dist, out_closest);                     \
     }
 
 #define DEFINE_API4(T, SUF, TREE, AABB, RAY, NODE, FLAT)                                                                   \

@@ -3,7 +3,8 @@
 // traversal's kernel, the self-overlap and two-tree overlap kernels, the host driver of count -> scan -> fill, and the device
 // drivers of the CSR families (queries, 4-D rays, nearest_candidates, ordered traversal, overlap, overlap between two trees), written
 // once over the tree type and instantiated in traverse.cu (Tree<T>: D = 3, and D = 2 through the z = 0 lift) and dim4.cu (Tree4<T>).
-// The triangle pairs (3-D only) reuse the overlap walk with a leaf policy and are instantiated in tripairs.cu.
+// The triangle pairs (3-D only) reuse the overlap walk with a leaf policy and are instantiated in tripairs.cu; the point-in-polygon
+// walk of 2-D trees (segments.cu) reuses its record loop, overlap_records.
 // The 3-D ray kernels of traverse.cu use the same fetch.
 //
 // CSR: offsets[n + 1] (u32, saturated to 0xFFFFFFFF) and the hit list hits[total]; the fill pass stores hits[0 .. cap) only, so a
@@ -215,6 +216,23 @@ __device__ __forceinline__ bool overlap_boxes(const T smn[D], const T smx[D], co
     for (int k = 0; k < D; ++k) hit = hit && !(smx[k] < mn[k] || mx[k] < smn[k]);
     return hit;
 }
+// The record loop of the overlap walks, from record i to n_rec: a record is entered when overlap_enter(smn, smx, its box) holds, and
+// visit(shape) is called for every entered leaf record, in DFS order.  The overlap kernels below and the point-in-polygon walk of
+// segments.cu (a point's box [px, +inf] x [py, py]) run it.
+template <int D, class T, class Rec, class Visit>
+__device__ __forceinline__ void overlap_records(const Rec* __restrict__ trec, uint32_t i, uint32_t n_rec, const T smn[D], const T smx[D], Visit visit) {
+    while (i < n_rec) {
+        T mn[D], mx[D];
+        uint32_t skip, shape;
+        fetch(trec + i, mn, mx, skip, shape);
+        if (overlap_enter<D, T>(smn, smx, mn, mx)) {
+            if (shape != BVH_INVALID) visit(shape);
+            ++i;
+        } else {
+            i = skip;
+        }
+    }
+}
 // The leaf policy of the overlap kernels: the boxes decide.  A policy has row(s), false when row s is empty whatever the boxes say,
 // and keep(t), which filters a shape whose box passed (TriPairsLeaf, tritri.cuh: the triangle pairs).
 struct BoxesDecide {
@@ -248,24 +266,14 @@ __device__ __forceinline__ void overlap_walk(const typename CsrRecords<D, T>::Re
     }
     uint32_t cnt = 0, i = CROSS ? 0u : __ldg(node_index + s);
     if (!leaf.row(s)) i = n_rec;
-    while (i < n_rec) {
-        T mn[D], mx[D];
-        uint32_t skip, shape;
-        fetch(trec + i, mn, mx, skip, shape);
-        if (overlap_enter<D, T>(smn, smx, mn, mx)) {
-            if (shape != BVH_INVALID) {
-                T tmn[D], tmx[D];
-                load_box(other + shape, tmn, tmx);
-                if (overlap_boxes<D, T>(smn, smx, tmn, tmx) && leaf.keep(shape)) {
-                    if (FILL) { if (w < cap) hits[w] = shape; ++w; }
-                    else ++cnt;
-                }
-            }
-            ++i;
-        } else {
-            i = skip;
+    overlap_records<D, T>(trec, i, n_rec, smn, smx, [&](uint32_t shape) {
+        T tmn[D], tmx[D];
+        load_box(other + shape, tmn, tmx);
+        if (overlap_boxes<D, T>(smn, smx, tmn, tmx) && leaf.keep(shape)) {
+            if (FILL) { if (w < cap) hits[w] = shape; ++w; }
+            else ++cnt;
         }
-    }
+    });
     if (!FILL) counts[s] = cnt;
 }
 template <int D, class T, bool FILL>

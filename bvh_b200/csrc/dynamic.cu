@@ -20,7 +20,7 @@
 // The host drivers of refit, update_shapes, add_shapes and remove_shapes are here too, one per operation for Tree<T> (D = 2, 3) and
 // Tree4<T> (D = 4) alike (DESIGN.md sections 4.12, 4.13).  What the two tree types do differently is an overload on the tree type:
 // building subtrees from seeded roots, the growth rebuild, the caches after boxes change in place and after a relocation, the
-// triangles and the deferred build status of a 3-D tree.
+// per-shape geometry (triangles of a 3-D tree, segments of a 2-D tree) and the deferred build status.
 #include "internal.h"
 #include "dynamic.cuh"
 #include <cub/device/device_scan.cuh>
@@ -173,12 +173,20 @@ template <class T> static int keep_build_error(Tree<T>* tree, uint32_t* saved, b
 }
 template <class T> static int keep_build_error(Tree4<T>*, uint32_t*, bool) { return BVHGPU_OK; }
 
-// The triangles of a 3-D tree (bvhgpu_tree_set_triangles_*): a removal permutes them with the boxes, an add drops them (the new
-// shapes' triangles are unknown until they are set again).
-template <class T> static const void* triangles(const Tree<T>* tree) { return tree->d_tris; }
-template <class T> static const void* triangles(const Tree4<T>*) { return nullptr; }
-template <class T> static void swap_triangles(Tree<T>* tree, void* tris) { dfree(tree->ctx, tree->d_tris); tree->d_tris = tris; }
-template <class T> static void swap_triangles(Tree4<T>*, void*) {}
+// The per-shape geometry a tree carries: the triangles of a 3-D tree (bvhgpu_tree_set_triangles_*, DTri<T>) or the segments of a 2-D
+// tree (bvhgpu_tree_set_segments_*, DSeg<T>).  A removal permutes it with the boxes (*words: its size in 16-byte words), an add drops
+// it (the new shapes' geometry is unknown until it is set again).
+template <class T> static const void* geometry(const Tree<T>* tree, uint32_t* words) {
+    *words = (uint32_t)((tree->dims == 2 ? sizeof(DSeg<T>) : sizeof(DTri<T>)) / 16);
+    return tree->dims == 2 ? tree->d_segs : tree->d_tris;
+}
+template <class T> static const void* geometry(const Tree4<T>*, uint32_t* words) { *words = 0; return nullptr; }
+template <class T> static void swap_geometry(Tree<T>* tree, void* g) {
+    void*& slot = tree->dims == 2 ? tree->d_segs : tree->d_tris;
+    dfree(tree->ctx, slot);
+    slot = g;
+}
+template <class T> static void swap_geometry(Tree4<T>*, void*) {}
 
 // ---- refit and update_shapes (Bvh::update_shapes, src/bvh/optimization.rs:304-351; DESIGN.md section 4.12) ----------------------
 template <class TreeT> int check_boxes(TreeT* tree, const uint32_t* d_changed, const typename TreeT::Aabb* d_fresh, uint32_t m, Scratch& scratch,
@@ -319,7 +327,7 @@ template <class TreeT> int add_shapes(TreeT* tree, typename TreeT::Box* aabb_all
     // the tree now is the new one (its boxes on the affected paths are still to be recomputed); from here on a failure leaves it
     // half-done, and the caller marks it failed
     dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
-    swap_triangles(tree, nullptr);
+    swap_geometry(tree, nullptr);
     tree->d_nodes = nw; tree->d_node_start = nstart; tree->d_node_index = nidx; tree->d_aabb = aabb_all; tree->d_sa_base = sa_new;
     tree->n = N; tree->n_nodes = nn2;
     uint32_t* h = ctx->h_pinned + 220;
@@ -358,10 +366,9 @@ template <class TreeT> int remove_shapes(TreeT* tree, const uint32_t* d_rm, uint
     bvhgpu_ctx* ctx = tree->ctx;
     cudaStream_t st = ctx->stream;
     const uint32_t n = tree->n, nn = tree->n_nodes, m = n - k, nn2 = m ? 2 * m - 1 : 0;
-    const uint32_t t_words = sizeof(T) == 4 ? 3 : 6;                          // DTri<T> (closest.cu) in 16-byte words
     if (m == 0) {                                                              // everything goes: the tree of an n == 0 build
         dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
-        swap_triangles(tree, nullptr);
+        swap_geometry(tree, nullptr);
         tree->d_nodes = nullptr; tree->d_node_start = nullptr; tree->d_node_index = nullptr; tree->d_aabb = nullptr; tree->d_sa_base = nullptr;
         tree->n = 0; tree->n_nodes = 0;
         return finish_relayout(tree);
@@ -379,7 +386,8 @@ template <class TreeT> int remove_shapes(TreeT* tree, const uint32_t* d_rm, uint
     survive_kernel<<<(nn + 256) / 256, 256, 0, st>>>(tree->d_nodes, tree->d_node_start, nn, rk.R, flag);
     ctx->launches++;
     BVH_TRY(exclusive_sum_u32(scratch, flag, newidx, (size_t)nn + 1, st));
-    const void* tris = triangles(tree);
+    uint32_t t_words = 0;
+    const void* tris = geometry(tree, &t_words);
     Node* nw = nullptr;
     uint32_t *nstart = nullptr, *nidx = nullptr;
     Box* a_new = nullptr;
@@ -398,7 +406,7 @@ template <class TreeT> int remove_shapes(TreeT* tree, const uint32_t* d_rm, uint
                                                            static_cast<uint4*>(t_new), t_words);
     ctx->launches += 2;
     dfree(ctx, tree->d_nodes); dfree(ctx, tree->d_node_start); dfree(ctx, tree->d_node_index); dfree(ctx, tree->d_aabb); dfree(ctx, tree->d_sa_base);
-    swap_triangles(tree, t_new);
+    swap_geometry(tree, t_new);
     tree->d_nodes = nw; tree->d_node_start = nstart; tree->d_node_index = nidx; tree->d_aabb = a_new; tree->d_sa_base = sa_new;
     tree->n = m; tree->n_nodes = nn2;
     if (nn2 > 1) {

@@ -85,6 +85,8 @@ namespace bvhb200 {
 
 // The device layout of a triangle of bvhgpu_tree_set_triangles_* (Tree::d_tris).
 template <class T> struct DTri { T a[3], pa, b[3], pb, c[3], pc; };       // 48 B / 96 B: three vector loads per triangle
+// The device layout of a segment of bvhgpu_tree_set_segments_* (Tree::d_segs, 2-D trees): the ABI's 4 T as they are.
+template <class T> struct DSeg { T a[2], b[2]; };                         // 16 B / 32 B: one / two vector loads per segment
 
 template <class T> struct Tree {
     using Tr = Traits<T>;
@@ -109,6 +111,7 @@ template <class T> struct Tree {
     uint8_t* d_bad = nullptr;                 // [2n-1] growth flags of the incremental update (all zero between calls)
     T* d_sa_base = nullptr;                   // [2n-1] surface area of every inner node when it was last (re)built: baseline of bvhgpu_optimize / update
     void* d_tris = nullptr;                   // [n] triangle vertices (padded), optional: bvhgpu_tree_set_triangles_*
+    void* d_segs = nullptr;                   // [n] dims == 2 only: segment end points (DSeg<T>), optional: bvhgpu_tree_set_segments_*
     typename Tr::Flat* d_flat = nullptr;      // [n_flat] reference-layout FlatBvh (built on demand)
     size_t n_flat = 0;
     bool have_flat = false;
@@ -345,6 +348,16 @@ template <class T> int contains_points_device(Tree<T>* tree, const T* d_points, 
 template <class T> int signed_distance_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint32_t* d_shape, T* d_dist, T* d_closest);
 template <class T> int rays_new_device(bvhgpu_ctx* ctx, const T* d_origins, const T* d_dirs, size_t n,
                                        typename Traits<T>::Ray* d_rays);
+// ---- segments.cu: polygons of 2-D trees (DESIGN.md §4.23) ----
+// The segments of every shape, host pointer: 4 T per segment (ax, ay, bx, by), n == tree->n.  Synchronises.
+template <class T> int set_segments(Tree<T>* tree, const T* segs4, size_t n);
+// Point-in-polygon, k nearest segments and signed distance, device pointers (2 T per point), on the context's stream, nothing
+// synchronises.  Each checks n (<= 2^31-1), its rule / k, the tree's status, then the segments; the pointers are checked by the caller.
+// d_winding and d_closest (2 T per slot) may be nullptr.
+template <class T> int polygon_contains_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint8_t* d_class, int32_t* d_winding);
+template <class T> int knn_seg_device(Tree<T>* tree, const T* d_points, size_t n, uint32_t k, const T* d_max_dist, uint32_t* d_shape, T* d_dist,
+                                      T* d_closest);
+template <class T> int polygon_distance_device(Tree<T>* tree, const T* d_points, size_t n, int rule, uint32_t* d_shape, T* d_dist, T* d_closest);
 
 // ---- dim4.cu: D = 4 ----
 // Traversal record: the AABB the node has in its parent, `skip` (first record behind the subtree) and the shape index of a leaf.

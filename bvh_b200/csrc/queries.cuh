@@ -145,6 +145,9 @@ template <int D, class T> __device__ __forceinline__ T aabb_min_d2(const T p[D],
     for (int k = 2; k < D; ++k) acc = add_rn(acc, mul_rn(o[k], o[k]));
     return acc;
 }
+template <class T> __device__ __forceinline__ T quiet_nan();                                      // the padding of out_closest
+template <> __device__ __forceinline__ float quiet_nan<float>() { return __int_as_float(0x7fc00000); }
+template <> __device__ __forceinline__ double quiet_nan<double>() { return __longlong_as_double(0x7ff8000000000000ll); }
 __device__ __forceinline__ float sqrt_rn(float x) { return __fsqrt_rn(x); }
 __device__ __forceinline__ double sqrt_rn(double x) { return __dsqrt_rn(x); }
 

@@ -1573,9 +1573,6 @@ template int knn_device<double>(Tree<double>*, const double*, size_t, uint32_t, 
 // nearest_kernel's triangle mode) at the leaves.  A NaN key fails knn_walk's `key <= r2` and never enters the list.  The closest points
 // are recomputed for the k final slots after the walk, in a loop of their own as the square roots are: the list carries no 3 K extra
 // values, and the recomputation performs the same operations on the same inputs, so q is the point the key was measured against. ----
-template <class T> __device__ __forceinline__ T quiet_nan();                                      // the padding of out_closest
-template <> __device__ __forceinline__ float quiet_nan<float>() { return __int_as_float(0x7fc00000); }
-template <> __device__ __forceinline__ double quiet_nan<double>() { return __longlong_as_double(0x7ff8000000000000ll); }
 template <class T, int K>
 __global__ void __launch_bounds__(128) knn_tri_kernel(const typename Traits<T>::Node* __restrict__ nodes, uint32_t n_shapes,
                                                       const T* __restrict__ tris, const T* __restrict__ points, const T* __restrict__ max_dist,

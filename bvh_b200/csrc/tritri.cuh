@@ -5,8 +5,8 @@
 // projection (degree 2).  A sign is first read from a double-precision evaluation with Shewchuk's static error bound (every operation
 // rounded explicitly: the library is built -fmad=false, and the bound assumes no contraction); only when the bound cannot decide it does
 // the exact evaluation run: every monomial of the determinant as a sum of doubles (two_prod through fma, differences through two_sum),
-// accumulated into a nonoverlapping expansion whose largest component carries the sign.  The exact evaluations are __noinline__ so the
-// walk's common path keeps its registers.
+// accumulated into a nonoverlapping expansion whose largest component carries the sign (exact.cuh holds the arithmetic and orient2d).
+// The exact evaluations are __noinline__ so the walk's common path keeps its registers.
 //
 // Exactness: f32 inputs promoted to double are multiples of 2^-149 below 2^128 in magnitude, f64 inputs that are zero or of magnitude
 // in [2^-300, 2^300] are multiples of 2^-352 below 2^301.  A degree-3 monomial of coordinate differences is then a multiple of 2^-447
@@ -14,36 +14,14 @@
 // or overflows, so two_prod and two_sum are exact and the filter's rounding errors are relative.  Outside that range (f64 only) a
 // triangle is "unchecked": the predicate does not run on it (TriPairsLeaf keeps its pairs).
 #pragma once
-#include "internal.h"
+#include "exact.cuh"
 
 namespace bvhb200 {
 #ifdef __CUDACC__
 
 constexpr double TRI_F64_LO = 0x1p-300, TRI_F64_HI = 0x1p+300;     // the f64 range the predicate is exact on (zero as well)
 
-// ---- exact arithmetic (Shewchuk, "Adaptive precision floating-point arithmetic and fast robust geometric predicates", 1997) ----
-__device__ __forceinline__ void two_sum(double a, double b, double& s, double& e) {
-    s = __dadd_rn(a, b);
-    const double bv = __dsub_rn(s, a), av = __dsub_rn(s, bv);
-    e = __dadd_rn(__dsub_rn(a, av), __dsub_rn(b, bv));
-}
-__device__ __forceinline__ void two_prod(double a, double b, double& p, double& e) {
-    p = __dmul_rn(a, b);
-    e = __fma_rn(a, b, -p);
-}
-// h[0 .. m) (nonoverlapping, increasing magnitude, no zeros) += b exactly (Grow-Expansion with zero elimination); returns the length.
-__device__ __forceinline__ int grow(double* h, int m, double b) {
-    double q = b;
-    int k = 0;
-    for (int i = 0; i < m; ++i) {
-        double s, e;
-        two_sum(q, h[i], s, e);
-        if (e != 0.0) h[k++] = e;
-        q = s;
-    }
-    if (q != 0.0) h[k++] = q;
-    return k;
-}
+// ---- exact arithmetic: two_sum, two_prod, grow, grow_prod2, orient2d_exact and orient2d_sign are in exact.cuh ----
 // h += sign * x * y * z exactly (four doubles); zero factors add nothing.
 __device__ __forceinline__ int grow_prod3(double* h, int m, double x, double y, double z, bool neg) {
     if (x == 0.0 || y == 0.0 || z == 0.0) return m;
@@ -55,15 +33,6 @@ __device__ __forceinline__ int grow_prod3(double* h, int m, double x, double y, 
     m = grow(h, m, e2); m = grow(h, m, e1); m = grow(h, m, p2);
     return grow(h, m, p1);
 }
-__device__ __forceinline__ int grow_prod2(double* h, int m, double x, double y, bool neg) {
-    if (x == 0.0 || y == 0.0) return m;
-    double p, e;
-    two_prod(x, y, p, e);
-    if (neg) { p = -p; e = -e; }
-    return grow(h, grow(h, m, e), p);
-}
-__device__ __forceinline__ int expansion_sign(const double* h, int m) { return m == 0 ? 0 : (h[m - 1] > 0.0 ? 1 : -1); }
-
 // Exact sign of orient3d(a, b, c, d) = det[a - d; b - d; c - d]: each difference is hi + lo (two_sum), the determinant the sum of its
 // 6 x 8 monomials of three such parts.  By value, so that the caller's points stay in registers.
 __device__ __noinline__ int orient3d_exact(double ax, double ay, double az, double bx, double by, double bz, double cx, double cy, double cz,
@@ -83,20 +52,6 @@ __device__ __noinline__ int orient3d_exact(double ax, double ay, double az, doub
     }
     return expansion_sign(h, m);
 }
-// Exact sign of orient2d(a, b, c) = (a - c) x (b - c).
-__device__ __noinline__ int orient2d_exact(double ax, double ay, double bx, double by, double cx, double cy) {
-    double A[2][2], B[2][2];
-    two_sum(ax, -cx, A[0][0], A[0][1]); two_sum(ay, -cy, A[1][0], A[1][1]);
-    two_sum(bx, -cx, B[0][0], B[0][1]); two_sum(by, -cy, B[1][0], B[1][1]);
-    double h[16];
-    int m = 0;
-    for (int u = 0; u < 4; ++u) {
-        m = grow_prod2(h, m, A[0][u & 1], B[1][u >> 1], false);
-        m = grow_prod2(h, m, A[1][u & 1], B[0][u >> 1], true);
-    }
-    return expansion_sign(h, m);
-}
-
 // ---- filtered signs (Shewchuk's orient3d / orient2d stage A: the same evaluation order and bounds) ----
 // A call, not inlined: tri_tri makes up to 24 of them, and inlined they would spill the walk's registers.
 __device__ __noinline__ int orient3_sign(double ax, double ay, double az, double bx, double by, double bz, double cx, double cy, double cz,
@@ -125,14 +80,7 @@ __device__ __forceinline__ int orient3(const double a[3], const double b[3], con
 __device__ __forceinline__ double comp(const double a[3], int i) { return i == 0 ? a[0] : i == 1 ? a[1] : a[2]; }
 // orient2d of the projection of a, b, c onto axes (i, j).
 __device__ __forceinline__ int orient2(const double a[3], const double b[3], const double c[3], int i, int j) {
-    constexpr double BOUND = (3.0 + 16.0 * 0x1p-53) * 0x1p-53;
-    const double ax = comp(a, i), ay = comp(a, j), bx = comp(b, i), by = comp(b, j), cx = comp(c, i), cy = comp(c, j);
-    const double l = __dmul_rn(__dsub_rn(ax, cx), __dsub_rn(by, cy));
-    const double r = __dmul_rn(__dsub_rn(ay, cy), __dsub_rn(bx, cx));
-    const double det = __dsub_rn(l, r), err = __dmul_rn(BOUND, __dadd_rn(fabs(l), fabs(r)));
-    if (det > err) return 1;
-    if (-det > err) return -1;
-    return orient2d_exact(ax, ay, bx, by, cx, cy);
+    return orient2d_sign(comp(a, i), comp(a, j), comp(b, i), comp(b, j), comp(c, i), comp(c, j));
 }
 
 // ---- the predicate on triangles of doubles ----

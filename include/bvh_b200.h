@@ -340,7 +340,8 @@ int bvhgpu_remove_shapes_dev_f64x4(bvhgpu_tree4d* tree, const void* dev_indices,
  * for each leaf (empty boxes of "no split wins" nodes: entry 0 / exit +inf), ties in DFS order, that distance in `dists`; closest =
  * the shape whose own AABB the ray enters first, key (entry distance, DFS order), exact, BVHGPU_INVALID_INDEX / +inf without a hit.
  * Differences:
- *   - there is no triangle mode: Ray::intersects_triangle needs a 3-D cross product.
+ *   - there is no triangle mode: Ray::intersects_triangle needs a 3-D cross product.  (The primitives of a 2-D tree are the segments
+ *     of bvhgpu_tree_set_segments_*x2, which serve point-in-polygon, k nearest segments and signed distance: see "polygons" below.)
  *   - a null argument or nrays > 2^31-1: BVHGPU_ERR_INVALID, nothing is read or written.  An empty tree gives all-zero offsets or
  *     no-hit results; a root leaf (n = 1) is decided by the shape's own box, as in the reference.
  *   - ordered, host pointers, `cap` entries in hits and dists: there is no fetch call.  When the hits do not fit `cap`, offsets and
@@ -721,6 +722,60 @@ int bvhgpu_signed_distance_dev_f32x3(bvhgpu_tree3f* tree, const void* dev_points
                                      void* dev_closest);
 int bvhgpu_signed_distance_dev_f64x3(bvhgpu_tree3d* tree, const void* dev_points, size_t n, int rule, void* dev_shape, void* dev_dist,
                                      void* dev_closest);
+
+/* ---- polygons (D = 2): exact point-in-polygon with winding numbers, k nearest segments and signed distance over line segments (GIS
+ * point-in-outline tests, 2-D physics and games, occupancy maps, font and vector SDFs).  bvhgpu_tree_set_segments_* gives shape s the
+ * segment (ax, ay, bx, by): 4 T per shape, n must equal the tree's shape count (else BVHGPU_ERR_INVALID).  The caller guarantees that
+ * shape s's current AABB contains segment s; it is not checked.  The segments follow their shapes through bvhgpu_remove_shapes_*,
+ * bvhgpu_add_shapes_* drops them (every segment call refuses until they are set again), bvhgpu_refit_* and bvhgpu_update_* keep them
+ * (they can go stale: a segment outside its box may then be missed).  Host pointers; set_segments synchronises.
+ *
+ * bvhgpu_contains_points_*x2: per point p (2 T), with every comparison exact and every sign decided in exact real arithmetic:
+ *   excluded   a segment with a non-finite coordinate or a == b contributes nothing and is never boundary.
+ *   relevant   a non-excluded s with min(ay, by) <= py <= max(ay, by) and max(ax, bx) >= px (its own end points, not its box).
+ *   o          sign(orient2d(a, b, p)), orient2d(a, b, c) = (a - c) x (b - c): positive when p lies left of a -> b.
+ *   contribution of a relevant s: +1 if ay <= py < by and o > 0; -1 if by <= py < ay and o < 0; else 0 (horizontal segments give 0).
+ *   boundary   o == 0 and p in the closed box of a and b.
+ *   out_winding[i] (may be NULL) = the sum of the contributions: the winding number of closed loops around a point not on them.
+ *   out_class[i] = BVHGPU_POINT_BOUNDARY when p is boundary of some relevant segment (this wins); else BVHGPU_POINT_UNDECIDED (f64 only,
+ *   below); else BVHGPU_POINT_INSIDE when the winding is odd (BVHGPU_FILL_EVEN_ODD) / nonzero (BVHGPU_FILL_NONZERO); else
+ *   BVHGPU_POINT_OUTSIDE.  A point with a non-finite coordinate: class 0, winding 0.
+ *   f64 range: the signs are exact for coordinates that are zero or of magnitude in [2^-300, 2^300] (f32: every finite value).  A point
+ *   with a nonzero coordinate outside it gets class 3 and winding 0 and is not walked; a relevant segment with such a coordinate
+ *   contributes nothing and makes the point class 3 unless it is boundary.
+ *   EXACT for every tree the library builds or maintains (the walk enters "no split wins" empty boxes), as long as every segment lies
+ *   in its shape's box.
+ * bvhgpu_knn_segments_*x2: as bvhgpu_knn_triangles_*x3 (radius rule, stable sort by (key_s, s), padding BVHGPU_INVALID_INDEX / +inf /
+ *   NaN x 2, out_dist = fl(sqrt(key_s)), refusals), out_closest 2 T per slot.  key_s in T, in this order, without FMA:
+ *     ex = bx - ax; ey = by - ay; wx = px - ax; wy = py - ay; num = wx*ex + wy*ey; den = ex*ex + ey*ey;
+ *     q = a if num <= 0; q = b if num >= den; otherwise t = num / den, q = (ax + t*ex, ay + t*ey) (a NaN num lands here);
+ *     key = (px - qx)*(px - qx) + (py - qy)*(py - qy).
+ *   A NaN key never qualifies; nothing else is excluded (a zero-length segment is a point).  Guarantee, with the wording of
+ *   bvhgpu_knn_triangles_*: a segment is bounded at p when its key is not below box_lower_d2(p, AABB_s); where every qualifying
+ *   segment is bounded the row is the brute-force row bit for bit.  Every finite segment inside its box is bounded at every finite
+ *   point, at every scale (DESIGN.md section 4.23); a stale segment outside its box need not be.
+ * bvhgpu_signed_distance_*x2: out_shape, |out_dist| and out_closest (may be NULL) are bvhgpu_knn_segments_* with k = 1 and no radius,
+ *   bit for bit; out_dist is negated exactly where bvhgpu_contains_points_*x2 with the same rule gives class 1 (inside at distance 0
+ *   gives -0).  Boundary and undecided points keep a non-negative distance; a point without a qualifying segment keeps +inf.
+ * Refusals (nothing written): a null argument, n > 2^31-1, an unknown rule, k outside 1 .. BVHGPU_KNN_MAX_K, or a non-empty tree
+ * without segments: BVHGPU_ERR_INVALID.  A failed build is reported sticky, before missing segments.  n = 0: no-op.  An empty tree:
+ * class 0 / winding 0, rows of padding. */
+#define BVHGPU_POINT_OUTSIDE 0
+#define BVHGPU_POINT_INSIDE 1
+#define BVHGPU_POINT_BOUNDARY 2
+#define BVHGPU_POINT_UNDECIDED 3
+int bvhgpu_tree_set_segments_f32x2(bvhgpu_tree2f* tree, const float* segments, size_t n);
+int bvhgpu_tree_set_segments_f64x2(bvhgpu_tree2d* tree, const double* segments, size_t n);
+int bvhgpu_contains_points_f32x2(bvhgpu_tree2f* tree, const float* points, size_t n, int rule, uint8_t* out_class, int32_t* out_winding);
+int bvhgpu_contains_points_f64x2(bvhgpu_tree2d* tree, const double* points, size_t n, int rule, uint8_t* out_class, int32_t* out_winding);
+int bvhgpu_knn_segments_f32x2(bvhgpu_tree2f* tree, const float* points, size_t n, uint32_t k, const float* max_dist, uint32_t* out_shape,
+                              float* out_dist, float* out_closest);
+int bvhgpu_knn_segments_f64x2(bvhgpu_tree2d* tree, const double* points, size_t n, uint32_t k, const double* max_dist, uint32_t* out_shape,
+                              double* out_dist, double* out_closest);
+int bvhgpu_signed_distance_f32x2(bvhgpu_tree2f* tree, const float* points, size_t n, int rule, uint32_t* out_shape, float* out_dist,
+                                 float* out_closest);
+int bvhgpu_signed_distance_f64x2(bvhgpu_tree2d* tree, const double* points, size_t n, int rule, uint32_t* out_shape, double* out_dist,
+                                 double* out_closest);
 
 /* ---- self-overlap pairs: every pair of shapes of the tree whose AABBs intersect, each once (the broad phase of physics, mesh
  * self-intersection, duplicate and contact detection in point and particle sets).  leaf(s) = the preorder node index of shape s's leaf
